@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py — the driver's measurement contract for the fused FFT-convolution hot path.
 
-  python bench.py --gpus N --steps K --warmup W            # our sm_100a engine
+  python bench.py --gpus N --steps K --warmup W            # our sm_90a engine
   python bench.py --impl reference --gpus N --steps K ...  # reference arm: the reference's CPU path
                                                            # (tests/test_flashfftconv.py:5-13 oracle port)
 
@@ -36,7 +36,7 @@ WORKLOADS = {
     'c2': (8192, 16, 768, 8192, False),       # BASELINE.json configs[1]: M2-BERT dims, the metric's config
     'c3': (32768, 8, 1024, 16384, True),      # configs[2]: Hyena-style, gated, implicit 2x causal padding
     'c4': (1048576, 2, 128, 1048576, False),  # configs[3]: HyenaDNA long range, B x H shard over 1..4 GPUs
-    'c5': (4194304, 8, 64, 4194304, False),   # configs[4]: 8 x B200 B x H shard (H = 64 / n_gpus per rank)
+    'c5': (4194304, 8, 64, 4194304, False),   # configs[4]: 8-GPU B x H shard (H = 64 / n_gpus per rank)
     # the shape of the reference's own published table (README.md:224-231: gated conv, forward, "batch size 64, hidden
     # dimension 768", H100-SXM: 0.29 ms at N=1K, 3.58 ms at N=8K) — the small-size path (8192/N batch members per unit of
     # the 8192-point engine) and the gated 8192 kernel get a measured line too
@@ -63,17 +63,17 @@ def workload_string(name, world=1):
 
 
 def fwd_bytes(N, B, H, L, gated):
-    """SURVEY.md §8(d): fwd ungated 4L per conv (+4L gates when gated) plus k_f once per channel (4N)."""
+    """fwd ungated 4L per conv (+4L gates when gated) plus k_f once per channel (4N)."""
     return (8 if gated else 4) * L * B * H + 4 * N * H
 
 
 def bwd_bytes(N, B, H, L, gated):
-    """SURVEY.md §8(d): bwd ungated 6L per conv + 8N per channel (dk_f fp32); gated 14L per conv."""
+    """bwd ungated 6L per conv + 8N per channel (dk_f fp32); gated 14L per conv."""
     return (14 if gated else 6) * L * B * H + 8 * N * H
 
 
 def issued_tensor_flops(N, B, H):
-    """Matmul flops the inner 8192-point kernel issues (DESIGN.md §6): 25.2 MFLOP per unit (a pair of sequences of one
+    """Matmul flops the inner 8192-point kernel issues: 25.2 MFLOP per unit (a pair of sequences of one
     channel; an odd batch still runs a full unit), N/8192 units per pair for the composite sizes; the outer radix-128
     stage of the 1M+ sizes adds 2 x 128 x 256 x 2 flops per complex column."""
     unit = 2.0 * 128 * 128 * (2 * 256 + 2 * 128)
@@ -87,14 +87,13 @@ def issued_tensor_flops(N, B, H):
 
 
 def reference_tensor_flops(N, B, H):
-    """SURVEY.md §8(d) 'algorithmic flops per conv' of the reference's own factorisation, forward."""
+    """Algorithmic flops per conv of the reference's own factorisation, forward."""
     per_conv = {8192: 6.29e6, 32768: 41.9e6, 1 << 20: 1.88e9, 1 << 22: 10.7e9}.get(N)
     return per_conv * B * H if per_conv else None
 
 
 class ClockSampler(threading.Thread):
-    """nvidia-smi clocks + throttle reasons while the GPU is under the benchmark load
-    (B200_PROFILING.md 'clocks line'): one persistent `nvidia-smi -lms 100`, samples are time-stamped and only
+    """nvidia-smi clocks + throttle reasons while the GPU is under the benchmark load: one persistent `nvidia-smi -lms 100`, samples are time-stamped and only
     those taken inside a marked load window are summarised."""
     Q = ('clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,'
          'clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,'
@@ -183,8 +182,7 @@ def dist_setup():
         torch.cuda.set_device(local)
         dist.init_process_group('nccl', device_id=torch.device('cuda', local))
         # first collectives now, not inside the first timed loop's barrier: NCCL builds its communicator lazily and the
-        # launches right after that set-up are slow (seen as 0.18-0.19 ms instead of 0.157 ms per C2 step at 2 and 8 ranks;
-        # the same loop with the communicator warmed is rank-count independent, profiles/r2_step_diag.md)
+        # launches right after that set-up are slow, which would land in the first timed loop
         t = torch.zeros(1, device=torch.device('cuda', local))
         dist.all_reduce(t)
         dist.barrier()
@@ -210,13 +208,32 @@ def run_reference(args):
         'gpu_launches': 0}), _OUT_FD)
 
 
+# at most 16M float32 values (64 MB) per dump; a larger output is sampled at fixed, seeded positions
+DUMP_MAX_ELEMS = 1 << 24
+
+
+def dump_outputs(out_dir, outputs):
+    """Write each output as <out_dir>/<name>.npy in float32: the whole array when it is small enough, else the values at
+    DUMP_MAX_ELEMS sorted flat positions drawn with a fixed seed (the same positions for the same shape)."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    for name, t in outputs.items():
+        flat = t.detach().reshape(-1)
+        if flat.numel() > DUMP_MAX_ELEMS:
+            g = torch.Generator().manual_seed(0)
+            idx = torch.randint(0, flat.numel(), (DUMP_MAX_ELEMS,), generator=g).sort().values
+            flat = flat[idx.to(flat.device)]
+        np.save(os.path.join(out_dir, f'{name}.npy'), flat.float().cpu().numpy())
+
+
 class Ctx:
     pass
 
 
 def measure(cx, name, steps, warmup, headline=False):
     """One BASELINE config on this rank's GPU: whole forward step through the public module, the conv kernels alone
-    (k_f pre-packed; CUDA events on the launching stream), autograd forward+backward, host-buffer end to end."""
+    (k_f pre-packed; CUDA events on the launching stream), autograd forward+backward, host-buffer end to end.  Every
+    timed loop runs `steps` iterations.  headline: the output of the last timed forward step is kept in res['outputs']."""
     from flashfftconv import FlashFFTConv, _lib
     from flashfftconv.conv import _pack_kf, _ptr, _stream
     dev, world = cx.dev, cx.world
@@ -244,13 +261,13 @@ def measure(cx, name, steps, warmup, headline=False):
 
     # ---- (1) device-resident whole step through the public forward (k -> k_f -> conv kernels)
     launches = [0]
+    last = {}
 
     def step():
-        conv(u, k, *gates)
+        last['y'] = conv(u, k, *gates)
         launches[0] += conv.last_launches
     # device wake-up before the W warm-up steps: ~10 ms of the same step so that the first timed loop does not run on
-    # clocks still ramping from idle (seen with small W under torchrun: 0.18 vs 0.158 ms at C2); far below the ~100 ms of
-    # continuous load after which the board's power cap starts to pull the clocks down
+    # clocks still ramping from idle
     e0 = torch.cuda.Event(enable_timing=True); e1 = torch.cuda.Event(enable_timing=True)
     step(); e0.record(); step(); e1.record(); torch.cuda.synchronize()
     for _ in range(min(60, int(10.0 / max(e0.elapsed_time(e1), 1e-3)))):
@@ -262,6 +279,8 @@ def measure(cx, name, steps, warmup, headline=False):
     launches[0] = 0
     step_ms = timed(step, steps)
     step_launches = launches[0]
+    outputs = {'y': last.pop('y')} if headline else None
+    last.clear()
     fwd_peak = torch.cuda.max_memory_allocated(dev) - base_mem
     # inference: eval mode keeps the engine-order spectrum while the filter tensor is unmodified (k -> k_f only once)
     conv.eval()
@@ -308,7 +327,7 @@ def measure(cx, name, steps, warmup, headline=False):
         conv(ug, kg, *gg).backward(dout)
     for _ in range(2):
         fb()
-    fb_ms = timed(fb, max(2, steps // 2))
+    fb_ms = timed(fb, steps)
     fb_peak = torch.cuda.max_memory_allocated(dev) - base_mem
     del ug, kg, gg, dout
 
@@ -326,7 +345,7 @@ def measure(cx, name, steps, warmup, headline=False):
         # pipelined over batch chunks inside bffc_fwd_host (include/bffc.h)
         conv.forward_host(u_h, k_h, *g_h, out=y_h, device=dev)
     e2e_step()
-    e2e_ms = timed(e2e_step, max(2, min(steps, 5)))
+    e2e_ms = timed(e2e_step, steps)
 
     fb_bytes = fwd_bytes(N, B, H, L, gated) + bwd_bytes(N, B, H, L, gated)
     ab = fwd_bytes(N, B, H, L, gated)
@@ -354,6 +373,8 @@ def measure(cx, name, steps, warmup, headline=False):
                                 'benchmarks/benchmark.py:137-147)'},
     }
     res['fwd_eval_cached_kf']['ratio_to_kernels'] = eval_ms / kern_ms
+    if headline:
+        res['outputs'] = outputs
     return res
 
 
@@ -399,9 +420,10 @@ def run_ours(args):
         peaks = json.load(open(os.path.join(ROOT, 'MEASURED_PEAKS.json')))
     except Exception:
         pass
-    cx.hbm_peak = float(peaks.get('hbm_gbs', 6650.0))
-    bf16_peak = float(peaks.get('bf16_tflops', 0) or 1590.0)
-    peak_src = 'measured (MEASURED_PEAKS.json hbm_gbs)' if 'hbm_gbs' in peaks else 'fallback 6.65 TB/s'
+    # fallbacks: NVIDIA's H100 SXM data sheet (3.35 TB/s HBM3, 989 TFLOP/s dense BF16 at up to 700 W)
+    cx.hbm_peak = float(peaks.get('hbm_gbs', 3350.0))
+    bf16_peak = float(peaks.get('bf16_tflops', 0) or 989.0)
+    peak_src = 'measured (MEASURED_PEAKS.json hbm_gbs)' if 'hbm_gbs' in peaks else 'H100 SXM data sheet 3.35 TB/s'
 
     cx.sampler = ClockSampler(local) if rank == 0 else None
     if cx.sampler:
@@ -412,22 +434,21 @@ def run_ours(args):
     if cx.sampler:
         time.sleep(0.15)
         cx.sampler.stop()
+    outputs = head.pop('outputs')           # dumped before the side configs allocate their own tensors
+    if rank == 0 and args.dump_outputs:
+        dump_outputs(args.dump_outputs, outputs)
+    del outputs
     configs = {head_name: head}
     if args.workload is None:
         for name in ('c3', 'c4', 'c5', 'r1k', 'r8k'):
             torch.cuda.empty_cache()
             try:
-                configs[name] = measure(cx, name, max(3, min(args.steps, 5)), 3)
+                configs[name] = measure(cx, name, args.steps, args.warmup)
             except Exception as e:        # a side config must never take the headline line down
                 configs[name] = {'error': f'{type(e).__name__}: {e}'[:300]}
     if rank != 0:
         return
     N, B, H, L, gated = shard_shape(head_name, world)
-    traffic = None
-    try:
-        traffic = json.load(open(os.path.join(ROOT, 'profiles', 'roofline_traffic.json'))).get(head_name)
-    except Exception:
-        pass
     kern = head['kernels']
     out = {
         'metric': 'fftconv_fwd_convs_per_sec', 'value': head['fwd']['convs_per_sec'], 'unit': 'convs/s',
@@ -436,13 +457,11 @@ def run_ours(args):
         'config': {'workload': workload_string(head_name, world),
                    'step': 'k -> k_f (one library launch; cached while k is unchanged only in eval mode) + conv kernels',
                    'wake_up': '~10 ms of untimed steps per config before the W warm-up steps (clock ramp from idle)',
-                   'l2': f'inputs+outputs {kern["algorithmic_bytes"] / 1e6:.0f} MB per step exceed the 126 MB L2 (no flush needed)',
+                   'l2': f'inputs+outputs {kern["algorithmic_bytes"] / 1e6:.0f} MB per step exceed the 50 MB L2 (no flush needed)',
                    'sharding': 'B x H sharded over ranks, no data-path collective',
                    'fwd_bwd_convs_per_sec': head['fwd_bwd']['convs_per_sec'], 'fwd_bwd_ms_per_step': head['fwd_bwd']['ms_per_step'],
                    'host_numa_binding': cx.numa},
         'roofline': {'bound': 'hbm', 'achieved': kern['gbs'], 'peak': cx.hbm_peak, 'unit': 'GB/s', 'frac': kern['frac'],
-                     'traffic': traffic,
-                     'traffic_source': 'ncu --set full capture of this kernel, profiles/ (not re-measured by this run)',
                      'kernel': 'bffc forward conv kernels of the headline config (k_f pre-packed)',
                      'kernel_ms': kern['ms'], 'algorithmic_bytes': kern['algorithmic_bytes'], 'peak_source': peak_src,
                      'kernel_convs_per_sec': kern['convs_per_sec_per_gpu'],
@@ -496,7 +515,11 @@ def _main(saved_fd):
     ap.add_argument('--impl', default='ours', choices=['ours', 'reference'])
     ap.add_argument('--workload', default=None, choices=sorted(WORKLOADS),
                     help='measure only this config (default: headline c2 + c3, c4, c5 under roofline.configs)')
+    ap.add_argument('--dump-outputs', default=None, metavar='DIR',
+                    help='write the output of the last timed headline step to DIR/<name>.npy (float32)')
     args = ap.parse_args()
+    if args.dump_outputs and args.impl == 'reference':
+        ap.error('--dump-outputs dumps the GPU path of --impl ours; the reference arm times a CPU sample only')
     args.warmup = max(args.warmup, 3) if args.impl == 'ours' else args.warmup
     if args.impl == 'reference':
         run_reference(args)

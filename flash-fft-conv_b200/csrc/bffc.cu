@@ -66,9 +66,9 @@ int check_device() {
     return fail(BFFC_ERR_NO_DEVICE, "no CUDA device available (bffc has no CPU fallback)");
   }
   int major = 0;
-  if (cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev) != cudaSuccess || major != 10) {
+  if (cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev) != cudaSuccess || major != 9) {
     cudaGetLastError();
-    return fail(BFFC_ERR_NO_DEVICE, "device %d is not sm_100 (compute capability major %d)", dev, major);
+    return fail(BFFC_ERR_NO_DEVICE, "device %d is not sm_90 (compute capability major %d)", dev, major);
   }
   return 0;
 }
@@ -143,7 +143,7 @@ __global__ void kf_pack_kernel(const float2* __restrict__ kf_nat, uint4* __restr
   (void)R;
 }
 
-// Tiled variant for a large outermost radix R0 (tcgen05 outer stage, R0 = 128): consecutive c0 are adjacent in the
+// Tiled variant for a large outermost radix R0 (tensor-core outer stage, R0 = 128): consecutive c0 are adjacent in the
 // natural order, consecutive words are adjacent in the engine rows, so a (32 c0) x (32 word pairs) tile goes
 // through shared memory and both sides are accessed in 256-byte runs.
 // grid: (8192/2/32 word-pair tiles, R0/32 * R1, H)
@@ -181,11 +181,11 @@ __global__ void kf_pack_tiled_kernel(const float2* __restrict__ kf_nat, uint2* _
   (void)R;
 }
 
-constexpr int kInner = 8192;   // the fused tcgen05 kernel's size
+constexpr int kInner = 8192;   // the fused tensor-core kernel's size
 
 }  // namespace
 
-struct bffc_level { int tc; int R; };   // tc = 1: tcgen05 radix-128 stage (outer_r128.cuh); 0: CUDA-core radix 2/4/8
+struct bffc_level { int tc; int R; };   // tc = 1: tensor-core radix-128 stage (outer_r128.cuh); 0: CUDA-core radix 2/4/8
 
 struct bffc_plan {
   int NE;        // engine FFT size: N for N >= 8192; 8192 for the small sizes (256..4096): 8192/N batch members of a
@@ -332,7 +332,7 @@ int bffc_plan_create(bffc_plan** out, int seqlen, int dtype) {
     PLAN_TRY(cudaFuncSetAttribute(fwd3_kernel<true, false, F>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemTotal3));
     PLAN_TRY(cudaFuncSetAttribute(dkf3_kernel<true, F>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemTotalDkf3));
     PLAN_TRY(cudaFuncSetAttribute(dkf3_kernel<false, F>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemTotalDkf3));
-    PLAN_TRY(cudaFuncSetAttribute(outer_tc_kernel<false, F>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemOuterGated));
+    PLAN_TRY(cudaFuncSetAttribute(outer_tc_kernel<false, F>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemOuter));
     PLAN_TRY(cudaFuncSetAttribute(outer_tc_kernel<true, F>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemOuter));
     PLAN_TRY(cudaFuncSetAttribute(bffc::ffft::kf_from_filter_kernel<F>, cudaFuncAttributeMaxDynamicSharedMemorySize, bffc::ffft::kSmemBytes));
   );
@@ -357,7 +357,7 @@ int bffc_fft_size(const bffc_plan* p) { return p ? p->NE : 0; }
 int bffc_length_multiple(const bffc_plan* p) {
   if (!p) return 0;
   if (p->nlev == 0) return 64;                       // fused kernel: TMA tiles of 64 columns
-  if (p->lev[0].tc) return p->N / 128;               // tcgen05 outer stage: whole rows of the [128][N/128] view
+  if (p->lev[0].tc) return p->N / 128;               // tensor-core outer stage: whole rows of the [128][N/128] view
   return 8;                                          // CUDA-core outer stage: 16-byte vectors
 }
 
@@ -422,8 +422,8 @@ static size_t filter_pair_bytes(const bffc_plan* p) { return size_t(2) * (p->R /
 size_t bffc_filter_workspace_bytes(const bffc_plan* p, int H) {
   if (!p || H <= 0 || p->NE == kInner) return 0;
   const size_t pairs = size_t(H + 1) / 2, per = filter_pair_bytes(p);
-  // one group when it fits 576 MB (C4: 128 channels x 65 rows x 64 KB = 520 MB): the two launches are latency / issue
-  // bound rather than HBM bound, so fewer, larger launches beat L2-sized groups (profiles/r2_filter_fft.md)
+  // one group when it fits 576 MB (C4: 128 channels x 65 rows x 64 KB = 520 MB): fewer, larger launches rather than
+  // L2-sized groups, each of which would pay the launch latency of the two kernels
   size_t group = (size_t(576) << 20) / per;
   if (group < 1) group = 1;
   return (pairs < group ? pairs : group) * per;
@@ -545,10 +545,9 @@ struct View { int B, H, Hs, h0; };
 
 // Composite sizes can run chunk by chunk: `sets` plane sets of one chunk take at most ~kPlaneBudget bytes.  Channels
 // first (the k_f rows of a channel are then shared by its batch pairs inside one chunk); a single channel that is too
-// large is cut over batch pairs.  Measured (profiles/r2_chunking.md): L2-sized chunks (40 MB, planes resident in the
-// 126 MB L2) LOSE — C3 0.72 -> 1.00 ms, C4 0.85 -> 1.23 ms, C5 1.16 -> 2.52 ms — because every chunk pays the launch
-// gaps, prologues and tails of 3-5 small persistent launches.  The budget therefore only bounds the workspace (and with
-// it the peak memory of a call): 4 GB of plane sets per chunk.
+// large is cut over batch pairs.  Every chunk pays the launch gaps, prologues and tails of 3-5 persistent launches, so
+// chunks are not cut to L2 size; the budget only bounds the workspace (and with it the peak memory of a call): 4 GB of
+// plane sets per chunk.
 constexpr size_t kPlaneBudget = size_t(4) << 30;
 static View chunk_view(const bffc_plan* p, int B, int H, int sets) {
   const size_t item = size_t(sets) * p->N * 4;                     // one (pair, channel) in all plane sets
@@ -627,29 +626,7 @@ static void fill_params(const bffc_plan* p, bffc::FwdParams& prm, const void* kf
   prm.y2 = nullptr;
   prm.xg_out = nullptr;
   prm.kf_conj_mask = 0;
-  prm.trace = nullptr;
 }
-
-#ifdef BFFC_BRINGUP
-// bring-up builds only (nvcc -DBFFC_BRINGUP): BFFC_TRACE=<file> makes every ungated fused launch record the phase
-// timeline of CTA 0 (tools/trace_fwd3.py).  Not compiled into the product library.
-static long long* g_trace = nullptr;
-static long long* trace_buffer() {
-  static bool init = false;
-  if (!init) {
-    init = true;
-    if (getenv("BFFC_TRACE")) cudaMalloc(&g_trace, 3 * 2 * 64 * 16 * sizeof(long long));
-  }
-  if (g_trace) cudaMemset(g_trace, 0, 3 * 2 * 64 * 16 * sizeof(long long));
-  return g_trace;
-}
-static void trace_dump(cudaStream_t st) {
-  std::vector<long long> h(3 * 2 * 64 * 16);
-  cudaStreamSynchronize(st);
-  cudaMemcpy(h.data(), g_trace, h.size() * sizeof(long long), cudaMemcpyDeviceToHost);
-  if (FILE* f = fopen(getenv("BFFC_TRACE"), "wb")) { fwrite(h.data(), sizeof(long long), h.size(), f); fclose(f); }
-}
-#endif
 
 // Segment geometry of the input tiles: S = 8192/N batch members per 8192-point unit for the small sizes, else 1.
 struct SegGeom { int S, seg_rows, groups, kmask; };
@@ -712,15 +689,8 @@ static int launch_fused(const bffc_plan* p, const void* u, const void* kf, const
   FMT_SWITCH(p->dtype,
     if (gated)
       fwd3_kernel<false, true, F><<<g3, kThreads3, kSmemTotal3, st>>>(tm_u, tm_y, tm_g, gm, prm);
-    else {
-#ifdef BFFC_BRINGUP
-      prm.trace = trace_buffer();
-#endif
+    else
       fwd3_kernel<false, false, F><<<g3, kThreads3, kSmemTotal3, st>>>(tm_u, tm_y, tm_g, gm, prm);
-#ifdef BFFC_BRINGUP
-      if (prm.trace) trace_dump(st);
-#endif
-    }
   );
   CUDA_TRY(cudaGetLastError());
   return BFFC_OK;
@@ -776,8 +746,7 @@ static void launch_cc(const bffc_plan* p, bool inverse, bool gated, bool planes,
                       int rows, cudaStream_t st) {
   using namespace bffc::outer;
   OuterParams op = op_in;
-  // read-ahead distance = the number of resident blocks (one residency period ahead; measured optimum at C3:
-  // 0 -> 0.827 ms, 296 -> 0.690, 592 -> 0.693, 1184 -> 0.725, 2368 -> 0.985 ms for the three kernels)
+  // read-ahead distance = the number of resident blocks (one residency period ahead)
   op.lookahead = p->num_sms * (R <= 4 ? 4 : 2);
   const int cb = op.M / (kVec * 128);
   if (planes) {
@@ -807,7 +776,7 @@ static int cc_stage(const bffc_plan* p, int R, bool inverse, bool gated, bool pl
   return BFFC_OK;
 }
 
-// tcgen05 radix-128 level 0: real endpoint x (u or y), gate g (pregate fwd / postgate inv), planes set A
+// tensor-core radix-128 level 0: real endpoint x (u or y), gate g (pregate fwd / postgate inv), planes set A
 static int tc_stage(const bffc_plan* p, bool inverse, const void* x, const void* gate, PlaneSet A, View v, int L,
                     cudaStream_t st, const void* gate2 = nullptr, void* x2 = nullptr) {
   const int B = v.B, H = v.H;
@@ -835,9 +804,9 @@ static int tc_stage(const bffc_plan* p, bool inverse, const void* x, const void*
   using namespace bffc::r128;
   FMT_SWITCH(p->dtype,
     if (!inverse)
-      outer_tc_kernel<false, F><<<grid, kThreads, prm.has_pregate ? kSmemOuterGated : kSmemOuter, st>>>(tm_x, tm_pr, tm_pi, tm_g, prm);
+      outer_tc_kernel<false, F><<<grid, kThreadsOuter, kSmemOuter, st>>>(tm_x, tm_pr, tm_pi, tm_g, prm);
     else
-      outer_tc_kernel<true, F><<<grid, kThreads, kSmemOuter, st>>>(tm_x, tm_pr, tm_pi, tm_g, prm);
+      outer_tc_kernel<true, F><<<grid, kThreadsOuter, kSmemOuter, st>>>(tm_x, tm_pr, tm_pi, tm_g, prm);
   );
   CUDA_TRY(cudaGetLastError());
   return BFFC_OK;
@@ -1115,8 +1084,8 @@ int bffc_bwd(const bffc_plan* p, const void* dout, const void* u, const void* kf
 }
 
 // ---------------------------------------------------------------------------------------------- host streaming
-// Chunk geometry of the host pipeline: bc batch members x hc channels per chunk, ~12 MB per chunk tensor — a copy of
-// ~0.25 ms (PCIe 5 x16) still runs at link speed, and the fill / drain of the three-stage pipeline (one chunk copy-in
+// Chunk geometry of the host pipeline: bc batch members x hc channels per chunk, ~12 MB per chunk tensor — large enough
+// that a copy runs at link speed, and the fill / drain of the three-stage pipeline (one chunk copy-in
 // before, one copy-out after the overlapped part) stays small.  bc is even so that batch pairs stay together; wide
 // rows (H*L*2 bytes > 6 MB) are split over channels instead and moved with pitched (2-D) copies.
 struct HostChunk { int bc, hc; };

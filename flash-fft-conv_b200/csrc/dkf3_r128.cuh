@@ -1,4 +1,4 @@
-// Backward filter-gradient kernel, N = 128 x 64 (= 8192), sm_100a: dk_f[h] = sum over batch pairs of
+// Backward filter-gradient kernel, N = 128 x 64 (= 8192), sm_90a: dk_f[h] = sum over batch pairs of
 // FFT(z_dout) * conj(FFT(z_u)), z = x_b + i x_{b+1}.
 //
 // Path replaced (reference): the dk_f part of monarch_conv_bwd_cuda_kernel
@@ -14,23 +14,12 @@
 // so summing the packed products over pairs gives exactly dk.  An odd batch is completed with an all-zero
 // partner (TMA out-of-bounds fill).
 //
-// Machine mapping (warp-specialised, software-pipelined): a strictly serial stage 1 -> pass 1 -> stage 2 -> accumulate
-// chain per pair leaves the tensor pipe idle during the passes and the CUDA cores during the MMAs (measured on the
-// first version of this kernel: tensor pipe 31 % active, 8.6 k cycles per pair against 3.1 k of MMA work).  Here
-//  * the stage-2 A operands live in shared memory (as in fwd3_r128.cuh), which leaves TMEM room for a THIRD 128-column
-//    accumulator: u and dout of pair n use buffers (2n) % 3 and (2n + 1) % 3, so stage 1 of u(n+1) runs while pair n is
-//    still being accumulated and stage 1 of dout(n+1) while pass 1 of u(n+1) runs;
-//  * a fifth warpgroup holds the ISSUER warp (TMA loads and every MMA, in program order).  A tcgen05.mma blocks its
-//    thread while the tensor pipe's short queue is full, i.e. for most of a stage; an issuer that also had a share of
-//    the passes would stall the other 15 warps at the next hand-over for exactly that long;
-//  * hand-overs are mbarriers only: tcgen05.commit -> compute warps, one arrive per compute warp -> issuer.  The
-//    compute warps never wait for each other.
-// Input slots are released as soon as stage 1 has consumed them (A tiles have their own buffers), so the TMA loads run
-// two pairs ahead.  Gated backward: the caller hands in u*pregate and dout*postgate (composite sizes: the outer stage
-// applies the gates on load; seqlen <= 8192: an elementwise pre-pass, see bffc_bwd).
-//
-//   tensor pipe:  S1d(n) | S2u(n) | S2d(n) | S1u(n+1) | S1d(n+1) | ...
-//   CUDA cores :  acc(n-1) | pass1 u(n) | pass1 d(n) | acc(n) | pass1 u(n+1) | ...
+// Machine mapping: two warpgroups, rows k1 = 0..63 / 64..127 of the 128 x 64 spectrum.  Per pair: stage 1 (DFT-128,
+// wgmma, A = DFT-128 image in shared memory) -> pass 1 (twiddles) -> stage 2 (radix 64, A from registers) for u, whose
+// spectrum is parked in a thread-private shared-memory area; the same for dout, then the product is accumulated in
+// registers.  The TMA loads of the next pair are issued as soon as stage 1 has consumed an input slot.  Gated
+// backward: the caller hands in u*pregate and dout*postgate (composite sizes: the outer stage applies the gates on
+// load; seqlen <= 8192: an elementwise pre-pass, see bffc_bwd).
 #pragma once
 #include "fwd3_r128.cuh"
 
@@ -49,73 +38,52 @@ struct DkfParams {
 
 namespace r128 {
 
-constexpr int kSmemDkf3Slots = 4 * kSlotBytes;                 // u slot 0/1, dout slot 0/1
-constexpr int kSmemDkf3A = 2 * kSlotBytes;                     // A tiles of u, of dout
-constexpr int kSmemTotalDkf3 = kSmemDkf3Slots + kSmemDkf3A + kSmemG + 128 + 1024;
-constexpr int kThreadsDkf3 = 640;                              // 4 compute warpgroups + the issuer's warpgroup
-constexpr int kComputeWarps = 16;
+constexpr int kThreadsDkf3 = kPipeThreads;
+constexpr int kSmemDkf3Slots = 2 * kSlotBytes;                 // u slot, dout slot
+constexpr int kSmemDkf3Park = kThreadsDkf3 * 64 * 4;           // spectrum of u: 64 fp32 per thread
+constexpr int kSmemTotalDkf3 = kSmemDkf3Slots + kSmemF + kSmemG + kSmemDkf3Park + 64 + 1024;
+static_assert(kSmemTotalDkf3 <= 227 * 1024, "shared memory per block");
 
 template <bool kPlanes, int kFmt = 1>
 __global__ void __launch_bounds__(kThreadsDkf3, 1)
 dkf3_kernel(const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CUtensorMap tm_d,
             const __grid_constant__ CUtensorMap tm_ui, const __grid_constant__ CUtensorMap tm_di, const DkfParams p) {
-  using NT = Num<kFmt>;
-  constexpr uint32_t ID_N128_MN = Idesc<kFmt>::N128_MN, ID_N64_MN = Idesc<kFmt>::N64_MN, ID_N64_MN_NEG = Idesc<kFmt>::N64_MN_NEG;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t sbase = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t s_au = sbase + kSmemDkf3Slots, s_ad = s_au + kSlotBytes;
-  const uint32_t s_g = s_ad + kSlotBytes;
-  const uint32_t s_bars = s_g + kSmemG;
   uint8_t* gen_base = smem_raw + (sbase - smem_u32(smem_raw));
+  const uint32_t s_f = sbase + kSmemDkf3Slots;
+  const uint32_t s_g = s_f + kSmemF;
+  const uint32_t s_park = s_g + kSmemG;
+  const uint32_t s_bars = s_park + kSmemDkf3Park;
 
   const int tid = threadIdx.x;
-  const int wg = __shfl_sync(0xffffffffu, tid >> 7, 0);     // warpgroup = column quarter (warp-uniform)
-  const int lane = tid & 127;                               // TMEM lane = k1
-  const int warp_q = (tid >> 5) & 3;
-  const bool issuer_warp = (tid >> 5) == kComputeWarps;     // first warp of the fifth warpgroup: stage 1 + loads
-  const bool issuer2_warp = (tid >> 5) == kComputeWarps + 1;  // second warp: stage 2
-  const bool compute = tid < 512;
+  const int hf = (tid >> 7) & 1;
+  const bool leader = tid == 0;
+  const FragPos fp(tid);
+  const uint32_t bar_tma_u = s_bars, bar_tma_d = s_bars + 8, bar_g = s_bars + 16;
 
-  // barriers: TMA full [which: u/d][slot]; MMA done: stage 1 of u, stage 1 of dout, stage 2 (both); DFT-64 tiles;
-  // compute -> issuer: pass 1 of u done, pass 1 of dout done, accumulate done (one arrival per compute warp)
-  const uint32_t bar_tma_u = s_bars, bar_tma_d = s_bars + 16;
-  const uint32_t bar_s1u = s_bars + 32, bar_s1d = s_bars + 40, bar_s2 = s_bars + 48, bar_g = s_bars + 56;
-  const uint32_t bar_p1u = s_bars + 72, bar_p1d = s_bars + 80, bar_acc = s_bars + 88;
-  const uint32_t bar_s1u_odd = s_bars + 96;          // stage 1 of u completes on bar_s1u (even pairs) / bar_s1u_odd (odd pairs)
-  const uint32_t s_tmemptr = s_bars + 64;
-
-  if (tid == 0) {
+  if (leader) {
     tma_prefetch_desc(&tm_u);
     tma_prefetch_desc(&tm_d);
     if (kPlanes) { tma_prefetch_desc(&tm_ui); tma_prefetch_desc(&tm_di); }
-    for (int i = 0; i < 8; ++i) mbar_init(s_bars + 8 * i, 1);
-    mbar_init(bar_p1u, kComputeWarps); mbar_init(bar_p1d, kComputeWarps); mbar_init(bar_acc, kComputeWarps);
-    mbar_init(bar_s1u_odd, 1);
+    mbar_init(bar_tma_u, 1); mbar_init(bar_tma_d, 1); mbar_init(bar_g, 1);
     fence_barrier_init();
   }
-  if (tid < 32) {
-    tmem_alloc(s_tmemptr, 512);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *reinterpret_cast<volatile uint32_t*>(gen_base + kSmemDkf3Slots + kSmemDkf3A + kSmemG + 64);
-  const uint32_t tlane = tmem_base + (uint32_t(warp_q * 32) << 16);
 
   // work split: the H * pairs units (channel-major: g = h * pairs + pr) are cut into gridDim.x contiguous ranges, so the
-  // grid is not limited by the channel count (H = 64 still fills 148 SMs) and no CTA carries a whole extra channel
-  // (768 channels on 148 CTAs used to be 6 vs 5).  A channel that straddles two CTAs is completed by both through
-  // fp32 reductions into the zero-initialised gradient (red.global.add), as is every other flush.
+  // grid is not limited by the channel count and no CTA carries a whole extra channel.  A channel that straddles two
+  // CTAs is completed by both through fp32 reductions into the zero-initialised gradient (red.global.add), as is every
+  // other flush.
   const long long total = (long long)p.H * p.pairs;
   const int g_begin = int(total * blockIdx.x / gridDim.x), g_end = int(total * (blockIdx.x + 1) / gridDim.x);
   const int n_units = g_end - g_begin;
   auto unit_h = [&](int n) { return (g_begin + n) / p.pairs; };
   auto unit_pr = [&](int n) { return (g_begin + n) % p.pairs; };
-  auto issue_load = [&](int n, int which) {          // which: 0 = u pair, 1 = dout pair; slot = n & 1
-    const int h = unit_h(n), pr = unit_pr(n), slot = n & 1;
-    const uint32_t bar = (which ? bar_tma_d : bar_tma_u) + 8 * slot;
-    const uint32_t dst = sbase + (2 * which + slot) * kSlotBytes;
+  auto issue_load = [&](int n, int which) {          // which: 0 = u pair, 1 = dout pair
+    const int h = unit_h(n), pr = unit_pr(n);
+    const uint32_t bar = which ? bar_tma_d : bar_tma_u;
+    const uint32_t dst = sbase + which * kSlotBytes;
     const CUtensorMap* tm = which ? &tm_d : &tm_u;
     mbar_expect_tx(bar, kSlotBytes);
     if (kPlanes) {
@@ -127,239 +95,80 @@ dkf3_kernel(const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CU
     }
   };
   // everything stage 1 needs from global memory is requested up front
-  if (issuer_warp) {
-    if (elect_one()) {
-      for (int n = 0; n < 2 && n < n_units; ++n) { issue_load(n, 0); issue_load(n, 1); }
-      mbar_expect_tx(bar_g, kSmemG);
-      for (int c = 0; c < kSmemG; c += 8192) bulk_load(s_g + c, reinterpret_cast<const uint8_t*>(p.gtiles) + c, 8192, bar_g);
-    }
-    __syncwarp();
+  if (leader) {
+    if (n_units > 0) { issue_load(0, 0); issue_load(0, 1); }
+    mbar_expect_tx(bar_g, kSmemG);
+    for (int c = 0; c < kSmemG; c += 8192) bulk_load(s_g + c, reinterpret_cast<const uint8_t*>(p.gtiles) + c, 8192, bar_g);
   }
-  // DFT-128 -> TMEM columns 0..127: warpgroups 0,1 load cos (32 columns each), 2,3 sin
-  if (compute) {
-    const int hf = wg & 1;
-    const uint4* row = reinterpret_cast<const uint4*>((wg < 2 ? p.dftC : p.dftS) + lane * 128) + hf * 8;
-    const uint32_t tcol = tlane + (wg < 2 ? kColC : kColS) + 32 * hf;
-#pragma unroll
-    for (int q = 0; q < 2; ++q) {
-      uint32_t v[16];
-#pragma unroll
-      for (int r = 0; r < 4; ++r) {
-        uint4 w = row[q * 4 + r];
-        v[4 * r + 0] = w.x; v[4 * r + 1] = w.y; v[4 * r + 2] = w.z; v[4 * r + 3] = w.w;
-      }
-      tmem_st16(tcol + 16 * q, v);
-    }
-    tmem_st_wait();
-  }
-  tc_fence_before();
-  __syncthreads();          // the only CTA-wide barrier after set-up: DFT-128 is in TMEM
-  tc_fence_after();
+  load_dft128(gen_base + kSmemDkf3Slots, p.dftC, p.dftS, tid, kThreadsDkf3);
+  RowTw tw[2];
+  const float tw_inv = 1.0f / float(p.tw_n);
+  tw[0].init(fp.r0 & p.tw_mask, fp.q, tw_inv);
+  tw[1].init((fp.r0 + 8) & p.tw_mask, fp.q, tw_inv);
+  fence_proxy_async_smem();
+  __syncthreads();
+  mbar_wait(bar_g, 0);
 
-  auto dcol = [&](int idx) { return uint32_t(128 + 128 * (idx % 3)); };      // accumulator buffer -> TMEM column
+  Acc d;
+  d.zero();
+  float acc[64];
+#pragma unroll
+  for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+  uint32_t are[4][4], aim[4][4];
+  float4* park = reinterpret_cast<float4*>(gen_base + (s_park - sbase)) + tid;
 
-  if (!compute) {
-    // ======================================================================================= issuer warpgroup
-    if ((!issuer_warp && !issuer2_warp) || n_units == 0) return;
-    const uint32_t tC0 = tmem_base + kColC, tS0 = tmem_base + kColS;
-    // stage 1 (TS): D = F128 * X, X = the two tiles of a slot
-    auto issue_s1 = [&](uint32_t sX, uint32_t tD0) {
-      const uint64_t dXr = tile_desc(sX), dXi = tile_desc(sX + kTileBytes);
-      if (p.kmask == 0xff) {
-#pragma unroll
-        for (int s = 0; s < 8; ++s) mma_ts(tD0, tC0 + 8 * s, dXr + 128 * s, ID_N128_MN, s > 0);
-#pragma unroll
-        for (int s = 0; s < 8; ++s) mma_ts(tD0, tS0 + 8 * s, dXi + 128 * s, ID_N64_MN, 1);
-#pragma unroll
-        for (int s = 0; s < 8; ++s) mma_ts(tD0 + 64, tS0 + 8 * s, dXr + 128 * s, ID_N64_MN_NEG, 1);
-      } else {
-        uint32_t acc = 0;
-        for (int s = 0; s < 8; ++s)
-          if ((p.kmask >> s) & 1) { mma_ts(tD0, tC0 + 8 * s, dXr + 128 * s, ID_N128_MN, acc); acc = 1; }
-        for (int s = 0; s < 8; ++s)
-          if ((p.kmask >> s) & 1) mma_ts(tD0, tS0 + 8 * s, dXi + 128 * s, ID_N64_MN, 1);
-        for (int s = 0; s < 8; ++s)
-          if ((p.kmask >> s) & 1) mma_ts(tD0 + 64, tS0 + 8 * s, dXr + 128 * s, ID_N64_MN_NEG, 1);
-      }
-    };
-    // stage 2 (SS): radix-64, A tiles in shared memory, accumulator rewritten in place
-    auto issue_s2 = [&](uint32_t sA, uint32_t tD0) {
-      const uint64_t dAr = atile_desc(sA), dAi = atile_desc(sA + kTileBytes);
-      const uint64_t dG0 = pair_desc(s_g, 8192), dG1 = pair_desc(s_g + 16384, 8192);
-#pragma unroll
-      for (int s = 0; s < 4; ++s) mma_ss(tD0, dAr + 2 * s, dG0 + 128 * s, ID_N128_MN, s > 0);
-#pragma unroll
-      for (int s = 0; s < 4; ++s) mma_ss(tD0, dAi + 2 * s, dG1 + 128 * s, ID_N128_MN, 1);
-    };
-    // Two issuing warps.  A single thread that waits on every hand-over, issues all 64 MMAs of a pair and the TMA loads
-    // runs ~600 dependent uniform-datapath instructions per pair: 7.2 k cycles against the 3.1 k cycles of tensor work
-    // it has to feed (profiles/r2_dkf3_ncu_summary.txt: tensor pipe 42 % active, compute warps waiting on stage
-    // completions).  Warp 16 issues stage 1 of both inputs and the loads, warp 17 stage 2.  Stage 1 of u(n+1) is queued
-    // right behind stage 1 of dout(n) (its accumulator held dout(n-1): free since acc(n-1)); because that lets its
-    // completion overtake slow observers of stage 1 of u(n), the two alternate between two barriers.
-    auto s1u_bar = [&](int n) { return (n & 1) ? bar_s1u_odd : bar_s1u; };
-    if (issuer2_warp) {
-      mbar_wait(bar_g, 0);
-      for (int n = 0; n < n_units; ++n) {
-        const uint32_t par = n & 1;
-        mbar_wait(bar_p1u, par);
-        tc_fence_after();
-        if (elect_one()) issue_s2(s_au, tmem_base + dcol(2 * n));
-        __syncwarp();
-        mbar_wait(bar_p1d, par);
-        tc_fence_after();
-        if (elect_one()) {
-          issue_s2(s_ad, tmem_base + dcol(2 * n + 1));
-          mma_commit(bar_s2);                         // this thread's MMAs: stage 2 of u(n) and of dout(n)
-        }
-        __syncwarp();
-      }
-      return;
-    }
-    mbar_wait(bar_tma_u, 0);
-    tc_fence_after();
-    if (elect_one()) {
-      issue_s1(sbase, tmem_base + dcol(0));
-      mma_commit(bar_s1u);
-    }
-    __syncwarp();
-    for (int n = 0; n < n_units; ++n) {
-      const int slot = n & 1;
-      const uint32_t par = n & 1;
-      // stage 1 of dout(n): its accumulator held u(n-1), released by the accumulate pass of pair n-1
-      mbar_wait(bar_tma_d + 8 * slot, (n >> 1) & 1);
-      if (n > 0) mbar_wait(bar_acc, (n - 1) & 1);
-      tc_fence_after();
-      if (elect_one()) {
-        issue_s1(sbase + (2 + slot) * kSlotBytes, tmem_base + dcol(2 * n + 1));
-        mma_commit(bar_s1d);
-      }
-      __syncwarp();
-      if (n + 1 < n_units) {                          // stage 1 of u(n+1) into the third accumulator
-        mbar_wait(bar_tma_u + 8 * (slot ^ 1), ((n + 1) >> 1) & 1);
-        tc_fence_after();
-        if (elect_one()) {
-          issue_s1(sbase + (slot ^ 1) * kSlotBytes, tmem_base + dcol(2 * n + 2));
-          mma_commit(s1u_bar(n + 1));                 // fires when this thread's earlier MMAs (incl. dout(n)) are done too
-        }
-        __syncwarp();
-      }
-      // input slots are free once their stage 1 has run: fetch pair n+2 into them
-      if (n + 2 < n_units) {
-        mbar_wait(s1u_bar(n), (n >> 1) & 1);
-        if (elect_one()) issue_load(n + 2, 0);
-        __syncwarp();
-        mbar_wait(bar_s1d, par);
-        if (elect_one()) issue_load(n + 2, 1);
-        __syncwarp();
-      }
-    }
-    return;
-  }
-
-  // ========================================================================================= compute warpgroups
-  // twiddles W_8192^{k1 j} of this thread's 16 columns j = 16 wg + (0..15), as 8 packed pairs (cos, sin), scaled
-  __half2 twc[8], tws[8];
-#pragma unroll
-  for (int q = 0; q < 8; ++q) {
-    float s0, c0, s1, c1;
-    const int kl = lane & p.tw_mask;
-    const float tw_inv = 1.0f / float(p.tw_n);
-    sincospif(-2.0f * float((kl * (16 * wg + 2 * q)) & (p.tw_n - 1)) * tw_inv, &s0, &c0);
-    sincospif(-2.0f * float((kl * (16 * wg + 2 * q + 1)) & (p.tw_n - 1)) * tw_inv, &s1, &c1);
-    twc[q] = __floats2half2_rn(c0 * p.tw_scale, c1 * p.tw_scale);
-    tws[q] = __floats2half2_rn(s0 * p.tw_scale, s1 * p.tw_scale);
-  }
-  // pass 1 of this warpgroup's column quarter: * W^{k1 j} -> K-major swizzled A tiles (re, im)
-  auto pass1 = [&](uint32_t tD, uint32_t sA) {
-    uint32_t re[16], im[16];
-    tmem_ld16(tD + 16 * wg, re);
-    tmem_ld16(tD + 64 + 16 * wg, im);
-    tmem_ld_wait();
-    reg_fence(re); reg_fence(im);
-#pragma unroll
-    for (int blk = 0; blk < 2; ++blk) {
-      uint32_t ore[4], oim[4];
-#pragma unroll
-      for (int q = 0; q < 4; ++q) {
-        const float2 c = __half22float2(twc[4 * blk + q]), sn = __half22float2(tws[4 * blk + q]);
-        f32x2 vr, vi;
-        cmul2(pk2u(re[8 * blk + 2 * q], re[8 * blk + 2 * q + 1]), pk2u(im[8 * blk + 2 * q], im[8 * blk + 2 * q + 1]),
-              pk2(c.x, c.y), pk2(sn.x, sn.y), vr, vi);
-        ore[q] = NT::pack_v(vr);
-        oim[q] = NT::pack_v(vi);
-      }
-      const uint32_t off = uint32_t(lane) * 128u + (uint32_t((2 * wg + blk) ^ (lane & 7)) << 4);
-      st_shared_v4(sA + off, ore[0], ore[1], ore[2], ore[3]);
-      st_shared_v4(sA + kTileBytes + off, oim[0], oim[1], oim[2], oim[3]);
-    }
+  // stage 1 -> pass 1 -> stage 2 of one input of pair n; the input slot is refilled with pair n + 1 once stage 1 of
+  // both warpgroups has read it
+  auto spectrum = [&](int n, int which) {
+    mbar_wait(which ? bar_tma_d : bar_tma_u, n & 1);
+    f128_stage<kFmt, false>(d, s_f, hf, sbase + which * kSlotBytes, p.kmask);
+    wgmma_wait_regs(d);
+    named_bar_sync(1, kThreadsDkf3);
+    if (leader && n + 1 < n_units) issue_load(n + 1, which);
+    twiddle_frag<false>(d, tw, p.tw_scale);
+    frag_to_a<kFmt>(d, are, aim);
+    r64_stage<kFmt>(d, are, aim, s_g, s_g + 2 * kGTileBytes, s_g + kGTileBytes, s_g);
+    wgmma_wait_regs(d);
   };
-  // this warp's TMEM reads / shared-memory writes are finished: tell the issuer
-  auto hand_over = [&](uint32_t bar) {
-    fence_proxy_async_smem();
-    tc_fence_before();
-    __syncwarp();
-    if ((tid & 31) == 0) mbar_arrive(bar);
-  };
-
-  f32x2 acc_r[8], acc_i[8];      // 16 complex accumulators: k2 = 16 wg + 2 q + {0, 1}
-#pragma unroll
-  for (int q = 0; q < 8; ++q) { acc_r[q] = 0ull; acc_i[q] = 0ull; }
 
   for (int n = 0; n < n_units; ++n) {
-    const uint32_t par = n & 1;                     // every per-pair barrier completes once per pair
-    const uint32_t tDu = tlane + dcol(2 * n), tDd = tlane + dcol(2 * n + 1);
-    // ---- pass 1 of u(n), of dout(n).  The A buffers are free: this thread saw stage 2 of pair n-1 complete (bar_s2).
-    mbar_wait((n & 1) ? bar_s1u_odd : bar_s1u, (n >> 1) & 1);
-    tc_fence_after();
-    pass1(tDu, s_au);
-    hand_over(bar_p1u);
-    mbar_wait(bar_s1d, par);
-    tc_fence_after();
-    pass1(tDd, s_ad);
-    hand_over(bar_p1d);
-    // ---- accumulate Zd * conj(Zu) over this thread's 16 frequencies
-    mbar_wait(bar_s2, par);
-    tc_fence_after();
+    spectrum(n, 0);
 #pragma unroll
-    for (int hf = 0; hf < 2; ++hf) {               // two halves of 8 columns keep the live registers low
-      uint32_t ur[8], ui[8], dr[8], di[8];
-      tmem_ld8(tDu + 16 * wg + 8 * hf, ur);
-      tmem_ld8(tDu + 64 + 16 * wg + 8 * hf, ui);
-      tmem_ld8(tDd + 16 * wg + 8 * hf, dr);
-      tmem_ld8(tDd + 64 + 16 * wg + 8 * hf, di);
-      tmem_ld_wait();
-      reg_fence(ur); reg_fence(ui); reg_fence(dr); reg_fence(di);
+    for (int i = 0; i < 8; ++i) {
+      park[i * kThreadsDkf3] = make_float4(d.r[4 * i], d.r[4 * i + 1], d.r[4 * i + 2], d.r[4 * i + 3]);
+      park[(8 + i) * kThreadsDkf3] = make_float4(d.i[4 * i], d.i[4 * i + 1], d.i[4 * i + 2], d.i[4 * i + 3]);
+    }
+    spectrum(n, 1);
+    // ---- accumulate Zd * conj(Zu): (a + ib)(c - id) = (ac + bd) + i(bc - ad)
 #pragma unroll
-      for (int q = 0; q < 4; ++q) {
-        const f32x2 a = pk2u(dr[2 * q], dr[2 * q + 1]), b = pk2u(di[2 * q], di[2 * q + 1]);
-        const f32x2 c = pk2u(ur[2 * q], ur[2 * q + 1]), d = pk2u(ui[2 * q], ui[2 * q + 1]);
-        // (a + ib)(c - id) = (ac + bd) + i(bc - ad)
-        acc_r[4 * hf + q] = fma2(a, c, fma2(b, d, acc_r[4 * hf + q]));
-        acc_i[4 * hf + q] = fma2(b, c, acc_i[4 * hf + q]);
-        acc_i[4 * hf + q] = sub2(acc_i[4 * hf + q], mul2(a, d));
+    for (int i = 0; i < 8; ++i) {
+      const float4 ur = park[i * kThreadsDkf3], ui = park[(8 + i) * kThreadsDkf3];
+      const float c[4] = {ur.x, ur.y, ur.z, ur.w}, dd[4] = {ui.x, ui.y, ui.z, ui.w};
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const int k = 4 * i + e;
+        const float a = d.r[k], b = d.i[k];
+        acc[k] = fmaf(a, c[e], fmaf(b, dd[e], acc[k]));
+        acc[32 + k] = fmaf(b, c[e], acc[32 + k]) - a * dd[e];
       }
     }
-    hand_over(bar_acc);    // both accumulators of pair n are free again (dout(n+1) and u(n+2) will overwrite them)
     // ---- channel (or this CTA's share of it) finished: add it to the gradient spectrum
     if (unit_pr(n) == p.pairs - 1 || n == n_units - 1) {
       const int h = unit_h(n);
-      float* out = reinterpret_cast<float*>(p.dkf + ((size_t(h) * 4 + wg) * 128 + lane) * 16);
 #pragma unroll
-      for (int q = 0; q < 8; ++q) {
-        float r0, r1, i0, i1;
-        upk2(acc_r[q], r0, r1);
-        upk2(acc_i[q], i0, i1);
-        red_add_v4(out + 4 * q, r0, i0, r1, i1);
-        acc_r[q] = 0ull; acc_i[q] = 0ull;
+      for (int rr = 0; rr < 2; ++rr) {
+        const int k1 = fp.r0 + 8 * rr;
+#pragma unroll
+        for (int i = 0; i < 8; ++i) {
+          const int k2 = 8 * i + 2 * fp.q, e = 4 * i + 2 * rr;
+          float* out = reinterpret_cast<float*>(p.dkf + ((size_t(h) * 4 + (k2 >> 4)) * 128 + k1) * 16 + (k2 & 15));
+          red_add_v4(out, acc[e], acc[32 + e], acc[e + 1], acc[32 + e + 1]);
+        }
       }
+#pragma unroll
+      for (int i = 0; i < 64; ++i) acc[i] = 0.f;
     }
   }
-
-  // every MMA has completed (the last bar_s2 was observed by every compute thread): release TMEM
-  tc_fence_before();
-  named_bar_sync(1, 512);
-  if (tid < 32) tmem_dealloc(tmem_base, 512);
 }
 
 // dk_f engine order -> natural order complex64 (reference analogue: the inverse permutation at conv.py:1818).
@@ -392,7 +201,7 @@ __global__ void dkf_unpack_kernel(const float2* __restrict__ eng, float2* __rest
 //     Xh[k] = (X[k] + conj X[(N - k) mod N]) / 2,   k = 0 .. N/2,
 // so that dk = irfft(Xh, n = N)[:Lk] — the same real part as the reference's ifft(dk_f).real (conv.py:1817-1820; the
 // pair-packed spectrum is not Hermitian, its anti-Hermitian part is exactly what `.real` discards) at half the FFT work
-// and without the full-spectrum round trips (C4: unpack 2.2 ms + c2c 0.99 ms + .real/slice 0.66 ms before).
+// and without the full-spectrum round trips (unpack, c2c FFT, .real / slice).
 // A block moves a tile of TR residues r (k = r + R kin, natural-fastest; engine row rho = (r % R0) R1 + r / R0) x the 16
 // consecutive k2 of one (k1, quarter): 128-byte runs on the engine side, TR x 8-byte runs on the natural side.
 // grid: (R / TR, 128 * 2, H), TR = min(32, R); 256 threads.

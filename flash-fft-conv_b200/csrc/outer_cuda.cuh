@@ -2,7 +2,7 @@
 //
 // Path replaced (reference): the butterfly kernels that wrap the inner Monarch convolution for N > 32K
 // (csrc/flashfftconv/butterfly/butterfly_padded_cuda_bf16.cu:17-157 forward, butterfly_padded_ifft_cuda_bf16.cu:
-// 15-319 inverse; gated variants :302/:326) — here used already from N = 16K because the fused tcgen05 kernel
+// 15-319 inverse; gated variants :302/:326) — here used already from N = 16K because the fused tensor-core kernel
 // is the 8192-point one.  Same role: outer DFT down the stride-M columns + (R x M) twiddle, with the implicit
 // zero padding (rows >= L/M are never read) and the gates applied on load / store.
 //
@@ -63,8 +63,6 @@ DEVINL void wr(int R, int e, float& c, float& s) {   // exp(-2 pi i e / R)
   c = cs[t]; s = sn[t];
 }
 
-DEVINL f32x2 add2(f32x2 a, f32x2 b) { f32x2 r; asm("add.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b)); return r; }
-
 // v += z * exp(-2 pi i e8 / 8)   (e8 = eighths of a turn, a compile-time constant after unrolling)
 DEVINL void rot_acc(int e8, f32x2 zr, f32x2 zi, f32x2& vr, f32x2& vi) {
   e8 &= 7;
@@ -110,8 +108,7 @@ DEVINL void twiddle8(int np, float inv_nl2, const float2* step, f32x2 (&wc)[4], 
 DEVINL void prefetch_l2(const void* p) { asm volatile("prefetch.global.L2 [%0];" ::"l"(p)); }
 
 // Software read-ahead for the streaming level-0 kernels.  A block lives for one load -> compute -> store round trip and
-// only 16 warps fit per SM (128 registers), so HBM latency is exposed (ncu: 70 % of the stall samples on the first use
-// of the loads, 4.1-4.7 TB/s).  Blocks are dispatched in linear order; each block therefore touches the lines the block
+// only 16 warps fit per SM (128 registers), so HBM latency is exposed at the first use of the loads.  Blocks are dispatched in linear order; each block therefore touches the lines the block
 // `lookahead` positions later will load (one thread per 128-byte line), turning those loads into L2 hits.
 template <int R, bool kGated>
 DEVINL void readahead_level0(const OuterParams& p, bool planes_in) {

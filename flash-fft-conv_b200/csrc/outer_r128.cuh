@@ -1,4 +1,4 @@
-// Outer radix-128 stages on tcgen05 for N = 128 x M (M = N/128 >= 8192: 1M, 2M, 4M), bf16, sm_100a.
+// Outer radix-128 stages on wgmma for N = 128 x M (M = N/128 >= 8192: 1M, 2M, 4M), bf16, sm_90a.
 //
 // Path replaced (reference): butterfly_padded[_gated]_bf16_forward / butterfly_ifft_padded[_gated]_bf16_forward
 // (csrc/flashfftconv/butterfly/butterfly_padded_cuda_bf16.cu:489-757 radix 128, :302 radix 64, :17/:165 radix
@@ -10,9 +10,10 @@
 //   inv_tc : z'[i, j] = sum_k0 conj F128[i,k0] * ( conj W_N^{k0 j} * T[k0, j] )
 //
 // Machine mapping: the unit is one 64-column chunk of one sequence pair: a (128 x 64) tile per member, TMA
-// loaded with a 4-D map (col, chunk, row, sequence); DFT-128 cos / sin planes resident in TMEM as the A operand
-// (exactly stage 1 / stage 4 of r128_common.cuh); the twiddle is applied by the CUDA cores on the accumulator
-// (forward) or on the tile in shared memory before the MMA (inverse).  Two pipelines x two warpgroups per CTA.
+// loaded with a 4-D map (col, chunk, row, sequence); DFT-128 cos / sin planes resident in shared memory as the A
+// operand (exactly stage 1 / stage 4 of r128_common.cuh); the twiddle is applied by the CUDA cores on the accumulator
+// (forward) or on the tile in shared memory before the MMA (inverse).  Two pipelines x two warpgroups (row halves)
+// per CTA.
 #pragma once
 #include "r128_common.cuh"
 
@@ -35,89 +36,69 @@ struct OuterTcParams {
 
 namespace r128 {
 
-// ungated: a ring of three (re, im) tile slots per pipeline so the next unit's TMA load never waits for the
-// previous unit's TMA store; gated forward keeps two slots + one gate slot (shared-memory budget)
-constexpr int kOuterSlots = 3;
+// ungated: two (re, im) tile slots per pipeline, the next unit's TMA load lands in one while the other is worked on;
+// gated forward: one work slot + one gate slot
+constexpr int kOuterSlots = 2;
+constexpr int kThreadsOuter = 2 * kPipeThreads;
 constexpr int kSmemOuterData = 2 * kOuterSlots * kSlotBytes;
-constexpr int kSmemOuter = kSmemOuterData + kSmemBars + 1024;
-constexpr int kSmemOuterGated = kSmemOuterData + kSmemBars + 1024;   // gate slot = third ring slot
+constexpr int kSmemOuter = kSmemOuterData + kSmemF + 64 + 1024;
+static_assert(kSmemOuter <= 227 * 1024, "shared memory per block");
 
 template <bool kInverse, int kFmt = 1>
-__global__ void __launch_bounds__(kThreads, 1)
+__global__ void __launch_bounds__(kThreadsOuter, 1)
 outer_tc_kernel(const __grid_constant__ CUtensorMap tm_x,    // real endpoint: u (fwd) / y (inv), 4-D
                 const __grid_constant__ CUtensorMap tm_pr,   // planes, real part, 4-D
                 const __grid_constant__ CUtensorMap tm_pi,   // planes, imaginary part
                 const __grid_constant__ CUtensorMap tm_g,    // pregate (fwd, optional)
                 const OuterTcParams p) {
   using NT = Num<kFmt>;
-  constexpr uint32_t ID_N128_MN = Idesc<kFmt>::N128_MN, ID_N64_MN = Idesc<kFmt>::N64_MN, ID_N64_MN_NEG = Idesc<kFmt>::N64_MN_NEG;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t sbase = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t s_bars = sbase + kSmemOuterData;
   uint8_t* gen_base = smem_raw + (sbase - smem_u32(smem_raw));
+  const uint32_t s_f = sbase + kSmemOuterData;
+  const uint32_t s_bars = s_f + kSmemF;
 
   const int tid = threadIdx.x;
-  const int pipe = __shfl_sync(0xffffffffu, tid >> 8, 0);   // warp-uniform for the compiler (uniform-register MMA issue)
-  const int half = (tid >> 7) & 1;
-  const int lane = tid & 127;
-  const int warp_q = (tid >> 5) & 3;
-  const bool lead_warp = ((tid & 255) < 32);
+  const int pipe = __shfl_sync(0xffffffffu, tid >> 8, 0);
+  const int hf = (tid >> 7) & 1;
+  const int lane = tid & 127;          // shared-memory passes: row `lane`, columns 32 hf .. 32 hf + 31
+  const bool leader = (tid & 255) == 0;
+  const FragPos fp(tid);
 
-  const uint32_t bar_tma0 = s_bars + pipe * 32;       // three TMA barriers
-  const uint32_t bar_mma = s_bars + pipe * 32 + 24;   // one MMA barrier
-  const uint32_t s_tmemptr = s_bars + 64;
+  const uint32_t bar_tma0 = s_bars + pipe * 16;       // one TMA barrier per slot
 
   if (tid == 0) {
     tma_prefetch_desc(&tm_x);
     tma_prefetch_desc(&tm_pr);
     tma_prefetch_desc(&tm_pi);
   }
-  if ((tid & 255) == 0) {
+  if (leader) {
     mbar_init(bar_tma0, 1);
     mbar_init(bar_tma0 + 8, 1);
-    mbar_init(bar_tma0 + 16, 1);
-    mbar_init(bar_mma, 1);
-    fence_barrier_init();
   }
-  if (tid < 32) {
-    tmem_alloc(s_tmemptr, 512);
-    tmem_relinquish();
-  }
-  tc_fence_before();
+  fence_barrier_init();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *reinterpret_cast<volatile uint32_t*>(gen_base + kSmemOuterData + 64);
-  const uint32_t tlane = tmem_base + (uint32_t(warp_q * 32) << 16);
-  {
-    const uint4* row = reinterpret_cast<const uint4*>((pipe == 0 ? p.dftC : p.dftS) + lane * 128) + half * 8;
-    const uint32_t tcol = tlane + (pipe == 0 ? kColC : kColS) + 32 * half;
-#pragma unroll
-    for (int q = 0; q < 2; ++q) {
-      uint32_t v[16];
-#pragma unroll
-      for (int r = 0; r < 4; ++r) {
-        uint4 w = row[q * 4 + r];
-        v[4 * r + 0] = w.x; v[4 * r + 1] = w.y; v[4 * r + 2] = w.z; v[4 * r + 3] = w.w;
-      }
-      tmem_st16(tcol + 16 * q, v);
-    }
-    tmem_st_wait();
-  }
-  // in-chunk twiddles W_N^{k0 * t}, t = 32*half + 2q + {0,1} (k0 = lane); the chunk base W_N^{k0*64*cj} is
-  // computed per unit in fp32
+  load_dft128(gen_base + kSmemOuterData, p.dftC, p.dftS, tid, kThreadsOuter);
+  // inverse: in-chunk twiddles W_N^{k0 * t}, t = 32*half + 2q + {0,1} (k0 = lane), applied in shared memory; the chunk
+  // base W_N^{k0*64*cj} is computed per unit in fp32
   __half2 twc[16], tws[16];
   const float invN2 = 2.0f / float(p.N);
+  if (kInverse) {
 #pragma unroll
-  for (int q = 0; q < 16; ++q) {
-    float s0, c0, s1, c1;
-    sincospif(-float(lane * (32 * half + 2 * q)) * invN2, &s0, &c0);
-    sincospif(-float(lane * (32 * half + 2 * q + 1)) * invN2, &s1, &c1);
-    twc[q] = __floats2half2_rn(c0 * p.tw_scale, c1 * p.tw_scale);
-    tws[q] = __floats2half2_rn(s0 * p.tw_scale, s1 * p.tw_scale);
+    for (int q = 0; q < 16; ++q) {
+      float s0, c0, s1, c1;
+      sincospif(-float(lane * (32 * hf + 2 * q)) * invN2, &s0, &c0);
+      sincospif(-float(lane * (32 * hf + 2 * q + 1)) * invN2, &s1, &c1);
+      twc[q] = __floats2half2_rn(c0 * p.tw_scale, c1 * p.tw_scale);
+      tws[q] = __floats2half2_rn(s0 * p.tw_scale, s1 * p.tw_scale);
+    }
   }
-  tc_fence_before();
+  // forward: W_N^{k0 t} of the accumulator fragment's rows, t = 8 i + 2 q + {0, 1}
+  RowTw tw[2];
+  tw[0].init(fp.r0, fp.q, 1.0f / float(p.N));
+  tw[1].init(fp.r0 + 8, fp.q, 1.0f / float(p.N));
+  fence_proxy_async_smem();
   __syncthreads();
-  tc_fence_after();
 
   const int gp = blockIdx.x * 2 + pipe;
   const int GP = gridDim.x * 2;
@@ -125,15 +106,11 @@ outer_tc_kernel(const __grid_constant__ CUtensorMap tm_x,    // real endpoint: u
   const int u_end = int((long long)p.units * (gp + 1) / GP);
 
   const uint32_t s_slot0 = sbase + pipe * kOuterSlots * kSlotBytes;
-  const uint32_t tD = tlane + colD(pipe);
-  const uint32_t tD0 = tmem_base + colD(pipe);
-  const uint32_t tC0 = tmem_base + kColC;
-  const uint32_t tS0 = tmem_base + kColS;
   const uint32_t bar_id = 1 + pipe;
   const int BH = p.B * p.Hs;      // out-of-bounds sequence index of the 4-D maps (zero fill / dropped)
   const bool gated_in = (!kInverse) && p.has_pregate;
-  const int nslots = gated_in ? 2 : kOuterSlots;
-  const uint32_t s_gate0 = s_slot0 + 2 * kSlotBytes;     // gated: the third ring slot holds the pregate tiles
+  const int nslots = gated_in ? 1 : kOuterSlots;
+  const uint32_t s_gate0 = s_slot0 + kSlotBytes;     // gated: the second slot holds the pregate tiles
 
   struct UnitIdx { int cj, h, pr; };
   auto decode = [&](int unit) {
@@ -155,9 +132,8 @@ outer_tc_kernel(const __grid_constant__ CUtensorMap tm_x,    // real endpoint: u
       tma_load_4d(dst, &tm_x, bar, 0, x.cj, 0, s0);
       tma_load_4d(dst + kTileBytes, &tm_x, bar, 0, x.cj, 0, s1);
       if (gated_in) {
-        const uint32_t gd = s_gate0;
-        tma_load_4d(gd, &tm_g, bar, 0, x.cj, 0, s0);
-        tma_load_4d(gd + kTileBytes, &tm_g, bar, 0, x.cj, 0, s1);
+        tma_load_4d(s_gate0, &tm_g, bar, 0, x.cj, 0, s0);
+        tma_load_4d(s_gate0 + kTileBytes, &tm_g, bar, 0, x.cj, 0, s1);
       }
     } else {
       const int row = x.pr * p.H + x.h;
@@ -165,45 +141,39 @@ outer_tc_kernel(const __grid_constant__ CUtensorMap tm_x,    // real endpoint: u
       tma_load_4d(dst + kTileBytes, &tm_pi, bar, 0, x.cj, 0, row);
     }
   };
-  uint32_t mma_phase = 0;
-  auto wait_mma = [&]() {
-    mbar_wait(bar_mma, mma_phase);
-    mma_phase ^= 1;
-    tc_fence_after();
-  };
 
-  if (lead_warp && u_begin < u_end) {
-    if (elect_one()) issue_load(u_begin, 0);
-    __syncwarp();
-  }
+  if (leader && u_begin < u_end) issue_load(u_begin, 0);
+
+  Acc d;
+  d.zero();
+  const bool has_post = kInverse && p.postgate != nullptr;
+  const bool has_y2 = kInverse && p.y2 != nullptr;
 
   for (int unit = u_begin, n = 0; unit < u_end; ++unit, ++n) {
     const int slot = n % nslots;
     const uint32_t tma_par = uint32_t(n / nslots) & 1u;
     const uint32_t sX = s_slot0 + slot * kSlotBytes;
     const UnitIdx x = decode(unit);
-    // chunk base twiddle W_N^{k0 * 64 * cj}
-    float bs, bc;
-    sincospif(-float((lane * 64 * x.cj) & (p.N - 1)) * invN2, &bs, &bc);
-    const f32x2 bc2 = pk2(bc, bc), bs2 = pk2(bs, bs);
 
-    if (kInverse || gated_in) mbar_wait(bar_tma0 + 8 * slot, tma_par);
+    mbar_wait(bar_tma0 + 8 * slot, tma_par);
     if (gated_in) {
-      const uint32_t sG = s_gate0;
 #pragma unroll
       for (int part = 0; part < 2; ++part)
 #pragma unroll
         for (int c = 0; c < 4; ++c) {
-          const uint32_t off = part * kTileBytes + uint32_t(lane) * 128u + uint32_t(4 * half + c) * 16u;
-          const uint4 a = ld_shared_v4(sX + off), g = ld_shared_v4(sG + off);
+          const uint32_t off = part * kTileBytes + uint32_t(lane) * 128u + uint32_t(4 * hf + c) * 16u;
+          const uint4 a = ld_shared_v4(sX + off), g = ld_shared_v4(s_gate0 + off);
           st_shared_v4(sX + off, NT::hmul2(a.x, g.x), NT::hmul2(a.y, g.y), NT::hmul2(a.z, g.z), NT::hmul2(a.w, g.w));
         }
     }
     if (kInverse) {
       // T[k0, j] *= conj(W_N^{k0 j}) in shared memory (row = lane = k0); logical chunk c lives at c ^ (lane & 7)
+      float bs, bc;
+      sincospif(-float((lane * 64 * x.cj) & (p.N - 1)) * invN2, &bs, &bc);
+      const f32x2 bc2 = pk2(bc, bc), bs2 = pk2(bs, bs);
 #pragma unroll
       for (int cc = 0; cc < 4; ++cc) {
-        const int c = 4 * half + cc;
+        const int c = 4 * hf + cc;
         const uint32_t off = uint32_t(lane) * 128u + (uint32_t(c ^ (lane & 7)) << 4);
         const uint4 vr = ld_shared_v4(sX + off), vi = ld_shared_v4(sX + kTileBytes + off);
         const uint32_t wr_[4] = {vr.x, vr.y, vr.z, vr.w}, wi_[4] = {vi.x, vi.y, vi.z, vi.w};
@@ -226,126 +196,76 @@ outer_tc_kernel(const __grid_constant__ CUtensorMap tm_x,    // real endpoint: u
       fence_proxy_async_smem();
       named_bar_sync(bar_id, kPipeThreads);
     }
-    // ---------------- radix-128 MMA
-    if (lead_warp) {
-      if (!(kInverse || gated_in)) mbar_wait(bar_tma0 + 8 * slot, tma_par);
-      tc_fence_after();
-      if (elect_one()) {
-        const int ks = kInverse ? 8 : p.ksteps;
-        const uint64_t dXr = tile_desc(sX), dXi = tile_desc(sX + kTileBytes);   // a K step = +(2048 >> 4) in the address field
-        // forward F = C - iS: D[:,0:64] += S*Xi, D[:,64:128] -= S*Xr ; inverse conj F: signs swapped
-        if (ks == 8) {
-#pragma unroll
-          for (int s = 0; s < 8; ++s) mma_ts(tD0, tC0 + 8 * s, dXr + 128 * s, ID_N128_MN, s > 0);
-#pragma unroll
-          for (int s = 0; s < 8; ++s) mma_ts(tD0, tS0 + 8 * s, dXi + 128 * s, kInverse ? ID_N64_MN_NEG : ID_N64_MN, 1);
-#pragma unroll
-          for (int s = 0; s < 8; ++s) mma_ts(tD0 + 64, tS0 + 8 * s, dXr + 128 * s, kInverse ? ID_N64_MN : ID_N64_MN_NEG, 1);
-        } else {
-          for (int s = 0; s < ks; ++s) mma_ts(tD0, tC0 + 8 * s, dXr + 128 * s, ID_N128_MN, s > 0);
-          for (int s = 0; s < ks; ++s) mma_ts(tD0, tS0 + 8 * s, dXi + 128 * s, kInverse ? ID_N64_MN_NEG : ID_N64_MN, 1);
-          for (int s = 0; s < ks; ++s) mma_ts(tD0 + 64, tS0 + 8 * s, dXr + 128 * s, kInverse ? ID_N64_MN : ID_N64_MN_NEG, 1);
-        }
-        mma_commit(bar_mma);
-        // next unit -> next ring slot (ungated: its last reader, a TMA store, was issued two units ago)
-        if (unit + 1 < u_end) {
-          if (nslots == 3) tma_store_wait_read1(); else tma_store_wait_read0();
-          issue_load(unit + 1, (n + 1) % nslots);
-        }
-      }
-      __syncwarp();
+    // ---------------- radix-128 MMA: forward F = C - iS; inverse conj F
+    {
+      const int ks = kInverse ? 8 : p.ksteps;
+      f128_stage<kFmt, kInverse>(d, s_f, hf, sX, (1 << ks) - 1);
     }
-    // postgate prefetch (inverse): rows i = lane of the [128][M] view
-    uint4 pg[2][4];
-    const bool has_post = kInverse && p.postgate != nullptr;
-    if (has_post) {
+    // next unit -> the other slot (ungated: its last reader was the previous unit's TMA store)
+    if (leader && nslots == 2 && unit + 1 < u_end) {
+      tma_store_wait_read0();
+      issue_load(unit + 1, (n + 1) % nslots);
+    }
+    wgmma_wait_regs(d);
+    if (!kInverse) {     // * W_N^{k0 (64 cj + t)}: chunk base per row times the in-chunk twiddles
+      float c0[2], s0[2];
+#pragma unroll
+      for (int rr = 0; rr < 2; ++rr) {
+        sincospif(-float(((fp.r0 + 8 * rr) * 64 * x.cj) & (p.N - 1)) * invN2, &s0[rr], &c0[rr]);
+        c0[rr] *= p.tw_scale; s0[rr] *= p.tw_scale;
+      }
+      twiddle_frag<false>(d, tw, c0, s0);
+    }
+    named_bar_sync(bar_id, kPipeThreads);     // both halves' MMAs have read the slot
+    frag_store_tile<kFmt>(sX, fp, d);
+    if (has_post || has_y2) {
+      // output gates on the rounded result, row `lane` of the [128][M] view, this thread's 32 columns
+      named_bar_sync(bar_id, kPipeThreads);
       const bool row_ok = (long long)lane * p.M < p.L;
 #pragma unroll
-      for (int part = 0; part < 2; ++part) {
-        const int b = 2 * x.pr + part;
-        const size_t e0 = (size_t(b < p.B ? b : p.B - 1) * p.Hs + p.h0 + x.h) * p.L + size_t(lane) * p.M + x.cj * 64 + 32 * half;
-        const uint4* gp_ = reinterpret_cast<const uint4*>(p.postgate + e0 / 2);
+      for (int cc = 0; cc < 4; ++cc) {
+        const int c = 4 * hf + cc;
+        const uint32_t off = uint32_t(lane) * 128u + (uint32_t(c ^ (lane & 7)) << 4);
 #pragma unroll
-        for (int c = 0; c < 4; ++c) pg[part][c] = row_ok ? __ldg(gp_ + c) : make_uint4(0, 0, 0, 0);
-      }
-    }
-    wait_mma();
-    // ---------------- accumulator -> bf16 tiles in the (now free) slot
-#pragma unroll
-    for (int sub = 0; sub < 2; ++sub) {
-      uint32_t re[16], im[16];
-      tmem_ld16(tD + 32 * half + 16 * sub, re);
-      tmem_ld16(tD + 64 + 32 * half + 16 * sub, im);
-      tmem_ld_wait();
-      reg_fence(re); reg_fence(im);
-      uint32_t ore[8], oim[8];
-#pragma unroll
-      for (int q = 0; q < 8; ++q) {
-        if (!kInverse) {
-          const float2 tc = __half22float2(twc[8 * sub + q]), ts = __half22float2(tws[8 * sub + q]);
-          f32x2 wcr, wci, vr, vi;
-          cmul2(bc2, bs2, pk2(tc.x, tc.y), pk2(ts.x, ts.y), wcr, wci);
-          cmul2(pk2u(re[2 * q], re[2 * q + 1]), pk2u(im[2 * q], im[2 * q + 1]), wcr, wci, vr, vi);
-          ore[q] = NT::pack_v(vr);
-          oim[q] = NT::pack_v(vi);
-        } else {
-          ore[q] = NT::pack(__uint_as_float(re[2 * q]), __uint_as_float(re[2 * q + 1]));
-          oim[q] = NT::pack(__uint_as_float(im[2 * q]), __uint_as_float(im[2 * q + 1]));
-        }
-      }
-#pragma unroll
-      for (int cc = 0; cc < 2; ++cc) {
-        const int chunk = 4 * half + 2 * sub + cc;
-        const uint32_t off = uint32_t(lane) * 128u + (uint32_t(chunk ^ (lane & 7)) << 4);
-        uint32_t a0 = ore[4 * cc], a1 = ore[4 * cc + 1], a2 = ore[4 * cc + 2], a3 = ore[4 * cc + 3];
-        uint32_t b0 = oim[4 * cc], b1 = oim[4 * cc + 1], b2 = oim[4 * cc + 2], b3 = oim[4 * cc + 3];
-        if (kInverse && p.y2 != nullptr && (long long)lane * p.M < p.L) {
-          // second gated output straight from registers (this thread owns 64 contiguous bytes of row `lane`)
-#pragma unroll
-          for (int part = 0; part < 2; ++part) {
-            const int b = 2 * x.pr + part;
-            if (b < p.B) {
-              const size_t e0 = (size_t(b) * p.Hs + p.h0 + x.h) * p.L + size_t(lane) * p.M + x.cj * 64 + 32 * half + 8 * (2 * sub + cc);
-              const uint4 g2 = __ldg(reinterpret_cast<const uint4*>(p.postgate2 + e0 / 2));
-              const uint32_t v0 = part ? b0 : a0, v1 = part ? b1 : a1, v2 = part ? b2 : a2, v3 = part ? b3 : a3;
-              *reinterpret_cast<uint4*>(p.y2 + e0 / 2) =
-                  make_uint4(NT::hmul2(v0, g2.x), NT::hmul2(v1, g2.y), NT::hmul2(v2, g2.z), NT::hmul2(v3, g2.w));
-            }
+        for (int part = 0; part < 2; ++part) {
+          const int b = 2 * x.pr + part;
+          const uint4 v = ld_shared_v4(sX + part * kTileBytes + off);
+          const size_t e0 = (size_t(b < p.B ? b : p.B - 1) * p.Hs + p.h0 + x.h) * p.L + size_t(lane) * p.M + x.cj * 64 + 8 * c;
+          if (has_y2 && row_ok && b < p.B) {
+            // second gated output straight to global memory
+            const uint4 g2 = __ldg(reinterpret_cast<const uint4*>(p.postgate2 + e0 / 2));
+            *reinterpret_cast<uint4*>(p.y2 + e0 / 2) =
+                make_uint4(NT::hmul2(v.x, g2.x), NT::hmul2(v.y, g2.y), NT::hmul2(v.z, g2.z), NT::hmul2(v.w, g2.w));
+          }
+          if (has_post) {
+            const uint4 g = row_ok ? __ldg(reinterpret_cast<const uint4*>(p.postgate + e0 / 2)) : make_uint4(0, 0, 0, 0);
+            st_shared_v4(sX + part * kTileBytes + off, NT::hmul2(v.x, g.x), NT::hmul2(v.y, g.y), NT::hmul2(v.z, g.z),
+                         NT::hmul2(v.w, g.w));
           }
         }
-        if (has_post) {
-          const uint4 g0 = pg[0][2 * sub + cc], g1 = pg[1][2 * sub + cc];
-          a0 = NT::hmul2(a0, g0.x); a1 = NT::hmul2(a1, g0.y); a2 = NT::hmul2(a2, g0.z); a3 = NT::hmul2(a3, g0.w);
-          b0 = NT::hmul2(b0, g1.x); b1 = NT::hmul2(b1, g1.y); b2 = NT::hmul2(b2, g1.z); b3 = NT::hmul2(b3, g1.w);
-        }
-        st_shared_v4(sX + off, a0, a1, a2, a3);
-        st_shared_v4(sX + kTileBytes + off, b0, b1, b2, b3);
       }
     }
     fence_proxy_async_smem();
-    tc_fence_before();
     named_bar_sync(bar_id, kPipeThreads);
-    if (lead_warp) {
-      if (elect_one()) {
-        if (!kInverse) {
-          const int row = x.pr * p.H + x.h;
-          tma_store_4d(&tm_pr, sX, 0, x.cj, 0, row);
-          tma_store_4d(&tm_pi, sX + kTileBytes, 0, x.cj, 0, row);
-        } else {
-          const int b0 = 2 * x.pr, b1 = 2 * x.pr + 1;
-          tma_store_4d(&tm_x, sX, 0, x.cj, 0, b0 * p.Hs + p.h0 + x.h);
-          if (b1 < p.B) tma_store_4d(&tm_x, sX + kTileBytes, 0, x.cj, 0, b1 * p.Hs + p.h0 + x.h);
-        }
-        tma_store_commit();
+    if (leader) {
+      if (!kInverse) {
+        const int row = x.pr * p.H + x.h;
+        tma_store_4d(&tm_pr, sX, 0, x.cj, 0, row);
+        tma_store_4d(&tm_pi, sX + kTileBytes, 0, x.cj, 0, row);
+      } else {
+        const int b0 = 2 * x.pr, b1 = 2 * x.pr + 1;
+        tma_store_4d(&tm_x, sX, 0, x.cj, 0, b0 * p.Hs + p.h0 + x.h);
+        if (b1 < p.B) tma_store_4d(&tm_x, sX + kTileBytes, 0, x.cj, 0, b1 * p.Hs + p.h0 + x.h);
       }
-      __syncwarp();
+      tma_store_commit();
+      if (nslots == 1 && unit + 1 < u_end) {   // gated: slot and gate slot are free once the store has read the slot
+        tma_store_wait_read0();
+        issue_load(unit + 1, 0);
+      }
     }
   }
 
-  if (lead_warp) tma_store_wait_all0();
-  tc_fence_before();
-  __syncthreads();
-  if (tid < 32) tmem_dealloc(tmem_base, 512);
+  if (leader) tma_store_wait_all0();
 }
 
 }  // namespace r128

@@ -1,5 +1,5 @@
-// Thin inline-PTX wrappers for sm_100a: mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (MMA, TMEM
-// alloc/ld/st, commit, fences).  Nothing here is derived from the reference (which uses wmma only).
+// Thin inline-PTX wrappers for sm_90a: mbarrier, TMA (cp.async.bulk.tensor), wgmma (warpgroup MMA, shared-memory
+// descriptors, fences).  Nothing here is derived from the reference (which uses wmma only).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
@@ -54,8 +54,6 @@ DEVINL void mbar_wait(uint32_t bar, uint32_t parity) {
 
 // ----------------------------------------------------------------------------- fences / barriers
 DEVINL void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-DEVINL void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-DEVINL void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 DEVINL void named_bar_sync(uint32_t id, uint32_t nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
@@ -96,130 +94,96 @@ DEVINL void tma_store_wait_read0() { asm volatile("cp.async.bulk.wait_group.read
 DEVINL void tma_store_wait_read1() { asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory"); }
 DEVINL void tma_store_wait_all0() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 
-// ----------------------------------------------------------------------------- TMEM alloc
-DEVINL void tmem_alloc(uint32_t dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(dst_smem), "r"(ncols)
-               : "memory");
-}
-DEVINL void tmem_relinquish() { asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory"); }
-DEVINL void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
+// ----------------------------------------------------------------------------- wgmma
+// Warpgroup MMA: every thread of the warpgroup executes these; m64 rows per instruction.  Accumulator fragment of
+// m64n64k16 (f32): thread t (warp w = t / 32, lane l) holds rows 16 w + l / 4 (+8) and columns 8 i + 2 (l % 4) + {0, 1}:
+// d[4 i + 0 / 1] = (row, col / col + 1), d[4 i + 2 / 3] = (row + 8, ...).  The 16-bit A fragment of k step s is exactly
+// the accumulator of column blocks 2 s and 2 s + 1 rounded and packed, which is how the radix-64 stages take their A
+// operand straight from the previous stage's result.
+DEVINL void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+DEVINL void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+DEVINL void wgmma_wait0() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
 
-// ----------------------------------------------------------------------------- tcgen05.mma
-// D[tmem] (+)= A[tmem] * B[smem desc].  kind::f16 covers bf16/fp16 inputs with fp32 accumulate.
-DEVINL void mma_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-DEVINL void mma_ss(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Arrive on an mbarrier when all MMAs previously issued by this thread have completed.
-DEVINL void mma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-
-// Instruction descriptor (32-bit) for kind::f16, fp32 accumulate, M=128.
-//   bits [4,6) c_format=1(F32) | [7,10) a_format | [10,13) b_format | 13 a_neg | 14 b_neg
-//   | 15 a_major | 16 b_major (0=K, 1=MN) | [17,23) N>>3 | [24,29) M>>4
-DEVINL constexpr uint32_t make_idesc(int fmt /*0=f16,1=bf16*/, int n, bool b_mn_major, bool a_neg) {
-  return (1u << 4) | (uint32_t(fmt) << 7) | (uint32_t(fmt) << 10) | (uint32_t(a_neg) << 13) |
-         (uint32_t(b_mn_major) << 16) | (uint32_t(n >> 3) << 17) | (uint32_t(128 >> 4) << 24);
-}
-
-// Shared-memory matrix descriptor (64-bit).
-//   [0,14) start>>4 | [16,30) LBO>>4 | [32,46) SBO>>4 | [46,48) version=1 | [61,64) layout
-//   layout: 0 = no swizzle (8x16B core matrices), 2 = 128B swizzle.
-DEVINL uint64_t make_sdesc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes, uint32_t layout) {
+// Shared-memory matrix descriptor (64-bit), 128B swizzle only:
+//   [0,14) start>>4 | [16,30) LBO>>4 | [32,46) SBO>>4 | [62,64) layout (1 = 128B swizzle)
+// The operand images must start on 1024-byte boundaries (base offset 0); a K step inside a swizzle atom moves the start
+// address field.
+DEVINL uint64_t make_sdesc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
   return uint64_t((saddr & 0x3FFFF) >> 4) | (uint64_t((lbo_bytes >> 4) & 0x3FFF) << 16) |
-         (uint64_t((sbo_bytes >> 4) & 0x3FFF) << 32) | (uint64_t(1) << 46) | (uint64_t(layout) << 61);
+         (uint64_t((sbo_bytes >> 4) & 0x3FFF) << 32) | (uint64_t(1) << 62);
 }
 
-// ----------------------------------------------------------------------------- TMEM ld / st
-DEVINL void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-DEVINL void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
-DEVINL void tmem_ld4(uint32_t taddr, uint32_t* v) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x4.b32 {%0,%1,%2,%3}, [%4];"
-               : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3])
-               : "r"(taddr));
+// D[64 x 64] (+)= (kScaleA) A[smem, K-major] * B[smem, MN-major]; accumulator registers d[kOff, kOff + 32)
+template <int kFmt, int kScaleA, int kOff, int kRegs>
+DEVINL void wgmma_ss_n64(float (&d)[kRegs], uint64_t da, uint64_t db, uint32_t acc) {
+  static_assert(kOff + 32 <= kRegs, "accumulator window");
+  if constexpr (kFmt == 1) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %34, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+        "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, %35, 1, 0, 1;\n\t}"
+        : "+f"(d[kOff + 0]), "+f"(d[kOff + 1]), "+f"(d[kOff + 2]), "+f"(d[kOff + 3]), "+f"(d[kOff + 4]), "+f"(d[kOff + 5]), "+f"(d[kOff + 6]), "+f"(d[kOff + 7]), "+f"(d[kOff + 8]), "+f"(d[kOff + 9]), "+f"(d[kOff + 10]), "+f"(d[kOff + 11]), "+f"(d[kOff + 12]), "+f"(d[kOff + 13]), "+f"(d[kOff + 14]), "+f"(d[kOff + 15]), "+f"(d[kOff + 16]), "+f"(d[kOff + 17]), "+f"(d[kOff + 18]), "+f"(d[kOff + 19]), "+f"(d[kOff + 20]), "+f"(d[kOff + 21]), "+f"(d[kOff + 22]), "+f"(d[kOff + 23]), "+f"(d[kOff + 24]), "+f"(d[kOff + 25]), "+f"(d[kOff + 26]), "+f"(d[kOff + 27]), "+f"(d[kOff + 28]), "+f"(d[kOff + 29]), "+f"(d[kOff + 30]), "+f"(d[kOff + 31])
+        : "l"(da), "l"(db), "r"(acc), "n"(kScaleA));
+  } else {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %34, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
+        "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, %35, 1, 0, 1;\n\t}"
+        : "+f"(d[kOff + 0]), "+f"(d[kOff + 1]), "+f"(d[kOff + 2]), "+f"(d[kOff + 3]), "+f"(d[kOff + 4]), "+f"(d[kOff + 5]), "+f"(d[kOff + 6]), "+f"(d[kOff + 7]), "+f"(d[kOff + 8]), "+f"(d[kOff + 9]), "+f"(d[kOff + 10]), "+f"(d[kOff + 11]), "+f"(d[kOff + 12]), "+f"(d[kOff + 13]), "+f"(d[kOff + 14]), "+f"(d[kOff + 15]), "+f"(d[kOff + 16]), "+f"(d[kOff + 17]), "+f"(d[kOff + 18]), "+f"(d[kOff + 19]), "+f"(d[kOff + 20]), "+f"(d[kOff + 21]), "+f"(d[kOff + 22]), "+f"(d[kOff + 23]), "+f"(d[kOff + 24]), "+f"(d[kOff + 25]), "+f"(d[kOff + 26]), "+f"(d[kOff + 27]), "+f"(d[kOff + 28]), "+f"(d[kOff + 29]), "+f"(d[kOff + 30]), "+f"(d[kOff + 31])
+        : "l"(da), "l"(db), "r"(acc), "n"(kScaleA));
+  }
 }
-DEVINL void tmem_ld8(uint32_t taddr, uint32_t* v) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-               : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7])
-               : "r"(taddr));
-}
-DEVINL void tmem_ld16(uint32_t taddr, uint32_t* v) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-        "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-      : "r"(taddr));
-}
-DEVINL void tmem_ld32(uint32_t taddr, uint32_t* v) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
-      "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-        "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]),
-        "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]),
-        "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr));
-}
-DEVINL void tmem_st4(uint32_t taddr, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x4.b32 [%0], {%1,%2,%3,%4};" ::"r"(taddr), "r"(a), "r"(b), "r"(c), "r"(d)
-               : "memory");
-}
-DEVINL void tmem_st8(uint32_t taddr, const uint32_t* v) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"r"(taddr), "r"(v[0]),
-               "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7])
-               : "memory");
-}
-DEVINL void tmem_st16(uint32_t taddr, const uint32_t* v) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16};"
-      ::"r"(taddr), "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]),
-      "r"(v[8]), "r"(v[9]), "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15])
-      : "memory");
+// D[64 x 64] (+)= A[registers, m64k16 fragment] * B[smem, MN-major]; accumulator registers d[kOff, kOff + 32)
+template <int kFmt, int kOff, int kRegs>
+DEVINL void wgmma_rs_n64(float (&d)[kRegs], const uint32_t (&a)[4], uint64_t db, uint32_t acc) {
+  static_assert(kOff + 32 <= kRegs, "accumulator window");
+  if constexpr (kFmt == 1) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %37, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+        "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, {%32,%33,%34,%35}, %36, p, 1, 1, 1;\n\t}"
+        : "+f"(d[kOff + 0]), "+f"(d[kOff + 1]), "+f"(d[kOff + 2]), "+f"(d[kOff + 3]), "+f"(d[kOff + 4]), "+f"(d[kOff + 5]), "+f"(d[kOff + 6]), "+f"(d[kOff + 7]), "+f"(d[kOff + 8]), "+f"(d[kOff + 9]), "+f"(d[kOff + 10]), "+f"(d[kOff + 11]), "+f"(d[kOff + 12]), "+f"(d[kOff + 13]), "+f"(d[kOff + 14]), "+f"(d[kOff + 15]), "+f"(d[kOff + 16]), "+f"(d[kOff + 17]), "+f"(d[kOff + 18]), "+f"(d[kOff + 19]), "+f"(d[kOff + 20]), "+f"(d[kOff + 21]), "+f"(d[kOff + 22]), "+f"(d[kOff + 23]), "+f"(d[kOff + 24]), "+f"(d[kOff + 25]), "+f"(d[kOff + 26]), "+f"(d[kOff + 27]), "+f"(d[kOff + 28]), "+f"(d[kOff + 29]), "+f"(d[kOff + 30]), "+f"(d[kOff + 31])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(acc));
+  } else {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %37, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
+        "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, {%32,%33,%34,%35}, %36, p, 1, 1, 1;\n\t}"
+        : "+f"(d[kOff + 0]), "+f"(d[kOff + 1]), "+f"(d[kOff + 2]), "+f"(d[kOff + 3]), "+f"(d[kOff + 4]), "+f"(d[kOff + 5]), "+f"(d[kOff + 6]), "+f"(d[kOff + 7]), "+f"(d[kOff + 8]), "+f"(d[kOff + 9]), "+f"(d[kOff + 10]), "+f"(d[kOff + 11]), "+f"(d[kOff + 12]), "+f"(d[kOff + 13]), "+f"(d[kOff + 14]), "+f"(d[kOff + 15]), "+f"(d[kOff + 16]), "+f"(d[kOff + 17]), "+f"(d[kOff + 18]), "+f"(d[kOff + 19]), "+f"(d[kOff + 20]), "+f"(d[kOff + 21]), "+f"(d[kOff + 22]), "+f"(d[kOff + 23]), "+f"(d[kOff + 24]), "+f"(d[kOff + 25]), "+f"(d[kOff + 26]), "+f"(d[kOff + 27]), "+f"(d[kOff + 28]), "+f"(d[kOff + 29]), "+f"(d[kOff + 30]), "+f"(d[kOff + 31])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(acc));
+  }
 }
 
-// The registers written by tcgen05.ld are only defined after tcgen05.wait::ld.  The wait has no data
-// dependence on them, so pin the order for the compiler: call reg_fence(v) after tmem_ld_wait().
-template <int N>
-DEVINL void reg_fence(uint32_t (&v)[N]) {
-#pragma unroll
-  for (int i = 0; i < N; ++i) asm volatile("" : "+r"(v[i]));
-}
-template <int N, int M>
-DEVINL void reg_fence(uint32_t (&v)[N][M]) {
-#pragma unroll
-  for (int i = 0; i < N; ++i) reg_fence(v[i]);
-}
-
-// ----------------------------------------------------------------------------- packed fp32x2 math (sm_100)
+// ----------------------------------------------------------------------------- fp32 pairs
+// Two fp32 lanes in one 64-bit value (lo, hi).  The arithmetic is lane-wise fp32; the pair form keeps the complex
+// arithmetic of the kernels compact.  An all-zero f32x2 is (0.f, 0.f).
 typedef unsigned long long f32x2;
 DEVINL f32x2 pk2(float a, float b) { f32x2 r; asm("mov.b64 %0, {%1,%2};" : "=l"(r) : "f"(a), "f"(b)); return r; }
 DEVINL f32x2 pk2u(uint32_t a, uint32_t b) { f32x2 r; asm("mov.b64 %0, {%1,%2};" : "=l"(r) : "r"(a), "r"(b)); return r; }
 DEVINL void upk2(f32x2 v, float& a, float& b) { asm("mov.b64 {%0,%1}, %2;" : "=f"(a), "=f"(b) : "l"(v)); }
-DEVINL f32x2 mul2(f32x2 a, f32x2 b) { f32x2 r; asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b)); return r; }
-DEVINL f32x2 fma2(f32x2 a, f32x2 b, f32x2 c) {
-  f32x2 r; asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(a), "l"(b), "l"(c)); return r;
+DEVINL f32x2 mul2(f32x2 a, f32x2 b) {
+  float a0, a1, b0, b1; upk2(a, a0, a1); upk2(b, b0, b1);
+  return pk2(__fmul_rn(a0, b0), __fmul_rn(a1, b1));
 }
-DEVINL f32x2 sub2(f32x2 a, f32x2 b) { f32x2 r; asm("sub.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b)); return r; }
+DEVINL f32x2 fma2(f32x2 a, f32x2 b, f32x2 c) {
+  float a0, a1, b0, b1, c0, c1; upk2(a, a0, a1); upk2(b, b0, b1); upk2(c, c0, c1);
+  return pk2(__fmaf_rn(a0, b0, c0), __fmaf_rn(a1, b1, c1));
+}
+DEVINL f32x2 sub2(f32x2 a, f32x2 b) {
+  float a0, a1, b0, b1; upk2(a, a0, a1); upk2(b, b0, b1);
+  return pk2(__fsub_rn(a0, b0), __fsub_rn(a1, b1));
+}
+DEVINL f32x2 add2(f32x2 a, f32x2 b) {
+  float a0, a1, b0, b1; upk2(a, a0, a1); upk2(b, b0, b1);
+  return pk2(__fadd_rn(a0, b0), __fadd_rn(a1, b1));
+}
 // two complex products at once: (ar + i ai) * (br + i bi), lanes = two different points
 DEVINL void cmul2(f32x2 ar, f32x2 ai, f32x2 br, f32x2 bi, f32x2& cr, f32x2& ci) {
-  cr = sub2(mul2(ar, br), mul2(ai, bi));   // ptxas fuses this into FMUL2 + FFMA2 (negated addend)
+  cr = sub2(mul2(ar, br), mul2(ai, bi));
   ci = fma2(ai, br, mul2(ar, bi));
 }
 // (ar + i ai) * conj(br + i bi)
@@ -234,7 +198,7 @@ DEVINL uint32_t pack_bf16x2_v(f32x2 v) {   // (lo, hi) fp32 pair -> bf16x2
 }
 
 DEVINL uint32_t pack_bf16x2(float lo, float hi);
-// 16-bit element formats.  kFmt follows the UMMA encoding: 1 = bf16, 0 = fp16 (fp32 accumulate either way).
+// 16-bit element formats.  kFmt: 1 = bf16, 0 = fp16 (fp32 accumulate either way).
 template <int kFmt> struct Num;
 template <> struct Num<1> {
   static DEVINL uint32_t pack(float lo, float hi) { return pack_bf16x2(lo, hi); }

@@ -1,17 +1,18 @@
-// r128_common.cuh — definitions shared by the tcgen05 kernels built on the 8192 = 128 x 64 split (fwd3_r128.cuh,
-// dkf3_r128.cuh, outer_r128.cuh): kernel parameter block, tile / slot geometry, TMEM column map, instruction and
-// shared-memory descriptors, the segmented TMA tile load.
+// r128_common.cuh — definitions shared by the wgmma kernels built on the 8192 = 128 x 64 split (fwd3_r128.cuh,
+// dkf3_r128.cuh, outer_r128.cuh): kernel parameter block, tile / slot geometry, the DFT-128 operand image, the stage
+// issuers, accumulator-fragment helpers, the segmented TMA tile load.
 //
 // Path replaced (reference): monarch_conv_cuda_kernel<32,8,8192,...>
 // (csrc/flashfftconv/monarch_cuda/kernels_bf16/monarch_cuda_32_16_16_kernel_bf16.h:15-801) and its launcher
 // (monarch_cuda_interface_fwd_bf16.cu:656-760).  Same math, different machine mapping:
 //  * two real sequences (b, b+1) of one channel h are packed as ONE complex sequence z = u_b + i u_{b+1};
 //    conv(z, k) = conv(u_b,k) + i conv(u_{b+1},k) because k is real, so no Hermitian split is needed.
-//  * N = 128 * 64, n = i*64 + j.  Stage 1 contracts i: the 128x128 DFT matrix (cos / sin planes) is the tcgen05 A
-//    operand and stays resident in TMEM for the whole kernel; the TMA-loaded (128 x 64) input tile is the MN-major B
-//    operand.  D1[k1, j] lands in TMEM with lane = k1.  Stages 2 / 3 are radix-64 transforms over j against DFT-64
-//    tiles resident in shared memory, stage 4 contracts k1 again; the CUDA-core passes between the MMAs apply the
-//    twiddles and k_f ("engine order", frequency k = k1 + 128*k2).  No intermediate touches HBM.
+//  * N = 128 * 64, n = i*64 + j.  Stage 1 contracts i: the 128x128 DFT matrix (cos / sin planes) is the wgmma A
+//    operand, resident in shared memory for the whole kernel; the TMA-loaded (128 x 64) input tile is the MN-major B
+//    operand.  The 128 rows k1 are split between two warpgroups (m64 each); D1[k1, j] lands in registers.  Stages 2 / 3
+//    are radix-64 transforms over j against DFT-64 tiles resident in shared memory, with the A operand taken straight
+//    from the registers of the previous stage; stage 4 contracts k1 again.  The CUDA-core passes between the MMAs apply
+//    the twiddles and k_f ("engine order", frequency k = k1 + 128*k2).  No intermediate touches HBM.
 #pragma once
 #include "ptx.cuh"
 #include <cuda.h>
@@ -25,48 +26,41 @@ struct FwdParams {
   const __nv_bfloat16* dftS; // [128][128] sin(2*pi*m*k/128)
   const uint8_t* gtiles;     // DFT-64 tiles Gr, Gi, -Gi, Gr: each 64 rows x 128 B, 128B-swizzled image
   float kf_scale;            // fp16 only: k_f is stored unscaled (1/N would underflow fp16) and scaled here in fp32
-  float tw_scale;            // folded into the twiddle table (fp16: 1/sqrt(128) keeps every stage near the input level)
+  float tw_scale;            // folded into the twiddles (fp16: 1/sqrt(128) keeps every stage near the input level)
   const uint32_t* pregate;   // optional (B,H,L) bf16, or null
   const uint32_t* postgate;
   const uint32_t* postgate2; // optional second output gate: y2 = postgate2 * conv(...)  (gated backward: du and dpregate
   uint32_t* y2;              //   come from ONE pass, reference kernels_bf16/monarch_cuda_32_16_16_bwd_kernel_bf16.h:836-870)
-  void* xg_out;              // gated three-pipeline kernel: also store u * pregate here (B,H,L), or null
+  void* xg_out;              // gated kernel: also store u * pregate here (B,H,L), or null
   int B, H, L;               // batch, channels, sequence length
   int pairs;                 // ceil(B/2)
   int kmask;                 // bit s set: 16-row K step s of the input tile can be non-zero (the rest is skipped)
   int nseg;                  // segments per tile (small sizes: 8192/N batch members share one 8192-point slot), else 1
   int seg_bytes;             // bytes of one segment inside a tile = (128 / nseg) rows x 128 B
-  int tw_n, tw_mask;         // stage-1 twiddles W_{tw_n}^{(lane & tw_mask) j}: 8192 / 127, small sizes N / (N/64 - 1)
+  int tw_n, tw_mask;         // stage-1 twiddles W_{tw_n}^{(k1 & tw_mask) j}: 8192 / 127, small sizes N / (N/64 - 1)
   int units;                 // H * pairs
   uint32_t kf_conj_mask;     // 0x80008000: multiply by conj(k_f) (du path of the backward: correlation), else 0
-  long long* trace;          // bring-up builds only (-DBFFC_BRINGUP): clock64 stamps of CTA 0, [pipe][warp 0|3][unit][16]
 };
 
 namespace r128 {
 
-constexpr int kThreads = 512;                  // outer radix-128 stage: two pipelines of
-constexpr int kPipeThreads = 256;              //   two warpgroups each
+constexpr int kPipeThreads = 256;              // one unit of work = two warpgroups (rows 0..63, 64..127)
 constexpr int kTileBytes = 128 * 128;          // one (128 rows x 64 bf16) tile
 constexpr int kSlotBytes = 2 * kTileBytes;     // re tile + im tile
 constexpr int kGTileBytes = 64 * 128;          // one DFT-64 plane
-constexpr int kSmemG = 4 * kGTileBytes;        // Gr, Gi, -Gi, Gr  (pairs at LBO 8K / 16K)
-constexpr int kSmemBars = 64;
-
-// TMEM columns
-constexpr uint32_t kColC = 0, kColS = 64;                 // DFT-128 cos / sin, bf16 K-major A operand
-DEVINL constexpr uint32_t colD(int pipe) { return 128 + 192 * pipe; }        // outer stage: 128 fp32 accumulator columns
-
-template <int kFmt> struct Idesc {
-  static constexpr uint32_t N128_MN = make_idesc(kFmt, 128, true, false);
-  static constexpr uint32_t N64_MN = make_idesc(kFmt, 64, true, false);
-  static constexpr uint32_t N64_MN_NEG = make_idesc(kFmt, 64, true, true);
-};
+constexpr int kSmemG = 4 * kGTileBytes;        // Gr, Gi, -Gi, Gr planes (r64_stage uses the first three)
+constexpr int kSmemF = 4 * kTileBytes;         // DFT-128: cos k 0..63, cos k 64..127, sin k 0..63, sin k 64..127
 
 DEVINL void cmul(float ar, float ai, float br, float bi, float& cr, float& ci) {
   cr = ar * br - ai * bi;
   ci = ar * bi + ai * br;
 }
-DEVINL uint64_t tile_desc(uint32_t saddr) { return make_sdesc(saddr, kTileBytes, 1024, 2); }
+// MN-major B operand (N = 64) of one tile; a 16-row K step = +(2048 >> 4)
+DEVINL uint64_t tile_desc(uint32_t saddr) { return make_sdesc(saddr, kTileBytes, 1024); }
+// K-major A operand: DFT-128 plane `plane` (0 = cos, 1 = sin), rows 64 hf .. 64 hf + 63, K step s (16 columns)
+DEVINL uint64_t f_desc(uint32_t s_f, int plane, int hf, int s) {
+  return make_sdesc(s_f + plane * 2 * kTileBytes + (s >> 2) * kTileBytes + hf * 64 * 128 + (s & 3) * 32, 16, 1024);
+}
 
 // One (128 x 64) input tile = nseg segments of 128/nseg rows; segment s holds batch member b = (g*nseg + s)*2 + which
 // of channel h (rows beyond L/64: TMA out-of-bounds zero fill = implicit padding).  nseg == 1 is the ordinary case
@@ -80,13 +74,165 @@ DEVINL void load_tile(uint32_t dst, const void* map, uint32_t bar, int B, int H,
     tma_load_3d(dst + s * seg_bytes, map, bar, 0, 0, b < B ? b * H + h : B * H);
   }
 }
-// N=128 B operand made of two 64-column tiles `lbo` bytes apart
-DEVINL uint64_t pair_desc(uint32_t saddr, uint32_t lbo) { return make_sdesc(saddr, lbo, 1024, 2); }
 
 DEVINL uint4 ld_shared_v4(uint32_t addr) {
   uint4 v;
   asm volatile("ld.shared.v4.b32 {%0,%1,%2,%3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(addr));
   return v;
+}
+DEVINL uint32_t ld_shared_u32(uint32_t addr) {
+  uint32_t v;
+  asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(addr));
+  return v;
+}
+DEVINL void st_shared_u32(uint32_t addr, uint32_t v) { asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(v) : "memory"); }
+
+// DFT-128 cos / sin planes (row-major 128 x 128 in global memory) -> the K-major, 128B-swizzled operand image at `dst`
+DEVINL void load_dft128(uint8_t* dst, const __nv_bfloat16* dftC, const __nv_bfloat16* dftS, int tid, int nthreads) {
+  for (int idx = tid; idx < 2 * 128 * 16; idx += nthreads) {
+    const int plane = idx >> 11, m = (idx >> 4) & 127, c16 = idx & 15;
+    const uint4 v = __ldg(reinterpret_cast<const uint4*>((plane ? dftS : dftC) + m * 128) + c16);
+    *reinterpret_cast<uint4*>(dst + plane * 2 * kTileBytes + (c16 >> 3) * kTileBytes + m * 128 +
+                              (((c16 & 7) ^ (m & 7)) << 4)) = v;
+  }
+}
+
+// This thread's place in the m64 accumulator fragment of its warpgroup: rows r0 and r0 + 8 of the 128, column pair 2 q.
+struct FragPos {
+  int r0, q;
+  DEVINL explicit FragPos(int tid) : r0(((tid >> 7) & 1) * 64 + ((tid >> 5) & 3) * 16 + ((tid & 31) >> 2)), q(tid & 3) {}
+};
+
+// Accumulator of one warpgroup's 64 rows x 64 complex columns: element (row r0 + 8 rr, column 8 i + 2 q + e) has its
+// real part at r[4 i + 2 rr + e] and its imaginary part at i[4 i + 2 rr + e].  The two halves are separate m64n64
+// accumulators, so every wgmma owns one whole register array.
+struct Acc {
+  float r[32], i[32];
+  DEVINL void zero() {
+#pragma unroll
+    for (int k = 0; k < 32; ++k) { r[k] = 0.f; i[k] = 0.f; }
+  }
+};
+
+// Issue (no wait) the radix-128 stage on this warpgroup's 64 rows: D = F128 X (kInv: conj F128 X), F = C - iS,
+// X = the (re, im) tile pair at sX.  Only the K steps set in kmask are issued (all-zero rows of X are skipped).
+//   D_re = C Xr + S Xi,  D_im = C Xi - S Xr     (kInv: D_re = C Xr - S Xi,  D_im = C Xi + S Xr)
+template <int kFmt, bool kInv>
+DEVINL void f128_stage(Acc& d, uint32_t s_f, int hf, uint32_t sX, int kmask) {
+  const uint64_t dXr = tile_desc(sX), dXi = tile_desc(sX + kTileBytes);
+  auto step = [&](int s, uint32_t acc) {
+    const uint64_t c = f_desc(s_f, 0, hf, s), sn = f_desc(s_f, 1, hf, s);
+    wgmma_ss_n64<kFmt, 1, 0>(d.r, c, dXr + 128 * s, acc);
+    wgmma_ss_n64<kFmt, 1, 0>(d.i, c, dXi + 128 * s, acc);
+    wgmma_ss_n64<kFmt, kInv ? -1 : 1, 0>(d.r, sn, dXi + 128 * s, 1);
+    wgmma_ss_n64<kFmt, kInv ? 1 : -1, 0>(d.i, sn, dXr + 128 * s, 1);
+  };
+  wgmma_fence();
+  if (kmask == 0xff) {
+#pragma unroll
+    for (int s = 0; s < 8; ++s) step(s, s > 0);
+  } else {
+    uint32_t acc = 0;
+    for (int s = 0; s < 8; ++s)
+      if ((kmask >> s) & 1) { step(s, acc); acc = 1; }
+  }
+  wgmma_commit();
+}
+// Issue (no wait) a radix-64 stage on DFT-64 planes (single 64 x 64 tiles):
+//   D_re = are * Brr + aim * Bir,  D_im = are * Bri + aim * Bii
+template <int kFmt>
+DEVINL void r64_stage(Acc& d, const uint32_t (&are)[4][4], const uint32_t (&aim)[4][4], uint32_t sBrr, uint32_t sBir,
+                      uint32_t sBri, uint32_t sBii) {
+  const uint64_t rr = tile_desc(sBrr), ir = tile_desc(sBir);
+  const uint64_t ri = tile_desc(sBri), ii = tile_desc(sBii);
+  wgmma_fence();
+#pragma unroll
+  for (int s = 0; s < 4; ++s) {
+    wgmma_rs_n64<kFmt, 0>(d.r, are[s], rr + 128 * s, s > 0);
+    wgmma_rs_n64<kFmt, 0>(d.i, are[s], ri + 128 * s, s > 0);
+  }
+#pragma unroll
+  for (int s = 0; s < 4; ++s) {
+    wgmma_rs_n64<kFmt, 0>(d.r, aim[s], ir + 128 * s, 1);
+    wgmma_rs_n64<kFmt, 0>(d.i, aim[s], ii + 128 * s, 1);
+  }
+  wgmma_commit();
+}
+// Wait for this warpgroup's MMAs.  The accumulator registers are only defined after the wait, which has no data
+// dependence on them: pin the order for the compiler.
+DEVINL void wgmma_wait_regs(Acc& d) {
+  wgmma_wait0();
+#pragma unroll
+  for (int k = 0; k < 32; ++k) asm volatile("" : "+f"(d.r[k]), "+f"(d.i[k]));
+}
+
+// Rounded 16-bit A fragments of the next stage (K = the 64 columns, four k steps).
+template <int kFmt>
+DEVINL void frag_to_a(const Acc& d, uint32_t (&are)[4][4], uint32_t (&aim)[4][4]) {
+#pragma unroll
+  for (int s = 0; s < 4; ++s)
+#pragma unroll
+    for (int h2 = 0; h2 < 2; ++h2)
+#pragma unroll
+      for (int rr = 0; rr < 2; ++rr) {
+        const int e = 4 * (2 * s + h2) + 2 * rr;
+        are[s][2 * h2 + rr] = Num<kFmt>::pack(d.r[e], d.r[e + 1]);
+        aim[s][2 * h2 + rr] = Num<kFmt>::pack(d.i[e], d.i[e + 1]);
+      }
+}
+// Byte offset of column pair 8 i + 2 q of row r in a row-major 128B-swizzled tile (the MN-major B operand image and
+// the TMA tile image are the same bytes)
+DEVINL uint32_t frag_off(int r, int i, int q) { return uint32_t(r) * 128u + (uint32_t(i ^ (r & 7)) << 4) + 4u * q; }
+// Rounded accumulator -> (re, im) tile pair at sT
+template <int kFmt>
+DEVINL void frag_store_tile(uint32_t sT, const FragPos& fp, const Acc& d) {
+#pragma unroll
+  for (int rr = 0; rr < 2; ++rr)
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      const uint32_t off = frag_off(fp.r0 + 8 * rr, i, fp.q);
+      const int e = 4 * i + 2 * rr;
+      st_shared_u32(sT + off, Num<kFmt>::pack(d.r[e], d.r[e + 1]));
+      st_shared_u32(sT + kTileBytes + off, Num<kFmt>::pack(d.i[e], d.i[e + 1]));
+    }
+}
+
+// Twiddles W_n^{kl j} of one accumulator row (kl = its stage-1 frequency), j = 8 i + 2 q + e: W^{kl (2q+e)} times the
+// block factor W^{8 kl i}, which is advanced block by block in fp32.
+struct RowTw {
+  float bc[2], bs[2], stc, sts;
+  DEVINL void init(int kl, int q, float tw_inv) {
+    sincospif(-2.0f * float(kl * 8) * tw_inv, &sts, &stc);
+#pragma unroll
+    for (int e = 0; e < 2; ++e) sincospif(-2.0f * float(kl * (2 * q + e)) * tw_inv, &bs[e], &bc[e]);
+  }
+};
+// d *= f_rr * W (kConj: * f_rr * conj W), element-wise over the fragment; f_rr = (c0 + i s0)[rr] is a per-row factor
+template <bool kConj>
+DEVINL void twiddle_frag(Acc& d, const RowTw (&tw)[2], const float (&c0)[2], const float (&s0)[2]) {
+#pragma unroll
+  for (int rr = 0; rr < 2; ++rr) {
+    float ac = c0[rr], as = s0[rr];
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const float wc = ac * tw[rr].bc[e] - as * tw[rr].bs[e], ws = ac * tw[rr].bs[e] + as * tw[rr].bc[e];
+        const int k = 4 * i + 2 * rr + e;
+        const float x = d.r[k], y = d.i[k];
+        if (!kConj) { d.r[k] = x * wc - y * ws; d.i[k] = x * ws + y * wc; }
+        else { d.r[k] = x * wc + y * ws; d.i[k] = y * wc - x * ws; }
+      }
+      const float nc = ac * tw[rr].stc - as * tw[rr].sts;
+      as = ac * tw[rr].sts + as * tw[rr].stc;
+      ac = nc;
+    }
+  }
+}
+template <bool kConj>
+DEVINL void twiddle_frag(Acc& d, const RowTw (&tw)[2], float scale) {
+  const float c0[2] = {scale, scale}, s0[2] = {0.f, 0.f};
+  twiddle_frag<kConj>(d, tw, c0, s0);
 }
 
 }  // namespace r128

@@ -1,6 +1,6 @@
 """ctypes binding of the bffc C ABI (include/bffc.h).  The shared library is built in-tree by
 `__graft_entry__.build()` as `flash-fft-conv_b200/libbffc.so`.  There is deliberately no fallback:
-if the library is missing or the device is not sm_100, every compute call raises."""
+if the library is missing or the device is not sm_90, every compute call raises."""
 import ctypes
 import os
 
@@ -52,7 +52,7 @@ def lib():
     if _lib is None:
         if not os.path.exists(LIB_PATH):
             raise BffcError(f'{LIB_PATH} not found: run `python -c "import __graft_entry__ as g; g.build()"` '
-                            'at the repo root (nvcc, sm_100a). There is no CPU/PyTorch fallback.')
+                            'at the repo root (nvcc, sm_90a). There is no CPU/PyTorch fallback.')
         l = ctypes.CDLL(LIB_PATH)
         for name, (res, args) in SYMBOLS.items():
             fn = getattr(l, name)

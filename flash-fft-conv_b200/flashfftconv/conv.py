@@ -5,7 +5,7 @@ Drop-in for `flashfftconv.FlashFFTConv` (reference flashfftconv/conv.py:71-560):
 `forward(u, k, pregate=None, postgate=None)`, same autograd contract
 (`backward -> (du, dk, None[, dpregate, dpostgate])`, conv.py:1822, :3939).
 
-All arithmetic on the hot path happens in libbffc.so (hand-written sm_100a CUDA, C ABI in
+All arithmetic on the hot path happens in libbffc.so (hand-written sm_90a CUDA, C ABI in
 include/bffc.h).  PyTorch is used for device memory and streams only: the filter-side transforms
 (k -> k_f, reference conv.py:575 + :640; dk_f -> dk, conv.py:1817-1820) are the library's own fp32 FFT launches
 for every supported size (bffc_kf_from_filter / bffc_dk_from_dkf) — no library FFT call is left in this module.
@@ -47,7 +47,7 @@ class _Plan:
         with torch.cuda.device(device):
             _lib.check(_lib.lib().bffc_plan_create(ctypes.byref(self.handle), int(seqlen), _DT[dtype]))
         # constants of the plan and memoised size queries: the per-call host path is a handful of ctypes calls, and at
-        # C2 a forward step is 0.16 ms of GPU work — Python overhead shows up as launch gaps (8 ranks per box: 0.18 ms)
+        # C2 a forward step is a fraction of a millisecond of GPU work — Python overhead shows up as launch gaps
         self.fft_size = _lib.lib().bffc_fft_size(self.handle)
         self.length_multiple = _lib.lib().bffc_length_multiple(self.handle)
         self._ws_bytes = {}

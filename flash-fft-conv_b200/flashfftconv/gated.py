@@ -1,4 +1,4 @@
-"""Routing the callers' gating through the fused operator (SURVEY.md §8f rank 3).
+"""Routing the callers' gating through the fused operator.
 
 Every model in the reference's examples wraps the convolution in two elementwise products that run as separate
 PyTorch kernels around an UNGATED call:

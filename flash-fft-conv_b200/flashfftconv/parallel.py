@@ -1,4 +1,4 @@
-"""B x H sharding of the FFT-convolution path across the GPUs of one box (SURVEY.md §8e).
+"""B x H sharding of the FFT-convolution path across the GPUs of one box.
 
 Every (b, h) convolution is independent and dk[h] is a sum over b only, so sharding the CHANNEL axis needs no
 collective in forward or backward: each rank owns a contiguous block of channels of u, k (and gates) and

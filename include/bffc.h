@@ -1,5 +1,5 @@
 /*
- * bffc.h — C ABI of the B200-native FFT long-convolution engine ("bffc").
+ * bffc.h — C ABI of the H100-native FFT long-convolution engine ("bffc").
  *
  * This is the drop-in boundary for ONE path of HazyResearch/flash-fft-conv: the fused
  * FFT convolution  y = postgate * irfft-like( FFT_N(pad(u*pregate)) * FFT_N(pad(k)) )[:L]
@@ -21,7 +21,7 @@
  * current CUDA device, all work is enqueued on the caller's `stream` (the reference used the
  * legacy default stream).  The caller owns every buffer.  Return value 0 = success, non-zero =
  * error; bffc_last_error() gives a message (thread-local).  No CPU fallback exists: on a machine
- * without an sm_100 GPU every compute entry point fails with BFFC_ERR_NO_DEVICE.
+ * without an sm_90 GPU every compute entry point fails with BFFC_ERR_NO_DEVICE.
  */
 #ifndef BFFC_H_
 #define BFFC_H_
@@ -43,7 +43,7 @@ extern "C" {
 #define BFFC_OK 0
 #define BFFC_ERR_INVALID 1     /* bad argument (shape, alignment, dtype)            */
 #define BFFC_ERR_UNSUPPORTED 2 /* seqlen / option not implemented                    */
-#define BFFC_ERR_NO_DEVICE 3   /* no CUDA device, or device is not sm_100            */
+#define BFFC_ERR_NO_DEVICE 3   /* no CUDA device, or device is not sm_90             */
 #define BFFC_ERR_CUDA 4        /* a CUDA runtime / driver call or a launch failed    */
 
 /* Opaque.  The tables are immutable after creation and bffc_fwd / bffc_bwd / the filter-side entry points may be called
@@ -73,7 +73,7 @@ int bffc_plan_destroy(bffc_plan* plan);
 int bffc_fft_size(const bffc_plan* plan);
 /* L passed to bffc_fwd / bffc_bwd / bffc_fwd_host must be a multiple of this: 64 for seqlen <= 8192 (TMA tiles of 64
  * columns), 8 for 16K..512K (16-byte vectors of the CUDA-core outer stage), seqlen/128 for 1M / 2M / 4M (whole rows of the
- * [128][seqlen/128] view of the tcgen05 outer stage).  Other lengths return BFFC_ERR_UNSUPPORTED; a caller holding such a
+ * [128][seqlen/128] view of the tensor-core outer stage).  Other lengths return BFFC_ERR_UNSUPPORTED; a caller holding such a
  * tensor zero-pads it to the next multiple (the operator is unchanged: implicit zero padding), as the host mirror does.
  * The reference itself only requires L even (README.md:270). */
 int bffc_length_multiple(const bffc_plan* plan);

@@ -8,7 +8,7 @@ Pinning: `tests/golden/*.npz` were produced by `tests/golden/make_golden.py`, wh
 reference's own `ref_fft_conv` (sliced out of /root/reference/tests/test_flashfftconv.py:5-13) and
 the reference's table builders (flashfftconv/conv.py:22-52) in this container; `tests/test_oracle.py`
 checks every function below against those fixtures.  Parity is therefore pinned to outputs of the
-reference's Python code (the reference ships no stored golden vectors, SURVEY.md §8c).
+reference's Python code (the reference ships no stored golden vectors.
 
 Each function cites the reference lines it restates (paths relative to the reference repo).
 """
@@ -77,7 +77,7 @@ def np_fft_conv(u, k, n, pregate=None, postgate=None):
 def make_inputs(B, H, N, L, dtype, seed=0, gated=False, unit_scale=False):
     """Inputs as the reference tests draw them (tests/test_flashfftconv.py:54-64, :120-128, :181-188):
     u = randn*0.02 in dtype, k = randn*0.02*exp(-0.1*arange) fp32, gates randn*0.02, dout randn*0.02.
-    unit_scale=True gives the 'set U' of SURVEY.md §8d (u~N(0,1), k~N(0,1/L)) where relative error is meaningful."""
+    unit_scale=True gives the input set (u~N(0,1), k~N(0,1/L)) where relative error is meaningful."""
     g = torch.Generator().manual_seed(seed)
     s = 1.0 if unit_scale else 0.02
     u = (torch.randn(B, H, L, generator=g) * s).to(dtype)
@@ -126,7 +126,7 @@ def kf_permute_3(k_f, n1, n2, n3):
 def monarch_conv_3(u, k, n1, n2, n3):
     """float64 restatement of the reference's fused three-radix kernel dataflow
     (kernels_bf16/monarch_cuda_32_16_16_kernel_bf16.h:590-763; tables conv.py:132-156;
-    index algebra SURVEY.md Appendix A).  u: (..., L<=N) real, k: (H, Lk) real with u[..., H, :]."""
+    index algebra of the reference's conv.py).  u: (..., L<=N) real, k: (H, Lk) real with u[..., H, :]."""
     N = n1 * n2 * n3
     M = n2 * n3
     u = np.asarray(u, dtype=np.float64)

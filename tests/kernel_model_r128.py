@@ -1,6 +1,6 @@
-"""Executable float64 model of the sm_100a kernel's dataflow for N = 128 x 64 (fwd3_r128.cuh).
+"""Executable float64 model of the sm_90a kernel's dataflow for N = 128 x 64 (fwd3_r128.cuh).
 
-Test infrastructure only.  It mirrors, stage by stage, the TMEM images the kernel produces
+Test infrastructure only.  It mirrors, stage by stage, the accumulator images the kernel produces
 (lane = row, 128 fp32 columns; round 1 compared them with stage dumps of a bring-up build of the kernel, agreement
 3e-7), and it proves (against numpy.fft) that the factorisation, the folded twiddles, the block
 layouts and the k_f "engine order" are right before any GPU time is spent.
@@ -35,7 +35,7 @@ def half_round(x):
 
 def model_fwd(x0, x1, kf_nat, quant=False, ksteps=8):
     """x0, x1: real sequences (length L <= N, zero padded here); kf_nat: FFT_N(k) natural order (complex).
-    Returns (y0, y1, stages) with stages = list of four (128,128) float64 TMEM images
+    Returns (y0, y1, stages) with stages = list of four (128,128) float64 accumulator images
     (cols [0,64) real part, [64,128) imaginary part): D1 outer DFT, D2 spectrum, D3 after inverse radix-64, D4."""
     q = bf16_round if quant else (lambda v: np.asarray(v, dtype=np.float64))
     qh = half_round if quant else (lambda v: np.asarray(v, dtype=np.float64))

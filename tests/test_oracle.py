@@ -37,8 +37,11 @@ def test_oracle_matches_reference_outputs(golden_dir, name):
         y = orc.ref_fft_conv_gated(u, k, pre, post, N)
     else:
         y = orc.ref_fft_conv(u, k, N)
-    # same algorithm, same library, same inputs: bit-exact
-    assert torch.equal(y.float(), torch.from_numpy(g['y']))
+    # same algorithm, same library, same inputs: identical up to the final rounding to the output dtype (the fp32 FFT
+    # may order its sums differently on another CPU, which can move a rounded output by one unit in the last place)
+    ref = torch.from_numpy(g['y'])
+    ulp = {torch.float32: 2.0 ** -23, torch.bfloat16: 2.0 ** -7, torch.float16: 2.0 ** -10}[dtype]
+    assert ((y.float() - ref).abs() <= ulp * ref.abs() + 2.0 ** -21 * ref.abs().max()).all()
     # float64 statement agrees to fp32/bf16 rounding of the reference output
     y64 = orc.np_fft_conv(g['u'], g['k'], N, g['pregate'] if gated else None, g['postgate'] if gated else None)
     tol = 1e-6 if dtype == torch.float32 else 8e-3

@@ -1,4 +1,4 @@
-"""GPU parity tests (run with `-m gpu` on a B200): the CUDA path, called through the reference-facing module
+"""GPU parity tests (run with `-m gpu` on an H100): the CUDA path, called through the reference-facing module
 (which goes through the C ABI), against the oracle on the same seeded inputs, the committed golden fixtures
 produced by the reference's own Python, and size-independent properties at BASELINE.json's full sizes.
 
@@ -220,7 +220,7 @@ def test_bwd_gated_golden(ffc, golden_dir):
     assert torch.allclose(k.grad.cpu(), torch.from_numpy(g['dk']), atol=1e-1)
 
 
-# ----------------------------------------------------------------------------- long sizes (two outer levels / tcgen05 outer stage)
+# ----------------------------------------------------------------------------- long sizes (two outer levels / tensor-core outer stage)
 LONG = [(131072, 2, 2, 131072), (262144, 1, 2, 131072), (524288, 2, 1, 524288), (1048576, 2, 2, 1048576),
         (1048576, 3, 2, 524288), (2097152, 2, 1, 2097152), (4194304, 2, 1, 4194304), (4194304, 1, 2, 2097152)]
 
@@ -396,7 +396,7 @@ def _unpack_kf(kf_engine, dtype):
     return torch.complex(re, im)
 
 
-# outer radices (outermost first) of the composite sizes, DESIGN.md §5: N = R0 * R1 * 8192
+# outer radices (outermost first) of the composite sizes: N = R0 * R1 * 8192
 OUTER = {8192: (1, 1), 16384: (2, 1), 32768: (4, 1), 65536: (8, 1), 131072: (8, 2), 262144: (8, 4), 524288: (8, 8),
          1048576: (128, 1), 2097152: (128, 2), 4194304: (128, 4)}
 
@@ -523,7 +523,7 @@ def test_filter_fft_entry_points_need_their_workspace(ffc):
 # ----------------------------------------------------------------------------- callers' gating routed through the fused gates
 @pytest.mark.parametrize('N,L', [(8192, 4096), (32768, 16384)])
 def test_hyena_mixer_matches_callers_pattern(ffc, N, L):
-    """SURVEY.md §8f-3: the examples' `x1v = x1 * v; y = conv(x1v, k); y = y * x2` (hyenadna_flashfftconv.py:279-284)
+    """The examples' `x1v = x1 * v; y = conv(x1v, k); y = y * x2` (hyenadna_flashfftconv.py:279-284)
     equals ONE gated call; outputs and all four gradients against autograd through the fp32 oracle of that pattern."""
     B, D = 2, 6
     torch.manual_seed(9)

@@ -1,7 +1,7 @@
-"""Precision study for the next inner kernel (DESIGN.md §6): rel-L2 error of the 8192-point pair-packed FFT convolution
+"""Precision study for the next inner kernel: rel-L2 error of the 8192-point pair-packed FFT convolution
 when every tensor-core operand is rounded to bf16, for the current two-radix split (128 x 64) and for flop-lean
 three-radix splits.  Generic mixed-radix decimation-in-frequency chain: after every stage the intermediate is multiplied
-by the inter-stage twiddle in fp32 and rounded to bf16 (what a TMEM -> register -> shared-memory pass does); DFT matrices
+by the inter-stage twiddle in fp32 and rounded to bf16 (what a register -> shared-memory pass does); DFT matrices
 are rounded to bf16; accumulation is exact (fp32 in the kernel, float64 here).  CPU only, numpy."""
 import sys
 import numpy as np
