@@ -19,7 +19,7 @@
 // spectrum is parked in a thread-private shared-memory area; the same for dout, then the product is accumulated in
 // registers.  The TMA loads of the next pair are issued as soon as stage 1 has consumed an input slot.  Gated
 // backward: the caller hands in u*pregate and dout*postgate (composite sizes: the outer stage applies the gates on
-// load; seqlen <= 8192: an elementwise pre-pass, see bffc_bwd).
+// load; seqlen <= 8192: the two fused passes of bffc_bwd store those products through FwdParams::xg_out).
 #pragma once
 #include "fwd3_r128.cuh"
 

@@ -19,17 +19,6 @@ namespace outer {
 constexpr int kVec = 8;
 
 template <int kFmt>
-DEVINL void unpack8(const uint4& v, float (&f)[8]) {
-  const uint32_t w[4] = {v.x, v.y, v.z, v.w};
-#pragma unroll
-  for (int i = 0; i < 4; ++i) upk2(Num<kFmt>::unpack(w[i]), f[2 * i], f[2 * i + 1]);
-}
-template <int kFmt>
-DEVINL uint4 pack8(const float (&f)[8]) {
-  using NT = Num<kFmt>;
-  return make_uint4(NT::pack(f[0], f[1]), NT::pack(f[2], f[3]), NT::pack(f[4], f[5]), NT::pack(f[6], f[7]));
-}
-template <int kFmt>
 DEVINL uint4 hmul8(const uint4& a, const uint4& b) {
   using NT = Num<kFmt>;
   return make_uint4(NT::hmul2(a.x, b.x), NT::hmul2(a.y, b.y), NT::hmul2(a.z, b.z), NT::hmul2(a.w, b.w));
@@ -53,15 +42,6 @@ struct OuterParams {
   int lookahead;         // blocks: a block pulls the input lines of block (its linear id + lookahead) into L2 (0 = off)
   float scale;           // applied to this stage's output (fp16: 1/sqrt(R) per direction; bf16: 1, 1/N lives in k_f)
 };
-
-// W_R^{a c} for R <= 8 as exact constants
-DEVINL void wr(int R, int e, float& c, float& s) {   // exp(-2 pi i e / R)
-  const int t = ((e % R) + R) % R * (8 / R);          // in eighths of a turn
-  const float h = 0.70710678118654752f;
-  const float cs[8] = {1.f, h, 0.f, -h, -1.f, -h, 0.f, h};
-  const float sn[8] = {0.f, -h, -1.f, -h, 0.f, h, 1.f, h};
-  c = cs[t]; s = sn[t];
-}
 
 // v += z * exp(-2 pi i e8 / 8)   (e8 = eighths of a turn, a compile-time constant after unrolling)
 DEVINL void rot_acc(int e8, f32x2 zr, f32x2 zi, f32x2& vr, f32x2& vi) {

@@ -19,9 +19,6 @@ DEVINL void mbar_init(uint32_t bar, uint32_t count) {
 DEVINL void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
 }
-DEVINL void mbar_arrive(uint32_t bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
-}
 DEVINL void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
 
 // Bounded wait: a protocol bug must not hang the GPU box (it traps instead; the host sees a launch error).  The bound
@@ -91,7 +88,6 @@ DEVINL void tma_store_4d(const void* map, uint32_t src_smem, int c0, int c1, int
 }
 DEVINL void tma_store_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 DEVINL void tma_store_wait_read0() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
-DEVINL void tma_store_wait_read1() { asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory"); }
 DEVINL void tma_store_wait_all0() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 
 // ----------------------------------------------------------------------------- wgmma
@@ -224,18 +220,6 @@ template <> struct Num<0> {
     return *reinterpret_cast<uint32_t*>(&r);
   }
 };
-
-// Warp-uniform single-thread election (elect.sync): lets the compiler keep MMA/TMA operands in uniform
-// registers instead of emitting a per-instruction uniformisation loop.
-DEVINL bool elect_one() {
-  uint32_t pred = 0;
-  asm volatile(
-      "{\n\t.reg .pred px;\n\t"
-      "elect.sync _|px, 0xffffffff;\n\t"
-      "selp.u32 %0, 1, 0, px;\n\t}"
-      : "=r"(pred));
-  return pred != 0;
-}
 
 // ----------------------------------------------------------------------------- misc
 DEVINL uint32_t pack_bf16x2(float lo, float hi) {

@@ -51,10 +51,6 @@ constexpr int kGTileBytes = 64 * 128;          // one DFT-64 plane
 constexpr int kSmemG = 4 * kGTileBytes;        // Gr, Gi, -Gi, Gr planes (r64_stage uses the first three)
 constexpr int kSmemF = 4 * kTileBytes;         // DFT-128: cos k 0..63, cos k 64..127, sin k 0..63, sin k 64..127
 
-DEVINL void cmul(float ar, float ai, float br, float bi, float& cr, float& ci) {
-  cr = ar * br - ai * bi;
-  ci = ar * bi + ai * br;
-}
 // MN-major B operand (N = 64) of one tile; a 16-row K step = +(2048 >> 4)
 DEVINL uint64_t tile_desc(uint32_t saddr) { return make_sdesc(saddr, kTileBytes, 1024); }
 // K-major A operand: DFT-128 plane `plane` (0 = cos, 1 = sin), rows 64 hf .. 64 hf + 63, K step s (16 columns)
