@@ -15,13 +15,18 @@
 #include "outer_cuda.cuh"
 #include "outer_r128.cuh"
 #include "filter_fft.cuh"
+#include "dwconv1d.cuh"
 
+#include <algorithm>
 #include <cmath>
 #include <cstdarg>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <initializer_list>
 #include <mutex>
+#include <type_traits>
+#include <utility>
 #include <vector>
 
 namespace {
@@ -1144,6 +1149,158 @@ int bffc_fwd_host(const bffc_plan* p, const void* u_host, const void* kf, const 
     return rc;
   }
   return BFFC_OK;
+}
+
+}  // extern "C"
+
+// ------------------------------------------------------------------------------------- depthwise convolution (no plan)
+namespace {
+
+template <class T>
+struct Tag {
+  using type = T;
+};
+
+// fn(Tag<T>, Tag<W>, integral_constant<KMAX>) for input type u_dtype, weight type w_dtype; K <= 4 (the models' short
+// filters) gets a kernel that keeps only four taps in registers
+template <class Fn>
+void dw_dispatch(int u_dtype, int w_dtype, int K, Fn&& fn) {
+  auto with_k = [&](auto tu, auto tw) {
+    if (K <= 4) fn(tu, tw, std::integral_constant<int, 4>());
+    else fn(tu, tw, std::integral_constant<int, bffc::dw::kMaxK>());
+  };
+  auto with_w = [&](auto tu) {
+    if (w_dtype == BFFC_DTYPE_FP32) with_k(tu, Tag<float>());
+    else if (w_dtype == BFFC_DTYPE_FP16) with_k(tu, Tag<__half>());
+    else with_k(tu, Tag<__nv_bfloat16>());
+  };
+  if (u_dtype == BFFC_DTYPE_FP32) with_w(Tag<float>());
+  else if (u_dtype == BFFC_DTYPE_FP16) with_w(Tag<__half>());
+  else with_w(Tag<__nv_bfloat16>());
+}
+
+size_t dw_elem(int dtype) { return dtype == BFFC_DTYPE_FP32 ? 4 : 2; }
+
+// Shape checks shared by the three entry points; fills the launch geometry (backward: its tiles cover du positions
+// [0, L) and dout positions [0, Lout), and `tiles` is the number of parts per batch member).
+int dw_geometry(const char* fn, int B, int D, int L, int K, int P, int layout, bool backward, bffc::dw::Shape* sh,
+                long long* ctas) {
+  using namespace bffc::dw;
+  if (layout != BFFC_LAYOUT_BHL && layout != BFFC_LAYOUT_BLH) return fail(BFFC_ERR_INVALID, "%s: layout %d is not BHL (0) or BLH (1)", fn, layout);
+  if (K < 1 || K > kMaxK) return fail(BFFC_ERR_INVALID, "%s: K=%d outside [1, %d]", fn, K, kMaxK);
+  if (P < 0 || P > K - 1) return fail(BFFC_ERR_INVALID, "%s: padding %d outside [0, K-1=%d]", fn, P, K - 1);
+  if (B < 1 || D < 1 || L < 1 || L > (1 << 30)) return fail(BFFC_ERR_INVALID, "%s: bad shape B=%d D=%d L=%d", fn, B, D, L);
+  const int Lout = L + 2 * P - K + 1;
+  if (Lout < 1) return fail(BFFC_ERR_INVALID, "%s: output length L + 2P - K + 1 = %d < 1", fn, Lout);
+  const long long span = backward ? std::max(L, Lout) : Lout;
+  long long n;
+  *sh = Shape{B, D, L, K, P, Lout, 0, 1};
+  if (layout == BFFC_LAYOUT_BHL) {
+    const long long tiles = (span + kTileL - 1) / kTileL;
+    sh->tiles = int(tiles);
+    n = static_cast<long long>(B) * D * tiles;
+  } else {
+    const long long tile = backward ? kStripL : blh_tile(K);       // the kernel for K <= 4 keeps at most 4 taps
+    const long long tiles = (span + tile - 1) / tile;
+    sh->tiles = int(tiles);
+    sh->dchunks = (D + kChunkD - 1) / kChunkD;
+    n = static_cast<long long>(B) * tiles * sh->dchunks;
+  }
+  if (n > 0x7fffffffLL) return fail(BFFC_ERR_INVALID, "%s: shape B=%d D=%d L=%d needs %lld CTAs (limit 2^31-1)", fn, B, D, L, n);
+  *ctas = n;
+  return 0;
+}
+
+int dw_dtypes(const char* fn, int u_dtype, int w_dtype) {
+  auto ok = [](int t) { return t == BFFC_DTYPE_BF16 || t == BFFC_DTYPE_FP16 || t == BFFC_DTYPE_FP32; };
+  if (!ok(u_dtype) || !ok(w_dtype)) return fail(BFFC_ERR_INVALID, "%s: dtype codes %d / %d (BF16 0, FP16 1, FP32 2)", fn, u_dtype, w_dtype);
+  return 0;
+}
+
+// every pointer non-null and aligned to its element size
+int dw_pointers(const char* fn, std::initializer_list<std::pair<const void*, size_t>> ptrs) {
+  for (auto& pe : ptrs) {
+    if (!pe.first) return fail(BFFC_ERR_INVALID, "%s: null pointer", fn);
+    if (reinterpret_cast<uintptr_t>(pe.first) % pe.second)
+      return fail(BFFC_ERR_INVALID, "%s: pointer not aligned to its %zu-byte element", fn, pe.second);
+  }
+  return 0;
+}
+
+}  // namespace
+
+extern "C" {
+
+size_t bffc_dwconv1d_workspace_bytes(int B, int D, int L, int K, int padding, int layout) {
+  bffc::dw::Shape sh;
+  long long ctas;
+  char msg[sizeof(g_err)];
+  memcpy(msg, g_err, sizeof(msg));               // a size query leaves the last error message alone
+  const int rc = dw_geometry("bffc_dwconv1d_workspace_bytes", B, D, L, K, padding, layout, true, &sh, &ctas);
+  memcpy(g_err, msg, sizeof(msg));
+  if (rc) return 0;
+  return size_t(K + 1) * D * B * sh.tiles * sizeof(float);
+}
+
+int bffc_dwconv1d_fwd(const void* u, int u_dtype, const void* w, const void* bias, int w_dtype, void* y, int B, int D,
+                      int L, int K, int padding, int layout, void* stream) {
+  const char* fn = "bffc_dwconv1d_fwd";
+  bffc::dw::Shape sh;
+  long long ctas;
+  if (int rc = dw_dtypes(fn, u_dtype, w_dtype)) return rc;
+  if (int rc = dw_geometry(fn, B, D, L, K, padding, layout, false, &sh, &ctas)) return rc;
+  const size_t eu = dw_elem(u_dtype), ew = dw_elem(w_dtype);
+  if (int rc = dw_pointers(fn, {{u, eu}, {w, ew}, {bias, ew}, {y, eu}})) return rc;
+  if (int rc = check_device()) return rc;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  g_launches = 0;
+  dw_dispatch(u_dtype, w_dtype, K, [&](auto tu, auto tw, auto km) {
+    using T = typename decltype(tu)::type;
+    using W = typename decltype(tw)::type;
+    constexpr int KM = decltype(km)::value;
+    auto kernel = layout == BFFC_LAYOUT_BHL ? bffc::dw::fwd_bhl<T, W, KM> : bffc::dw::fwd_blh<T, W, KM>;
+    kernel<<<unsigned(ctas), bffc::dw::kThreads, 0, st>>>(static_cast<const T*>(u), static_cast<const W*>(w),
+                                                         static_cast<const W*>(bias), static_cast<T*>(y), sh);
+  });
+  return launched();
+}
+
+int bffc_dwconv1d_bwd(const void* dout, const void* u, int u_dtype, const void* w, int w_dtype, void* du, void* dw,
+                      void* dbias, int B, int D, int L, int K, int padding, int layout, void* workspace,
+                      size_t workspace_bytes, void* stream) {
+  const char* fn = "bffc_dwconv1d_bwd";
+  bffc::dw::Shape sh;
+  long long ctas;
+  if (int rc = dw_dtypes(fn, u_dtype, w_dtype)) return rc;
+  if (int rc = dw_geometry(fn, B, D, L, K, padding, layout, true, &sh, &ctas)) return rc;
+  const size_t eu = dw_elem(u_dtype), ew = dw_elem(w_dtype);
+  if (int rc = dw_pointers(fn, {{dout, eu}, {u, eu}, {w, ew}, {du, eu}, {dw, ew}, {dbias, ew}, {workspace, 4}})) return rc;
+  const size_t need = bffc_dwconv1d_workspace_bytes(B, D, L, K, padding, layout);
+  if (workspace_bytes < need) return fail(BFFC_ERR_INVALID, "%s: workspace of %zu bytes required", fn, need);
+  if (int rc = check_device()) return rc;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  float* part = static_cast<float*>(workspace);
+  g_launches = 0;
+  dw_dispatch(u_dtype, w_dtype, K, [&](auto tu, auto tw, auto km) {
+    using T = typename decltype(tu)::type;
+    using W = typename decltype(tw)::type;
+    constexpr int KM = decltype(km)::value;
+    auto kernel = layout == BFFC_LAYOUT_BHL ? bffc::dw::bwd_bhl<T, W, KM> : bffc::dw::bwd_blh<T, W, KM>;
+    kernel<<<unsigned(ctas), bffc::dw::kThreads, 0, st>>>(static_cast<const T*>(dout), static_cast<const T*>(u),
+                                                         static_cast<const W*>(w), static_cast<T*>(du), part, sh);
+  });
+  if (int rc = launched()) return rc;
+  const long long rows = static_cast<long long>(K + 1) * D, per_cta = bffc::dw::kThreads / 32;
+  const long long parts = static_cast<long long>(B) * sh.tiles;
+  auto reduce = [&](auto tw) {
+    using W = typename decltype(tw)::type;
+    bffc::dw::reduce_parts<W><<<unsigned((rows + per_cta - 1) / per_cta), bffc::dw::kThreads, 0, st>>>(
+        part, static_cast<W*>(dw), static_cast<W*>(dbias), D, K, parts, layout == BFFC_LAYOUT_BLH);
+  };
+  if (w_dtype == BFFC_DTYPE_FP32) reduce(Tag<float>());
+  else if (w_dtype == BFFC_DTYPE_FP16) reduce(Tag<__half>());
+  else reduce(Tag<__nv_bfloat16>());
+  return launched();
 }
 
 }  // extern "C"

@@ -9,6 +9,9 @@ LIB_PATH = os.path.join(os.path.dirname(_HERE), 'libbffc.so')
 
 BFFC_DTYPE_BF16 = 0
 BFFC_DTYPE_FP16 = 1
+BFFC_DTYPE_FP32 = 2          # depthwise convolution only
+BFFC_LAYOUT_BHL = 0
+BFFC_LAYOUT_BLH = 1
 
 _lib = None
 
@@ -39,6 +42,11 @@ SYMBOLS = {
     'bffc_host_workspace_bytes': (_c.c_size_t, [_c.c_void_p, _c.c_int, _c.c_int, _c.c_int, _c.c_int]),
     'bffc_fwd_host': (_c.c_int, [_c.c_void_p] * 6 + [_c.c_int] * 3 + [_c.c_void_p, _c.c_size_t, _c.c_void_p]),
     'bffc_last_launch_count': (_c.c_int, []),
+    'bffc_dwconv1d_fwd': (_c.c_int, [_c.c_void_p, _c.c_int, _c.c_void_p, _c.c_void_p, _c.c_int, _c.c_void_p]
+                          + [_c.c_int] * 6 + [_c.c_void_p]),
+    'bffc_dwconv1d_workspace_bytes': (_c.c_size_t, [_c.c_int] * 6),
+    'bffc_dwconv1d_bwd': (_c.c_int, [_c.c_void_p, _c.c_void_p, _c.c_int, _c.c_void_p, _c.c_int, _c.c_void_p, _c.c_void_p,
+                                     _c.c_void_p] + [_c.c_int] * 6 + [_c.c_void_p, _c.c_size_t, _c.c_void_p]),
 }
 
 

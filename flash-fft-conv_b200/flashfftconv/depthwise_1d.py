@@ -1,0 +1,120 @@
+"""Depthwise 1-D convolution: drop-in for `flashfftconv.FlashDepthWiseConv1d` (reference flashfftconv/depthwise_1d.py).
+
+The operator is exactly `torch.nn.Conv1d(D, D, K, groups=D, padding=P)` on `(B, D, L)` input (`is_bhl=True`) or the same
+convolution along L of `(B, L, D)` input (`is_bhl=False`).  Both passes run in libbffc.so (bffc_dwconv1d_fwd /
+bffc_dwconv1d_bwd, include/bffc.h): the forward is one kernel, the backward two (du with per-CTA partial sums of the
+weight and bias gradients, then their fixed-order reduction).  All arithmetic is fp32 whatever the input and weight
+types.
+
+Differences from the reference, each deliberate:
+- it accumulates in fp32 (the reference accumulates in the 16-bit input type);
+- the backward allocates no (B, D, K, L) tensor (the reference materialises one and runs a matmul over it);
+- the BLH weight gradient is in the (K, D) layout of the parameter (the reference returns the (D, K) gradient
+  reinterpreted with .view);
+- any K in [1, 32] and any padding in [0, K - 1] (the reference requires odd K, and its BHL kernel is wrong whenever
+  padding != (K - 1) // 2), and any D in BLH (the reference assumes even D);
+- the module keeps torch.nn.Module's own load_state_dict (the reference overrides it with a no-op).
+"""
+import torch
+
+from . import _lib
+from .conv import _on_device, _ptr, _stream
+
+_DT = {torch.bfloat16: _lib.BFFC_DTYPE_BF16, torch.float16: _lib.BFFC_DTYPE_FP16, torch.float32: _lib.BFFC_DTYPE_FP32}
+MAX_KERNEL_SIZE = 32
+
+
+def _check(u, weights, bias, padding, is_bhl):
+    """Shape (B, D, L, K) of a valid call; RuntimeError otherwise."""
+    for name, t in (('input', u), ('weights', weights), ('bias', bias)):
+        if not t.is_cuda:
+            raise RuntimeError(f'{name} must be a CUDA tensor (there is no CPU path)')
+        if t.device != u.device:
+            raise RuntimeError(f'{name} is on {t.device}, input on {u.device}')
+        if not t.is_contiguous():
+            raise RuntimeError(f'{name} must be contiguous')
+        if t.dtype not in _DT:
+            raise RuntimeError(f'{name} has dtype {t.dtype}; supported: float32, float16, bfloat16')
+    if weights.dtype != bias.dtype:
+        raise RuntimeError(f'weights ({weights.dtype}) and bias ({bias.dtype}) must have the same dtype')
+    if u.dim() != 3 or weights.dim() != 2 or bias.dim() != 1:
+        raise RuntimeError(f'expected input of rank 3, weights of rank 2 and bias of rank 1, got {u.dim()}, '
+                           f'{weights.dim()}, {bias.dim()}')
+    if is_bhl:
+        B, D, L = u.shape
+        K = weights.shape[1]
+        wshape = (D, K)
+    else:
+        B, L, D = u.shape
+        K = weights.shape[0]
+        wshape = (K, D)
+    if tuple(weights.shape) != wshape or tuple(bias.shape) != (D,):
+        raise RuntimeError(f'input has {D} channels: expected weights {wshape} and bias ({D},), got '
+                           f'{tuple(weights.shape)} and {tuple(bias.shape)}')
+    if not 1 <= K <= MAX_KERNEL_SIZE:
+        raise RuntimeError(f'kernel size {K} outside [1, {MAX_KERNEL_SIZE}]')
+    if not 0 <= padding <= K - 1:
+        raise RuntimeError(f'padding {padding} outside [0, K - 1 = {K - 1}]')
+    if L + 2 * padding - K + 1 < 1:
+        raise RuntimeError(f'output length L + 2 * padding - K + 1 = {L + 2 * padding - K + 1} < 1')
+    if min(B, D, L) < 1:
+        raise RuntimeError(f'empty input {tuple(u.shape)}')
+    return B, D, L, K
+
+
+class DepthWiseConv1dFunc(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, u, weights, bias, padding, is_bhl=True):
+        padding = int(padding)
+        B, D, L, K = _check(u, weights, bias, padding, is_bhl)
+        Lout = L + 2 * padding - K + 1
+        layout = _lib.BFFC_LAYOUT_BHL if is_bhl else _lib.BFFC_LAYOUT_BLH
+        with _on_device(u.device):
+            y = torch.empty((B, D, Lout) if is_bhl else (B, Lout, D), dtype=u.dtype, device=u.device)
+            _lib.check(_lib.lib().bffc_dwconv1d_fwd(_ptr(u), _DT[u.dtype], _ptr(weights), _ptr(bias), _DT[weights.dtype],
+                                                    _ptr(y), B, D, L, K, padding, layout, _stream()))
+        ctx.shape = (B, D, L, K, padding, layout)
+        ctx.save_for_backward(u, weights, bias)
+        return y
+
+    @staticmethod
+    def backward(ctx, dout):
+        u, weights, bias = ctx.saved_tensors
+        B, D, L, K, padding, layout = ctx.shape
+        dout = dout.contiguous()                                      # reference depthwise_1d.py:19
+        with _on_device(u.device):
+            du = torch.empty_like(u)
+            dw = torch.empty_like(weights)
+            dbias = torch.empty_like(bias)
+            nws = _lib.lib().bffc_dwconv1d_workspace_bytes(B, D, L, K, padding, layout)
+            ws = torch.empty(nws, dtype=torch.uint8, device=u.device)
+            _lib.check(_lib.lib().bffc_dwconv1d_bwd(_ptr(dout), _ptr(u), _DT[u.dtype], _ptr(weights), _DT[weights.dtype],
+                                                    _ptr(du), _ptr(dw), _ptr(dbias), B, D, L, K, padding, layout,
+                                                    _ptr(ws), nws, _stream()))
+        return du, dw, dbias, None, None
+
+
+class FlashDepthWiseConv1d(torch.nn.Module):
+    """Depthwise convolution with the reference's constructor.  `weights` / `bias` are the tensors of an
+    `nn.Conv1d(channels, channels, kernel_size, groups=channels)`: weights (D, 1, K), bias (D,).  They are copied into
+    the parameters `weights` ((D, K) for BHL, (K, D) for BLH, the reference's layouts, so state dicts interchange with
+    it) and `bias`, converted to `device` / `dtype` when those are given."""
+
+    def __init__(self, channels, kernel_size, padding, weights, bias, is_bhl=True, device=None, dtype=None):
+        super().__init__()
+        self.d = channels
+        self.k = kernel_size
+        self.padding = padding
+        self.is_bhl = is_bhl
+        w = weights.detach().reshape(channels, kernel_size)
+        if not is_bhl:
+            w = w.t()
+        factory_kwargs = {'device': device, 'dtype': dtype}
+        self.weights = torch.nn.Parameter(w.to(**factory_kwargs).contiguous().clone())
+        self.bias = torch.nn.Parameter(bias.detach().reshape(channels).to(**factory_kwargs).contiguous().clone())
+
+    def extra_repr(self):
+        return f'channels={self.d}, kernel_size={self.k}, padding={self.padding}, is_bhl={self.is_bhl}'
+
+    def forward(self, input):
+        return DepthWiseConv1dFunc.apply(input, self.weights, self.bias, self.padding, self.is_bhl)

@@ -1,9 +1,10 @@
 /*
  * bffc.h — C ABI of the H100-native FFT long-convolution engine ("bffc").
  *
- * This is the drop-in boundary for ONE path of HazyResearch/flash-fft-conv: the fused
- * FFT convolution  y = postgate * irfft-like( FFT_N(pad(u*pregate)) * FFT_N(pad(k)) )[:L]
- * behind  FlashFFTConv(seqlen, dtype)(u, k, pregate, postgate).
+ * This is the drop-in boundary for the two operators HazyResearch/flash-fft-conv exports:
+ *   - the fused FFT convolution  y = postgate * irfft-like( FFT_N(pad(u*pregate)) * FFT_N(pad(k)) )[:L]
+ *     behind  FlashFFTConv(seqlen, dtype)(u, k, pregate, postgate)  (plan-based entry points below);
+ *   - the short depthwise convolution behind  FlashDepthWiseConv1d(...)(u)  (bffc_dwconv1d_*, no plan).
  *
  * Reference interfaces each entry point replaces (paths relative to the reference repo):
  *   bffc_fwd          <- monarch_conv_forward_* / butterfly_*_forward pybind ops
@@ -16,6 +17,8 @@
  *                        Python per call (conv.py:575, :640, :676, :1423-1424, :1632-1633)
  *   bffc_dk_from_dkf / bffc_dkf_unpack* <- their inverses for dk_f + torch.fft.ifft(...).real (conv.py:1817-1820, :1862, :2954)
  *   bffc_plan_*       <- FlashFFTConv.__init__ constant tables (conv.py:72-551)
+ *   bffc_dwconv1d_*   <- conv1d_forward / conv1d_backward pybind ops (monarch.cpp:58-59, conv1d/conv1d.h), called from
+ *                        flashfftconv/depthwise_1d.py
  *
  * Conventions: plain pointers and sizes only, all data pointers are DEVICE pointers on the
  * current CUDA device, all work is enqueued on the caller's `stream` (the reference used the
@@ -169,7 +172,35 @@ int bffc_fwd_host(const bffc_plan* plan, const void* u_host, const void* kf_engi
                   const void* pregate_host, const void* postgate_host, void* y_host, int B, int H,
                   int L, void* dev_workspace, size_t dev_workspace_bytes, void* stream);
 
-/* Number of kernel launches the last bffc_fwd / bffc_bwd / bffc_fwd_host on this thread enqueued (bench.py). */
+/*
+ * Depthwise 1-D convolution, the short filter of the reference's FlashDepthWiseConv1d (reference conv1d_forward /
+ * conv1d_backward, csrc/flashfftconv/conv1d/).  No plan: these entry points need no tables.  Exactly
+ * torch.nn.Conv1d(D, D, K, groups=D, padding=P):
+ *
+ *     y[b, d, l] = bias[d] + sum_{k<K} w[d, k] * u[b, d, l - P + k]      (u = 0 outside [0, L)),  0 <= l < Lout
+ *     Lout = L + 2P - K + 1
+ *
+ * layout BFFC_LAYOUT_BHL: u, y (B, D, L) and w (D, K); BFFC_LAYOUT_BLH: u, y (B, L, D) and w (K, D) (the reference's
+ * parameter layouts).  bias (D).  All contiguous device memory.  1 <= K <= 32, 0 <= P <= K - 1, Lout >= 1.
+ * u_dtype (u, y, dout, du) and w_dtype (w, bias, dw, dbias) are each BF16, FP16 or FP32; arithmetic is fp32.
+ * Forward is one launch.  Backward is two: du and per-CTA fp32 partial sums of dw / dbias into `workspace` (at least
+ * bffc_dwconv1d_workspace_bytes, a function of the shape only), then a fixed-order reduction of the partials, so results
+ * are bit-identical across runs and devices.  dw is in the layout of w.  Arguments are validated before the device is
+ * looked at: a bad argument is BFFC_ERR_INVALID on any machine.
+ */
+#define BFFC_DTYPE_FP32 2 /* depthwise entry points only; bffc_supported / bffc_plan_create take BF16 / FP16 */
+#define BFFC_LAYOUT_BHL 0
+#define BFFC_LAYOUT_BLH 1
+int bffc_dwconv1d_fwd(const void* u, int u_dtype, const void* w, const void* bias, int w_dtype, void* y, int B, int D,
+                      int L, int K, int padding, int layout, void* stream);
+/* 0 for invalid arguments */
+size_t bffc_dwconv1d_workspace_bytes(int B, int D, int L, int K, int padding, int layout);
+int bffc_dwconv1d_bwd(const void* dout, const void* u, int u_dtype, const void* w, int w_dtype, void* du, void* dw,
+                      void* dbias, int B, int D, int L, int K, int padding, int layout, void* workspace,
+                      size_t workspace_bytes, void* stream);
+
+/* Number of kernel launches the last bffc_fwd / bffc_bwd / bffc_fwd_host / filter-side transform /
+ * bffc_dwconv1d_fwd (1) / bffc_dwconv1d_bwd (2) on this thread enqueued (bench.py). */
 int bffc_last_launch_count(void);
 
 #ifdef __cplusplus
