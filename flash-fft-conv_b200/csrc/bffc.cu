@@ -474,21 +474,27 @@ size_t bffc_filter_workspace_bytes(const bffc_plan* p, int H) {
   return (pairs < group ? pairs : group) * per;
 }
 
-int bffc_kf_from_filter(const bffc_plan* p, const void* k, int Lk, void* kf_engine, int H, int conj, void* workspace,
-                        size_t workspace_bytes, void* stream) {
-  if (!p || !k || !kf_engine || H <= 0 || Lk <= 0) return fail(BFFC_ERR_INVALID, "bffc_kf_from_filter: bad argument");
-  if (Lk > p->N) return fail(BFFC_ERR_INVALID, "bffc_kf_from_filter: Lk=%d exceeds seqlen %d", Lk, p->N);
+// band that keeps every frequency of the plan's seqlen grid (min(f, N - f) <= N/2 < band)
+static int full_band(const bffc_plan* p) { return p->N / 2 + 1; }
+
+// bffc_kf_from_filter / bffc_kf_from_filter_band
+static int kf_from_filter(const bffc_plan* p, const void* k, int Lk, void* kf_engine, int H, int conj, int band,
+                          void* workspace, size_t workspace_bytes, void* stream, const char* name) {
+  if (!p || !k || !kf_engine || H <= 0 || Lk <= 0) return fail(BFFC_ERR_INVALID, "%s: bad argument", name);
+  if (band < 0) return fail(BFFC_ERR_INVALID, "%s: band=%d is negative", name, band);
+  if (Lk > p->N) return fail(BFFC_ERR_INVALID, "%s: Lk=%d exceeds seqlen %d", name, Lk, p->N);
   using namespace bffc::ffft;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   g_launches = 0;
   if (p->NE == kInner) {
     FMT_SWITCH(p->dtype, (kf_from_filter_kernel<F><<<(H + 1) / 2, kThreads, kSmemBytes, st>>>(
-        static_cast<const float*>(k), Lk, static_cast<uint4*>(kf_engine), H, p->kf_pack_scale, conj, p->tw8192, p->N)););
+        static_cast<const float*>(k), Lk, static_cast<uint4*>(kf_engine), H, p->kf_pack_scale, conj, p->tw8192, p->N,
+        band)););
     return launched();
   }
   const size_t per = filter_pair_bytes(p);
   if (!workspace || workspace_bytes < per)
-    return fail(BFFC_ERR_INVALID, "bffc_kf_from_filter: workspace %zu B < %zu B (one channel pair; see bffc_filter_workspace_bytes)", workspace_bytes, per);
+    return fail(BFFC_ERR_INVALID, "%s: workspace %zu B < %zu B (one channel pair; see bffc_filter_workspace_bytes)", name, workspace_bytes, per);
   const int group = int(std::min<size_t>(workspace_bytes / per, size_t(H + 1) / 2)) * 2;   // channels per group
   float2* T = static_cast<float2*>(workspace);
   for (int h0 = 0; h0 < H; h0 += group) {
@@ -499,27 +505,29 @@ int bffc_kf_from_filter(const bffc_plan* p, const void* k, int Lk, void* kf_engi
         kc, Lk, T, Hc, p->kf_pack_scale, p->tw512, p->tw_lo, p->tw_hi)););
     if (int rc = launched()) return rc;
     FMT_SWITCH(p->dtype, (filter_rows_kernel<F><<<dim3(p->R / 2 + 1, Hc), kThreads, kSmemBytes, st>>>(
-        T, out, p->R, p->R0, p->R1, conj, p->tw8192)););
+        T, out, p->R, p->R0, p->R1, conj, p->tw8192, band)););
     if (int rc = launched()) return rc;
   }
   return BFFC_OK;
 }
 
-int bffc_dk_from_dkf(const bffc_plan* p, const void* dkf_engine, void* dk, int Lk, int H, void* workspace,
-                     size_t workspace_bytes, void* stream) {
-  if (!p || !dkf_engine || !dk || H <= 0 || Lk <= 0) return fail(BFFC_ERR_INVALID, "bffc_dk_from_dkf: bad argument");
-  if (Lk > p->N) return fail(BFFC_ERR_INVALID, "bffc_dk_from_dkf: Lk=%d exceeds seqlen %d", Lk, p->N);
+// bffc_dk_from_dkf / bffc_dk_from_dkf_band
+static int dk_from_dkf(const bffc_plan* p, const void* dkf_engine, void* dk, int Lk, int H, int band, void* workspace,
+                       size_t workspace_bytes, void* stream, const char* name) {
+  if (!p || !dkf_engine || !dk || H <= 0 || Lk <= 0) return fail(BFFC_ERR_INVALID, "%s: bad argument", name);
+  if (band < 0) return fail(BFFC_ERR_INVALID, "%s: band=%d is negative", name, band);
+  if (Lk > p->N) return fail(BFFC_ERR_INVALID, "%s: Lk=%d exceeds seqlen %d", name, Lk, p->N);
   using namespace bffc::ffft;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   g_launches = 0;
   if (p->NE == kInner) {
     dk_from_dkf_kernel<<<H, kThreads, kSmemBytes, st>>>(static_cast<const float2*>(dkf_engine), static_cast<float*>(dk), Lk,
-                                                         p->dk_scale, p->N, p->tw8192);
+                                                         p->dk_scale, p->N, p->tw8192, band);
     return launched();
   }
   const size_t per = filter_pair_bytes(p);
   if (!workspace || workspace_bytes < per)
-    return fail(BFFC_ERR_INVALID, "bffc_dk_from_dkf: workspace %zu B < %zu B (one channel pair; see bffc_filter_workspace_bytes)", workspace_bytes, per);
+    return fail(BFFC_ERR_INVALID, "%s: workspace %zu B < %zu B (one channel pair; see bffc_filter_workspace_bytes)", name, workspace_bytes, per);
   const int group = int(std::min<size_t>(workspace_bytes / per, size_t(H + 1) / 2)) * 2;
   float2* T = static_cast<float2*>(workspace);
   for (int h0 = 0; h0 < H; h0 += group) {
@@ -527,13 +535,34 @@ int bffc_dk_from_dkf(const bffc_plan* p, const void* dkf_engine, void* dk, int L
     const float2* in = static_cast<const float2*>(dkf_engine) + size_t(h0) * p->NE;
     float* out = static_cast<float*>(dk) + size_t(h0) * Lk;
     dk_rows_kernel<<<dim3(p->R / 2 + 1, Hc), kThreads, kSmemBytes, st>>>(in, T, p->R, p->R0, p->R1, p->tw8192, p->tw_lo,
-                                                                          p->tw_hi);
+                                                                          p->tw_hi, band);
     if (int rc = launched()) return rc;
     COLS_SWITCH(p->R, (dk_cols_kernel<RR><<<dim3(kInner / ColRadix<RR>::kTC, (Hc + 1) / 2), kColThreads, ColRadix<RR>::kSmem, st>>>(
         T, out, Lk, Hc, p->dk_scale / float(p->NE), p->tw512)););
     if (int rc = launched()) return rc;
   }
   return BFFC_OK;
+}
+
+int bffc_kf_from_filter(const bffc_plan* p, const void* k, int Lk, void* kf_engine, int H, int conj, void* workspace,
+                        size_t workspace_bytes, void* stream) {
+  return kf_from_filter(p, k, Lk, kf_engine, H, conj, p ? full_band(p) : 0, workspace, workspace_bytes, stream,
+                        "bffc_kf_from_filter");
+}
+
+int bffc_kf_from_filter_band(const bffc_plan* p, const void* k, int Lk, void* kf_engine, int H, int conj, int band,
+                             void* workspace, size_t workspace_bytes, void* stream) {
+  return kf_from_filter(p, k, Lk, kf_engine, H, conj, band, workspace, workspace_bytes, stream, "bffc_kf_from_filter_band");
+}
+
+int bffc_dk_from_dkf(const bffc_plan* p, const void* dkf_engine, void* dk, int Lk, int H, void* workspace,
+                     size_t workspace_bytes, void* stream) {
+  return dk_from_dkf(p, dkf_engine, dk, Lk, H, p ? full_band(p) : 0, workspace, workspace_bytes, stream, "bffc_dk_from_dkf");
+}
+
+int bffc_dk_from_dkf_band(const bffc_plan* p, const void* dkf_engine, void* dk, int Lk, int H, int band, void* workspace,
+                          size_t workspace_bytes, void* stream) {
+  return dk_from_dkf(p, dkf_engine, dk, Lk, H, band, workspace, workspace_bytes, stream, "bffc_dk_from_dkf_band");
 }
 
 int bffc_dkf_unpack(const bffc_plan* p, const void* dkf_engine, void* dkf_natural, int H, void* stream) {

@@ -11,6 +11,8 @@
 // plan table that stays in L1.  Output frequency f = q1 + 16 q2 + 256 q3 ends at position 512 q1 + 32 q2 + q3;
 // the engine-order pack / the time-domain read-out undo that permutation on the fly, so nothing goes through HBM
 // between the FFT and the layout change.  Two real filters share one complex FFT (z = k_a + i k_b).
+// Every filter-side kernel that knows a frequency (the pack side and the read side of dk_f) also applies an optional band
+// limit there (in_band below): the frequency-sparse convolution's mask, free when it keeps everything.
 #pragma once
 #include "ptx.cuh"
 
@@ -129,13 +131,18 @@ DEVINL void fft8192(float2* buf, int tid, const float2* __restrict__ tw) {
 
 DEVINL int pos_of_freq(int f) { return 512 * (f & 15) + 32 * ((f >> 4) & 15) + (f >> 8); }
 
+// Band limit of the filter-side kernels: a frequency f of the seqlen-point grid N is kept iff min(f, N - f) < band
+// (zeroed otherwise).  The mask is real and symmetric, so it commutes with the Hermitian separation and with conjugation;
+// any band >= N/2 + 1 keeps every frequency.
+DEVINL bool in_band(int f, int N, int band) { return min(f, N - f) < band; }
+
 // grid = ceil(H / 2): channels 2*blockIdx.x (real part) and 2*blockIdx.x + 1 (imaginary part)
 // N < 8192 (small sizes): the engine row holds the N-point spectrum K_N[f] = K_8192[f * 8192/N] (k has support < N) at
 // (lane k1, column k2) -> f = (k1 mod N/64) + (N/64) k2, i.e. replicated over the 8192/N stage-1 blocks of the kernel.
 template <int kFmt>
 __global__ void __launch_bounds__(kThreads, 3) kf_from_filter_kernel(const float* __restrict__ k, int Lk, uint4* __restrict__ kf_eng,
                                                                      int H, float scale, int conj, const float2* __restrict__ tw,
-                                                                     int N) {
+                                                                     int N, int band) {
   extern __shared__ float2 fbuf[];
   const int tid = threadIdx.x, ha = 2 * blockIdx.x, hb = ha + 1;
   const float* ka = k + size_t(ha) * Lk;
@@ -164,10 +171,11 @@ __global__ void __launch_bounds__(kThreads, 3) kf_from_filter_kernel(const float
     float2 A[4], Bv[4];
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
-      const int f = ((k1 & (r - 1)) + r * (4 * c + j)) * q8;
+      const int fn = (k1 & (r - 1)) + r * (4 * c + j), f = fn * q8;     // frequency on the N grid, on the 8192 grid
       const float2 z = fbuf[slot(pos_of_freq(f))], zc = fbuf[slot(pos_of_freq((kN - f) & (kN - 1)))];
-      A[j] = make_float2((z.x + zc.x) * sa, (z.y - zc.y) * sa * sgn);
-      Bv[j] = make_float2((z.y + zc.y) * sa, (zc.x - z.x) * sa * sgn);
+      const bool keep = in_band(fn, N, band);
+      A[j] = keep ? make_float2((z.x + zc.x) * sa, (z.y - zc.y) * sa * sgn) : make_float2(0.f, 0.f);
+      Bv[j] = keep ? make_float2((z.y + zc.y) * sa, (zc.x - z.x) * sa * sgn) : make_float2(0.f, 0.f);
     }
     kf_eng[size_t(ha) * (kN / 4) + v] = make_uint4(NT::pack(A[0].x, A[1].x), NT::pack(A[0].y, A[1].y),
                                                     NT::pack(A[2].x, A[3].x), NT::pack(A[2].y, A[3].y));
@@ -181,9 +189,10 @@ __global__ void __launch_bounds__(kThreads, 3) kf_from_filter_kernel(const float
 // Engine order of dk_f (dkf3_r128.cuh): index ((qd*128 + k1)*16 + k2l) holds (lane k1, column k2 = 16 qd + k2l).
 // N = 8192: frequency k1 + 128 k2.  N < 8192: the 8192/N stage-1 blocks hold different batch members at the same
 // N-point frequency f = (k1 mod r) + r k2, r = N/64; their sum D_N[f] goes to 8192-point frequency f * 8192/N (the rest
-// is zero), whose inverse transform is the N-periodic gradient.
+// is zero), whose inverse transform is the N-periodic gradient.  The band limit masks D_N[f] as it is read (Re ifft of
+// the masked spectrum = ifft of the masked Hermitian part, the mask being symmetric).
 __global__ void __launch_bounds__(kThreads, 3) dk_from_dkf_kernel(const float2* __restrict__ dkf_eng, float* __restrict__ dk, int Lk,
-                                                                  float scale, int N, const float2* __restrict__ tw) {
+                                                                  float scale, int N, const float2* __restrict__ tw, int band) {
   extern __shared__ float2 fbuf[];
   const int tid = threadIdx.x, h = blockIdx.x;
   const float2* src = dkf_eng + size_t(h) * kN;
@@ -191,7 +200,9 @@ __global__ void __launch_bounds__(kThreads, 3) dk_from_dkf_kernel(const float2* 
 #pragma unroll 16
     for (int e = tid; e < kN; e += kThreads) {
       const int k2l = e & 15, k1 = (e >> 4) & 127, qd = e >> 11;
-      fbuf[slot(k1 + 128 * (16 * qd + k2l))] = __ldg(src + e);
+      const int f = k1 + 128 * (16 * qd + k2l);
+      const float2 d = __ldg(src + e);
+      fbuf[slot(f)] = in_band(f, kN, band) ? d : make_float2(0.f, 0.f);
     }
   } else {
     const int r = N >> 6, q8 = kN / N;
@@ -205,7 +216,8 @@ __global__ void __launch_bounds__(kThreads, 3) dk_from_dkf_kernel(const float2* 
       float2 acc = make_float2(0.f, 0.f);
 #pragma unroll 4
       for (int m = 0; m < q8; ++m) acc = cadd(acc, __ldg(b0 + ((r * m) << 4)));
-      fbuf[slot((k1p + r * (16 * qd + k2l)) * q8)] = acc;
+      const int fn = k1p + r * (16 * qd + k2l);                       // frequency on the N grid
+      fbuf[slot(fn * q8)] = in_band(fn, N, band) ? acc : make_float2(0.f, 0.f);
     }
   }
   __syncthreads();
@@ -369,11 +381,12 @@ DEVINL void load_row(float2* fbuf, const float2* __restrict__ src, int tid) {
 }
 
 // engine vector v = c*128 + k1 holds the frequencies f_j = k1 + 128 (4c + j); with k1 fixed per thread (v = tid + 256 i)
-// pos_of_freq(f_j) = 512 (k1 & 15) + 32 ((k1 >> 4) + 8 (j & 1)) + 2c + (j >> 1); the mirrored row reads 8191 - f_j
+// pos_of_freq(f_j) = 512 (k1 & 15) + 32 ((k1 >> 4) + 8 (j & 1)) + 2c + (j >> 1); the mirrored row reads 8191 - f_j.
+// rho_w: residue of the row written, whose word f_j holds natural frequency rho_w + R f_j (band-limited there)
 template <int kFmt, bool kMirror>
-DEVINL void store_engine_row(const float2* fbuf, uint4* __restrict__ row, int tid, float sgn) {
+DEVINL void store_engine_row(const float2* fbuf, uint4* __restrict__ row, int tid, float sgn, int rho_w, int R, int band) {
   using NT = Num<kFmt>;
-  const int k1 = tid & 127;
+  const int k1 = tid & 127, N = R * kN;
 #pragma unroll 4
   for (int i = 0; i < 8; ++i) {
     const int c = (tid >> 7) + 2 * i;
@@ -386,7 +399,7 @@ DEVINL void store_engine_row(const float2* fbuf, uint4* __restrict__ row, int ti
         const int k1m = 127 - k1, jm = 3 - j, cm = 15 - c;
         p = 512 * (k1m & 15) + 32 * ((k1m >> 4) + 8 * (jm & 1)) + 2 * cm + (jm >> 1);
       }
-      A[j] = fbuf[slot(p)];
+      A[j] = in_band(rho_w + R * (k1 + 128 * (4 * c + j)), N, band) ? fbuf[slot(p)] : make_float2(0.f, 0.f);
     }
     row[tid + 256 * i] = make_uint4(NT::pack(A[0].x, A[1].x), NT::pack(sgn * A[0].y, sgn * A[1].y),
                                     NT::pack(A[2].x, A[3].x), NT::pack(sgn * A[2].y, sgn * A[3].y));
@@ -396,17 +409,19 @@ DEVINL void store_engine_row(const float2* fbuf, uint4* __restrict__ row, int ti
 // grid (R/2 + 1, Hc).  kf_eng: (Hc, R rows, 2048 vectors of 16 bytes); row of residue rho = (rho % R0) * R1 + rho / R0
 template <int kFmt>
 __global__ void __launch_bounds__(kThreads, 3) filter_rows_kernel(const float2* __restrict__ T, uint4* __restrict__ kf_eng, int R, int R0,
-                                                                  int R1, int conj, const float2* __restrict__ tw) {
+                                                                  int R1, int conj, const float2* __restrict__ tw, int band) {
   extern __shared__ float2 fbuf[];
   const int tid = threadIdx.x, rho = blockIdx.x, h = blockIdx.y;
   load_row(fbuf, T + (size_t(h) * (R / 2 + 1) + rho) * kN, tid);
   __syncthreads();
   fft8192<-1>(fbuf, tid, tw);
   const float sgn = conj ? -1.f : 1.f;
-  store_engine_row<kFmt, false>(fbuf, kf_eng + (size_t(h) * R + (rho % R0) * R1 + rho / R0) * (kN / 4), tid, sgn);
+  store_engine_row<kFmt, false>(fbuf, kf_eng + (size_t(h) * R + (rho % R0) * R1 + rho / R0) * (kN / 4), tid, sgn, rho, R,
+                                band);
   if (rho == 0 || 2 * rho == R) return;
   const int rm = R - rho;
-  store_engine_row<kFmt, true>(fbuf, kf_eng + (size_t(h) * R + (rm % R0) * R1 + rm / R0) * (kN / 4), tid, -sgn);
+  store_engine_row<kFmt, true>(fbuf, kf_eng + (size_t(h) * R + (rm % R0) * R1 + rm / R0) * (kN / 4), tid, -sgn, rm, R,
+                               band);
 }
 
 // ---- inverse: dk (Hc, Lk) fp32 from dk_f engine rows (fp32 complex, row layout [quarter 4][k1 128][k2l 16], frequency
@@ -416,10 +431,11 @@ __global__ void __launch_bounds__(kThreads, 3) filter_rows_kernel(const float2* 
 // grid (R/2 + 1, Hc).  T: (Hc, R/2 + 1, 8192) = Y[rho][n2] = sum_{n1} W_R^{n1 rho} dk[n1*8192 + n2], unscaled.
 __global__ void __launch_bounds__(kThreads, 3) dk_rows_kernel(const float2* __restrict__ dkf_eng, float2* __restrict__ T, int R, int R0,
                                                               int R1, const float2* __restrict__ tw,
-                                                              const float2* __restrict__ tw_lo, const float2* __restrict__ tw_hi) {
+                                                              const float2* __restrict__ tw_lo, const float2* __restrict__ tw_hi,
+                                                              int band) {
   extern __shared__ float2 fbuf[];
   const int tid = threadIdx.x, rho = blockIdx.x, h = blockIdx.y;
-  const int rm = (R - rho) & (R - 1);
+  const int rm = (R - rho) & (R - 1), N = R * kN;
   const float2* row = dkf_eng + (size_t(h) * R + (rho % R0) * R1 + rho / R0) * kN;
   const float2* mrow = dkf_eng + (size_t(h) * R + (rm % R0) * R1 + rm / R0) * kN;
 #pragma unroll 8
@@ -432,7 +448,7 @@ __global__ void __launch_bounds__(kThreads, 3) dk_rows_kernel(const float2* __re
       em = ((k2m >> 4) * 128 + (fm & 127)) * 16 + (k2m & 15);
     }
     const float2 a = row[e], b = mrow[em];
-    fbuf[slot(f)] = make_float2(0.5f * (a.x + b.x), 0.5f * (a.y - b.y));
+    fbuf[slot(f)] = in_band(rho + R * f, N, band) ? make_float2(0.5f * (a.x + b.x), 0.5f * (a.y - b.y)) : make_float2(0.f, 0.f);
   }
   __syncthreads();
   fft8192<1>(fbuf, tid, tw);

@@ -93,7 +93,7 @@ class FlashFFTConv(torch.nn.Module):
         d = self.__dict__
         d['_plans'] = {}
         d['_host_ws'] = {}
-        d['_kf_cache'] = None          # (weakref(k), k._version, device, kf_engine)
+        d['_kf_cache'] = None          # (weakref(k), k._version, device, kf_engine, band)
         d['last_launches'] = 0         # kernels enqueued by the most recent forward / backward (bench.py)
 
     def __getstate__(self):
@@ -215,32 +215,39 @@ def _filter_workspace(plan, H, device):
     return (torch.empty(n, dtype=torch.uint8, device=device) if n else None), n
 
 
-def _pack_kf(mod, plan, k, conj=0):
+def _pack_kf(mod, plan, k, conj=0, band=None):
     """k (H, Lk) fp32 device -> engine-order packed spectrum (H, N) int32 words by the library's own fp32 FFT
     (bffc_kf_from_filter): one launch for engine size 8192, column + row FFT launches per L2-sized channel group for
-    the composite sizes (replaces conv.py:575 + :640)."""
+    the composite sizes (replaces conv.py:575 + :640).  band: None for the full spectrum, else the band limit of
+    bffc_kf_from_filter_band (frequencies with min(f, seqlen - f) >= band are zeroed)."""
     k32 = k.detach()
     if k32.dtype != torch.float32 or not k32.is_contiguous():
         k32 = k32.to(torch.float32).contiguous()
     H, Lk = k32.shape
     kf_engine = torch.empty((H, plan.fft_size), dtype=torch.int32, device=k.device)
     ws, ws_bytes = _filter_workspace(plan, H, k.device)
-    _lib.check(_lib.lib().bffc_kf_from_filter(plan.handle, _ptr(k32), int(Lk), _ptr(kf_engine), int(H), int(conj),
-                                              _ptr(ws), ws_bytes, _stream()))
+    if band is None:
+        _lib.check(_lib.lib().bffc_kf_from_filter(plan.handle, _ptr(k32), int(Lk), _ptr(kf_engine), int(H), int(conj),
+                                                  _ptr(ws), ws_bytes, _stream()))
+    else:
+        _lib.check(_lib.lib().bffc_kf_from_filter_band(plan.handle, _ptr(k32), int(Lk), _ptr(kf_engine), int(H),
+                                                       int(conj), int(band), _ptr(ws), ws_bytes, _stream()))
     mod.__dict__['last_launches'] = _lib.lib().bffc_last_launch_count()
     return kf_engine
 
 
-def _kf_engine_for(mod, plan, k, cache_key=None):
-    """Engine-order spectrum of `k`, cached in eval mode while the same tensor object is unmodified."""
+def _kf_engine_for(mod, plan, k, cache_key=None, band=None, use_cache=None):
+    """Engine-order spectrum of `k` (band-limited unless band is None), cached in eval mode (use_cache=None: the
+    module's own mode) while the same tensor object is unmodified and the band is the same."""
     key = k if cache_key is None else cache_key
-    use_cache = not mod.training
+    if use_cache is None:
+        use_cache = not mod.training
     if use_cache and mod._kf_cache is not None:
-        ref, ver, dev, kf = mod._kf_cache
-        if ref() is key and ver == key._version and dev == k.device:
+        ref, ver, dev, kf, kf_band = mod._kf_cache
+        if ref() is key and ver == key._version and dev == k.device and kf_band == band:
             return kf
-    kf = _pack_kf(mod, plan, k)
-    mod.__dict__['_kf_cache'] = (weakref.ref(key), key._version, k.device, kf) if use_cache else None
+    kf = _pack_kf(mod, plan, k, band=band)
+    mod.__dict__['_kf_cache'] = (weakref.ref(key), key._version, k.device, kf, band) if use_cache else None
     return kf
 
 
@@ -277,17 +284,18 @@ class _on_device:
             self.ctx.__exit__(*a)
 
 
-def _fwd(mod, u, k, pregate, postgate):
+def _fwd(mod, u, k, pregate, postgate, band=None, use_cache=None):
+    """y and the engine-order filter spectrum it used.  band / use_cache: see _kf_engine_for."""
     L0 = u.shape[-1]
     Lp = _pad_len(mod, u.device, L0)
     if Lp != L0:
-        y, kf = _fwd(mod, _padded(u, Lp), k, _padded(pregate, Lp), _padded(postgate, Lp))
+        y, kf = _fwd(mod, _padded(u, Lp), k, _padded(pregate, Lp), _padded(postgate, Lp), band, use_cache)
         return y[..., :L0].contiguous(), kf
     B, H, L = u.shape
     plan = mod.plan(u.device)
     with _on_device(u.device):
         mod.__dict__['last_launches'] = 0
-        kf_engine = _kf_engine_for(mod, plan, k)
+        kf_engine = _kf_engine_for(mod, plan, k, band=band, use_cache=use_cache)
         y = torch.empty_like(u)
         ws, ws_bytes = _workspace(plan, B, H, L, pregate is not None, False, u.device)
         _lib.check(_lib.lib().bffc_fwd(plan.handle, _ptr(u), _ptr(kf_engine), _ptr(pregate), _ptr(postgate),
@@ -296,12 +304,14 @@ def _fwd(mod, u, k, pregate, postgate):
     return y, kf_engine
 
 
-def _bwd(mod, dout, u, kf_engine, k_len, pregate, postgate):
-    """du, dk[, dpregate, dpostgate] — reference: FlashFFTConvFunc.backward, conv.py:1737-1822."""
+def _bwd(mod, dout, u, kf_engine, k_len, pregate, postgate, band=None):
+    """du, dk[, dpregate, dpostgate] — reference: FlashFFTConvFunc.backward, conv.py:1737-1822.  band: the forward's
+    band limit (None: full spectrum); kf_engine is then the band-limited spectrum and dk gets the same mask."""
     L0 = u.shape[-1]
     Lp = _pad_len(mod, u.device, L0)
     if Lp != L0:
-        r = _bwd(mod, _padded(dout, Lp), _padded(u, Lp), kf_engine, k_len, _padded(pregate, Lp), _padded(postgate, Lp))
+        r = _bwd(mod, _padded(dout, Lp), _padded(u, Lp), kf_engine, k_len, _padded(pregate, Lp), _padded(postgate, Lp),
+                 band)
         cut = lambda t: None if t is None else t[..., :L0].contiguous()
         return cut(r[0]), r[1], cut(r[2]), cut(r[3])
     B, H, L = u.shape
@@ -324,8 +334,12 @@ def _bwd(mod, dout, u, kf_engine, k_len, pregate, postgate):
         # (only the Hermitian part of dk_f contributes), sum over the batch-member blocks of the small sizes, [:k_len]
         dk = torch.empty((H, k_len), dtype=torch.float32, device=u.device)
         fws, fws_bytes = _filter_workspace(plan, H, u.device)
-        _lib.check(_lib.lib().bffc_dk_from_dkf(plan.handle, _ptr(dkf_engine), _ptr(dk), int(k_len), H, _ptr(fws), fws_bytes,
-                                               _stream()))
+        if band is None:
+            _lib.check(_lib.lib().bffc_dk_from_dkf(plan.handle, _ptr(dkf_engine), _ptr(dk), int(k_len), H, _ptr(fws),
+                                                   fws_bytes, _stream()))
+        else:
+            _lib.check(_lib.lib().bffc_dk_from_dkf_band(plan.handle, _ptr(dkf_engine), _ptr(dk), int(k_len), H, int(band),
+                                                        _ptr(fws), fws_bytes, _stream()))
         mod.__dict__['last_launches'] += _lib.lib().bffc_last_launch_count()
     return du, dk, dpre, dpost
 

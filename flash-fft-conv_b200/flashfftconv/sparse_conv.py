@@ -2,19 +2,21 @@
 
 The reference ships these two operators as plain-PyTorch examples (flashfftconv/sparse_conv.py:9-38: `PartialFFTConv`
 truncates the filter to its first N_partial taps, `FrequencySparseFFTConv` zeroes the rfft bins from N_partial // 2 up;
-both convolve at FFT size N = 2 L and keep the first L outputs).  Same classes, same call `forward(x, k)`, but the
-convolution itself is one `FlashFFTConv(2 L)` launch sequence on the 16-bit engine:
+both convolve at FFT size N = 2 L and keep the first L outputs).  Same classes, same call `forward(x, k)`, and gradients
+reach both `x` and `k` as they do through the reference's torch operations, but the convolution itself is one
+`FlashFFTConv(2 L)` launch sequence on the 16-bit engine:
 
 * partial: the engine takes filters shorter than the sequence natively (`k: (H, Lk <= seqlen)`, zero-extended inside the
-  filter-side FFT kernel), so truncation is a view;
-* frequency-sparse: the masked half-spectrum goes through `bffc_kf_pack_rfft` (Hermitian completion, engine order, 1/N,
-  cast) — the one place this package computes an FFT outside the library, because the caller's operator is defined on
-  `torch.fft.rfft` bins.  Forward only (the reference example has no custom backward either; use it for inference).
+  filter-side FFT kernel), so truncation is a differentiable view;
+* frequency-sparse: the band limit is part of the library's fp32 filter transforms.  With c = N_partial // 2 and M the
+  mask that zeroes the frequencies f of the N-point grid with min(f, N - f) >= c (the rfft bins j >= c and their
+  mirrors), the forward packs M * FFT_N(k) (bffc_kf_from_filter_band) and runs bffc_fwd; M is real and symmetric, so
+  the backward is bffc_bwd with that same masked spectrum for dx, and dk = ifft(M * dk_f).real[:, :Lk]
+  (bffc_dk_from_dkf_band).  No FFT runs outside the library.
 """
 import torch
 
-from . import _lib
-from .conv import FlashFFTConv, _pack_kf_from_natural, _ptr, _stream, _workspace, _check_inputs, _on_device
+from .conv import FlashFFTConv, _bwd, _check_inputs, _fwd
 
 
 class _EngineCache(torch.nn.Module):
@@ -41,32 +43,45 @@ class PartialFFTConv(_EngineCache):
         return self.conv(2 * L, x.dtype, x.device)(x, k[..., : self.N_partial].contiguous())
 
 
+class FrequencySparseFFTConvFunc(torch.autograd.Function):
+    """y = irfft(rfft(x, N) * M * rfft(k, N), N)[..., :L] on the engine `mod` (seqlen N = 2 L), band = N_partial // 2.
+    save: keep x and the masked spectrum for backward (only when a gradient is wanted).  use_cache: reuse the masked
+    spectrum across calls while the same `k` is unmodified (the eval-mode filter cache of FlashFFTConv)."""
+
+    @staticmethod
+    def forward(ctx, x, k, mod, band, save, use_cache):
+        _check_inputs(x, k, mod)
+        y, kf_engine = _fwd(mod, x, k, None, None, band=band, use_cache=use_cache)
+        ctx.mod, ctx.k_len, ctx.band = mod, k.shape[-1], band
+        if save:
+            ctx.save_for_backward(x, kf_engine)
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        x, kf_engine = ctx.saved_tensors
+        dx, dk, _, _ = _bwd(ctx.mod, dy, x, kf_engine, ctx.k_len, None, None, band=ctx.band)
+        return dx, dk, None, None, None, None
+
+
 class FrequencySparseFFTConv(_EngineCache):
     """y = irfft(rfft(x, 2L) * mask(rfft(k, 2L)))[..., :L] with the bins from N_partial // 2 up zeroed
-    (reference sparse_conv.py:25-38)."""
+    (reference sparse_conv.py:25-38), trainable: gradients flow to x and to k.
+
+    Any L the engine takes at seqlen 2L works; lengths that are not a multiple of bffc_length_multiple() are zero-padded
+    as FlashFFTConv pads them.  In eval mode the masked filter spectrum is cached while the same `k` tensor is
+    unmodified and N_partial is unchanged.  `self.conv(2 * L, dtype, device).last_launches` counts the kernels of the
+    most recent call: forward = filter transform (1 launch at seqlen <= 8192, 2 per channel group above; 0 on a cache
+    hit) + bffc_fwd; backward = bffc_bwd + the band-limited dk transform."""
 
     def __init__(self, N_partial):
         super().__init__()
         self.N_partial = N_partial
 
-    @torch.no_grad()
     def forward(self, x, k):
-        B, H, L = x.shape
+        L = x.shape[-1]
         mod = self.conv(2 * L, x.dtype, x.device)
-        _check_inputs(x, k, mod)
-        plan = mod.plan(x.device)
-        if L % plan.length_multiple:
-            raise RuntimeError(f'L={L} must be a multiple of {plan.length_multiple} for seqlen {2 * L}')
-        with _on_device(x.device):
-            # the caller's bins are those of an rfft at 2L; the small sizes live on the 8192-point grid, where bin j of 2L
-            # is bin j * q (the pack kernel samples exactly those), so the cut-off scales by q
-            n = plan.fft_size
-            q = n // (2 * L)
-            k_f = torch.fft.rfft(k.float(), n=n)
-            k_f[..., (self.N_partial // 2) * q:] = 0
-            kf_engine = _pack_kf_from_natural(mod, plan, k_f.contiguous(), 0)
-            y = torch.empty_like(x)
-            ws, ws_bytes = _workspace(plan, B, H, L, False, False, x.device)
-            _lib.check(_lib.lib().bffc_fwd(plan.handle, _ptr(x), _ptr(kf_engine), None, None, _ptr(y), B, H, L,
-                                           _ptr(ws), ws_bytes, _stream()))
-        return y
+        # the engines sit in a plain dict (no .train() / .eval() reaches them): this module's own mode and the grad
+        # state decide caching and saving
+        save = torch.is_grad_enabled() and (x.requires_grad or k.requires_grad)
+        return FrequencySparseFFTConvFunc.apply(x, k, mod, self.N_partial // 2, save, not self.training)

@@ -124,6 +124,22 @@ int bffc_kf_from_filter(const bffc_plan* plan, const void* k, int Lk, void* kf_e
 int bffc_dk_from_dkf(const bffc_plan* plan, const void* dkf_engine, void* dk, int Lk, int H,
                      void* workspace, size_t workspace_bytes, void* stream);
 
+/*
+ * Band-limited filter-side transforms (the reference's FrequencySparseFFTConv, flashfftconv/sparse_conv.py:25-38):
+ * with N = seqlen (not bffc_fft_size) and M the real, symmetric mask that zeroes every frequency f of the N-point grid
+ * with min(f, N - f) >= band (the rfft bins j >= band and their mirrors),
+ *   bffc_kf_from_filter_band: kf_engine = pack(M * FFT_N(k))                       -> y = irfft(rfft(u) * M * rfft(k))
+ *   bffc_dk_from_dkf_band:    dk = ifft(M * unpack(dkf)).real[:, :Lk]              (the filter gradient of that operator)
+ * P = F^-1 M F is a real self-adjoint projection, so the input gradient needs nothing new: bffc_bwd with the masked
+ * kf_engine (kf_engine_conj NULL).  band = 0: an all-zero spectrum (y and dk are zero); band >= N/2 + 1: identical to
+ * bffc_kf_from_filter / bffc_dk_from_dkf, which are these calls with that band; band < 0: BFFC_ERR_INVALID.  Workspace
+ * rule and launch count are those of the unbanded pair.
+ */
+int bffc_kf_from_filter_band(const bffc_plan* plan, const void* k, int Lk, void* kf_engine, int H, int conj, int band,
+                             void* workspace, size_t workspace_bytes, void* stream);
+int bffc_dk_from_dkf_band(const bffc_plan* plan, const void* dkf_engine, void* dk, int Lk, int H, int band,
+                          void* workspace, size_t workspace_bytes, void* stream);
+
 /* Scratch the caller must provide.  bffc_workspace_bytes_ex: exact need of bffc_fwd (backward = 0) or bffc_bwd
  * (backward = 1) for a gated / ungated call; bffc_workspace_bytes: enough for any call with these shapes.
  * seqlen <= 8192: 0, except the gated backward (two (B,H,L) tensors: the gated inputs handed to the dk_f kernel).
