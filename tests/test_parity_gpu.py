@@ -14,6 +14,7 @@ import torch
 pytestmark = pytest.mark.gpu
 
 from oracle import fftconv_oracle as orc  # noqa: E402
+from oracle.spectral_oracle import OUTER, _engine_freqs, _unpack_kf  # noqa: E402
 
 REL_L2 = 1e-2
 MAX_REL = 1e-2
@@ -388,35 +389,6 @@ def test_forward_host_rejects_bad_arguments(ffc):
 
 
 # ----------------------------------------------------------------------------- filter-side FFT kernels (every size)
-def _unpack_kf(kf_engine, dtype):
-    """engine words (H, N) int32 = (re01, im01, re23, im23) groups -> (H, N/4, 4) complex64, engine order"""
-    w = kf_engine.view(torch.int16).view(dtype).float().reshape(kf_engine.shape[0], -1, 4, 2)     # [v][re01 im01 re23 im23][2]
-    re = torch.stack([w[:, :, 0, 0], w[:, :, 0, 1], w[:, :, 2, 0], w[:, :, 2, 1]], dim=-1)
-    im = torch.stack([w[:, :, 1, 0], w[:, :, 1, 1], w[:, :, 3, 0], w[:, :, 3, 1]], dim=-1)
-    return torch.complex(re, im)
-
-
-# outer radices (outermost first) of the composite sizes: N = R0 * R1 * 8192
-OUTER = {8192: (1, 1), 16384: (2, 1), 32768: (4, 1), 65536: (8, 1), 131072: (8, 2), 262144: (8, 4), 524288: (8, 8),
-         1048576: (128, 1), 2097152: (128, 2), 4194304: (128, 4)}
-
-
-def _engine_freqs(N):
-    """(NE/4, 4) frequency of the N-point spectrum held by component j of engine vector v of one channel.
-    N >= 8192: row = v // 2048 = c0*R1 + c1, inside a row vector cc*128 + k1 holds inner frequencies
-    k'' = k1 + 128*(4cc + j); k = c0 + R0*(c1 + R1*k'').  N < 8192 (one row): lane k1 belongs to stage-1 block k1 // r,
-    r = N/64, and holds frequency (k1 mod r) + r*(4cc + j) — the N-point spectrum replicated over the 8192/N blocks."""
-    if N < 8192:
-        r = N // 64
-        rem = torch.arange(2048)
-        return ((rem % 128) % r)[:, None] + r * (4 * (rem // 128)[:, None] + torch.arange(4)[None, :])
-    R0, R1 = OUTER[N]
-    v = torch.arange(N // 4)
-    row, rem = v // 2048, v % 2048
-    inner = (rem % 128)[:, None] + 128 * (4 * (rem // 128)[:, None] + torch.arange(4)[None, :])
-    return (row // R1)[:, None] + R0 * ((row % R1)[:, None] + R1 * inner)
-
-
 def _rfft_natural(mod, k):
     return torch.fft.rfft(k.to(torch.float32), n=mod.fft_size(k.device)).contiguous()
 
