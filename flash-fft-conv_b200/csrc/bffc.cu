@@ -626,10 +626,18 @@ extern "C" size_t bffc_workspace_bytes(const bffc_plan* p, int B, int H, int L) 
   return bffc_workspace_bytes_ex(p, B, H, L, 1, 1);     // enough for every call with these shapes
 }
 
-// 128B-swizzled tensor map of rank 3 or 4 over 16-bit elements of the plan's dtype; dims[0] = 64 elements (128 B)
+// A (B, H, L) tensor argument of the engine: rows contiguous (channel stride L), element (b, h, l) at
+// p + b * bs + h * L + l; bs (elements) is a multiple of 8 and >= H * L.  Composite sizes offset p chunk by chunk.
+struct Seq {
+  void* p = nullptr;
+  int64_t bs = 0;
+};
+static Seq seq(const void* p, int64_t bs) { return Seq{const_cast<void*>(p), bs}; }
+
+// 128B-swizzled tensor map of rank 3 to 5 over 16-bit elements of the plan's dtype; dims[0] = 64 elements (128 B)
 static int encode_map(const bffc_plan* p, CUtensorMap* map, const void* base, cuuint32_t rank, const cuuint64_t* dims,
                       const cuuint64_t* strides, const cuuint32_t* box) {
-  const cuuint32_t estr[4] = {1, 1, 1, 1};
+  const cuuint32_t estr[5] = {1, 1, 1, 1, 1};
   CUresult r = g_encode(map, p->dtype == BFFC_DTYPE_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16,
                         rank, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                         CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
@@ -637,13 +645,21 @@ static int encode_map(const bffc_plan* p, CUtensorMap* map, const void* base, cu
   return 0;
 }
 
-static int make_map(const bffc_plan* p, CUtensorMap* map, const void* base, int rows, int L, int box_rows = 128) {
-  // (rows, L) bf16 viewed as [row][L/64][64]; box = one (128 x 64) tile, 128B swizzle;
-  // tile rows >= L/64 are out of bounds: zero-filled on load (implicit padding), dropped on store.
+static int make_map(const bffc_plan* p, CUtensorMap* map, const void* base, int rows, int L) {
+  // complex-row planes: (rows, L) viewed as [row][L/64][64]; box = one (128 x 64) tile, 128B swizzle
   const cuuint64_t dims[3] = {64, cuuint64_t(L / 64), cuuint64_t(rows)};
   const cuuint64_t strides[2] = {128, cuuint64_t(L) * 2};
-  const cuuint32_t box[3] = {64, cuuint32_t(box_rows), 1};
+  const cuuint32_t box[3] = {64, 128, 1};
   return encode_map(p, map, base, 3, dims, strides, box);
+}
+
+static int make_seq_map(const bffc_plan* p, CUtensorMap* map, Seq t, int B, int H, int L, int box_rows) {
+  // (B, H, L) tensor viewed as [b][h][L/64][64]; box = one (box_rows x 64) tile of one sequence, 128B swizzle;
+  // tile rows >= L/64 and members b >= B are out of bounds: zero-filled on load (implicit padding), dropped on store.
+  const cuuint64_t dims[4] = {64, cuuint64_t(L / 64), cuuint64_t(H), cuuint64_t(B)};
+  const cuuint64_t strides[3] = {128, cuuint64_t(L) * 2, cuuint64_t(t.bs) * 2};
+  const cuuint32_t box[4] = {64, cuuint32_t(box_rows), 1, 1};
+  return encode_map(p, map, t.p, 4, dims, strides, box);
 }
 
 static int make_map4(const bffc_plan* p, CUtensorMap* map, const void* base, int chunks, int rows, int seqs,
@@ -653,6 +669,15 @@ static int make_map4(const bffc_plan* p, CUtensorMap* map, const void* base, int
   const cuuint64_t strides[3] = {128, cuuint64_t(row_stride_bytes), cuuint64_t(seq_stride_bytes)};
   const cuuint32_t box[4] = {64, 1, 128, 1};
   return encode_map(p, map, base, 4, dims, strides, box);
+}
+
+static int make_endpoint_map(const bffc_plan* p, CUtensorMap* map, Seq t, int chunks, int M, int L, int Hs, int B) {
+  // (B, Hs, L) tensor viewed as [b][h][L/M][chunk][64]: the [L/M][M] rows of each sequence cut into 64-column
+  // chunks; box = 128 rows x 64 columns of one chunk of one sequence, 128B swizzle.
+  const cuuint64_t dims[5] = {64, cuuint64_t(chunks), cuuint64_t(L / M), cuuint64_t(Hs), cuuint64_t(B)};
+  const cuuint64_t strides[4] = {128, cuuint64_t(M) * 2, cuuint64_t(L) * 2, cuuint64_t(t.bs) * 2};
+  const cuuint32_t box[5] = {64, 1, 128, 1, 1};
+  return encode_map(p, map, t.p, 5, dims, strides, box);
 }
 
 // Persistent kernels: one block per `per_block` units of work, at most one block per SM.
@@ -707,38 +732,39 @@ static bffc::FwdParams fwd_params(const bffc_plan* p, const void* kf, int conj) 
 // optional extras of one pass of the forward path
 struct PassOpts {
   int conj = 0;                     // 1: conjugate k_f inside the kernel's pointwise multiply (else kf is pre-conjugated)
-  const void* postgate2 = nullptr;  // second gated output y2 = postgate2 * conv(...) from the same pass
-  void* y2 = nullptr;
+  Seq postgate2;                    // second gated output y2 = postgate2 * conv(...) from the same pass
+  Seq y2;
   void* xg_out = nullptr;           // seqlen <= 8192, gated: the pass also stores its gated input u * pregate here
+                                    // (contiguous (B, H, L) workspace)
 };
 
 // fused 8192-point kernel on (B, H, L) real sequences (seqlen <= 8192)
-static int launch_fused(const bffc_plan* p, const void* u, const void* kf, const void* pregate, const void* postgate,
-                        void* y, int B, int H, int L, cudaStream_t st,
-                        const PassOpts& po = PassOpts()) {
+static int launch_fused(const bffc_plan* p, Seq u, const void* kf, Seq pregate, Seq postgate, Seq y, int B, int H,
+                        int L, cudaStream_t st, const PassOpts& po = PassOpts()) {
   if (L % 64 != 0) return fail(BFFC_ERR_UNSUPPORTED, "L=%d must be a multiple of 64 for seqlen <= 8192 in this build", L);
   bffc::FwdParams prm = fwd_params(p, kf, po.conj);
   fill_seq_tiles(p, prm, B, H, L);
-  prm.pregate = static_cast<const uint32_t*>(pregate);
-  prm.postgate = static_cast<const uint32_t*>(postgate);
-  prm.postgate2 = static_cast<const uint32_t*>(po.postgate2);
-  prm.y2 = static_cast<uint32_t*>(po.y2);
-  prm.xg_out = pregate ? po.xg_out : nullptr;
+  prm.pregate = static_cast<const uint32_t*>(pregate.p);
+  prm.postgate = static_cast<const uint32_t*>(postgate.p);
+  prm.postgate2 = static_cast<const uint32_t*>(po.postgate2.p);
+  prm.y2 = static_cast<uint32_t*>(po.y2.p);
+  prm.xg_out = pregate.p ? po.xg_out : nullptr;
   prm.units = H * prm.pairs;
   const int seg_rows = p->rblk;
+  auto map = [&](CUtensorMap* m, Seq t) { return make_seq_map(p, m, t, B, H, L, seg_rows); };
   CUtensorMap tm_u, tm_y, tm_g;
-  if (int rc = make_map(p, &tm_u, u, B * H, L, seg_rows)) return rc;
-  if (int rc = make_map(p, &tm_y, y, B * H, L, seg_rows)) return rc;
-  if (int rc = make_map(p, &tm_g, pregate ? pregate : u, B * H, L, seg_rows)) return rc;
+  if (int rc = map(&tm_u, u)) return rc;
+  if (int rc = map(&tm_y, y)) return rc;
+  if (int rc = map(&tm_g, pregate.p ? pregate : u)) return rc;
   using namespace bffc::r128;
-  const bool gated = pregate || postgate || prm.y2;
+  const bool gated = pregate.p || postgate.p || prm.y2;
   // gate tiles travel by TMA like the inputs: pregate with the (segmented) geometry of u, output gates with that of y
   GateMaps gm{tm_g, tm_u, tm_u, tm_u, tm_u};
-  if (prm.xg_out) { if (int rc = make_map(p, &gm.xg, prm.xg_out, B * H, L, seg_rows)) return rc; }
-  if (postgate) { if (int rc = make_map(p, &gm.post, postgate, B * H, L, seg_rows)) return rc; }
+  if (prm.xg_out) { if (int rc = map(&gm.xg, seq(prm.xg_out, int64_t(H) * L))) return rc; }
+  if (postgate.p) { if (int rc = map(&gm.post, postgate)) return rc; }
   if (prm.y2) {
-    if (int rc = make_map(p, &gm.post2, prm.postgate2, B * H, L, seg_rows)) return rc;
-    if (int rc = make_map(p, &gm.y2, prm.y2, B * H, L, seg_rows)) return rc;
+    if (int rc = map(&gm.post2, po.postgate2)) return rc;
+    if (int rc = map(&gm.y2, po.y2)) return rc;
   }
   const int g3 = persistent_grid(p, prm.units, kPipes3);
   FMT_SWITCH(p->dtype,
@@ -845,22 +871,23 @@ static int cc_stage(const bffc_plan* p, int lev, bool inverse, bool gated, const
 }
 
 // tensor-core radix-128 level 0: real endpoint x (u or y), gate g (pregate fwd / postgate inv), planes set A
-static int tc_stage(const bffc_plan* p, bool inverse, const void* x, const void* gate, PlaneSet A, View v, int L,
-                    cudaStream_t st, const void* gate2 = nullptr, void* x2 = nullptr) {
+static int tc_stage(const bffc_plan* p, bool inverse, Seq x, Seq gate, PlaneSet A, View v, int L, cudaStream_t st,
+                    Seq gate2 = Seq(), Seq x2 = Seq()) {
   const int B = v.B, H = v.H;
   const int M = p->N / 128, chunks = M / 64, pairs = (B + 1) / 2;
   if (L % M != 0) return fail(BFFC_ERR_UNSUPPORTED, "seqlen %d needs L to be a multiple of %d in this build (L=%d)", p->N, M, L);
   CUtensorMap tm_x, tm_pr, tm_pi, tm_g;
-  if (int rc = make_map4(p, &tm_x, x, chunks, L / M, B * v.Hs, size_t(M) * 2, size_t(L) * 2)) return rc;
+  if (int rc = make_endpoint_map(p, &tm_x, x, chunks, M, L, v.Hs, B)) return rc;
   if (int rc = make_map4(p, &tm_pr, A.re, chunks, 128, pairs * H, size_t(M) * 2, size_t(p->N) * 2)) return rc;
   if (int rc = make_map4(p, &tm_pi, A.im, chunks, 128, pairs * H, size_t(M) * 2, size_t(p->N) * 2)) return rc;
-  if (int rc = make_map4(p, &tm_g, (!inverse && gate) ? gate : x, chunks, L / M, B * v.Hs, size_t(M) * 2, size_t(L) * 2)) return rc;
+  if (int rc = make_endpoint_map(p, &tm_g, (!inverse && gate.p) ? gate : x, chunks, M, L, v.Hs, B)) return rc;
   bffc::OuterTcParams prm;
   prm.dftC = p->dftC; prm.dftS = p->dftS;
-  prm.postgate = inverse ? static_cast<const uint32_t*>(gate) : nullptr;
-  prm.postgate2 = inverse ? static_cast<const uint32_t*>(gate2) : nullptr;
-  prm.y2 = inverse ? static_cast<uint32_t*>(x2) : nullptr;
-  prm.has_pregate = (!inverse && gate) ? 1 : 0;
+  prm.postgate = inverse ? static_cast<const uint32_t*>(gate.p) : nullptr;
+  prm.postgate2 = inverse ? static_cast<const uint32_t*>(gate2.p) : nullptr;
+  prm.y2 = inverse ? static_cast<uint32_t*>(x2.p) : nullptr;
+  prm.postgate_bs = gate.bs; prm.postgate2_bs = gate2.bs; prm.y2_bs = x2.bs;
+  prm.has_pregate = (!inverse && gate.p) ? 1 : 0;
   prm.tw_scale = p->lev[0].scale;
   prm.B = B; prm.H = H; prm.L = L; prm.pairs = pairs;
   prm.Hs = v.Hs; prm.h0 = v.h0;
@@ -885,15 +912,16 @@ static PlaneSet plane_set(const bffc_plan* p, void* ws, int idx, int B, int H) {
 
 // all outer levels, forward: real (B,H,L) x (* pregate) -> complex 8192-point rows.  Level 0 writes set `s0`,
 // level 1 (if any) reads `s0` and writes `s1`; returns the set holding the rows.
-static int transform_fwd(const bffc_plan* p, const void* x, const void* pregate, View v, int L, PlaneSet s0,
-                         PlaneSet s1, PlaneSet* out, cudaStream_t st) {
+static int transform_fwd(const bffc_plan* p, Seq x, Seq pregate, View v, int L, PlaneSet s0, PlaneSet s1,
+                         PlaneSet* out, cudaStream_t st) {
   if (p->lev[0].tc) {
     if (int rc = tc_stage(p, false, x, pregate, s0, v, L, st)) return rc;
   } else {
     bffc::outer::OuterParams op = outer_params(p, 0, v, L, s0, s1);
-    op.u = static_cast<const uint4*>(x);
-    op.pregate = static_cast<const uint4*>(pregate);
-    if (int rc = cc_stage(p, 0, false, pregate != nullptr, op, st)) return rc;
+    op.u = static_cast<const uint4*>(x.p);
+    op.pregate = static_cast<const uint4*>(pregate.p);
+    op.u_bs = x.bs / 8; op.pregate_bs = pregate.bs / 8;
+    if (int rc = cc_stage(p, 0, false, pregate.p != nullptr, op, st)) return rc;
   }
   *out = s0;
   if (p->nlev == 2) {
@@ -904,33 +932,33 @@ static int transform_fwd(const bffc_plan* p, const void* x, const void* pregate,
 }
 
 // all outer levels, inverse: rows in `rows` (set s1 if two levels, else s0) -> real y (* postgate)
-static int transform_inv(const bffc_plan* p, void* y, const void* postgate, View v, int L, PlaneSet s0, PlaneSet s1,
-                         cudaStream_t st, const void* postgate2 = nullptr, void* y2 = nullptr) {
+static int transform_inv(const bffc_plan* p, Seq y, Seq postgate, View v, int L, PlaneSet s0, PlaneSet s1,
+                         cudaStream_t st, Seq postgate2 = Seq(), Seq y2 = Seq()) {
   if (p->nlev == 2) {
     if (int rc = cc_stage(p, 1, true, false, outer_params(p, 1, v, L, s0, s1), st)) return rc;
   }
   if (p->lev[0].tc) return tc_stage(p, true, y, postgate, s0, v, L, st, postgate2, y2);
   bffc::outer::OuterParams op = outer_params(p, 0, v, L, s0, s1);
-  op.y = static_cast<uint4*>(y);
-  op.postgate = static_cast<const uint4*>(postgate);
-  op.postgate2 = static_cast<const uint4*>(postgate2);
-  op.y2 = static_cast<uint4*>(y2);
-  return cc_stage(p, 0, true, postgate != nullptr, op, st);
+  op.y = static_cast<uint4*>(y.p);
+  op.postgate = static_cast<const uint4*>(postgate.p);
+  op.postgate2 = static_cast<const uint4*>(postgate2.p);
+  op.y2 = static_cast<uint4*>(y2.p);
+  op.y_bs = y.bs / 8; op.postgate_bs = postgate.bs / 8; op.postgate2_bs = postgate2.bs / 8; op.y2_bs = y2.bs / 8;
+  return cc_stage(p, 0, true, postgate.p != nullptr, op, st);
 }
 
 // A composite-size call chunk by chunk (see chunk_view; `sets` plane sets per chunk): f(v, at, set) for each chunk.
-// v is the chunk's View, at(t) the chunk's first batch member in a (B, H, L) tensor t, input or output (null stays
-// null), and set(i) plane set i of the workspace, sized for a full chunk.
+// v is the chunk's View, at(t) tensor t (input or output, each with its own batch stride; null stays null) from the
+// chunk's first batch member on, and set(i) plane set i of the workspace, sized for a full chunk.
 template <class Fn>
 static int for_each_chunk(const bffc_plan* p, int B, int H, int L, void* ws, int sets, Fn&& f) {
   const View c = chunk_view(p, B, H, sets);
-  const size_t bstride = size_t(H) * L * 2;                       // bytes of one batch member of the (B, H, L) tensors
   auto set = [&](int i) { return plane_set(p, ws, i, c.B, c.H); };
   for (int b0 = 0; b0 < B; b0 += c.B)
     for (int h0 = 0; h0 < H; h0 += c.H) {
       const View v{B - b0 < c.B ? B - b0 : c.B, H - h0 < c.H ? H - h0 : c.H, H, h0};
-      auto at = [&](const void* t) -> void* {
-        return t ? static_cast<uint8_t*>(const_cast<void*>(t)) + size_t(b0) * bstride : nullptr;
+      auto at = [&](Seq t) -> Seq {
+        return t.p ? Seq{static_cast<uint8_t*>(t.p) + size_t(b0) * size_t(t.bs) * 2, t.bs} : Seq();
       };
       if (int rc = f(v, at, set)) return rc;
     }
@@ -949,9 +977,18 @@ static int check_common(const bffc_plan* p, int B, int H, int L, const void* a, 
   return 0;
 }
 
+// batch stride of every given (non-null) tensor: a multiple of 8 elements (16-byte aligned members) and >= H * L
+static int check_strides(const char* fn, int H, int L, std::initializer_list<Seq> ts) {
+  for (const Seq& t : ts)
+    if (t.p && (t.bs % 8 != 0 || t.bs < int64_t(H) * L))
+      return fail(BFFC_ERR_INVALID, "%s: batch stride %lld must be a multiple of 8 and >= H*L = %lld", fn,
+                  (long long)t.bs, (long long)H * L);
+  return 0;
+}
+
 // y = postgate * conv(u * pregate, k) for any supported size.  `ws`: workspace (plane sets 0 and 1) for composite sizes.
-static int conv_forward(const bffc_plan* p, const void* u, const void* kf, const void* pregate, const void* postgate,
-                        void* y, int B, int H, int L, void* ws, cudaStream_t st, const PassOpts& po = PassOpts()) {
+static int conv_forward(const bffc_plan* p, Seq u, const void* kf, Seq pregate, Seq postgate, Seq y, int B, int H, int L,
+                        void* ws, cudaStream_t st, const PassOpts& po = PassOpts()) {
   if (p->nlev == 0) return launch_fused(p, u, kf, pregate, postgate, y, B, H, L, st, po);
   // composite sizes: outer stage(s) -> inner kernel in place -> inverse outer stage(s)
   return for_each_chunk(p, B, H, L, ws, p->nlev, [&](const View& v, auto at, auto set) {
@@ -966,16 +1003,19 @@ static int conv_forward(const bffc_plan* p, const void* u, const void* kf, const
 
 extern "C" {
 
-int bffc_fwd(const bffc_plan* p, const void* u, const void* kf, const void* pregate, const void* postgate, void* y,
-             int B, int H, int L, void* workspace, size_t workspace_bytes, void* stream) {
-  if ((pregate == nullptr) != (postgate == nullptr))
+int bffc_fwd_strided(const bffc_plan* p, const void* u_, int64_t u_bs, const void* kf, const void* pregate_,
+                     int64_t pregate_bs, const void* postgate_, int64_t postgate_bs, void* y_, int64_t y_bs, int B, int H,
+                     int L, void* workspace, size_t workspace_bytes, void* stream) {
+  if ((pregate_ == nullptr) != (postgate_ == nullptr))
     return fail(BFFC_ERR_INVALID, "bffc_fwd: pregate and postgate must both be given or both be null");
-  if (!u || !kf || !y) return fail(BFFC_ERR_INVALID, "bffc_fwd: null pointer");
-  if (int rc = check_common(p, B, H, L, u, y, kf)) return rc;
-  if (!aligned16(pregate, postgate, workspace))
+  if (!u_ || !kf || !y_) return fail(BFFC_ERR_INVALID, "bffc_fwd: null pointer");
+  if (int rc = check_common(p, B, H, L, u_, y_, kf)) return rc;
+  if (!aligned16(pregate_, postgate_, workspace))
     return fail(BFFC_ERR_INVALID, "bffc_fwd: gates / workspace must be 16-byte aligned");
+  const Seq u = seq(u_, u_bs), pregate = seq(pregate_, pregate_bs), postgate = seq(postgate_, postgate_bs), y = seq(y_, y_bs);
+  if (int rc = check_strides("bffc_fwd", H, L, {u, pregate, postgate, y})) return rc;
   {
-    const size_t need = bffc_workspace_bytes_ex(p, B, H, L, pregate != nullptr, 0);
+    const size_t need = bffc_workspace_bytes_ex(p, B, H, L, pregate.p != nullptr, 0);
     if (need && (!workspace || workspace_bytes < need))
       return fail(BFFC_ERR_INVALID, "bffc_fwd: workspace of %zu bytes required", need);
   }
@@ -983,19 +1023,32 @@ int bffc_fwd(const bffc_plan* p, const void* u, const void* kf, const void* preg
   return conv_forward(p, u, kf, pregate, postgate, y, B, H, L, workspace, static_cast<cudaStream_t>(stream));
 }
 
-int bffc_bwd(const bffc_plan* p, const void* dout, const void* u, const void* kf, const void* kf_conj,
-             const void* pregate, const void* postgate, void* du, void* dkf, void* dpregate, void* dpostgate, int B, int H,
-             int L, void* workspace, size_t workspace_bytes, void* stream) {
-  if ((pregate == nullptr) != (postgate == nullptr))
+int bffc_fwd(const bffc_plan* p, const void* u, const void* kf, const void* pregate, const void* postgate, void* y,
+             int B, int H, int L, void* workspace, size_t workspace_bytes, void* stream) {
+  const int64_t s = int64_t(H) * L;
+  return bffc_fwd_strided(p, u, s, kf, pregate, s, postgate, s, y, s, B, H, L, workspace, workspace_bytes, stream);
+}
+
+int bffc_bwd_strided(const bffc_plan* p, const void* dout_, int64_t dout_bs, const void* u_, int64_t u_bs, const void* kf,
+                     const void* kf_conj, const void* pregate_, int64_t pregate_bs, const void* postgate_,
+                     int64_t postgate_bs, void* du_, int64_t du_bs, void* dkf, void* dpregate_, int64_t dpregate_bs,
+                     void* dpostgate_, int64_t dpostgate_bs, int B, int H, int L, void* workspace, size_t workspace_bytes,
+                     void* stream) {
+  if ((pregate_ == nullptr) != (postgate_ == nullptr))
     return fail(BFFC_ERR_INVALID, "bffc_bwd: pregate and postgate must both be given or both be null");
-  const bool gated = pregate != nullptr;
-  if (!dout || !u || (!kf && !kf_conj) || !du || !dkf) return fail(BFFC_ERR_INVALID, "bffc_bwd: null pointer");
-  if (gated && (!kf || !dpregate || !dpostgate)) return fail(BFFC_ERR_INVALID, "bffc_bwd: gated backward needs kf, dpregate, dpostgate");
-  if (!aligned16(pregate, postgate, dpregate, dpostgate, kf))
+  const bool gated = pregate_ != nullptr;
+  if (!dout_ || !u_ || (!kf && !kf_conj) || !du_ || !dkf) return fail(BFFC_ERR_INVALID, "bffc_bwd: null pointer");
+  if (gated && (!kf || !dpregate_ || !dpostgate_)) return fail(BFFC_ERR_INVALID, "bffc_bwd: gated backward needs kf, dpregate, dpostgate");
+  if (!aligned16(pregate_, postgate_, dpregate_, dpostgate_, kf))
     return fail(BFFC_ERR_INVALID, "bffc_bwd: gate pointers must be 16-byte aligned");
-  if (int rc = check_common(p, B, H, L, u, du, dout)) return rc;
+  if (int rc = check_common(p, B, H, L, u_, du_, dout_)) return rc;
   if (!aligned16(dkf, kf_conj, workspace))
     return fail(BFFC_ERR_INVALID, "bffc_bwd: dkf / kf / workspace must be 16-byte aligned");
+  // an ungated call has no gate gradients: whatever it passes there is ignored
+  const Seq dout = seq(dout_, dout_bs), u = seq(u_, u_bs), pregate = seq(pregate_, pregate_bs);
+  const Seq postgate = seq(postgate_, postgate_bs), du = seq(du_, du_bs);
+  const Seq dpregate = gated ? seq(dpregate_, dpregate_bs) : Seq(), dpostgate = gated ? seq(dpostgate_, dpostgate_bs) : Seq();
+  if (int rc = check_strides("bffc_bwd", H, L, {dout, u, pregate, postgate, du, dpregate, dpostgate})) return rc;
   {
     const size_t need = bffc_workspace_bytes_ex(p, B, H, L, gated, 1);
     if (need && (!workspace || workspace_bytes < need))
@@ -1013,7 +1066,7 @@ int bffc_bwd(const bffc_plan* p, const void* dout, const void* u, const void* kf
   if (p->nlev > 0) {
     // composite sizes: all passes share the transformed rows, chunk by chunk, below
   } else if (!gated) {
-    if (int rc = conv_forward(p, dout, kfc, nullptr, nullptr, du, B, H, L, workspace, st, dx)) return rc;
+    if (int rc = conv_forward(p, dout, kfc, Seq(), Seq(), du, B, H, L, workspace, st, dx)) return rc;
   } else {
     // y = q * conv(u*p, k)  (conv.py:3856-3939; kernels_bf16/..._bwd_kernel_bf16.h:836-906; host recompute
     // monarch_cuda_interface_bwd_bf16.cu:798-808).  With dx = corr(dout*q, k):
@@ -1039,10 +1092,11 @@ int bffc_bwd(const bffc_plan* p, const void* dout, const void* u, const void* kf
   if (p->nlev == 0) {
     if (L % 64 != 0) return fail(BFFC_ERR_UNSUPPORTED, "L=%d must be a multiple of 64 for seqlen <= 8192 in this build", L);
     // gated loads (reference: ..._bwd_kernel_bf16.h:505-509,571-581): the products stored by the two passes above
-    const void *xu = gated ? gate_x : u, *xd = gated ? gate_d : dout;
+    // (contiguous workspace), else u and dout themselves
+    const Seq xu = gated ? seq(gate_x, int64_t(H) * L) : u, xd = gated ? seq(gate_d, int64_t(H) * L) : dout;
     CUtensorMap tm_u, tm_d;
-    if (int rc = make_map(p, &tm_u, xu, B * H, L, p->rblk)) return rc;
-    if (int rc = make_map(p, &tm_d, xd, B * H, L, p->rblk)) return rc;
+    if (int rc = make_seq_map(p, &tm_u, xu, B, H, L, p->rblk)) return rc;
+    if (int rc = make_seq_map(p, &tm_d, xd, B, H, L, p->rblk)) return rc;
     fill_seq_tiles(p, prm, B, H, L);
     return launch_dkf(p, false, tm_u, tm_d, tm_u, tm_d, prm, st);
   }
@@ -1074,8 +1128,16 @@ int bffc_bwd(const bffc_plan* p, const void* dout, const void* u, const void* kf
     }
     if (int rc = launch_planes(p, rd.re, rd.im, static_cast<const uint8_t*>(kfc) + kf_off, vpairs, rows, st, dx.conj)) return rc;
     return transform_inv(p, at(du), at(pregate), v, L, p->nlev == 2 ? s0 : sD, sD, st,
-                         gated ? at(u) : nullptr, gated ? at(dpregate) : nullptr);
+                         gated ? at(u) : Seq(), gated ? at(dpregate) : Seq());
   });
+}
+
+int bffc_bwd(const bffc_plan* p, const void* dout, const void* u, const void* kf, const void* kf_conj,
+             const void* pregate, const void* postgate, void* du, void* dkf, void* dpregate, void* dpostgate, int B, int H,
+             int L, void* workspace, size_t workspace_bytes, void* stream) {
+  const int64_t s = int64_t(H) * L;
+  return bffc_bwd_strided(p, dout, s, u, s, kf, kf_conj, pregate, s, postgate, s, du, s, dkf, dpregate, s, dpostgate, s,
+                          B, H, L, workspace, workspace_bytes, stream);
 }
 
 // ---------------------------------------------------------------------------------------------- host streaming
@@ -1156,8 +1218,9 @@ int bffc_fwd_host(const bffc_plan* p, const void* u_host, const void* kf, const 
         CUDA_TRY(cudaEventRecord(ev_in[slot], s_in));
         CUDA_TRY(cudaStreamWaitEvent(s_cmp, ev_in[slot], 0));
         if (c >= 2) CUDA_TRY(cudaStreamWaitEvent(s_cmp, ev_out[slot], 0));
-        if (int rc = conv_forward(p, d_u, static_cast<const uint8_t*>(kf) + size_t(h0) * kf_row, d_p, d_q, d_y, nb, nh, L,
-                                  conv_ws ? d_ws : nullptr, s_cmp)) return rc;
+        const int64_t cs = int64_t(nh) * L;                          // the device chunk is a contiguous (nb, nh, L)
+        if (int rc = conv_forward(p, seq(d_u, cs), static_cast<const uint8_t*>(kf) + size_t(h0) * kf_row, seq(d_p, cs),
+                                  seq(d_q, cs), seq(d_y, cs), nb, nh, L, conv_ws ? d_ws : nullptr, s_cmp)) return rc;
         CUDA_TRY(cudaEventRecord(ev_cmp[slot], s_cmp));
         CUDA_TRY(cudaStreamWaitEvent(s_out, ev_cmp[slot], 0));
         CUDA_TRY(cudaMemcpy2DAsync(static_cast<uint8_t*>(y_host) + off, host_pitch, d_y, width, width, nb, cudaMemcpyDeviceToHost, s_out));

@@ -90,8 +90,8 @@ dkf3_kernel(const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CU
       tma_load_3d(dst, tm, bar, 0, 0, pr * p.H + h);
       tma_load_3d(dst + kTileBytes, which ? &tm_di : &tm_ui, bar, 0, 0, pr * p.H + h);
     } else {
-      load_tile(dst, tm, bar, p.B, p.H, h, pr, 0, p.nseg, p.seg_bytes);              // members beyond the batch: zeros
-      load_tile(dst + kTileBytes, tm, bar, p.B, p.H, h, pr, 1, p.nseg, p.seg_bytes);
+      load_tile<true>(dst, tm, bar, h, pr, 0, p.nseg, p.seg_bytes);              // members beyond the batch: zeros
+      load_tile<true>(dst + kTileBytes, tm, bar, h, pr, 1, p.nseg, p.seg_bytes);
     }
   };
   // everything stage 1 needs from global memory is requested up front

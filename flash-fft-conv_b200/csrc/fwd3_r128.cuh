@@ -94,11 +94,11 @@ fwd3_kernel(const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CU
     if (kGated) {                        // input tiles -> slot 0, pregate tiles -> slot 1, one barrier
       const int uh = unit / p.pairs, ug = unit - uh * p.pairs;
       mbar_expect_tx(bar_tma0, has_pre ? 2 * kSlotBytes : kSlotBytes);
-      load_tile(s_slot0, &tm_u, bar_tma0, p.B, p.H, uh, ug, 0, p.nseg, p.seg_bytes);
-      load_tile(s_slot0 + kTileBytes, &tm_u, bar_tma0, p.B, p.H, uh, ug, 1, p.nseg, p.seg_bytes);
+      load_tile(s_slot0, &tm_u, bar_tma0, uh, ug, 0, p.nseg, p.seg_bytes);
+      load_tile(s_slot0 + kTileBytes, &tm_u, bar_tma0, uh, ug, 1, p.nseg, p.seg_bytes);
       if (has_pre) {
-        load_tile(s_slot0 + kSlotBytes, &gm.pre, bar_tma0, p.B, p.H, uh, ug, 0, p.nseg, p.seg_bytes);
-        load_tile(s_slot0 + kSlotBytes + kTileBytes, &gm.pre, bar_tma0, p.B, p.H, uh, ug, 1, p.nseg, p.seg_bytes);
+        load_tile(s_slot0 + kSlotBytes, &gm.pre, bar_tma0, uh, ug, 0, p.nseg, p.seg_bytes);
+        load_tile(s_slot0 + kSlotBytes + kTileBytes, &gm.pre, bar_tma0, uh, ug, 1, p.nseg, p.seg_bytes);
       }
       return;
     }
@@ -108,8 +108,8 @@ fwd3_kernel(const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CU
       tma_load_3d(dst + kTileBytes, &tm_g, bar, 0, 0, seq_index(unit));
     } else {
       const int uh = unit / p.pairs, ug = unit - uh * p.pairs;
-      load_tile(dst, &tm_u, bar, p.B, p.H, uh, ug, 0, p.nseg, p.seg_bytes);
-      load_tile(dst + kTileBytes, &tm_u, bar, p.B, p.H, uh, ug, 1, p.nseg, p.seg_bytes);
+      load_tile(dst, &tm_u, bar, uh, ug, 0, p.nseg, p.seg_bytes);
+      load_tile(dst + kTileBytes, &tm_u, bar, uh, ug, 1, p.nseg, p.seg_bytes);
     }
   };
   // Everything the first stage needs from global memory is requested up front and lands while the tables below are
@@ -141,7 +141,7 @@ fwd3_kernel(const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CU
     for (int w = 0; w < 2; ++w)
       for (int sg = 0; sg < p.nseg; ++sg) {
         const int b = (ug * p.nseg + sg) * 2 + w;
-        if (b < p.B) tma_store_3d(my, sT + w * kTileBytes + sg * p.seg_bytes, 0, 0, b * p.H + uh);
+        if (b < p.B) tma_store_4d(my, sT + w * kTileBytes + sg * p.seg_bytes, 0, 0, uh, b);
       }
     tma_store_commit();
   };
@@ -173,8 +173,8 @@ fwd3_kernel(const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CU
         if (has_post) {
           const int ug = unit - h * p.pairs;
           mbar_expect_tx(bar_gate, kSlotBytes);
-          load_tile(sGate, &gm.post, bar_gate, p.B, p.H, h, ug, 0, p.nseg, p.seg_bytes);
-          load_tile(sGate + kTileBytes, &gm.post, bar_gate, p.B, p.H, h, ug, 1, p.nseg, p.seg_bytes);
+          load_tile(sGate, &gm.post, bar_gate, h, ug, 0, p.nseg, p.seg_bytes);
+          load_tile(sGate + kTileBytes, &gm.post, bar_gate, h, ug, 1, p.nseg, p.seg_bytes);
         }
       }
     }
@@ -272,8 +272,8 @@ fwd3_kernel(const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CU
       if (has_post2) {                    // slot 1 has been read by every thread (barrier above): second gate -> slot 1
         const int ug = unit - h * p.pairs;
         mbar_expect_tx(bar_gate, kSlotBytes);
-        load_tile(sGate, &gm.post2, bar_gate, p.B, p.H, h, ug, 0, p.nseg, p.seg_bytes);
-        load_tile(sGate + kTileBytes, &gm.post2, bar_gate, p.B, p.H, h, ug, 1, p.nseg, p.seg_bytes);
+        load_tile(sGate, &gm.post2, bar_gate, h, ug, 0, p.nseg, p.seg_bytes);
+        load_tile(sGate + kTileBytes, &gm.post2, bar_gate, h, ug, 1, p.nseg, p.seg_bytes);
         tma_store_wait_read0();           // the first output has left slot 0
       }
     }

@@ -24,6 +24,8 @@ DEVINL uint4 hmul8(const uint4& a, const uint4& b) {
   return make_uint4(NT::hmul2(a.x, b.x), NT::hmul2(a.y, b.y), NT::hmul2(a.z, b.z), NT::hmul2(a.w, b.w));
 }
 
+// The real endpoints are (B, Hs, L) tensors with contiguous rows and a batch stride of their own (`*_bs`, counted in
+// 16-byte vectors): element (b, h, l) of u is u[b * u_bs + h * L/8 + l/8].
 struct OuterParams {
   const uint4* u;        // (B, H, L) bf16                                  (real endpoint, level 0)
   const uint4* pregate;  // optional
@@ -31,6 +33,7 @@ struct OuterParams {
   uint4* y;              // (B, H, L) bf16 (inverse only)
   const uint4* postgate2; // optional second gated output of the inverse: y2 = postgate2 * z' (gated backward: du, dpregate)
   uint4* y2;
+  long long u_bs, pregate_bs, postgate_bs, y_bs, postgate2_bs, y2_bs;   // batch strides of the pointers above
   uint4* xre;            // kPlanes: outer-side complex rows (rows x R*M), read by fwd / written by inv
   uint4* xim;
   uint4* pre;            // inner-side planes: real parts,  rows*R rows of M bf16 each
@@ -99,7 +102,7 @@ DEVINL void readahead_level0(const OuterParams& p, bool planes_in) {
   if (id >= total) return;
   const int bx = int(id % gx), h = int((id / gx) % gy), pr = int(id / (gx * (unsigned long long)gy));
   const int np = (bx * blockDim.x + threadIdx.x) * kVec;
-  const size_t L8 = size_t(p.L) / kVec;
+  const size_t c8 = size_t(p.h0 + h) * (p.L / kVec);            // channel offset inside a batch member
   const int b0 = 2 * pr, b1 = 2 * pr + 1;
   if (planes_in) {      // inverse: R rows of both planes
 #pragma unroll
@@ -113,15 +116,16 @@ DEVINL void readahead_level0(const OuterParams& p, bool planes_in) {
   for (int a = 0; a < R; ++a) {
     const int n = a * p.M + np;
     if (n >= p.L) break;
-    const size_t o0 = (size_t(b0) * p.Hs + p.h0 + h) * L8 + n / kVec, o1 = (size_t(b1) * p.Hs + p.h0 + h) * L8 + n / kVec;
+    const size_t o = c8 + n / kVec;
     if (!planes_in) {
-      prefetch_l2(p.u + o0);
-      if (b1 < p.B) prefetch_l2(p.u + o1);
+      prefetch_l2(p.u + b0 * p.u_bs + o);
+      if (b1 < p.B) prefetch_l2(p.u + b1 * p.u_bs + o);
     }
     if (kGated) {
       const uint4* g = planes_in ? p.postgate : p.pregate;
-      prefetch_l2(g + o0);
-      if (b1 < p.B) prefetch_l2(g + o1);
+      const long long gbs = planes_in ? p.postgate_bs : p.pregate_bs;
+      prefetch_l2(g + b0 * gbs + o);
+      if (b1 < p.B) prefetch_l2(g + b1 * gbs + o);
     }
   }
 }
@@ -152,7 +156,7 @@ __global__ void __launch_bounds__(128, (R <= 4) ? 4 : 2) fwd_kernel(const OuterP
   const int np = ((kPlanes ? blockIdx.y : blockIdx.x) * blockDim.x + threadIdx.x) * kVec;   // n'
   const int h = blockIdx.y, pr = blockIdx.z;
   const int b0 = 2 * pr, b1 = 2 * pr + 1;
-  const size_t L8 = size_t(p.L) / kVec;
+  const size_t c8 = size_t(p.h0 + h) * (p.L / kVec);            // channel offset inside a batch member
   if (kPlanes) readahead_planes<R>(p, false); else readahead_level0<R, kGated>(p, false);
   f32x2 zr[R][4], zi[R][4];
   int rows = 0;
@@ -166,14 +170,13 @@ __global__ void __launch_bounds__(128, (R <= 4) ? 4 : 2) fwd_kernel(const OuterP
       unpack8v<kFmt>(__ldg(p.xim + o), zi[a]);
     } else if (n < p.L) {
       rows = a + 1;
-      const size_t o0 = (size_t(b0) * p.Hs + p.h0 + h) * L8 + n / kVec;
-      uint4 v0 = __ldg(p.u + o0);
-      if (kGated) v0 = hmul8<kFmt>(v0, __ldg(p.pregate + o0));
+      const size_t o = c8 + n / kVec;
+      uint4 v0 = __ldg(p.u + b0 * p.u_bs + o);
+      if (kGated) v0 = hmul8<kFmt>(v0, __ldg(p.pregate + b0 * p.pregate_bs + o));
       unpack8v<kFmt>(v0, zr[a]);
       if (b1 < p.B) {
-        const size_t o1 = (size_t(b1) * p.Hs + p.h0 + h) * L8 + n / kVec;
-        uint4 v1 = __ldg(p.u + o1);
-        if (kGated) v1 = hmul8<kFmt>(v1, __ldg(p.pregate + o1));
+        uint4 v1 = __ldg(p.u + b1 * p.u_bs + o);
+        if (kGated) v1 = hmul8<kFmt>(v1, __ldg(p.pregate + b1 * p.pregate_bs + o));
         unpack8v<kFmt>(v1, zi[a]);
       } else {
 #pragma unroll
@@ -224,8 +227,25 @@ __global__ void __launch_bounds__(128, (R <= 4) ? 4 : 2) inv_kernel(const OuterP
   const int np = ((kPlanes ? blockIdx.y : blockIdx.x) * blockDim.x + threadIdx.x) * kVec;
   const int h = blockIdx.y, pr = blockIdx.z;
   const int b0 = 2 * pr, b1 = 2 * pr + 1;
-  const size_t L8 = size_t(p.L) / kVec;
+  const size_t c8 = size_t(p.h0 + h) * (p.L / kVec);            // channel offset inside a batch member
   if (kPlanes) readahead_planes<R>(p, true); else readahead_level0<R, kGated>(p, true);
+  // Level 0: this channel's rows in the endpoint tensors.  Ungated: the row of member b0 in y (b1: one batch stride
+  // further).  Gated: the rows of y, postgate, y2, postgate2 in members b0 (0..3) and b1 (4..7) go to a block-wide table
+  // in shared memory and are re-read at each store; held in registers across the transform they would cost the kernel
+  // registers (and at R = 4 a resident block per SM).
+  uint4* y0 = nullptr;
+  __shared__ uint4* volatile rows[8];
+  if (!kPlanes && !kGated) y0 = p.y + b0 * p.y_bs + c8;
+  if (!kPlanes && kGated) {
+    if (threadIdx.x < 8) {
+      const int t = threadIdx.x & 3;
+      const long long m = b0 + (threadIdx.x >> 2);
+      uint4* base = t == 0 ? p.y : t == 1 ? const_cast<uint4*>(p.postgate) : t == 2 ? p.y2 : const_cast<uint4*>(p.postgate2);
+      const long long bs = t == 0 ? p.y_bs : t == 1 ? p.postgate_bs : t == 2 ? p.y2_bs : p.postgate2_bs;
+      rows[threadIdx.x] = base ? base + m * bs + c8 : nullptr;
+    }
+    __syncthreads();
+  }
   f32x2 w1c[4], w1s[4];                      // conj twiddle: exp(+2 pi i (n'+t) / N)
   float2 stepc[8];
 #pragma unroll
@@ -269,17 +289,19 @@ __global__ void __launch_bounds__(128, (R <= 4) ? 4 : 2) inv_kernel(const OuterP
         p.xim[o] = pack8v<kFmt>(yi);
         continue;
       }
-      const size_t o0 = (size_t(b0) * p.Hs + p.h0 + h) * L8 + n / kVec;
+      const int o = n / kVec;
       uint4 v0 = pack8v<kFmt>(yr);
-      if (kGated && p.y2) p.y2[o0] = hmul8<kFmt>(v0, __ldg(p.postgate2 + o0));
-      if (kGated) v0 = hmul8<kFmt>(v0, __ldg(p.postgate + o0));
-      p.y[o0] = v0;
+      if (!kGated) {
+        y0[o] = v0;
+        if (b1 < p.B) y0[p.y_bs + o] = pack8v<kFmt>(yi);
+        continue;
+      }
+      if (p.y2) rows[2][o] = hmul8<kFmt>(v0, __ldg(rows[3] + o));
+      rows[0][o] = hmul8<kFmt>(v0, __ldg(rows[1] + o));
       if (b1 < p.B) {
-        const size_t o1 = (size_t(b1) * p.Hs + p.h0 + h) * L8 + n / kVec;
-        uint4 v1 = pack8v<kFmt>(yi);
-        if (kGated && p.y2) p.y2[o1] = hmul8<kFmt>(v1, __ldg(p.postgate2 + o1));
-        if (kGated) v1 = hmul8<kFmt>(v1, __ldg(p.postgate + o1));
-        p.y[o1] = v1;
+        const uint4 v1 = pack8v<kFmt>(yi);
+        if (p.y2) rows[6][o] = hmul8<kFmt>(v1, __ldg(rows[7] + o));
+        rows[4][o] = hmul8<kFmt>(v1, __ldg(rows[5] + o));
       }
     }
   }

@@ -10,7 +10,7 @@
 //   inv_tc : z'[i, j] = sum_k0 conj F128[i,k0] * ( conj W_N^{k0 j} * T[k0, j] )
 //
 // Machine mapping: the unit is one 64-column chunk of one sequence pair: a (128 x 64) tile per member, TMA
-// loaded with a 4-D map (col, chunk, row, sequence); DFT-128 cos / sin planes resident in shared memory as the A
+// loaded with a 5-D map (col, chunk, row, channel, batch member: any batch stride); DFT-128 cos / sin planes resident in shared memory as the A
 // operand (exactly stage 1 / stage 4 of r128_common.cuh); the twiddle is applied by the CUDA cores on the accumulator
 // (forward) or on the tile in shared memory before the MMA (inverse).  Two pipelines x two warpgroups (row halves)
 // per CTA.
@@ -25,6 +25,7 @@ struct OuterTcParams {
   const uint32_t* postgate;   // inverse only, (B,H,L) bf16 or null
   const uint32_t* postgate2;  // inverse only: optional second gated output y2 = postgate2 * z' (gated backward)
   uint32_t* y2;
+  long long postgate_bs, postgate2_bs, y2_bs;   // batch strides (elements) of the three pointers above
   int has_pregate;            // forward only: tm_g is the pregate map
   float tw_scale;             // folded into the twiddle table (fp16: 1/sqrt(128))
   int B, H, L, pairs;         // this launch: batch members [0, B), channels [h0, h0 + H) of tensors with Hs channels
@@ -46,10 +47,10 @@ static_assert(kSmemOuter <= 227 * 1024, "shared memory per block");
 
 template <bool kInverse, int kFmt = 1>
 __global__ void __launch_bounds__(kThreadsOuter, 1)
-outer_tc_kernel(const __grid_constant__ CUtensorMap tm_x,    // real endpoint: u (fwd) / y (inv), 4-D
+outer_tc_kernel(const __grid_constant__ CUtensorMap tm_x,    // real endpoint: u (fwd) / y (inv), 5-D
                 const __grid_constant__ CUtensorMap tm_pr,   // planes, real part, 4-D
                 const __grid_constant__ CUtensorMap tm_pi,   // planes, imaginary part
-                const __grid_constant__ CUtensorMap tm_g,    // pregate (fwd, optional)
+                const __grid_constant__ CUtensorMap tm_g,    // pregate (fwd, optional), 5-D
                 const OuterTcParams p) {
   using NT = Num<kFmt>;
   extern __shared__ uint8_t smem_raw[];
@@ -107,7 +108,6 @@ outer_tc_kernel(const __grid_constant__ CUtensorMap tm_x,    // real endpoint: u
 
   const uint32_t s_slot0 = sbase + pipe * kOuterSlots * kSlotBytes;
   const uint32_t bar_id = 1 + pipe;
-  const int BH = p.B * p.Hs;      // out-of-bounds sequence index of the 4-D maps (zero fill / dropped)
   const bool gated_in = (!kInverse) && p.has_pregate;
   const int nslots = gated_in ? 1 : kOuterSlots;
   const uint32_t s_gate0 = s_slot0 + kSlotBytes;     // gated: the second slot holds the pregate tiles
@@ -127,13 +127,13 @@ outer_tc_kernel(const __grid_constant__ CUtensorMap tm_x,    // real endpoint: u
     const uint32_t dst = s_slot0 + slot * kSlotBytes;
     mbar_expect_tx(bar, gated_in ? 2 * kSlotBytes : kSlotBytes);
     if (!kInverse) {
-      const int b0 = 2 * x.pr, b1 = 2 * x.pr + 1;
-      const int s0 = b0 * p.Hs + p.h0 + x.h, s1 = b1 < p.B ? b1 * p.Hs + p.h0 + x.h : BH;    // BH: out of bounds -> zeros
-      tma_load_4d(dst, &tm_x, bar, 0, x.cj, 0, s0);
-      tma_load_4d(dst + kTileBytes, &tm_x, bar, 0, x.cj, 0, s1);
+      const int b0 = 2 * x.pr, b1 = 2 * x.pr + 1 < p.B ? 2 * x.pr + 1 : p.B;   // b = B: out of bounds -> zeros
+      const int hc = p.h0 + x.h;
+      tma_load_5d(dst, &tm_x, bar, 0, x.cj, 0, hc, b0);
+      tma_load_5d(dst + kTileBytes, &tm_x, bar, 0, x.cj, 0, hc, b1);
       if (gated_in) {
-        tma_load_4d(s_gate0, &tm_g, bar, 0, x.cj, 0, s0);
-        tma_load_4d(s_gate0 + kTileBytes, &tm_g, bar, 0, x.cj, 0, s1);
+        tma_load_5d(s_gate0, &tm_g, bar, 0, x.cj, 0, hc, b0);
+        tma_load_5d(s_gate0 + kTileBytes, &tm_g, bar, 0, x.cj, 0, hc, b1);
       }
     } else {
       const int row = x.pr * p.H + x.h;
@@ -230,15 +230,18 @@ outer_tc_kernel(const __grid_constant__ CUtensorMap tm_x,    // real endpoint: u
         for (int part = 0; part < 2; ++part) {
           const int b = 2 * x.pr + part;
           const uint4 v = ld_shared_v4(sX + part * kTileBytes + off);
-          const size_t e0 = (size_t(b < p.B ? b : p.B - 1) * p.Hs + p.h0 + x.h) * p.L + size_t(lane) * p.M + x.cj * 64 + 8 * c;
+          // element offset inside batch member bb (a real member: the zero partner reads member B - 1 and drops it)
+          const long long bb = b < p.B ? b : p.B - 1;
+          const size_t e0 = size_t(p.h0 + x.h) * p.L + size_t(lane) * p.M + x.cj * 64 + 8 * c;
           if (has_y2 && row_ok && b < p.B) {
             // second gated output straight to global memory
-            const uint4 g2 = __ldg(reinterpret_cast<const uint4*>(p.postgate2 + e0 / 2));
-            *reinterpret_cast<uint4*>(p.y2 + e0 / 2) =
+            const uint4 g2 = __ldg(reinterpret_cast<const uint4*>(p.postgate2 + (bb * p.postgate2_bs + e0) / 2));
+            *reinterpret_cast<uint4*>(p.y2 + (bb * p.y2_bs + e0) / 2) =
                 make_uint4(NT::hmul2(v.x, g2.x), NT::hmul2(v.y, g2.y), NT::hmul2(v.z, g2.z), NT::hmul2(v.w, g2.w));
           }
           if (has_post) {
-            const uint4 g = row_ok ? __ldg(reinterpret_cast<const uint4*>(p.postgate + e0 / 2)) : make_uint4(0, 0, 0, 0);
+            const uint4 g = row_ok ? __ldg(reinterpret_cast<const uint4*>(p.postgate + (bb * p.postgate_bs + e0) / 2))
+                                   : make_uint4(0, 0, 0, 0);
             st_shared_v4(sX + part * kTileBytes + off, NT::hmul2(v.x, g.x), NT::hmul2(v.y, g.y), NT::hmul2(v.z, g.z),
                          NT::hmul2(v.w, g.w));
           }
@@ -254,8 +257,8 @@ outer_tc_kernel(const __grid_constant__ CUtensorMap tm_x,    // real endpoint: u
         tma_store_4d(&tm_pi, sX + kTileBytes, 0, x.cj, 0, row);
       } else {
         const int b0 = 2 * x.pr, b1 = 2 * x.pr + 1;
-        tma_store_4d(&tm_x, sX, 0, x.cj, 0, b0 * p.Hs + p.h0 + x.h);
-        if (b1 < p.B) tma_store_4d(&tm_x, sX + kTileBytes, 0, x.cj, 0, b1 * p.Hs + p.h0 + x.h);
+        tma_store_5d(&tm_x, sX, 0, x.cj, 0, p.h0 + x.h, b0);
+        if (b1 < p.B) tma_store_5d(&tm_x, sX + kTileBytes, 0, x.cj, 0, p.h0 + x.h, b1);
       }
       tma_store_commit();
       if (nslots == 1 && unit + 1 < u_end) {   // gated: slot and gate slot are free once the store has read the slot

@@ -86,6 +86,17 @@ DEVINL void tma_store_4d(const void* map, uint32_t src_smem, int c0, int c1, int
                ::"l"(reinterpret_cast<uint64_t>(map)), "r"(src_smem), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
                : "memory");
 }
+DEVINL void tma_load_5d(uint32_t dst_smem, const void* map, uint32_t bar, int c0, int c1, int c2, int c3, int c4) {
+  asm volatile(
+      "cp.async.bulk.tensor.5d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6, %7}], [%2];"
+      ::"r"(dst_smem), "l"(reinterpret_cast<uint64_t>(map)), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4)
+      : "memory");
+}
+DEVINL void tma_store_5d(const void* map, uint32_t src_smem, int c0, int c1, int c2, int c3, int c4) {
+  asm volatile("cp.async.bulk.tensor.5d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5, %6}], [%1];"
+               ::"l"(reinterpret_cast<uint64_t>(map)), "r"(src_smem), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4)
+               : "memory");
+}
 DEVINL void tma_store_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 DEVINL void tma_store_wait_read0() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
 DEVINL void tma_store_wait_all0() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }

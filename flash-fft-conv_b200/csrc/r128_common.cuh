@@ -62,12 +62,17 @@ DEVINL uint64_t f_desc(uint32_t s_f, int plane, int hf, int s) {
 // of channel h (rows beyond L/64: TMA out-of-bounds zero fill = implicit padding).  nseg == 1 is the ordinary case
 // b = 2g + which.  Small sizes N < 8192: nseg = 8192/N members, each an independent N-point circular convolution —
 // stage 1 uses the block-diagonal matrix I_nseg (x) F_{N/64} instead of F_128, the rest of the kernel is unchanged.
-// A member beyond the batch is fetched from sequence index B*H, out of bounds for the tensor map: an all-zero tile.
-DEVINL void load_tile(uint32_t dst, const void* map, uint32_t bar, int B, int H, int h, int g, int which, int nseg,
-                      int seg_bytes) {
-  for (int s = 0; s < nseg; ++s) {
-    const int b = (g * nseg + s) * 2 + which;
-    tma_load_3d(dst + s * seg_bytes, map, bar, 0, 0, b < B ? b * H + h : B * H);
+// The map is the rank-4 [b][h][L/64][64] view of a (B, H, L) tensor (any batch stride, see make_seq_map in bffc.cu); a
+// member beyond the batch (b >= B) is out of bounds for the map: an all-zero tile.
+// kRolled: keep the segment loop rolled (the dk_f kernel: unrolled copies cost it spill slots; the fused forward kernel
+// spills less with the compiler's choice).
+template <bool kRolled = false>
+DEVINL void load_tile(uint32_t dst, const void* map, uint32_t bar, int h, int g, int which, int nseg, int seg_bytes) {
+  if (kRolled) {
+#pragma unroll 1
+    for (int s = 0; s < nseg; ++s) tma_load_4d(dst + s * seg_bytes, map, bar, 0, 0, h, (g * nseg + s) * 2 + which);
+  } else {
+    for (int s = 0; s < nseg; ++s) tma_load_4d(dst + s * seg_bytes, map, bar, 0, 0, h, (g * nseg + s) * 2 + which);
   }
 }
 

@@ -184,12 +184,38 @@ def _forward_host(mod, u, k, pregate, postgate, out, device):
     return out
 
 
-def _check_inputs(u, k, mod, gates=()):
+def batch_stride(t, dtype, device_type='cuda'):
+    """Batch stride (elements) of a (B, H, L) tensor the engine reads or writes in place, or None when `t` does not
+    qualify.  It qualifies when it lives on `device_type` with `dtype`, its rows are contiguous (stride (s, L, 1)), s is
+    a multiple of 8 that is >= H*L, and its data is 16-byte aligned: channel slices of one (B, 3H, L) projection do."""
+    if t.device.type != device_type or t.dtype != dtype or t.dim() != 3:
+        return None
+    _, H, L = t.shape
+    s = t.stride(0)
+    if (H > 1 and t.stride(1) != L) or (L > 1 and t.stride(2) != 1) or s % 8 or s < H * L or t.data_ptr() % 16:
+        return None
+    return s
+
+
+def _engine_view(t, dtype):
+    """(tensor, batch stride) as the engine takes it: `t` itself when it qualifies (batch_stride), else a contiguous
+    copy.  (None, 0) for an absent tensor."""
+    if t is None:
+        return None, 0
+    s = batch_stride(t, dtype)
+    if s is None:
+        t = t.contiguous()
+        s = t.shape[1] * t.shape[2]
+    return t, s
+
+
+def _check_inputs(u, k, mod, gates=(), views=False):
+    """views: u and the gates may be any (B, H, L) layout (channel slices are used in place, others copied)."""
     if not u.is_cuda:
         raise RuntimeError('u must be a CUDA tensor (bffc has no CPU path)')          # monarch_fwd.h:7-13
     if u.dtype != mod.dtype:
         raise RuntimeError(f'u must have dtype {mod.dtype}, got {u.dtype}')
-    if u.dim() != 3 or not u.is_contiguous():
+    if u.dim() != 3 or not (views or u.is_contiguous()):
         raise RuntimeError('u must be a contiguous (B, H, L) tensor')
     B, H, L = u.shape
     if k.dim() != 2 or k.shape[0] != H or k.shape[1] > mod.seqlen:
@@ -197,7 +223,7 @@ def _check_inputs(u, k, mod, gates=()):
     if L > mod.seqlen:
         raise RuntimeError(f'L={L} exceeds seqlen={mod.seqlen}')
     for g in gates:
-        if g.shape != u.shape or g.dtype != u.dtype or not g.is_contiguous() or not g.is_cuda:
+        if g.shape != u.shape or g.dtype != u.dtype or not (views or g.is_contiguous()) or not g.is_cuda:
             raise RuntimeError('gates must match u in shape, dtype, device and be contiguous')
     return B, H, L
 
@@ -284,50 +310,74 @@ class _on_device:
             self.ctx.__exit__(*a)
 
 
-def _fwd(mod, u, k, pregate, postgate, band=None, use_cache=None):
-    """y and the engine-order filter spectrum it used.  band / use_cache: see _kf_engine_for."""
+def _fwd(mod, u, k, pregate, postgate, band=None, use_cache=None, kf_engine=None):
+    """y (contiguous) and the engine-order filter spectrum it used.  u and the gates: any (B, H, L) layout; those that
+    qualify (batch_stride) are read in place, others copied.  band / use_cache: see _kf_engine_for; kf_engine: a
+    spectrum of k already at hand."""
     L0 = u.shape[-1]
     Lp = _pad_len(mod, u.device, L0)
     if Lp != L0:
-        y, kf = _fwd(mod, _padded(u, Lp), k, _padded(pregate, Lp), _padded(postgate, Lp), band, use_cache)
+        y, kf = _fwd(mod, _padded(u, Lp), k, _padded(pregate, Lp), _padded(postgate, Lp), band, use_cache, kf_engine)
         return y[..., :L0].contiguous(), kf
     B, H, L = u.shape
     plan = mod.plan(u.device)
+    (u, u_bs), (pre, pre_bs), (post, post_bs) = (_engine_view(t, mod.dtype) for t in (u, pregate, postgate))
     with _on_device(u.device):
         mod.__dict__['last_launches'] = 0
-        kf_engine = _kf_engine_for(mod, plan, k, band=band, use_cache=use_cache)
-        y = torch.empty_like(u)
-        ws, ws_bytes = _workspace(plan, B, H, L, pregate is not None, False, u.device)
-        _lib.check(_lib.lib().bffc_fwd(plan.handle, _ptr(u), _ptr(kf_engine), _ptr(pregate), _ptr(postgate),
-                                       _ptr(y), B, H, L, _ptr(ws), ws_bytes, _stream()))
+        if kf_engine is None:
+            kf_engine = _kf_engine_for(mod, plan, k, band=band, use_cache=use_cache)
+        y = torch.empty((B, H, L), dtype=u.dtype, device=u.device)
+        ws, ws_bytes = _workspace(plan, B, H, L, pre is not None, False, u.device)
+        _lib.check(_lib.lib().bffc_fwd_strided(plan.handle, _ptr(u), u_bs, _ptr(kf_engine), _ptr(pre), pre_bs,
+                                               _ptr(post), post_bs, _ptr(y), H * L, B, H, L, _ptr(ws), ws_bytes,
+                                               _stream()))
         mod.__dict__['last_launches'] += _lib.lib().bffc_last_launch_count()
     return y, kf_engine
 
 
-def _bwd(mod, dout, u, kf_engine, k_len, pregate, postgate, band=None):
+def _bwd(mod, dout, u, kf_engine, k_len, pregate, postgate, band=None, out=None):
     """du, dk[, dpregate, dpostgate] — reference: FlashFFTConvFunc.backward, conv.py:1737-1822.  band: the forward's
-    band limit (None: full spectrum); kf_engine is then the band-limited spectrum and dk gets the same mask."""
+    band limit (None: full spectrum); kf_engine is then the band-limited spectrum and dk gets the same mask.  Inputs:
+    any (B, H, L) layout, as for _fwd.  out: optional (du, dpregate, dpostgate) tensors to write the gradients into
+    (channel slices of one buffer are written in place) and return; otherwise they are new contiguous tensors."""
     L0 = u.shape[-1]
     Lp = _pad_len(mod, u.device, L0)
     if Lp != L0:
         r = _bwd(mod, _padded(dout, Lp), _padded(u, Lp), kf_engine, k_len, _padded(pregate, Lp), _padded(postgate, Lp),
                  band)
         cut = lambda t: None if t is None else t[..., :L0].contiguous()
-        return cut(r[0]), r[1], cut(r[2]), cut(r[3])
+        res = [cut(r[0]), r[1], cut(r[2]), cut(r[3])]
+        for i, o in zip((0, 2, 3), out or ()):
+            if o is not None and res[i] is not None:
+                res[i] = o.copy_(res[i])
+        return tuple(res)
     B, H, L = u.shape
     N = mod.fft_size(u.device)
     plan = mod.plan(u.device)
-    dout = dout.contiguous()                                          # conv.py:1742
+    gated = pregate is not None
+    (dout, dout_bs), (u, u_bs), (pre, pre_bs), (post, post_bs) = (_engine_view(t, mod.dtype)
+                                                                  for t in (dout, u, pregate, postgate))
+    outs = list(out) if out is not None else [None, None, None]
+    dst = []                       # (tensor the library writes, its batch stride, where the result must end up)
+    for i, o in enumerate(outs):
+        if i > 0 and not gated:
+            dst.append((None, 0, None))
+            continue
+        s = None if o is None else batch_stride(o, mod.dtype)
+        t = o if s is not None else torch.empty((B, H, L), dtype=u.dtype, device=u.device)
+        dst.append((t, s if s is not None else H * L, o if s is None else None))
+    (du, du_bs, _), (dpre, dpre_bs, _), (dpost, dpost_bs, _) = dst
     with _on_device(u.device):
-        du = torch.empty_like(u)
         dkf_engine = torch.empty((H, N, 2), dtype=torch.float32, device=u.device)
-        dpre = torch.empty_like(u) if pregate is not None else None
-        dpost = torch.empty_like(u) if pregate is not None else None
-        ws, ws_bytes = _workspace(plan, B, H, L, pregate is not None, True, u.device)
+        ws, ws_bytes = _workspace(plan, B, H, L, gated, True, u.device)
         # kf_engine_conj = NULL: the kernels conjugate the forward's spectrum in their pointwise multiply
-        _lib.check(_lib.lib().bffc_bwd(plan.handle, _ptr(dout), _ptr(u), _ptr(kf_engine), None, _ptr(pregate),
-                                       _ptr(postgate), _ptr(du), _ptr(dkf_engine), _ptr(dpre), _ptr(dpost),
-                                       B, H, L, _ptr(ws), ws_bytes, _stream()))
+        _lib.check(_lib.lib().bffc_bwd_strided(plan.handle, _ptr(dout), dout_bs, _ptr(u), u_bs, _ptr(kf_engine), None,
+                                               _ptr(pre), pre_bs, _ptr(post), post_bs, _ptr(du), du_bs,
+                                               _ptr(dkf_engine), _ptr(dpre), dpre_bs, _ptr(dpost), dpost_bs,
+                                               B, H, L, _ptr(ws), ws_bytes, _stream()))
+        for t, _, o in dst:
+            if o is not None:
+                o.copy_(t)
         mod.__dict__['last_launches'] = _lib.lib().bffc_last_launch_count()
         # the kernels accumulate unnormalised pair-packed spectra in engine order; the reference takes
         # ifft(dk_f).real[..., :k_len] (conv.py:1817-1820): inverse fp32 FFT straight from engine order, 1/N, real part
@@ -341,6 +391,7 @@ def _bwd(mod, dout, u, kf_engine, k_len, pregate, postgate, band=None):
             _lib.check(_lib.lib().bffc_dk_from_dkf_band(plan.handle, _ptr(dkf_engine), _ptr(dk), int(k_len), H, int(band),
                                                         _ptr(fws), fws_bytes, _stream()))
         mod.__dict__['last_launches'] += _lib.lib().bffc_last_launch_count()
+    du, dpre, dpost = (o if o is not None else t for t, _, o in dst)
     return du, dk, dpre, dpost
 
 
@@ -364,8 +415,9 @@ class FlashFFTConvFunc(torch.autograd.Function):
 
 class GatedFlashFFTConvFunc(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, u, k, mod, pregate, postgate):
-        _check_inputs(u, k, mod, (pregate, postgate))
+    def forward(ctx, u, k, mod, pregate, postgate, views=False):
+        """views=True (gated_long_conv): u and the gates may be channel slices or other non-contiguous layouts."""
+        _check_inputs(u, k, mod, (pregate, postgate), views)
         y, kf_engine = _fwd(mod, u, k, pregate, postgate)
         ctx.mod = mod
         ctx.k_len = k.shape[-1]
@@ -377,4 +429,4 @@ class GatedFlashFFTConvFunc(torch.autograd.Function):
     def backward(ctx, dout):
         u, kf_engine, pregate, postgate = ctx.saved_tensors
         du, dk, dpre, dpost = _bwd(ctx.mod, dout, u, kf_engine, ctx.k_len, pregate, postgate)
-        return du, dk, None, dpre, dpost                              # conv.py:3939
+        return du, dk, None, dpre, dpost, None                        # conv.py:3939

@@ -171,6 +171,27 @@ int bffc_bwd(const bffc_plan* plan, const void* dout, const void* u, const void*
              void* workspace, size_t workspace_bytes, void* stream);
 
 /*
+ * bffc_fwd / bffc_bwd on batch-strided (B, H, L) tensors, e.g. channel slices x1, x2, v of one (B, 3H, L) projection
+ * (the Hyena / M2 mixers) read and written in place.  Rows stay contiguous (channel stride L); every tensor argument
+ * carries its own batch stride, counted in elements: element (b, h, l) of u lives at u + b * u_bstride + h * L + l.
+ * Each stride of a given (non-NULL) tensor must be a multiple of 8 and >= H * L, else BFFC_ERR_INVALID; pointers are
+ * 16-byte aligned as for bffc_fwd / bffc_bwd.  No two outputs may overlap (the caller's rule; not checked).  Inputs may
+ * overlap each other.  An ungated bffc_bwd_strided ignores dpregate / dpostgate and their strides.
+ * Workspace sizes and launch counts are those of bffc_fwd / bffc_bwd at the same shape; bffc_fwd / bffc_bwd are these
+ * calls with every stride H * L.
+ */
+int bffc_fwd_strided(const bffc_plan* plan, const void* u, int64_t u_bstride, const void* kf_engine,
+                     const void* pregate, int64_t pregate_bstride, const void* postgate, int64_t postgate_bstride,
+                     void* y, int64_t y_bstride, int B, int H, int L, void* workspace, size_t workspace_bytes,
+                     void* stream);
+int bffc_bwd_strided(const bffc_plan* plan, const void* dout, int64_t dout_bstride, const void* u, int64_t u_bstride,
+                     const void* kf_engine, const void* kf_engine_conj,
+                     const void* pregate, int64_t pregate_bstride, const void* postgate, int64_t postgate_bstride,
+                     void* du, int64_t du_bstride, void* dkf_engine, void* dpregate, int64_t dpregate_bstride,
+                     void* dpostgate, int64_t dpostgate_bstride, int B, int H, int L,
+                     void* workspace, size_t workspace_bytes, void* stream);
+
+/*
  * Forward on HOST buffers (the reference has no counterpart: its user writes u.cuda() -> conv -> y.cpu(),
  * README.md:108-149, three serial steps on one stream).  u_host, pregate_host, postgate_host, y_host: (B, H, L)
  * contiguous host memory of the plan dtype — page-locked for the copies to overlap; kf_engine: DEVICE, from
