@@ -404,6 +404,7 @@ int bffc_plan_create(bffc_plan** out, int seqlen, int dtype) {
   FMT_SWITCH(dtype,
     PLAN_TRY(cudaFuncSetAttribute(fwd3_kernel<false, false, F>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemTotal3));
     PLAN_TRY(cudaFuncSetAttribute(fwd3_kernel<false, true, F>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemTotal3));
+    PLAN_TRY(cudaFuncSetAttribute(fwd3_kernel<false, true, F, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemTotal3));
     PLAN_TRY(cudaFuncSetAttribute(fwd3_kernel<true, false, F>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemTotal3));
     PLAN_TRY(cudaFuncSetAttribute(dkf3_kernel<true, F>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemTotalDkf3));
     PLAN_TRY(cudaFuncSetAttribute(dkf3_kernel<false, F>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemTotalDkf3));
@@ -736,6 +737,7 @@ struct PassOpts {
   Seq y2;
   void* xg_out = nullptr;           // seqlen <= 8192, gated: the pass also stores its gated input u * pregate here
                                     // (contiguous (B, H, L) workspace)
+  const bffc::ShortParams* sf = nullptr;   // short filter on u / pregate / postgate (bffc_fwd_short_strided)
 };
 
 // fused 8192-point kernel on (B, H, L) real sequences (seqlen <= 8192)
@@ -767,8 +769,15 @@ static int launch_fused(const bffc_plan* p, Seq u, const void* kf, Seq pregate, 
     if (int rc = map(&gm.y2, po.y2)) return rc;
   }
   const int g3 = persistent_grid(p, prm.units, kPipes3);
+  bffc::FwdShortParams sprm;
+  if (po.sf) {
+    static_cast<bffc::FwdParams&>(sprm) = prm;
+    sprm.sf = *po.sf;
+  }
   FMT_SWITCH(p->dtype,
-    if (gated)
+    if (po.sf)             // the gated pipeline, also for a filtered u without gates
+      fwd3_kernel<false, true, F, true><<<g3, kThreads3, kSmemTotal3, st>>>(tm_u, tm_y, tm_g, gm, sprm);
+    else if (gated)
       fwd3_kernel<false, true, F><<<g3, kThreads3, kSmemTotal3, st>>>(tm_u, tm_y, tm_g, gm, prm);
     else
       fwd3_kernel<false, false, F><<<g3, kThreads3, kSmemTotal3, st>>>(tm_u, tm_y, tm_g, gm, prm);
@@ -834,8 +843,8 @@ static bffc::outer::OuterParams outer_params(const bffc_plan* p, int lev, View v
 }
 
 template <int R, int F>
-static void launch_cc(const bffc_plan* p, bool inverse, bool gated, bool planes, const bffc::outer::OuterParams& op_in,
-                      int rows, cudaStream_t st) {
+static void launch_cc(const bffc_plan* p, bool inverse, bool gated, bool planes, bool shrt,
+                      const bffc::outer::OuterParams& op_in, int rows, cudaStream_t st) {
   using namespace bffc::outer;
   OuterParams op = op_in;
   // read-ahead distance = the number of resident blocks (one residency period ahead)
@@ -845,6 +854,15 @@ static void launch_cc(const bffc_plan* p, bool inverse, bool gated, bool planes,
     dim3 grid(rows, cb, 1);
     if (!inverse) fwd_kernel<R, false, true, F><<<grid, 128, 0, st>>>(op);
     else inv_kernel<R, false, true, F><<<grid, 128, 0, st>>>(op);
+  } else if (shrt) {      // level 0 on the raw projection: short filter on u / pregate (forward), postgate (inverse)
+    dim3 grid(cb, op.H, op.pairs);
+    if (!inverse) {
+      if (gated) fwd_kernel<R, true, false, F, true><<<grid, 128, 0, st>>>(op);
+      else fwd_kernel<R, false, false, F, true><<<grid, 128, 0, st>>>(op);
+    } else {
+      if (gated) inv_kernel<R, true, false, F, true><<<grid, 128, 0, st>>>(op);
+      else inv_kernel<R, false, false, F><<<grid, 128, 0, st>>>(op);     // no gate, nothing to filter
+    }
   } else {
     dim3 grid(cb, op.H, op.pairs);
     if (!inverse) {
@@ -857,14 +875,15 @@ static void launch_cc(const bffc_plan* p, bool inverse, bool gated, bool planes,
   }
 }
 // CUDA-core outer level `lev` (level 1 works on the complex rows of level 0: pairs * H * R0 of them)
+// shrt (level 0 only): op.sf holds short filter taps for the endpoint tensors
 static int cc_stage(const bffc_plan* p, int lev, bool inverse, bool gated, const bffc::outer::OuterParams& op,
-                    cudaStream_t st) {
+                    cudaStream_t st, bool shrt = false) {
   const bool planes = lev == 1;
   const int rows = op.pairs * op.H * p->R0;
   switch (p->lev[lev].R) {
-    case 2: FMT_SWITCH(p->dtype, (launch_cc<2, F>(p, inverse, gated, planes, op, rows, st));); break;
-    case 4: FMT_SWITCH(p->dtype, (launch_cc<4, F>(p, inverse, gated, planes, op, rows, st));); break;
-    case 8: FMT_SWITCH(p->dtype, (launch_cc<8, F>(p, inverse, gated, planes, op, rows, st));); break;
+    case 2: FMT_SWITCH(p->dtype, (launch_cc<2, F>(p, inverse, gated, planes, shrt, op, rows, st));); break;
+    case 4: FMT_SWITCH(p->dtype, (launch_cc<4, F>(p, inverse, gated, planes, shrt, op, rows, st));); break;
+    case 8: FMT_SWITCH(p->dtype, (launch_cc<8, F>(p, inverse, gated, planes, shrt, op, rows, st));); break;
     default: return fail(BFFC_ERR_UNSUPPORTED, "outer radix %d not supported", p->lev[lev].R);
   }
   return launched();
@@ -912,16 +931,19 @@ static PlaneSet plane_set(const bffc_plan* p, void* ws, int idx, int B, int H) {
 
 // all outer levels, forward: real (B,H,L) x (* pregate) -> complex 8192-point rows.  Level 0 writes set `s0`,
 // level 1 (if any) reads `s0` and writes `s1`; returns the set holding the rows.
+// sf: short filter taps applied to x / pregate as level 0 loads them (CUDA-core outer stage only)
 static int transform_fwd(const bffc_plan* p, Seq x, Seq pregate, View v, int L, PlaneSet s0, PlaneSet s1,
-                         PlaneSet* out, cudaStream_t st) {
+                         PlaneSet* out, cudaStream_t st, const bffc::ShortParams* sf = nullptr) {
   if (p->lev[0].tc) {
+    if (sf) return fail(BFFC_ERR_UNSUPPORTED, "the short filter is not fused into the seqlen %d outer stage", p->N);
     if (int rc = tc_stage(p, false, x, pregate, s0, v, L, st)) return rc;
   } else {
     bffc::outer::OuterParams op = outer_params(p, 0, v, L, s0, s1);
     op.u = static_cast<const uint4*>(x.p);
     op.pregate = static_cast<const uint4*>(pregate.p);
     op.u_bs = x.bs / 8; op.pregate_bs = pregate.bs / 8;
-    if (int rc = cc_stage(p, 0, false, pregate.p != nullptr, op, st)) return rc;
+    if (sf) op.sf = *sf;
+    if (int rc = cc_stage(p, 0, false, pregate.p != nullptr, op, st, sf != nullptr)) return rc;
   }
   *out = s0;
   if (p->nlev == 2) {
@@ -932,19 +954,24 @@ static int transform_fwd(const bffc_plan* p, Seq x, Seq pregate, View v, int L, 
 }
 
 // all outer levels, inverse: rows in `rows` (set s1 if two levels, else s0) -> real y (* postgate)
+// sf: short filter taps applied to postgate where the output is multiplied by it
 static int transform_inv(const bffc_plan* p, Seq y, Seq postgate, View v, int L, PlaneSet s0, PlaneSet s1,
-                         cudaStream_t st, Seq postgate2 = Seq(), Seq y2 = Seq()) {
+                         cudaStream_t st, Seq postgate2 = Seq(), Seq y2 = Seq(), const bffc::ShortParams* sf = nullptr) {
   if (p->nlev == 2) {
     if (int rc = cc_stage(p, 1, true, false, outer_params(p, 1, v, L, s0, s1), st)) return rc;
   }
-  if (p->lev[0].tc) return tc_stage(p, true, y, postgate, s0, v, L, st, postgate2, y2);
+  if (p->lev[0].tc) {
+    if (sf) return fail(BFFC_ERR_UNSUPPORTED, "the short filter is not fused into the seqlen %d outer stage", p->N);
+    return tc_stage(p, true, y, postgate, s0, v, L, st, postgate2, y2);
+  }
   bffc::outer::OuterParams op = outer_params(p, 0, v, L, s0, s1);
   op.y = static_cast<uint4*>(y.p);
   op.postgate = static_cast<const uint4*>(postgate.p);
   op.postgate2 = static_cast<const uint4*>(postgate2.p);
   op.y2 = static_cast<uint4*>(y2.p);
   op.y_bs = y.bs / 8; op.postgate_bs = postgate.bs / 8; op.postgate2_bs = postgate2.bs / 8; op.y2_bs = y2.bs / 8;
-  return cc_stage(p, 0, true, postgate.p != nullptr, op, st);
+  if (sf) op.sf = *sf;
+  return cc_stage(p, 0, true, postgate.p != nullptr, op, st, sf != nullptr);
 }
 
 // A composite-size call chunk by chunk (see chunk_view; `sets` plane sets per chunk): f(v, at, set) for each chunk.
@@ -994,10 +1021,10 @@ static int conv_forward(const bffc_plan* p, Seq u, const void* kf, Seq pregate, 
   return for_each_chunk(p, B, H, L, ws, p->nlev, [&](const View& v, auto at, auto set) {
     const PlaneSet s0 = set(0), s1 = set(p->nlev == 2 ? 1 : 0);
     PlaneSet rows;
-    if (int rc = transform_fwd(p, at(u), at(pregate), v, L, s0, s1, &rows, st)) return rc;
+    if (int rc = transform_fwd(p, at(u), at(pregate), v, L, s0, s1, &rows, st, po.sf)) return rc;
     const uint8_t* kfc = static_cast<const uint8_t*>(kf) + size_t(v.h0) * p->NE * 4;
     if (int rc = launch_planes(p, rows.re, rows.im, kfc, (v.B + 1) / 2, v.H * p->R, st, po.conj)) return rc;
-    return transform_inv(p, at(y), at(postgate), v, L, s0, s1, st, at(po.postgate2), at(po.y2));
+    return transform_inv(p, at(y), at(postgate), v, L, s0, s1, st, at(po.postgate2), at(po.y2), po.sf);
   });
 }
 
@@ -1027,6 +1054,53 @@ int bffc_fwd(const bffc_plan* p, const void* u, const void* kf, const void* preg
              int B, int H, int L, void* workspace, size_t workspace_bytes, void* stream) {
   const int64_t s = int64_t(H) * L;
   return bffc_fwd_strided(p, u, s, kf, pregate, s, postgate, s, y, s, B, H, L, workspace, workspace_bytes, stream);
+}
+
+int bffc_fwd_short_strided(const bffc_plan* p, const void* u_, int64_t u_bs, const void* kf, const void* pregate_,
+                           int64_t pregate_bs, const void* postgate_, int64_t postgate_bs, void* y_, int64_t y_bs, int B,
+                           int H, int L, const void* u_w, const void* u_bias, const void* pregate_w,
+                           const void* pregate_bias, const void* postgate_w, const void* postgate_bias, int w_dtype, int K,
+                           int padding, void* workspace, size_t workspace_bytes, void* stream) {
+  const char* fn = "bffc_fwd_short_strided";
+  // arguments first, the device last (as the depthwise entry points): a bad argument is BFFC_ERR_INVALID on any machine
+  if (K < 1 || K > 4) return fail(BFFC_ERR_INVALID, "%s: K=%d outside [1, 4]", fn, K);
+  if (padding < 0 || padding > K - 1 || 2 * padding < K - 1)
+    return fail(BFFC_ERR_INVALID, "%s: padding %d outside [(K-1)/2, K-1] for K=%d", fn, padding, K);
+  if (w_dtype != BFFC_DTYPE_BF16 && w_dtype != BFFC_DTYPE_FP16 && w_dtype != BFFC_DTYPE_FP32)
+    return fail(BFFC_ERR_INVALID, "%s: w_dtype %d (BF16 0, FP16 1, FP32 2)", fn, w_dtype);
+  if ((u_bias && !u_w) || (pregate_bias && !pregate_w) || (postgate_bias && !postgate_w))
+    return fail(BFFC_ERR_INVALID, "%s: a bias needs the taps of its tensor", fn);
+  if ((pregate_w && !pregate_) || (postgate_w && !postgate_))
+    return fail(BFFC_ERR_INVALID, "%s: taps for an absent gate", fn);
+  const size_t ew = w_dtype == BFFC_DTYPE_FP32 ? 4 : 2;
+  for (const void* t : {u_w, u_bias, pregate_w, pregate_bias, postgate_w, postgate_bias})
+    if (reinterpret_cast<uintptr_t>(t) % ew) return fail(BFFC_ERR_INVALID, "%s: taps not aligned to their element", fn);
+  if (B <= 0 || H <= 0 || L <= 0) return fail(BFFC_ERR_INVALID, "%s: bad shape B=%d H=%d L=%d", fn, B, H, L);
+  if (int rc = check_strides(fn, H, L, {seq(u_, u_bs), seq(pregate_, pregate_bs), seq(postgate_, postgate_bs), seq(y_, y_bs)}))
+    return rc;
+  if (!p) return fail(BFFC_ERR_INVALID, "%s: null plan", fn);
+  if (p->nlev > 0 && p->lev[0].tc)
+    return fail(BFFC_ERR_UNSUPPORTED, "%s: seqlen %d (tensor-core outer stage) does not take the short filter", fn, p->N);
+  if ((pregate_ == nullptr) != (postgate_ == nullptr))
+    return fail(BFFC_ERR_INVALID, "%s: pregate and postgate must both be given or both be null", fn);
+  if (!u_ || !kf || !y_) return fail(BFFC_ERR_INVALID, "%s: null pointer", fn);
+  if (int rc = check_common(p, B, H, L, u_, y_, kf)) return rc;
+  if (!aligned16(pregate_, postgate_, workspace)) return fail(BFFC_ERR_INVALID, "%s: gates / workspace must be 16-byte aligned", fn);
+  {
+    const size_t need = bffc_workspace_bytes_ex(p, B, H, L, pregate_ != nullptr, 0);
+    if (need && (!workspace || workspace_bytes < need))
+      return fail(BFFC_ERR_INVALID, "%s: workspace of %zu bytes required", fn, need);
+  }
+  bffc::ShortParams sf{};
+  sf.u = {u_w, u_bias};
+  sf.pre = {pregate_w, pregate_bias};
+  sf.post = {postgate_w, postgate_bias};
+  sf.wdt = w_dtype; sf.K = K; sf.P = padding;
+  PassOpts po;
+  po.sf = &sf;
+  g_launches = 0;
+  return conv_forward(p, seq(u_, u_bs), kf, seq(pregate_, pregate_bs), seq(postgate_, postgate_bs), seq(y_, y_bs), B, H, L,
+                      workspace, static_cast<cudaStream_t>(stream), po);
 }
 
 int bffc_bwd_strided(const bffc_plan* p, const void* dout_, int64_t dout_bs, const void* u_, int64_t u_bs, const void* kf,

@@ -19,6 +19,7 @@
 // elementwise pre-pass re-reading all four tensors.
 #pragma once
 #include "r128_common.cuh"
+#include <type_traits>
 
 namespace bffc {
 namespace r128 {
@@ -32,11 +33,68 @@ static_assert(kSmemTotal3 <= 227 * 1024, "shared memory per block");
 
 struct GateMaps { CUtensorMap pre, post, post2, y2, xg; };
 
-template <bool kPlanes, bool kGated, int kFmt>
+// Where a row of a slot sits in its sequence (kShort).  The slot's 256 tile rows are the two pair members' tiles; tile
+// row r belongs to segment r / rblk, i.e. batch member b = (g * nseg + r / rblk) * 2 + tile, at rows (r % rblk) * 64 ..
+// + 63 of it.  A row is `valid` when that member exists and the row lies inside [0, L); its left / right neighbour row
+// is part of the same sequence when `lvalid` / `rvalid`.
+struct ShortRow {
+  bool valid, lvalid, rvalid;
+  DEVINL ShortRow(const FwdParams& p, int g, int row) {
+    const int r = row & 127, rblk = p.seg_bytes >> 7, sg = r / rblk, ris = r - sg * rblk, used = p.L >> 6;
+    valid = (g * p.nseg + sg) * 2 + (row >> 7) < p.B && ris < used;
+    lvalid = ris > 0;
+    rvalid = ris + 1 < used;
+  }
+};
+
+// kShort: the short filter (short_filter.cuh) on the raw tiles of slot sA, in place; thread ptid owns row `row` = ptid
+// (64 elements in 8 swizzled 16-byte chunks).  A row's neighbours are its own chunks, the last chunk of the row before
+// and the first of the row after, when those belong to the same sequence (never across a segment or a pair member):
+// those two are read before `sync`, then the row is swept left to right, each chunk read before the one before it is
+// overwritten.  Rows that are not `valid` are left alone: their tiles are zero (TMA zero fill), and s is implicitly
+// zero-padded beyond L, so no bias leaks there.  sB != 0: a second slot filtered the same way (its own taps, not
+// written); the row becomes s(A) * s(B), the 16-bit product of pass 0.  fa / fb: whether A / B have taps (else raw).
+template <int kFmt, class Sync>
+DEVINL void short_slot(uint32_t sA, uint32_t sB, const Taps& ta, const Taps& tb, bool fa, bool fb, int row,
+                       const ShortRow& g, Sync&& sync) {
+  using NT = Num<kFmt>;
+  const uint4 z = make_uint4(0u, 0u, 0u, 0u);
+  auto at = [&](uint32_t s, int r, int c) { return s + uint32_t(r) * 128u + (uint32_t(c ^ (r & 7)) << 4); };
+  uint4 la = z, ra = z, lb = z, rb = z;
+  if (g.valid && g.lvalid) {
+    la = ld_shared_v4(at(sA, row - 1, 7));
+    if (sB) lb = ld_shared_v4(at(sB, row - 1, 7));
+  }
+  if (g.valid && g.rvalid) {
+    ra = ld_shared_v4(at(sA, row + 1, 0));
+    if (sB) rb = ld_shared_v4(at(sB, row + 1, 0));
+  }
+  sync();
+  if (!g.valid) return;
+  uint4 pa = la, ca = ld_shared_v4(at(sA, row, 0)), pb = lb, cb = sB ? ld_shared_v4(at(sB, row, 0)) : z;
+#pragma unroll 1
+  for (int c = 0; c < 8; ++c) {
+    const uint4 na = c < 7 ? ld_shared_v4(at(sA, row, c + 1)) : ra;
+    const uint4 nb = !sB ? z : c < 7 ? ld_shared_v4(at(sB, row, c + 1)) : rb;
+    uint4 o = fa ? short8<kFmt>(pa, ca, na, ta) : ca;
+    if (sB) {
+      const uint4 q = fb ? short8<kFmt>(pb, cb, nb, tb) : cb;
+      o = make_uint4(NT::hmul2(o.x, q.x), NT::hmul2(o.y, q.y), NT::hmul2(o.z, q.z), NT::hmul2(o.w, q.w));
+    }
+    st_shared_v4(at(sA, row, c), o.x, o.y, o.z, o.w);
+    pa = ca; ca = na; pb = cb; cb = nb;
+  }
+}
+
+// kShort (with kGated): the gated pipeline on the raw projection — u and pregate filtered in pass 0, the postgate after
+// it lands in slot 1 (bffc_fwd_short_strided).  With no gates it is the residual filter's call: s(u) alone.
+template <bool kPlanes, bool kGated, int kFmt, bool kShort = false>
 __global__ void __launch_bounds__(kThreads3, 1)
 fwd3_kernel(const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CUtensorMap tm_y,
-            const __grid_constant__ CUtensorMap tm_g, const __grid_constant__ GateMaps gm, const FwdParams p) {
+            const __grid_constant__ CUtensorMap tm_g, const __grid_constant__ GateMaps gm,
+            const std::conditional_t<kShort, FwdShortParams, FwdParams> p) {
   static_assert(!(kPlanes && kGated), "composite sizes apply their gates in the outer stages");
+  static_assert(!kShort || kGated, "the short filter runs in the gated pipeline");
   using NT = Num<kFmt>;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t sbase = (smem_u32(smem_raw) + 1023u) & ~1023u;
@@ -158,8 +216,18 @@ fwd3_kernel(const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CU
 
     mbar_wait(bar_tma0 + 8 * slot, kGated ? (n & 1) : ((n >> 1) & 1));
     if (kGated) {
-      // ---------------- pass 0: u * pregate in place (same swizzled image on both sides: linear 16-byte chunks)
-      if (has_pre) {
+      if constexpr (kShort) {
+        // ---------------- pass 0: s(u) [* s(pregate)] in place
+        const ShortParams& sf = p.sf;
+        if (has_pre || sf.u.w) {
+          const Taps ta = sf.u.w ? load_taps(sf.u, sf, h) : Taps{};
+          const Taps tb = has_pre && sf.pre.w ? load_taps(sf.pre, sf, h) : Taps{};
+          short_slot<kFmt>(sX, has_pre ? sGate : 0u, ta, tb, sf.u.w != nullptr, sf.pre.w != nullptr, ptid,
+                           ShortRow(p, unit - h * p.pairs, ptid), pipe_sync);
+          publish_smem();                 // filtered products visible to the tensor cores; slot 1 is free again
+        }
+      } else if (has_pre) {
+        // ---------------- pass 0: u * pregate in place (same swizzled image on both sides: linear 16-byte chunks)
 #pragma unroll 4
         for (int i = 0; i < kSlotBytes / 16 / kPipeThreads; ++i) {
           const uint32_t off = uint32_t(i * kPipeThreads + ptid) * 16u;
@@ -265,6 +333,13 @@ fwd3_kernel(const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CU
       }
     };
     if (has_post) { mbar_wait(bar_gate, gate_phase); gate_phase ^= 1; }
+    if constexpr (kShort) {
+      if (has_post && p.sf.post.w) {      // s(postgate) in place in slot 1, then pass 6 multiplies by it
+        const Taps tq = load_taps(p.sf.post, p.sf, h);
+        short_slot<kFmt>(sGate, 0u, tq, tq, true, false, ptid, ShortRow(p, unit - h * p.pairs, ptid), pipe_sync);
+        pipe_sync();
+      }
+    }
     pass6(has_post);
     publish_smem();
     if (leader) {

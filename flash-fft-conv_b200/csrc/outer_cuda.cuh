@@ -12,6 +12,7 @@
 // Each thread owns 8 consecutive n' (one 16-byte vector per row).
 #pragma once
 #include "ptx.cuh"
+#include "short_filter.cuh"
 
 namespace bffc {
 namespace outer {
@@ -44,7 +45,18 @@ struct OuterParams {
   float2 step[8];        // exp(-2 pi i t / (R*M)), t = 0..7: neighbour twiddle steps (host computed, double precision)
   int lookahead;         // blocks: a block pulls the input lines of block (its linear id + lookahead) into L2 (0 = off)
   float scale;           // applied to this stage's output (fp16: 1/sqrt(R) per direction; bf16: 1, 1/N lives in k_f)
+  ShortParams sf;        // kShort kernels: short filter taps of u, pregate (forward) and postgate (inverse)
 };
+
+// kShort: s (short_filter.cuh) of vector i of the raw row x of nv vectors, or the raw vector when `on` is false.  The
+// neighbours are vectors i - 1 and i + 1 of the same row (an L1 / L2 hit: the neighbouring threads load them); L is a
+// multiple of 8, so no vector straddles the end of the sequence, and positions beyond it are zero.
+template <int kFmt>
+DEVINL uint4 short_vec(const uint4* x, int i, int nv, const Taps& t, bool on) {
+  if (!on) return __ldg(x + i);
+  const uint4 z = make_uint4(0u, 0u, 0u, 0u);
+  return short8<kFmt>(i > 0 ? __ldg(x + i - 1) : z, __ldg(x + i), i + 1 < nv ? __ldg(x + i + 1) : z, t);
+}
 
 // v += z * exp(-2 pi i e8 / 8)   (e8 = eighths of a turn, a compile-time constant after unrolling)
 DEVINL void rot_acc(int e8, f32x2 zr, f32x2 zi, f32x2& vr, f32x2& vi) {
@@ -150,14 +162,30 @@ DEVINL void readahead_planes(const OuterParams& p, bool inverse) {
 }
 
 // forward: grid (M / (kVec*blockDim.x), H, pairs)   [kPlanes: (rows, M / (kVec*blockDim.x), 1)]
-template <int R, bool kGated, bool kPlanes, int kFmt>
+// kShort (level 0): u and pregate are the raw tensors, filtered on load (bffc_fwd_short_strided)
+template <int R, bool kGated, bool kPlanes, int kFmt, bool kShort = false>
 __global__ void __launch_bounds__(128, (R <= 4) ? 4 : 2) fwd_kernel(const OuterParams p) {
+  static_assert(!(kShort && kPlanes), "the short filter applies to the real endpoint");
   const int kM = p.M;
   const int np = ((kPlanes ? blockIdx.y : blockIdx.x) * blockDim.x + threadIdx.x) * kVec;   // n'
   const int h = blockIdx.y, pr = blockIdx.z;
   const int b0 = 2 * pr, b1 = 2 * pr + 1;
   const size_t c8 = size_t(p.h0 + h) * (p.L / kVec);            // channel offset inside a batch member
   if (kPlanes) readahead_planes<R>(p, false); else readahead_level0<R, kGated>(p, false);
+  // kShort: a block works on one channel; its taps live in shared memory rather than in registers next to z
+  __shared__ Taps s_taps[kShort ? 2 : 1];
+  if constexpr (kShort) {
+    if (threadIdx.x == 0 && p.sf.u.w) s_taps[0] = load_taps(p.sf.u, p.sf, p.h0 + h);
+    if (threadIdx.x == 1 && kGated && p.sf.pre.w) s_taps[1] = load_taps(p.sf.pre, p.sf, p.h0 + h);
+    __syncthreads();
+  }
+  const Taps& ta = s_taps[0];
+  const Taps& tp = s_taps[kShort ? 1 : 0];
+  // vector o = c8 + n / 8 of member b of a real endpoint (kShort: filtered, when `on`)
+  auto load_x = [&](const uint4* x, long long bs, int b, size_t o, const Taps& t, bool on) -> uint4 {
+    if constexpr (kShort) return short_vec<kFmt>(x + b * bs + c8, int(o - c8), p.L / kVec, t, on);
+    else return __ldg(x + b * bs + o);
+  };
   f32x2 zr[R][4], zi[R][4];
   int rows = 0;
 #pragma unroll
@@ -171,12 +199,13 @@ __global__ void __launch_bounds__(128, (R <= 4) ? 4 : 2) fwd_kernel(const OuterP
     } else if (n < p.L) {
       rows = a + 1;
       const size_t o = c8 + n / kVec;
-      uint4 v0 = __ldg(p.u + b0 * p.u_bs + o);
-      if (kGated) v0 = hmul8<kFmt>(v0, __ldg(p.pregate + b0 * p.pregate_bs + o));
+      const bool fu = kShort && p.sf.u.w, fp = kShort && p.sf.pre.w;
+      uint4 v0 = load_x(p.u, p.u_bs, b0, o, ta, fu);
+      if (kGated) v0 = hmul8<kFmt>(v0, load_x(p.pregate, p.pregate_bs, b0, o, tp, fp));
       unpack8v<kFmt>(v0, zr[a]);
       if (b1 < p.B) {
-        uint4 v1 = __ldg(p.u + b1 * p.u_bs + o);
-        if (kGated) v1 = hmul8<kFmt>(v1, __ldg(p.pregate + b1 * p.pregate_bs + o));
+        uint4 v1 = load_x(p.u, p.u_bs, b1, o, ta, fu);
+        if (kGated) v1 = hmul8<kFmt>(v1, load_x(p.pregate, p.pregate_bs, b1, o, tp, fp));
         unpack8v<kFmt>(v1, zi[a]);
       } else {
 #pragma unroll
@@ -221,8 +250,10 @@ __global__ void __launch_bounds__(128, (R <= 4) ? 4 : 2) fwd_kernel(const OuterP
 }
 
 // inverse: same grid
-template <int R, bool kGated, bool kPlanes, int kFmt>
+// kShort (level 0, gated): the postgate is the raw tensor, filtered where the output is multiplied by it
+template <int R, bool kGated, bool kPlanes, int kFmt, bool kShort = false>
 __global__ void __launch_bounds__(128, (R <= 4) ? 4 : 2) inv_kernel(const OuterParams p) {
+  static_assert(!kShort || (kGated && !kPlanes), "the short filter applies to the gated real endpoint");
   const int kM = p.M;
   const int np = ((kPlanes ? blockIdx.y : blockIdx.x) * blockDim.x + threadIdx.x) * kVec;
   const int h = blockIdx.y, pr = blockIdx.z;
@@ -246,6 +277,13 @@ __global__ void __launch_bounds__(128, (R <= 4) ? 4 : 2) inv_kernel(const OuterP
     }
     __syncthreads();
   }
+  __shared__ Taps s_tq[1];                    // kShort: the block's channel's postgate taps
+  const bool fq = kShort && p.sf.post.w;
+  if constexpr (kShort) {
+    if (threadIdx.x == 0 && fq) s_tq[0] = load_taps(p.sf.post, p.sf, p.h0 + h);
+    __syncthreads();
+  }
+  const Taps& tq = s_tq[0];
   f32x2 w1c[4], w1s[4];                      // conj twiddle: exp(+2 pi i (n'+t) / N)
   float2 stepc[8];
 #pragma unroll
@@ -297,11 +335,19 @@ __global__ void __launch_bounds__(128, (R <= 4) ? 4 : 2) inv_kernel(const OuterP
         continue;
       }
       if (p.y2) rows[2][o] = hmul8<kFmt>(v0, __ldg(rows[3] + o));
-      rows[0][o] = hmul8<kFmt>(v0, __ldg(rows[1] + o));
+      if constexpr (kShort) {
+        rows[0][o] = hmul8<kFmt>(v0, short_vec<kFmt>(rows[1], o, p.L / kVec, tq, fq));
+      } else {
+        rows[0][o] = hmul8<kFmt>(v0, __ldg(rows[1] + o));
+      }
       if (b1 < p.B) {
         const uint4 v1 = pack8v<kFmt>(yi);
         if (p.y2) rows[6][o] = hmul8<kFmt>(v1, __ldg(rows[7] + o));
-        rows[4][o] = hmul8<kFmt>(v1, __ldg(rows[5] + o));
+        if constexpr (kShort) {
+          rows[4][o] = hmul8<kFmt>(v1, short_vec<kFmt>(rows[5], o, p.L / kVec, tq, fq));
+        } else {
+          rows[4][o] = hmul8<kFmt>(v1, __ldg(rows[5] + o));
+        }
       }
     }
   }

@@ -15,6 +15,7 @@
 //    the twiddles and k_f ("engine order", frequency k = k1 + 128*k2).  No intermediate touches HBM.
 #pragma once
 #include "ptx.cuh"
+#include "short_filter.cuh"
 #include <cuda.h>
 #include <cuda_fp16.h>
 
@@ -40,6 +41,10 @@ struct FwdParams {
   int tw_n, tw_mask;         // stage-1 twiddles W_{tw_n}^{(k1 & tw_mask) j}: 8192 / 127, small sizes N / (N/64 - 1)
   int units;                 // H * pairs
   uint32_t kf_conj_mask;     // 0x80008000: multiply by conj(k_f) (du path of the backward: correlation), else 0
+};
+// parameters of the fused kernel's kShort instantiations: the short filter taps of u, pregate, postgate (short_filter.cuh)
+struct FwdShortParams : FwdParams {
+  ShortParams sf;
 };
 
 namespace r128 {

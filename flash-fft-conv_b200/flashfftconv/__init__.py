@@ -1,4 +1,4 @@
 from .conv import FlashFFTConv  # noqa: F401  (reference flashfftconv/__init__.py:1)
 from .depthwise_1d import FlashDepthWiseConv1d  # noqa: F401  (reference flashfftconv/__init__.py:2)
-from .gated import gated_long_conv, hyena_mixer  # noqa: F401
+from .gated import gated_long_conv, hyena_mixer, hyena_operator  # noqa: F401
 from .sparse_conv import PartialFFTConv, FrequencySparseFFTConv  # noqa: F401  (reference flashfftconv/sparse_conv.py)

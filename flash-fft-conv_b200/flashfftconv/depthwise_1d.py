@@ -62,35 +62,46 @@ def _check(u, weights, bias, padding, is_bhl):
     return B, D, L, K
 
 
+def _forward(u, weights, bias, padding, is_bhl=True):
+    """(y, shape) of one bffc_dwconv1d_fwd launch; shape = (B, D, L, K, padding, layout) is what _backward takes."""
+    padding = int(padding)
+    B, D, L, K = _check(u, weights, bias, padding, is_bhl)
+    Lout = L + 2 * padding - K + 1
+    layout = _lib.BFFC_LAYOUT_BHL if is_bhl else _lib.BFFC_LAYOUT_BLH
+    with _on_device(u.device):
+        y = torch.empty((B, D, Lout) if is_bhl else (B, Lout, D), dtype=u.dtype, device=u.device)
+        _lib.check(_lib.lib().bffc_dwconv1d_fwd(_ptr(u), _DT[u.dtype], _ptr(weights), _ptr(bias), _DT[weights.dtype],
+                                                _ptr(y), B, D, L, K, padding, layout, _stream()))
+    return y, (B, D, L, K, padding, layout)
+
+
+def _backward(dout, u, weights, bias, shape):
+    """(du, dw, dbias) of the bffc_dwconv1d_bwd launches; dout must be contiguous."""
+    B, D, L, K, padding, layout = shape
+    with _on_device(u.device):
+        du = torch.empty_like(u)
+        dw = torch.empty_like(weights)
+        dbias = torch.empty_like(bias)
+        nws = _lib.lib().bffc_dwconv1d_workspace_bytes(B, D, L, K, padding, layout)
+        ws = torch.empty(nws, dtype=torch.uint8, device=u.device)
+        _lib.check(_lib.lib().bffc_dwconv1d_bwd(_ptr(dout), _ptr(u), _DT[u.dtype], _ptr(weights), _DT[weights.dtype],
+                                                _ptr(du), _ptr(dw), _ptr(dbias), B, D, L, K, padding, layout,
+                                                _ptr(ws), nws, _stream()))
+    return du, dw, dbias
+
+
 class DepthWiseConv1dFunc(torch.autograd.Function):
     @staticmethod
     def forward(ctx, u, weights, bias, padding, is_bhl=True):
-        padding = int(padding)
-        B, D, L, K = _check(u, weights, bias, padding, is_bhl)
-        Lout = L + 2 * padding - K + 1
-        layout = _lib.BFFC_LAYOUT_BHL if is_bhl else _lib.BFFC_LAYOUT_BLH
-        with _on_device(u.device):
-            y = torch.empty((B, D, Lout) if is_bhl else (B, Lout, D), dtype=u.dtype, device=u.device)
-            _lib.check(_lib.lib().bffc_dwconv1d_fwd(_ptr(u), _DT[u.dtype], _ptr(weights), _ptr(bias), _DT[weights.dtype],
-                                                    _ptr(y), B, D, L, K, padding, layout, _stream()))
-        ctx.shape = (B, D, L, K, padding, layout)
+        y, ctx.shape = _forward(u, weights, bias, padding, is_bhl)
         ctx.save_for_backward(u, weights, bias)
         return y
 
     @staticmethod
     def backward(ctx, dout):
         u, weights, bias = ctx.saved_tensors
-        B, D, L, K, padding, layout = ctx.shape
         dout = dout.contiguous()                                      # reference depthwise_1d.py:19
-        with _on_device(u.device):
-            du = torch.empty_like(u)
-            dw = torch.empty_like(weights)
-            dbias = torch.empty_like(bias)
-            nws = _lib.lib().bffc_dwconv1d_workspace_bytes(B, D, L, K, padding, layout)
-            ws = torch.empty(nws, dtype=torch.uint8, device=u.device)
-            _lib.check(_lib.lib().bffc_dwconv1d_bwd(_ptr(dout), _ptr(u), _DT[u.dtype], _ptr(weights), _DT[weights.dtype],
-                                                    _ptr(du), _ptr(dw), _ptr(dbias), B, D, L, K, padding, layout,
-                                                    _ptr(ws), nws, _stream()))
+        du, dw, dbias = _backward(dout, u, weights, bias, ctx.shape)
         return du, dw, dbias, None, None
 
 

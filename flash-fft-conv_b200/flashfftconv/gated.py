@@ -17,10 +17,16 @@ and writes such slices in place (bffc_fwd_strided / bffc_bwd_strided: rows conti
 multiple of 8 elements), so neither function copies them; a view that does not qualify (conv.batch_stride) is copied
 to a contiguous tensor first, with the same result.  `hyena_mixer` also writes the three gate / input gradients
 straight into one (B, 3H, L) gradient of the projection, so its backward does not concatenate them either.
+
+`hyena_operator` also runs the short depthwise filter that produces the projection's three slices
+(x1x2v = short_filter(in_proj(u))) inside the engine's loads, so the filtered (B, 3H, L) tensor is neither written nor
+read back in the forward, nor kept for the backward.
 """
 import torch
 
+from . import _lib
 from . import conv as _conv
+from . import depthwise_1d as _dw
 
 
 def gated_long_conv(conv, v, k, x1, x2):
@@ -59,17 +65,22 @@ class HyenaMixerFunc(torch.autograd.Function):
     @staticmethod
     def backward(ctx, dout):
         x1x2v, kf, kf2 = ctx.saved_tensors
-        mod, D = ctx.mod, ctx.d_model
-        x1, x2, v = x1x2v.split(D, dim=1)
-        grad = torch.empty_like(x1x2v, memory_format=torch.contiguous_format)
-        dx1, dx2, dv = grad.split(D, dim=1)
-        # u = v, pregate = x1, postgate = x2: du -> [:, 2D:], dpregate -> [:, :D], dpostgate -> [:, D:2D]
-        _, dk, _, _ = _conv._bwd(mod, dout, v, kf, ctx.k_len, x1, x2, out=(dv, dx1, dx2))
-        dk2 = None
-        if kf2 is not None:
-            dv2, dk2, _, _ = _conv._bwd(mod, dout, v, kf2, ctx.k2_len, None, None)
-            dv.add_(dv2)
+        grad, dk, dk2 = _mixer_backward(ctx.mod, ctx.d_model, dout, x1x2v, kf, ctx.k_len, kf2, ctx.k2_len)
         return grad, dk, dk2, None, None
+
+
+def _mixer_backward(mod, D, dout, x1x2v, kf, k_len, kf2, k2_len):
+    """(d x1x2v, dk, dk2) of y = x2 * conv(x1 * v, k) [+ conv(v, k2)]; d x1x2v is one contiguous (B, 3D, L) tensor."""
+    x1, x2, v = x1x2v.split(D, dim=1)
+    grad = torch.empty_like(x1x2v, memory_format=torch.contiguous_format)
+    dx1, dx2, dv = grad.split(D, dim=1)
+    # u = v, pregate = x1, postgate = x2: du -> [:, 2D:], dpregate -> [:, :D], dpostgate -> [:, D:2D]
+    _, dk, _, _ = _conv._bwd(mod, dout, v, kf, k_len, x1, x2, out=(dv, dx1, dx2))
+    dk2 = None
+    if kf2 is not None:
+        dv2, dk2, _, _ = _conv._bwd(mod, dout, v, kf2, k2_len, None, None)
+        dv.add_(dv2)
+    return grad, dk, dk2
 
 
 def hyena_mixer(conv, x1x2v, k, d_model, residual_filter=None):
@@ -83,3 +94,122 @@ def hyena_mixer(conv, x1x2v, k, d_model, residual_filter=None):
     its input gradient is added into the v slice of that gradient with one add.  Like gated_long_conv, this calls the
     engine directly rather than conv(...): forward hooks registered on the module do not run for it."""
     return HyenaMixerFunc.apply(x1x2v, k, residual_filter, conv, d_model)
+
+
+# the short filter runs inside the engine's loads for kernel sizes up to this, and for seqlen below FUSED_SEQLEN_LIMIT
+# (1M..4M use the tensor-core outer stage, which does not take it)
+FUSED_MAX_KERNEL_SIZE = 4
+FUSED_SEQLEN_LIMIT = 1 << 20
+
+
+def _short_fused(conv, short_filter, x):
+    """True when hyena_operator runs as one fused forward; otherwise it is short_filter(x) followed by hyena_mixer."""
+    L = x.shape[-1]
+    return (short_filter.k <= FUSED_MAX_KERNEL_SIZE and conv.seqlen < FUSED_SEQLEN_LIMIT
+            and L % conv.plan(x.device).length_multiple == 0)
+
+
+class ShortHyenaFunc(torch.autograd.Function):
+    """y = s_x2 * conv(s_x1 * s_v, k) [+ conv(s_v, k2)] with s = short(x), s_x1, s_x2, s_v = s.split(D, dim=1).
+
+    Forward: one bffc_fwd_short_strided call (one more for k2) on the raw projection; s is never materialised.  Saved for
+    backward: x, the filter spectra and the short filter's parameters.  Backward: s is recomputed (bffc_dwconv1d_fwd),
+    the mixer's backward runs on it into one (B, 3D, L) gradient of s, and bffc_dwconv1d_bwd turns that into the
+    gradients of x, the taps and the bias."""
+
+    @staticmethod
+    def forward(ctx, x, weights, bias, k, k2, mod, d_model, padding):
+        D, K, P = d_model, weights.shape[1], padding
+        if _conv.batch_stride(x, mod.dtype) is None:
+            x = x.contiguous()
+        B, _, L = x.shape
+        x1, x2, v = x.split(D, dim=1)
+        bs = x.stride(0)
+        w1, w2, wv = weights.split(D)            # rows of a contiguous (3D, K) weight: plain pointer offsets
+        b1, b2, bv = bias.split(D)
+        wdt = _dw._DT[weights.dtype]
+        plan = mod.plan(x.device)
+        with _conv._on_device(x.device):
+            mod.__dict__['last_launches'] = 0
+            kf = _conv._kf_engine_for(mod, plan, k)
+            launches = mod.last_launches
+
+            def call(y, ws, ws_bytes, kf_engine, gated):
+                g = (lambda t: _conv._ptr(t if gated else None))
+                _lib.check(_lib.lib().bffc_fwd_short_strided(
+                    plan.handle, _conv._ptr(v), bs, _conv._ptr(kf_engine), g(x1), bs if gated else 0, g(x2),
+                    bs if gated else 0, _conv._ptr(y), D * L, B, D, L, _conv._ptr(wv), _conv._ptr(bv), g(w1), g(b1),
+                    g(w2), g(b2), wdt, K, P, _conv._ptr(ws), ws_bytes, _conv._stream()))
+                return _lib.lib().bffc_last_launch_count()
+
+            y = torch.empty((B, D, L), dtype=x.dtype, device=x.device)
+            ws, ws_bytes = _conv._workspace(plan, B, D, L, True, False, x.device)
+            launches += call(y, ws, ws_bytes, kf, True)
+            kf2 = None
+            if k2 is not None:
+                mod.__dict__['last_launches'] = 0
+                kf2 = _conv._kf_engine_for(mod, plan, k2)
+                launches += mod.last_launches
+                y2 = torch.empty((B, D, L), dtype=x.dtype, device=x.device)
+                ws, ws_bytes = _conv._workspace(plan, B, D, L, False, False, x.device)
+                launches += call(y2, ws, ws_bytes, kf2, False)
+                y.add_(y2)
+        mod.__dict__['last_launches'] = launches
+        ctx.mod, ctx.d_model, ctx.padding = mod, D, P
+        ctx.k_len = k.shape[-1]
+        ctx.k2_len = None if k2 is None else k2.shape[-1]
+        if any(ctx.needs_input_grad[:5]):
+            ctx.save_for_backward(x, weights, bias, kf, kf2)
+        return y
+
+    @staticmethod
+    def backward(ctx, dout):
+        x, weights, bias, kf, kf2 = ctx.saved_tensors
+        L = x.shape[-1]
+        s, shape = _dw._forward(x, weights, bias, ctx.padding, True)
+        Lout = s.shape[-1]
+        # padding = K - 1 (the original models): nn.Conv1d gives L + K - 1 outputs, of which the mixer uses the first L.
+        # Those slices do not qualify for in-place use and are copied, and the gradient of s is zero-extended: both
+        # costs fall on the backward only.
+        grad, dk, dk2 = _mixer_backward(ctx.mod, ctx.d_model, dout, s if Lout == L else s[..., :L], kf, ctx.k_len, kf2,
+                                        ctx.k2_len)
+        if Lout != L:
+            grad = torch.nn.functional.pad(grad, (0, Lout - L))
+        dx, dw, dbias = _dw._backward(grad, x, weights, bias, shape)
+        return dx, dw, dbias, dk, dk2, None, None, None
+
+
+def hyena_operator(conv, short_filter, x, k, d_model, residual_filter=None):
+    """The whole Hyena / M2 sequence mixer from the raw (B, 3*d_model, L) projection x (the output of in_proj):
+
+        s = short_filter(x)[..., :L];  x1, x2, v = s.split(d_model, dim=1)
+        y = x2 * conv(x1 * v, k) [+ conv(v, k2)]
+
+    short_filter: a BHL FlashDepthWiseConv1d(3 * d_model, K, padding) with 2 * padding >= K - 1 (so that it produces at
+    least L outputs: padding = (K - 1) // 2 as in the flash examples, or K - 1 followed by [..., :L] as in the original
+    models); its `weights` and `bias` receive gradients, as do x, k and the residual filter k2.
+
+    For K <= 4, seqlen < 1M and L a multiple of bffc_length_multiple, the forward is one engine call (two with k2) that
+    applies the short filter where the kernels load x1, x2 and v: s is not written to memory, and not kept for the
+    backward, which recomputes it.  Results are bit for bit those of short_filter followed by hyena_mixer, which is what
+    every other call runs.  Like hyena_mixer, the call goes to the engine directly: forward hooks on `conv` and
+    `short_filter` do not run for it."""
+    if not isinstance(short_filter, _dw.FlashDepthWiseConv1d) or not short_filter.is_bhl:
+        raise RuntimeError('short_filter must be a BHL FlashDepthWiseConv1d')
+    if short_filter.d != 3 * d_model:
+        raise RuntimeError(f'short_filter has {short_filter.d} channels, the projection needs 3 * d_model = {3 * d_model}')
+    K, P = short_filter.k, int(short_filter.padding)
+    if 2 * P < K - 1:
+        raise RuntimeError(f'short filter padding {P} < (K - 1) / 2 for K={K}: it would produce fewer than L outputs')
+    if x.dim() != 3 or x.shape[1] != 3 * d_model:
+        raise RuntimeError(f'x must be (B, 3 * d_model = {3 * d_model}, L), got {tuple(x.shape)}')
+    L = x.shape[-1]
+    if not _short_fused(conv, short_filter, x):
+        return hyena_mixer(conv, short_filter(x)[..., :L], k, d_model, residual_filter)
+    w, b = short_filter.weights, short_filter.bias
+    x1, x2, v = x.split(d_model, dim=1)
+    _conv._check_inputs(v, k, conv, (x1, x2), views=True)
+    if residual_filter is not None:
+        _conv._check_inputs(v, residual_filter, conv, views=True)
+    _dw._check(x, w, b, P, True)
+    return ShortHyenaFunc.apply(x, w, b, k, residual_filter, conv, d_model, P)

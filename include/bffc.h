@@ -192,6 +192,29 @@ int bffc_bwd_strided(const bffc_plan* plan, const void* dout, int64_t dout_bstri
                      void* workspace, size_t workspace_bytes, void* stream);
 
 /*
+ * bffc_fwd_strided with the Hyena / M2 short filter applied to its tensors as the kernels load them: each of u, pregate
+ * and postgate is replaced by
+ *
+ *     s[b, h, l] = bias[h] + sum_{j<K} w[h, j] * x[b, h, l - P + j]      (x = 0 outside [0, L)),  0 <= l < L
+ *
+ * the first L outputs of torch.nn.Conv1d(H, H, K, groups=H, padding=P) (bffc_dwconv1d_fwd, BHL), with the same rounding:
+ * an fp32 accumulation from the bias, taps in ascending order, rounded once to the plan dtype.  The result is bit for bit
+ * bffc_fwd_strided on the outputs of bffc_dwconv1d_fwd.  s is zero beyond L (implicit padding of s, not of x).
+ * *_w: (H, K) taps, *_bias: (H), contiguous device memory of w_dtype (BF16, FP16 or FP32); NULL taps = no short filter on
+ * that tensor, NULL bias = bias 0.  Rows of one (3H, K) weight are plain pointer offsets.  1 <= K <= 4,
+ * (K - 1) / 2 <= padding <= K - 1 (2P >= K - 1: nn.Conv1d produces at least L outputs).  Arguments are validated before the
+ * device is looked at.  Strides, workspace and launch count are those of bffc_fwd_strided.  Without gates, u is still
+ * filtered (a residual filter on the v slice).  Seqlens of the tensor-core outer stage (1M, 2M, 4M) return
+ * BFFC_ERR_UNSUPPORTED.
+ */
+int bffc_fwd_short_strided(const bffc_plan* plan, const void* u, int64_t u_bstride, const void* kf_engine,
+                           const void* pregate, int64_t pregate_bstride, const void* postgate, int64_t postgate_bstride,
+                           void* y, int64_t y_bstride, int B, int H, int L, const void* u_w, const void* u_bias,
+                           const void* pregate_w, const void* pregate_bias, const void* postgate_w,
+                           const void* postgate_bias, int w_dtype, int K, int padding, void* workspace,
+                           size_t workspace_bytes, void* stream);
+
+/*
  * Forward on HOST buffers (the reference has no counterpart: its user writes u.cuda() -> conv -> y.cpu(),
  * README.md:108-149, three serial steps on one stream).  u_host, pregate_host, postgate_host, y_host: (B, H, L)
  * contiguous host memory of the plan dtype — page-locked for the copies to overlap; kf_engine: DEVICE, from
