@@ -4,7 +4,8 @@
 // Same algorithm and stage list as r128_common.cuh.  A pipeline owns one unit (a sequence pair of one channel) at a
 // time; its two warpgroups hold rows 0..63 / 64..127 of every stage's accumulator in registers.  The two pipelines of
 // a CTA share the tensor cores: while one runs a CUDA-core pass the other's MMAs execute.  Shared memory (227 KB per
-// block): 2 pipelines x 2 slots of (re, im) tiles, the DFT-128 operand image and the DFT-64 tiles.  A slot holds the
+// block): 2 pipelines x 2 slots of (re, im) tiles, the DFT-128 operand image, the DFT-64 tiles and the stage-1 twiddle
+// table (loop-invariant per-thread state kept out of the 128 registers a thread has).  A slot holds the
 // unit's input tiles (stage-1 B operand), then the Y tiles (stage-4 B operand), then the output tiles (TMA store);
 // the radix-64 stages take their A operand from registers.  Ungated, the other slot receives the next unit's tiles.
 //
@@ -28,7 +29,9 @@ constexpr int kPipes3 = 2;
 constexpr int kThreads3 = kPipes3 * kPipeThreads;
 constexpr int kSmemData3 = kPipes3 * 2 * kSlotBytes;
 constexpr int kSmemBars3 = 128;
-constexpr int kSmemTotal3 = kSmemData3 + kSmemF + kSmemG + kSmemBars3 + 1024;
+constexpr int kSmemTwSt3 = 128 * 8;             // (stc, sts) of every row (RowTw::store); the (bc, bs) part of the
+                                                // table takes the fourth DFT-64 plane, which no stage reads
+constexpr int kSmemTotal3 = kSmemData3 + kSmemF + kSmemG + kSmemBars3 + kSmemTwSt3 + 1024;
 static_assert(kSmemTotal3 <= 227 * 1024, "shared memory per block");
 
 struct GateMaps { CUtensorMap pre, post, post2, y2, xg; };
@@ -102,10 +105,13 @@ fwd3_kernel(const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CU
   const uint32_t s_f = sbase + kSmemData3;
   const uint32_t s_g = s_f + kSmemF;
   const uint32_t s_bars = s_g + kSmemG;
+  const uint32_t s_twb = s_g + 3 * kGTileBytes;    // stage-1 twiddle table (RowTw::store)
+  const uint32_t s_tws = s_bars + kSmemBars3;
 
   const int tid = threadIdx.x;
+  // warp-uniform by construction, so that the addresses and wgmma descriptors built from them live in uniform registers
   const int pipe = __shfl_sync(0xffffffffu, tid >> 8, 0);
-  const int hf = (tid >> 7) & 1;       // row half of the unit
+  const int hf = __shfl_sync(0xffffffffu, (tid >> 7) & 1, 0);   // row half of the unit
   const int ptid = tid & 255;
   const bool leader = ptid == 0;       // issues this pipeline's TMA loads / stores (bulk groups are per thread)
   const FragPos fp(tid);
@@ -171,18 +177,30 @@ fwd3_kernel(const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CU
     }
   };
   // Everything the first stage needs from global memory is requested up front and lands while the tables below are
-  // built: the first unit's tiles (TMA), the DFT-64 tiles (one bulk copy, needed before the first stage 2 only).
+  // built: the first unit's tiles (TMA), the three DFT-64 tiles the stages read (one bulk copy, needed before the first
+  // stage 2 only).
   if (leader && u_begin < u_end) issue_load(u_begin, 0);
   if (tid == 0) {
-    mbar_expect_tx(bar_g, kSmemG);
-    for (int c = 0; c < kSmemG; c += 8192) bulk_load(s_g + c, reinterpret_cast<const uint8_t*>(p.gtiles) + c, 8192, bar_g);
+    mbar_expect_tx(bar_g, 3 * kGTileBytes);
+    for (int c = 0; c < 3 * kGTileBytes; c += 8192)
+      bulk_load(s_g + c, reinterpret_cast<const uint8_t*>(p.gtiles) + c, 8192, bar_g);
   }
   load_dft128(gen_base + kSmemData3, p.dftC, p.dftS, tid, kThreads3);
-  // stage-1 twiddles W_{tw_n}^{(k1 & tw_mask) j} of this thread's two rows (small sizes: N/64-point blocks)
-  RowTw tw[2];
-  const float tw_inv = 1.0f / float(p.tw_n);
-  tw[0].init(fp.r0 & p.tw_mask, fp.q, tw_inv);
-  tw[1].init((fp.r0 + 8) & p.tw_mask, fp.q, tw_inv);
+  // stage-1 twiddles W_{tw_n}^{(k1 & tw_mask) j} of every row (small sizes: N/64-point blocks); the threads of pipeline
+  // 0 cover each (row, column pair) once
+  if (pipe == 0) {
+    const float tw_inv = 1.0f / float(p.tw_n);
+#pragma unroll
+    for (int rr = 0; rr < 2; ++rr) {
+      RowTw t;
+      t.init((fp.r0 + 8 * rr) & p.tw_mask, fp.q, tw_inv);
+      t.store(s_twb, s_tws, fp.r0 + 8 * rr, fp.q);
+    }
+  }
+  auto row_tw = [&](RowTw (&tw)[2]) {
+    tw[0].load(s_twb, s_tws, fp.r0, fp.q);
+    tw[1].load(s_twb, s_tws, fp.r0 + 8, fp.q);
+  };
   fence_proxy_async_smem();             // DFT-128 image: generic stores -> wgmma operand reads
   __syncthreads();
   mbar_wait(bar_g, 0);
@@ -260,7 +278,11 @@ fwd3_kernel(const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CU
     }
 
     // ---------------- pass 1: * W^{k1 j} -> A operand of stage 2
-    twiddle_frag<false>(d, tw, p.tw_scale);
+    {
+      RowTw tw[2];
+      row_tw(tw);
+      twiddle_frag<false>(d, tw, p.tw_scale);
+    }
     frag_to_a<kFmt>(d, are, aim);
     // ---------------- stage 2: D_re = re * Gr + im * (-Gi),  D_im = re * Gi + im * Gr
     r64_stage<kFmt>(d, are, aim, s_g, s_g + 2 * kGTileBytes, s_g + kGTileBytes, s_g);
@@ -295,7 +317,11 @@ fwd3_kernel(const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CU
     wgmma_wait_regs(d);
 
     // ---------------- pass 5: * conj W -> Y tiles in the slot (MN-major B operand of stage 4)
-    twiddle_frag<true>(d, tw, p.tw_scale);
+    {
+      RowTw tw[2];
+      row_tw(tw);
+      twiddle_frag<true>(d, tw, p.tw_scale);
+    }
     pipe_sync();                          // both halves' stage 1 has read X (and the xg store has left the slot)
     frag_store_tile<kFmt>(sX, fp, d);
     publish_smem();

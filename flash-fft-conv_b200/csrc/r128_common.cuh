@@ -91,6 +91,11 @@ DEVINL uint32_t ld_shared_u32(uint32_t addr) {
   asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(addr));
   return v;
 }
+DEVINL uint2 ld_shared_v2(uint32_t addr) {
+  uint2 v;
+  asm volatile("ld.shared.v2.b32 {%0,%1}, [%2];" : "=r"(v.x), "=r"(v.y) : "r"(addr));
+  return v;
+}
 DEVINL void st_shared_u32(uint32_t addr, uint32_t v) { asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(v) : "memory"); }
 
 // DFT-128 cos / sin planes (row-major 128 x 128 in global memory) -> the K-major, 128B-swizzled operand image at `dst`
@@ -211,6 +216,23 @@ struct RowTw {
     sincospif(-2.0f * float(kl * 8) * tw_inv, &sts, &stc);
 #pragma unroll
     for (int e = 0; e < 2; ++e) sincospif(-2.0f * float(kl * (2 * q + e)) * tw_inv, &bs[e], &bc[e]);
+  }
+  // Shared-memory table of a CTA's rows (fused forward kernel): (bc, bs) of row r, column pair q at s_b + (4 r + q) * 16
+  // (a warp reads 512 contiguous bytes), (stc, sts) at s_st + 8 r.  Read at the point of use, the twiddles hold no
+  // registers across the unit loop, and the compiler cannot hoist the 64 products W^{kl j} out of it.
+  DEVINL void store(uint32_t s_b, uint32_t s_st, int r, int q) const {
+    st_shared_v4(s_b + uint32_t(4 * r + q) * 16u, __float_as_uint(bc[0]), __float_as_uint(bs[0]), __float_as_uint(bc[1]),
+                 __float_as_uint(bs[1]));
+    if (q == 0) {
+      st_shared_u32(s_st + uint32_t(r) * 8u, __float_as_uint(stc));
+      st_shared_u32(s_st + uint32_t(r) * 8u + 4u, __float_as_uint(sts));
+    }
+  }
+  DEVINL void load(uint32_t s_b, uint32_t s_st, int r, int q) {
+    const uint4 b = ld_shared_v4(s_b + uint32_t(4 * r + q) * 16u);
+    const uint2 st = ld_shared_v2(s_st + uint32_t(r) * 8u);
+    bc[0] = __uint_as_float(b.x); bs[0] = __uint_as_float(b.y); bc[1] = __uint_as_float(b.z); bs[1] = __uint_as_float(b.w);
+    stc = __uint_as_float(st.x); sts = __uint_as_float(st.y);
   }
 };
 // d *= f_rr * W (kConj: * f_rr * conj W), element-wise over the fragment; f_rr = (c0 + i s0)[rr] is a per-row factor
