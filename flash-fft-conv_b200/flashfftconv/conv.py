@@ -8,7 +8,7 @@ Drop-in for `flashfftconv.FlashFFTConv` (reference flashfftconv/conv.py:71-560):
 All arithmetic on the hot path happens in libbffc.so (hand-written sm_90a CUDA, C ABI in
 include/bffc.h).  PyTorch is used for device memory and streams only: the filter-side transforms
 (k -> k_f, reference conv.py:575 + :640; dk_f -> dk, conv.py:1817-1820) are the library's own fp32 FFT launches
-for every supported size (bffc_kf_from_filter / bffc_dk_from_dkf) — no library FFT call is left in this module.
+for every supported size (bffc_kf_from_filter_band / bffc_dk_from_dkf_band) — no library FFT call is left in this module.
 
 The filter spectrum in engine order is what forward keeps for backward (the reference keeps its permuted
 k_f, conv.py:587-588), so a training step transforms the filter once; in eval mode it is additionally cached
@@ -94,7 +94,7 @@ class FlashFFTConv(torch.nn.Module):
         d['_plans'] = {}
         d['_host_ws'] = {}
         d['_kf_cache'] = None          # (weakref(k), k._version, device, kf_engine, band)
-        d['last_launches'] = 0         # kernels enqueued by the most recent forward / backward (bench.py)
+        d['last_launches'] = 0         # kernels enqueued by the most recent operator call (bench.py); see _launched
 
     def __getstate__(self):
         state = self.__dict__.copy()
@@ -143,8 +143,8 @@ class FlashFFTConv(torch.nn.Module):
     def forward(self, u, k, pregate=None, postgate=None):
         if pregate is not None or postgate is not None:
             assert pregate is not None and postgate is not None       # conv.py:557-558
-            return GatedFlashFFTConvFunc.apply(u, k, self, pregate, postgate)
-        return FlashFFTConvFunc.apply(u, k, self)
+            return FlashFFTConvFunc.apply(u, k, self, self.training, pregate, postgate)
+        return FlashFFTConvFunc.apply(u, k, self, self.training)
 
 
 def _forward_host(mod, u, k, pregate, postgate, out, device):
@@ -167,6 +167,7 @@ def _forward_host(mod, u, k, pregate, postgate, out, device):
         raise RuntimeError('forward_host: out must be a contiguous host tensor like u')
     plan = mod.plan(device)
     with torch.cuda.device(device):
+        mod.__dict__['last_launches'] = 0
         kf_engine = _kf_engine_for(mod, plan, k if k.is_cuda else k.to(device, non_blocking=True), cache_key=k)
         nws = _lib.lib().bffc_host_workspace_bytes(plan.handle, B, H, L, 1 if gates else 0)
         ws = mod._host_ws.get((device, nws))
@@ -177,8 +178,7 @@ def _forward_host(mod, u, k, pregate, postgate, out, device):
                                       _ptr(out), B, H, L, _ptr(ws), nws, _stream())
         if rc:
             torch.cuda.synchronize(device)     # nothing may still be copying into / out of buffers we are about to drop
-            _lib.check(rc)
-        mod.__dict__['last_launches'] = 1 + _lib.lib().bffc_last_launch_count()
+        _launched(mod, rc)
         # the library joins its internal streams back into the current stream before returning, so the caching
         # allocator (stream-ordered on the current stream) may recycle kf_engine / ws after this point
     return out
@@ -191,8 +191,8 @@ def batch_stride(t, dtype, device_type='cuda'):
     if t.device.type != device_type or t.dtype != dtype or t.dim() != 3:
         return None
     _, H, L = t.shape
-    s = t.stride(0)
-    if (H > 1 and t.stride(1) != L) or (L > 1 and t.stride(2) != 1) or s % 8 or s < H * L or t.data_ptr() % 16:
+    s, sh, sl = t.stride()
+    if (H > 1 and sh != L) or (L > 1 and sl != 1) or s % 8 or s < H * L or t.data_ptr() % 16:
         return None
     return s
 
@@ -236,6 +236,14 @@ def _pack_kf_from_natural(mod, plan, k_f, conj):
     return kf_engine
 
 
+def _launched(mod, rc):
+    """Raise on a library error code, else add the kernels the call enqueued to mod.last_launches.  The count covers the
+    plan-based entry points (filter-side transforms, bffc_fwd*, bffc_bwd*, bffc_fwd_host); each operator call (autograd
+    forward, autograd backward, forward_host) zeroes it once at its start."""
+    _lib.check(rc)
+    mod.__dict__['last_launches'] += _lib.lib().bffc_last_launch_count()
+
+
 def _filter_workspace(plan, H, device):
     n = plan.filter_workspace_bytes(H)
     return (torch.empty(n, dtype=torch.uint8, device=device) if n else None), n
@@ -243,22 +251,18 @@ def _filter_workspace(plan, H, device):
 
 def _pack_kf(mod, plan, k, conj=0, band=None):
     """k (H, Lk) fp32 device -> engine-order packed spectrum (H, N) int32 words by the library's own fp32 FFT
-    (bffc_kf_from_filter): one launch for engine size 8192, column + row FFT launches per L2-sized channel group for
-    the composite sizes (replaces conv.py:575 + :640).  band: None for the full spectrum, else the band limit of
-    bffc_kf_from_filter_band (frequencies with min(f, seqlen - f) >= band are zeroed)."""
+    (bffc_kf_from_filter_band): one launch for engine size 8192, column + row FFT launches per L2-sized channel group
+    for the composite sizes (replaces conv.py:575 + :640).  band: None for the full spectrum (band seqlen / 2 + 1 keeps
+    every frequency), else the band limit (frequencies with min(f, seqlen - f) >= band are zeroed)."""
     k32 = k.detach()
     if k32.dtype != torch.float32 or not k32.is_contiguous():
         k32 = k32.to(torch.float32).contiguous()
     H, Lk = k32.shape
     kf_engine = torch.empty((H, plan.fft_size), dtype=torch.int32, device=k.device)
     ws, ws_bytes = _filter_workspace(plan, H, k.device)
-    if band is None:
-        _lib.check(_lib.lib().bffc_kf_from_filter(plan.handle, _ptr(k32), int(Lk), _ptr(kf_engine), int(H), int(conj),
-                                                  _ptr(ws), ws_bytes, _stream()))
-    else:
-        _lib.check(_lib.lib().bffc_kf_from_filter_band(plan.handle, _ptr(k32), int(Lk), _ptr(kf_engine), int(H),
+    band = mod.seqlen // 2 + 1 if band is None else band
+    _launched(mod, _lib.lib().bffc_kf_from_filter_band(plan.handle, _ptr(k32), int(Lk), _ptr(kf_engine), int(H),
                                                        int(conj), int(band), _ptr(ws), ws_bytes, _stream()))
-    mod.__dict__['last_launches'] = _lib.lib().bffc_last_launch_count()
     return kf_engine
 
 
@@ -277,8 +281,8 @@ def _kf_engine_for(mod, plan, k, cache_key=None, band=None, use_cache=None):
     return kf
 
 
-def _pad_len(mod, device, L):
-    q = mod.plan(device).length_multiple
+def _pad_len(plan, L):
+    q = plan.length_multiple
     return (L + q - 1) // q * q
 
 
@@ -310,28 +314,36 @@ class _on_device:
             self.ctx.__exit__(*a)
 
 
-def _fwd(mod, u, k, pregate, postgate, band=None, use_cache=None, kf_engine=None):
+def _fwd(mod, u, k, pregate, postgate, band=None, use_cache=None, kf_engine=None, taps=None):
     """y (contiguous) and the engine-order filter spectrum it used.  u and the gates: any (B, H, L) layout; those that
     qualify (batch_stride) are read in place, others copied.  band / use_cache: see _kf_engine_for; kf_engine: a
-    spectrum of k already at hand."""
-    L0 = u.shape[-1]
-    Lp = _pad_len(mod, u.device, L0)
-    if Lp != L0:
-        y, kf = _fwd(mod, _padded(u, Lp), k, _padded(pregate, Lp), _padded(postgate, Lp), band, use_cache, kf_engine)
-        return y[..., :L0].contiguous(), kf
+    spectrum of k already at hand.  taps: ((u_w, u_bias, pregate_w, pregate_bias, postgate_w, postgate_bias), w_dtype,
+    K, padding), a short depthwise filter bffc_fwd_short_strided applies to u and the gates as it loads them; the rows
+    are device addresses of (H, K) taps and (H) biases, None for a tensor that is not filtered."""
     B, H, L = u.shape
-    plan = mod.plan(u.device)
-    (u, u_bs), (pre, pre_bs), (post, post_bs) = (_engine_view(t, mod.dtype) for t in (u, pregate, postgate))
-    with _on_device(u.device):
-        mod.__dict__['last_launches'] = 0
+    dev = u.device
+    plan = mod.plan(dev)
+    Lp = _pad_len(plan, L)
+    if Lp != L:
+        if taps is not None:       # the filter's bias would reach past L: padding the input is not padding its output
+            raise RuntimeError(f'L={L} must be a multiple of bffc_length_multiple() to fuse a short filter')
+        y, kf = _fwd(mod, _padded(u, Lp), k, _padded(pregate, Lp), _padded(postgate, Lp), band, use_cache, kf_engine)
+        return y[..., :L].contiguous(), kf
+    (u, u_bs), (pre, pre_bs), (post, post_bs) = [_engine_view(t, mod.dtype) for t in (u, pregate, postgate)]
+    with _on_device(dev):
         if kf_engine is None:
             kf_engine = _kf_engine_for(mod, plan, k, band=band, use_cache=use_cache)
-        y = torch.empty((B, H, L), dtype=u.dtype, device=u.device)
-        ws, ws_bytes = _workspace(plan, B, H, L, pre is not None, False, u.device)
-        _lib.check(_lib.lib().bffc_fwd_strided(plan.handle, _ptr(u), u_bs, _ptr(kf_engine), _ptr(pre), pre_bs,
-                                               _ptr(post), post_bs, _ptr(y), H * L, B, H, L, _ptr(ws), ws_bytes,
-                                               _stream()))
-        mod.__dict__['last_launches'] += _lib.lib().bffc_last_launch_count()
+        y = torch.empty((B, H, L), dtype=u.dtype, device=dev)
+        ws, ws_bytes = _workspace(plan, B, H, L, pre is not None, False, dev)
+        if taps is None:
+            rc = _lib.lib().bffc_fwd_strided(plan.handle, _ptr(u), u_bs, _ptr(kf_engine), _ptr(pre), pre_bs, _ptr(post),
+                                             post_bs, _ptr(y), H * L, B, H, L, _ptr(ws), ws_bytes, _stream())
+        else:
+            rows, w_dtype, K, P = taps
+            rc = _lib.lib().bffc_fwd_short_strided(plan.handle, _ptr(u), u_bs, _ptr(kf_engine), _ptr(pre), pre_bs,
+                                                   _ptr(post), post_bs, _ptr(y), H * L, B, H, L, *rows, w_dtype, K, P,
+                                                   _ptr(ws), ws_bytes, _stream())
+        _launched(mod, rc)
     return y, kf_engine
 
 
@@ -340,20 +352,19 @@ def _bwd(mod, dout, u, kf_engine, k_len, pregate, postgate, band=None, out=None)
     band limit (None: full spectrum); kf_engine is then the band-limited spectrum and dk gets the same mask.  Inputs:
     any (B, H, L) layout, as for _fwd.  out: optional (du, dpregate, dpostgate) tensors to write the gradients into
     (channel slices of one buffer are written in place) and return; otherwise they are new contiguous tensors."""
-    L0 = u.shape[-1]
-    Lp = _pad_len(mod, u.device, L0)
-    if Lp != L0:
+    B, H, L = u.shape
+    plan = mod.plan(u.device)
+    Lp = _pad_len(plan, L)
+    if Lp != L:
         r = _bwd(mod, _padded(dout, Lp), _padded(u, Lp), kf_engine, k_len, _padded(pregate, Lp), _padded(postgate, Lp),
                  band)
-        cut = lambda t: None if t is None else t[..., :L0].contiguous()
+        cut = lambda t: None if t is None else t[..., :L].contiguous()
         res = [cut(r[0]), r[1], cut(r[2]), cut(r[3])]
         for i, o in zip((0, 2, 3), out or ()):
             if o is not None and res[i] is not None:
                 res[i] = o.copy_(res[i])
         return tuple(res)
-    B, H, L = u.shape
-    N = mod.fft_size(u.device)
-    plan = mod.plan(u.device)
+    N = plan.fft_size
     gated = pregate is not None
     (dout, dout_bs), (u, u_bs), (pre, pre_bs), (post, post_bs) = (_engine_view(t, mod.dtype)
                                                                   for t in (dout, u, pregate, postgate))
@@ -371,62 +382,43 @@ def _bwd(mod, dout, u, kf_engine, k_len, pregate, postgate, band=None, out=None)
         dkf_engine = torch.empty((H, N, 2), dtype=torch.float32, device=u.device)
         ws, ws_bytes = _workspace(plan, B, H, L, gated, True, u.device)
         # kf_engine_conj = NULL: the kernels conjugate the forward's spectrum in their pointwise multiply
-        _lib.check(_lib.lib().bffc_bwd_strided(plan.handle, _ptr(dout), dout_bs, _ptr(u), u_bs, _ptr(kf_engine), None,
-                                               _ptr(pre), pre_bs, _ptr(post), post_bs, _ptr(du), du_bs,
-                                               _ptr(dkf_engine), _ptr(dpre), dpre_bs, _ptr(dpost), dpost_bs,
-                                               B, H, L, _ptr(ws), ws_bytes, _stream()))
+        _launched(mod, _lib.lib().bffc_bwd_strided(plan.handle, _ptr(dout), dout_bs, _ptr(u), u_bs, _ptr(kf_engine),
+                                                   None, _ptr(pre), pre_bs, _ptr(post), post_bs, _ptr(du), du_bs,
+                                                   _ptr(dkf_engine), _ptr(dpre), dpre_bs, _ptr(dpost), dpost_bs,
+                                                   B, H, L, _ptr(ws), ws_bytes, _stream()))
         for t, _, o in dst:
             if o is not None:
                 o.copy_(t)
-        mod.__dict__['last_launches'] = _lib.lib().bffc_last_launch_count()
         # the kernels accumulate unnormalised pair-packed spectra in engine order; the reference takes
         # ifft(dk_f).real[..., :k_len] (conv.py:1817-1820): inverse fp32 FFT straight from engine order, 1/N, real part
         # (only the Hermitian part of dk_f contributes), sum over the batch-member blocks of the small sizes, [:k_len]
         dk = torch.empty((H, k_len), dtype=torch.float32, device=u.device)
         fws, fws_bytes = _filter_workspace(plan, H, u.device)
-        if band is None:
-            _lib.check(_lib.lib().bffc_dk_from_dkf(plan.handle, _ptr(dkf_engine), _ptr(dk), int(k_len), H, _ptr(fws),
-                                                   fws_bytes, _stream()))
-        else:
-            _lib.check(_lib.lib().bffc_dk_from_dkf_band(plan.handle, _ptr(dkf_engine), _ptr(dk), int(k_len), H, int(band),
-                                                        _ptr(fws), fws_bytes, _stream()))
-        mod.__dict__['last_launches'] += _lib.lib().bffc_last_launch_count()
+        band = mod.seqlen // 2 + 1 if band is None else band
+        _launched(mod, _lib.lib().bffc_dk_from_dkf_band(plan.handle, _ptr(dkf_engine), _ptr(dk), int(k_len), H,
+                                                        int(band), _ptr(fws), fws_bytes, _stream()))
     du, dpre, dpost = (o if o is not None else t for t, _, o in dst)
     return du, dk, dpre, dpost
 
 
 class FlashFFTConvFunc(torch.autograd.Function):
-    @staticmethod
-    def forward(ctx, u, k, mod):
-        _check_inputs(u, k, mod)
-        y, kf_engine = _fwd(mod, u, k, None, None)
-        ctx.mod = mod
-        ctx.k_len = k.shape[-1]
-        if mod.training:                                              # conv.py:587-588
-            ctx.save_for_backward(u, kf_engine)
-        return y
+    """y = postgate * conv(u * pregate, k), the gates both given or both None.  save: keep what backward reads (the
+    caller's rule: the module's training mode, or whether a gradient is wanted).  band / use_cache: see _kf_engine_for.
+    views: u and the gates may be channel slices or other non-contiguous (B, H, L) layouts (gated_long_conv)."""
 
     @staticmethod
-    def backward(ctx, dout):
-        u, kf_engine = ctx.saved_tensors
-        du, dk, _, _ = _bwd(ctx.mod, dout, u, kf_engine, ctx.k_len, None, None)
-        return du, dk, None                                           # conv.py:1822
-
-
-class GatedFlashFFTConvFunc(torch.autograd.Function):
-    @staticmethod
-    def forward(ctx, u, k, mod, pregate, postgate, views=False):
-        """views=True (gated_long_conv): u and the gates may be channel slices or other non-contiguous layouts."""
-        _check_inputs(u, k, mod, (pregate, postgate), views)
-        y, kf_engine = _fwd(mod, u, k, pregate, postgate)
-        ctx.mod = mod
-        ctx.k_len = k.shape[-1]
-        if mod.training:
+    def forward(ctx, u, k, mod, save, pregate=None, postgate=None, band=None, use_cache=None, views=False):
+        _check_inputs(u, k, mod, () if pregate is None else (pregate, postgate), views)
+        mod.__dict__['last_launches'] = 0
+        y, kf_engine = _fwd(mod, u, k, pregate, postgate, band, use_cache)
+        ctx.mod, ctx.k_len, ctx.band = mod, k.shape[-1], band
+        if save:                                                      # conv.py:587-588
             ctx.save_for_backward(u, kf_engine, pregate, postgate)
         return y
 
     @staticmethod
     def backward(ctx, dout):
         u, kf_engine, pregate, postgate = ctx.saved_tensors
-        du, dk, dpre, dpost = _bwd(ctx.mod, dout, u, kf_engine, ctx.k_len, pregate, postgate)
-        return du, dk, None, dpre, dpost, None                        # conv.py:3939
+        ctx.mod.__dict__['last_launches'] = 0
+        du, dk, dpre, dpost = _bwd(ctx.mod, dout, u, kf_engine, ctx.k_len, pregate, postgate, ctx.band)
+        return du, dk, None, None, dpre, dpost, None, None, None      # conv.py:1822, :3939

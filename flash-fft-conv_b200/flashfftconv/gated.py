@@ -24,7 +24,6 @@ read back in the forward, nor kept for the backward.
 """
 import torch
 
-from . import _lib
 from . import conv as _conv
 from . import depthwise_1d as _dw
 
@@ -33,9 +32,9 @@ def gated_long_conv(conv, v, k, x1, x2):
     """y = x2 * conv(v * x1, k) through FlashFFTConv's fused gates.
 
     conv: a FlashFFTConv module; v, x1, x2: (B, H, L) tensors of conv.dtype (channel slices are read in place); k: (H, Lk)
-    fp32 filter.  Gradients flow to v, k, x1 and x2 (GatedFlashFFTConvFunc).  The call goes to the autograd function,
-    not through conv(...), so forward hooks registered on the module do not run for it."""
-    return _conv.GatedFlashFFTConvFunc.apply(v, k, conv, x1, x2, True)
+    fp32 filter.  Gradients flow to v, k, x1 and x2 (FlashFFTConvFunc).  The call goes to the autograd function, not
+    through conv(...), so forward hooks registered on the module do not run for it."""
+    return _conv.FlashFFTConvFunc.apply(v, k, conv, conv.training, x1, x2, None, None, True)
 
 
 class HyenaMixerFunc(torch.autograd.Function):
@@ -47,14 +46,8 @@ class HyenaMixerFunc(torch.autograd.Function):
         _conv._check_inputs(v, k, mod, (x1, x2), views=True)
         if k2 is not None:
             _conv._check_inputs(v, k2, mod, views=True)     # k2 must be (d_model, Lk <= seqlen), as k
-        y, kf = _conv._fwd(mod, v, k, x1, x2, use_cache=None)
-        launches = mod.last_launches
-        kf2 = None
-        if k2 is not None:
-            y2, kf2 = _conv._fwd(mod, v, k2, None, None)
-            launches += mod.last_launches
-            y.add_(y2)
-        mod.__dict__['last_launches'] = launches
+        mod.__dict__['last_launches'] = 0
+        y, kf, kf2 = _mixer_forward(mod, x1, x2, v, k, k2)
         ctx.mod, ctx.d_model = mod, d_model
         ctx.k_len = k.shape[-1]
         ctx.k2_len = None if k2 is None else k2.shape[-1]
@@ -65,8 +58,32 @@ class HyenaMixerFunc(torch.autograd.Function):
     @staticmethod
     def backward(ctx, dout):
         x1x2v, kf, kf2 = ctx.saved_tensors
+        ctx.mod.__dict__['last_launches'] = 0
         grad, dk, dk2 = _mixer_backward(ctx.mod, ctx.d_model, dout, x1x2v, kf, ctx.k_len, kf2, ctx.k2_len)
         return grad, dk, dk2, None, None
+
+
+def _mixer_forward(mod, x1, x2, v, k, k2, short=None):
+    """(y, kf, kf2) of y = x2 * conv(x1 * v, k) [+ conv(v, k2)] on the slices x1, x2, v of one (B, 3D, L) projection.
+    short: (weights (3D, K), bias (3D), padding) of a short depthwise filter the engine applies to the three slices as
+    it loads them (bffc_fwd_short_strided); the residual call filters only v."""
+    taps = taps2 = None
+    if short is not None:
+        w, b, P = short
+        D, K = v.shape[1], w.shape[1]
+        # the rows of x1, x2, v in the contiguous (3D, K) weight and (3D) bias: plain pointer offsets (a split would
+        # cost several microseconds of host time per call)
+        w1, w2, wv = (w.data_ptr() + i * D * K * w.element_size() for i in range(3))
+        b1, b2, bv = (b.data_ptr() + i * D * b.element_size() for i in range(3))
+        wdt = _dw._DT[w.dtype]
+        taps = ((wv, bv, w1, b1, w2, b2), wdt, K, P)
+        taps2 = ((wv, bv, None, None, None, None), wdt, K, P)
+    y, kf = _conv._fwd(mod, v, k, x1, x2, taps=taps)
+    kf2 = None
+    if k2 is not None:
+        y2, kf2 = _conv._fwd(mod, v, k2, None, None, taps=taps2)
+        y.add_(y2)
+    return y, kf, kf2
 
 
 def _mixer_backward(mod, D, dout, x1x2v, kf, k_len, kf2, k2_len):
@@ -119,43 +136,11 @@ class ShortHyenaFunc(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, x, weights, bias, k, k2, mod, d_model, padding):
-        D, K, P = d_model, weights.shape[1], padding
-        if _conv.batch_stride(x, mod.dtype) is None:
+        if _conv.batch_stride(x, mod.dtype) is None:     # then the slices of the copy qualify: L is a multiple of 8
             x = x.contiguous()
-        B, _, L = x.shape
-        x1, x2, v = x.split(D, dim=1)
-        bs = x.stride(0)
-        w1, w2, wv = weights.split(D)            # rows of a contiguous (3D, K) weight: plain pointer offsets
-        b1, b2, bv = bias.split(D)
-        wdt = _dw._DT[weights.dtype]
-        plan = mod.plan(x.device)
-        with _conv._on_device(x.device):
-            mod.__dict__['last_launches'] = 0
-            kf = _conv._kf_engine_for(mod, plan, k)
-            launches = mod.last_launches
-
-            def call(y, ws, ws_bytes, kf_engine, gated):
-                g = (lambda t: _conv._ptr(t if gated else None))
-                _lib.check(_lib.lib().bffc_fwd_short_strided(
-                    plan.handle, _conv._ptr(v), bs, _conv._ptr(kf_engine), g(x1), bs if gated else 0, g(x2),
-                    bs if gated else 0, _conv._ptr(y), D * L, B, D, L, _conv._ptr(wv), _conv._ptr(bv), g(w1), g(b1),
-                    g(w2), g(b2), wdt, K, P, _conv._ptr(ws), ws_bytes, _conv._stream()))
-                return _lib.lib().bffc_last_launch_count()
-
-            y = torch.empty((B, D, L), dtype=x.dtype, device=x.device)
-            ws, ws_bytes = _conv._workspace(plan, B, D, L, True, False, x.device)
-            launches += call(y, ws, ws_bytes, kf, True)
-            kf2 = None
-            if k2 is not None:
-                mod.__dict__['last_launches'] = 0
-                kf2 = _conv._kf_engine_for(mod, plan, k2)
-                launches += mod.last_launches
-                y2 = torch.empty((B, D, L), dtype=x.dtype, device=x.device)
-                ws, ws_bytes = _conv._workspace(plan, B, D, L, False, False, x.device)
-                launches += call(y2, ws, ws_bytes, kf2, False)
-                y.add_(y2)
-        mod.__dict__['last_launches'] = launches
-        ctx.mod, ctx.d_model, ctx.padding = mod, D, P
+        mod.__dict__['last_launches'] = 0
+        y, kf, kf2 = _mixer_forward(mod, *x.split(d_model, dim=1), k, k2, (weights, bias, padding))
+        ctx.mod, ctx.d_model, ctx.padding = mod, d_model, padding
         ctx.k_len = k.shape[-1]
         ctx.k2_len = None if k2 is None else k2.shape[-1]
         if any(ctx.needs_input_grad[:5]):
@@ -165,6 +150,7 @@ class ShortHyenaFunc(torch.autograd.Function):
     @staticmethod
     def backward(ctx, dout):
         x, weights, bias, kf, kf2 = ctx.saved_tensors
+        ctx.mod.__dict__['last_launches'] = 0
         L = x.shape[-1]
         s, shape = _dw._forward(x, weights, bias, ctx.padding, True)
         Lout = s.shape[-1]

@@ -16,7 +16,7 @@ reach both `x` and `k` as they do through the reference's torch operations, but 
 """
 import torch
 
-from .conv import FlashFFTConv, _bwd, _check_inputs, _fwd
+from .conv import FlashFFTConv, FlashFFTConvFunc
 
 
 class _EngineCache(torch.nn.Module):
@@ -43,27 +43,6 @@ class PartialFFTConv(_EngineCache):
         return self.conv(2 * L, x.dtype, x.device)(x, k[..., : self.N_partial].contiguous())
 
 
-class FrequencySparseFFTConvFunc(torch.autograd.Function):
-    """y = irfft(rfft(x, N) * M * rfft(k, N), N)[..., :L] on the engine `mod` (seqlen N = 2 L), band = N_partial // 2.
-    save: keep x and the masked spectrum for backward (only when a gradient is wanted).  use_cache: reuse the masked
-    spectrum across calls while the same `k` is unmodified (the eval-mode filter cache of FlashFFTConv)."""
-
-    @staticmethod
-    def forward(ctx, x, k, mod, band, save, use_cache):
-        _check_inputs(x, k, mod)
-        y, kf_engine = _fwd(mod, x, k, None, None, band=band, use_cache=use_cache)
-        ctx.mod, ctx.k_len, ctx.band = mod, k.shape[-1], band
-        if save:
-            ctx.save_for_backward(x, kf_engine)
-        return y
-
-    @staticmethod
-    def backward(ctx, dy):
-        x, kf_engine = ctx.saved_tensors
-        dx, dk, _, _ = _bwd(ctx.mod, dy, x, kf_engine, ctx.k_len, None, None, band=ctx.band)
-        return dx, dk, None, None, None, None
-
-
 class FrequencySparseFFTConv(_EngineCache):
     """y = irfft(rfft(x, 2L) * mask(rfft(k, 2L)))[..., :L] with the bins from N_partial // 2 up zeroed
     (reference sparse_conv.py:25-38), trainable: gradients flow to x and to k.
@@ -82,6 +61,6 @@ class FrequencySparseFFTConv(_EngineCache):
         L = x.shape[-1]
         mod = self.conv(2 * L, x.dtype, x.device)
         # the engines sit in a plain dict (no .train() / .eval() reaches them): this module's own mode and the grad
-        # state decide caching and saving
+        # state decide caching and saving (x and the masked spectrum, only when a gradient is wanted)
         save = torch.is_grad_enabled() and (x.requires_grad or k.requires_grad)
-        return FrequencySparseFFTConvFunc.apply(x, k, mod, self.N_partial // 2, save, not self.training)
+        return FlashFFTConvFunc.apply(x, k, mod, save, None, None, self.N_partial // 2, not self.training)

@@ -362,11 +362,20 @@ def test_forward_host_matches_device_path(ffc, N, B, H, L, gated):
     u_h = d['u'].pin_memory()
     g_h = [g.pin_memory() for g in gates]
     out = torch.full(u_h.shape, float('nan'), dtype=torch.bfloat16).pin_memory()
+    lib = ffc._lib.lib()
+    filter_launches = 1 if N <= 8192 else 2              # one channel group at these H
     for _ in range(2):                                   # second call reuses streams, events and the staging workspace
         y = conv.forward_host(u_h, d['k'], *g_h, out=out)
+        assert conv.last_launches == filter_launches + lib.bffc_last_launch_count()
         torch.cuda.current_stream().synchronize()        # asynchronous like every entry point: joined into this stream
         assert y is out
         assert torch.equal(y, y_dev)
+    conv.eval()                                          # the second call finds the filter spectrum cached
+    for want in (filter_launches, 0):
+        conv.forward_host(u_h, d['k'], *g_h, out=out)
+        assert conv.last_launches == want + lib.bffc_last_launch_count()
+    torch.cuda.current_stream().synchronize()
+    assert torch.equal(out, y_dev)
     if B <= 9:
         ref = orc.ref_fft_conv_gated(d['u'], d['k'], *gates, N) if gated else orc.ref_fft_conv(d['u'], d['k'], N)
         _check(y, ref, 'forward_host vs oracle')

@@ -15,6 +15,7 @@
 4. Negative control: perturbing one tap of x1, x2 or v alone changes y.
 5. Fusion: no depthwise kernel in the forward (torch.profiler); forward peak memory above the inputs at least 6*B*D*L
    bytes (the s tensor) below the composition's; no s-sized tensor saved for backward.
+6. Launch counts: forward and backward with a residual filter count both engine calls.
 """
 import pytest
 import torch
@@ -147,6 +148,28 @@ def test_fp64_reference(ffc, N, half, dtype):
         rel = so.rel_l2(got, ref)
         assert stat <= THRESH[(dtype, 'y')], f'N={N} K={K}: spectral error {stat:.3e}'
         assert rel <= REL_L2, f'N={N} K={K}: rel-L2 {rel:.3e}'
+
+
+@pytest.mark.parametrize('N', [8192, 32 * KI])
+def test_launch_counts(ffc, N):
+    """last_launches of the fused hyena_operator with a residual filter, forward and backward, is the sum over the same
+    two engine calls made through FlashFFTConv on the filtered slices (the depthwise launches are not counted)."""
+    D = 4
+    conv, sf, x, k, k2, dout = _make(ffc, N, N, 3, D, 3, 1, torch.bfloat16, torch.float32, seed=2, residual=True)
+    xs, ks, k2s = (t.detach().clone().requires_grad_(True) for t in (x, k, k2))
+    y = ffc.hyena_operator(conv, sf, xs, ks, D, residual_filter=k2s)
+    got = [conv.last_launches]
+    y.backward(dout)
+    got.append(conv.last_launches)
+    with torch.no_grad():
+        x1, x2, v = (t.contiguous().requires_grad_(True) for t in sf(x).split(D, dim=1))
+    want = [0, 0]
+    for args in ((v, ks, x1, x2), (v, k2s)):
+        yr = conv(*args)
+        want[0] += conv.last_launches
+        yr.backward(dout)
+        want[1] += conv.last_launches
+    assert got == want, f'(forward, backward) launches {got}, expected {want}'
 
 
 @pytest.mark.parametrize('N', [1024, 32 * KI])

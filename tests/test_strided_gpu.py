@@ -13,7 +13,8 @@ Hyena / M2 mixer on channel slices of its (B, 3D, L) projection in place (run wi
    projection, forward and backward, bit for bit against the contiguous call.
 4. No copies: hyena_mixer forward + backward launches library kernels and memsets only, as many launches as one gated
    forward + backward of contiguous tensors; a misaligned projection (the copying fallback) does show copy kernels.
-5. Gradients: hyena_mixer with and without residual_filter against autograd through the fp32 reference formula.
+5. Gradients: hyena_mixer with and without residual_filter against autograd through the fp32 reference formula; the
+   backward's launch count is that of FlashFFTConv's backward calls on the same slices (both with a residual filter).
 """
 import ctypes
 
@@ -242,6 +243,7 @@ def test_hyena_mixer_gradients(ffc, N, L, residual):
     y = ffc.hyena_mixer(conv, proj, k, D, residual_filter=k2)
     dout = torch.randn_like(y)
     y.backward(dout)
+    bwd_launches = conv.last_launches
     p32 = proj.detach().float().cpu().requires_grad_(True)
     k32 = k.detach().cpu().requires_grad_(True)
     x1, x2, v = p32.split(D, dim=1)
@@ -255,6 +257,13 @@ def test_hyena_mixer_gradients(ffc, N, L, residual):
     _check(k.grad, k32.grad, 'mixer dk')
     if residual:
         _check(k2.grad, k232.grad, 'mixer dk2')
+    # the backward counts the launches of every engine call it makes: the gated one, and the ungated one with k2
+    x1, x2, v = (t.detach().contiguous().requires_grad_(True) for t in proj.split(D, dim=1))
+    want = 0
+    for args in [(v, k, x1, x2)] + ([(v, k2)] if residual else []):
+        conv(*args).backward(dout)
+        want += conv.last_launches
+    assert bwd_launches == want, (bwd_launches, want)
 
 
 def test_hyena_mixer_checks_residual_filter(ffc):
