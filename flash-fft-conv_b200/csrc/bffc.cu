@@ -226,8 +226,7 @@ struct bffc_plan {
   float dk_scale;        // dk_f: 1 (bf16), rblk * R (fp16)
   int dtype;
   int device;
-  __nv_bfloat16* dftC = nullptr;
-  __nv_bfloat16* dftS = nullptr;
+  __nv_bfloat16* dft = nullptr;   // stage-1 / stage-4 A operand: conjugate-pair rows of the DFT-128, see bffc_plan_create
   uint8_t* gtiles = nullptr;
   float2* tw8192 = nullptr;   // e^{-2 pi i t / 8192}, t < 8192: twiddles of the fp32 filter-side FFTs (filter_fft.cuh)
   float2* tw512 = nullptr;    // composite sizes: e^{-2 pi i t / 512} (column FFTs), W_N^{j} j < 2048, W_N^{2048 i} i < N/2048
@@ -344,21 +343,25 @@ int bffc_plan_create(bffc_plan** out, int seqlen, int dtype) {
   PLAN_TRY(cudaGetDevice(&p->device));
   PLAN_TRY(cudaDeviceGetAttribute(&p->num_sms, cudaDevAttrMultiProcessorCount, p->device));
 
-  // stage-1 DFT of the fused kernel, cos / sin planes (symmetric, K-major rows): F_128, or for the small sizes the
-  // block-diagonal I_{8192/N} (x) F_r, r = N/64 (one block per batch member sharing the unit)
-  std::vector<uint16_t> c(128 * 128), s(128 * 128);
-  const int rblk = p->rblk;
-  for (int m = 0; m < 128; ++m)
+  // stage-1 DFT of the fused kernel (symmetric, K-major rows): F_128, or for the small sizes the block-diagonal
+  // I_{8192/N} (x) F_r, r = N/64 (one block per batch member sharing the unit).  One conjugate-pair image: A row f holds
+  // the cos row and A row f + 8 the sin row of the natural row of conjugate pair p that FragPos (r128_common.cuh) gives
+  // the thread owning fragment rows f, f + 8; for a pair with kk = 0 the cos row of its partner row b r + r/2 instead.
+  std::vector<uint16_t> a(128 * 128);
+  const int rblk = p->rblk, half = rblk / 2;
+  for (int f = 0; f < 128; ++f) {
+    const int slot = (f >> 3) & 1, pr = (f >> 6) * 32 + ((f >> 4) & 3) * 8 + (f & 7);
+    const int b = pr / half, kk = pr % half;
+    const bool sine = slot == 1 && kk != 0;
+    const int m = b * rblk + (slot == 1 && kk == 0 ? half : kk);      // natural row whose cos / sin goes here
     for (int k = 0; k < 128; ++k) {
       const bool same = m / rblk == k / rblk;
       const double ang = 2.0 * kPi * double(((m % rblk) * (k % rblk)) % rblk) / double(rblk);
-      c[m * 128 + k] = f2h16(same ? cos(ang) : 0.0, dtype);
-      s[m * 128 + k] = f2h16(same ? sin(ang) : 0.0, dtype);
+      a[f * 128 + k] = f2h16(same ? (sine ? sin(ang) : cos(ang)) : 0.0, dtype);
     }
-  PLAN_TRY(cudaMalloc(&p->dftC, c.size() * 2));
-  PLAN_TRY(cudaMalloc(&p->dftS, s.size() * 2));
-  PLAN_TRY(cudaMemcpy(p->dftC, c.data(), c.size() * 2, cudaMemcpyHostToDevice));
-  PLAN_TRY(cudaMemcpy(p->dftS, s.data(), s.size() * 2, cudaMemcpyHostToDevice));
+  }
+  PLAN_TRY(cudaMalloc(&p->dft, a.size() * 2));
+  PLAN_TRY(cudaMemcpy(p->dft, a.data(), a.size() * 2, cudaMemcpyHostToDevice));
 
   // DFT-64 planes for the row-local stage: G = exp(-2 pi i k n / 64) = Gr + i Gi.  Stored as the MN-major
   // B operand image: row k (K index) = 64 bf16 = 128 B, 16-byte chunk c of row k at chunk position c ^ (k & 7)
@@ -439,8 +442,7 @@ int bffc_length_multiple(const bffc_plan* p) {
 
 int bffc_plan_destroy(bffc_plan* p) {
   if (!p) return BFFC_OK;
-  cudaFree(p->dftC);
-  cudaFree(p->dftS);
+  cudaFree(p->dft);
   cudaFree(p->gtiles);
   cudaFree(p->tw8192);
   cudaFree(p->tw512);
@@ -690,8 +692,7 @@ static int persistent_grid(const bffc_plan* p, long long units, int per_block) {
 // Stage-1 fields shared by the fused kernel (FwdParams) and the dk_f kernel (DkfParams)
 template <class P>
 static void fill_stage1(const bffc_plan* p, P& prm) {
-  prm.dftC = p->dftC;
-  prm.dftS = p->dftS;
+  prm.dft = p->dft;
   prm.gtiles = p->gtiles;
   prm.tw_scale = p->tw_scale;
   prm.tw_n = p->rblk * 64;
@@ -901,7 +902,7 @@ static int tc_stage(const bffc_plan* p, bool inverse, Seq x, Seq gate, PlaneSet 
   if (int rc = make_map4(p, &tm_pi, A.im, chunks, 128, pairs * H, size_t(M) * 2, size_t(p->N) * 2)) return rc;
   if (int rc = make_endpoint_map(p, &tm_g, (!inverse && gate.p) ? gate : x, chunks, M, L, v.Hs, B)) return rc;
   bffc::OuterTcParams prm;
-  prm.dftC = p->dftC; prm.dftS = p->dftS;
+  prm.dft = p->dft;
   prm.postgate = inverse ? static_cast<const uint32_t*>(gate.p) : nullptr;
   prm.postgate2 = inverse ? static_cast<const uint32_t*>(gate2.p) : nullptr;
   prm.y2 = inverse ? static_cast<uint32_t*>(x2.p) : nullptr;

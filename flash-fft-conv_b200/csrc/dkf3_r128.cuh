@@ -14,8 +14,8 @@
 // so summing the packed products over pairs gives exactly dk.  An odd batch is completed with an all-zero
 // partner (TMA out-of-bounds fill).
 //
-// Machine mapping: two warpgroups, rows k1 = 0..63 / 64..127 of the 128 x 64 spectrum.  Per pair: stage 1 (DFT-128,
-// wgmma, A = DFT-128 image in shared memory) -> pass 1 (twiddles) -> stage 2 (radix 64, A from registers) for u, whose
+// Machine mapping: two warpgroups, 32 conjugate row pairs k1 each of the 128 x 64 spectrum (FragPos).  Per pair: stage 1
+// (DFT-128, wgmma, A = DFT-128 image in shared memory, then the pair butterfly) -> pass 1 (twiddles) -> stage 2 (radix 64, A from registers) for u, whose
 // spectrum is parked in a thread-private shared-memory area; the same for dout, then the product is accumulated in
 // registers.  The TMA loads of the next pair are issued as soon as stage 1 has consumed an input slot.  Gated
 // backward: the caller hands in u*pregate and dout*postgate (composite sizes: the outer stage applies the gates on
@@ -26,8 +26,7 @@
 namespace bffc {
 
 struct DkfParams {
-  const __nv_bfloat16* dftC;
-  const __nv_bfloat16* dftS;
+  const __nv_bfloat16* dft;  // see FwdParams
   const uint8_t* gtiles;
   float2* dkf;               // [H][4][128][16] complex fp32: k2 = 16*q + t, frequency k = k1 + 128*k2
   int B, H, L, pairs, kmask;  // pairs = batch groups per channel; kmask as in FwdParams
@@ -59,7 +58,7 @@ dkf3_kernel(const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CU
   const int tid = threadIdx.x;
   const int hf = (tid >> 7) & 1;
   const bool leader = tid == 0;
-  const FragPos fp(tid);
+  const FragPos fp(tid, p.seg_bytes >> 7);
   const uint32_t bar_tma_u = s_bars, bar_tma_d = s_bars + 8, bar_g = s_bars + 16;
 
   if (leader) {
@@ -100,11 +99,11 @@ dkf3_kernel(const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CU
     mbar_expect_tx(bar_g, kSmemG);
     for (int c = 0; c < kSmemG; c += 8192) bulk_load(s_g + c, reinterpret_cast<const uint8_t*>(p.gtiles) + c, 8192, bar_g);
   }
-  load_dft128(gen_base + kSmemDkf3Slots, p.dftC, p.dftS, tid, kThreadsDkf3);
+  load_dft128(gen_base + kSmemDkf3Slots, p.dft, tid, kThreadsDkf3);
   RowTw tw[2];
   const float tw_inv = 1.0f / float(p.tw_n);
-  tw[0].init(fp.r0 & p.tw_mask, fp.q, tw_inv);
-  tw[1].init((fp.r0 + 8) & p.tw_mask, fp.q, tw_inv);
+  tw[0].init(fp.row[0] & p.tw_mask, fp.q, tw_inv);
+  tw[1].init(fp.row[1] & p.tw_mask, fp.q, tw_inv);
   fence_proxy_async_smem();
   __syncthreads();
   mbar_wait(bar_g, 0);
@@ -121,8 +120,8 @@ dkf3_kernel(const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CU
   // both warpgroups has read it
   auto spectrum = [&](int n, int which) {
     mbar_wait(which ? bar_tma_d : bar_tma_u, n & 1);
-    f128_stage<kFmt, false>(d, s_f, hf, sbase + which * kSlotBytes, p.kmask);
-    wgmma_wait_regs(d);
+    f128_stage<kFmt>(d, s_f, hf, sbase + which * kSlotBytes, p.kmask);
+    f128_wait<false>(d, fp);
     named_bar_sync(1, kThreadsDkf3);
     if (leader && n + 1 < n_units) issue_load(n + 1, which);
     twiddle_frag<false>(d, tw, p.tw_scale);
@@ -157,7 +156,7 @@ dkf3_kernel(const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CU
       const int h = unit_h(n);
 #pragma unroll
       for (int rr = 0; rr < 2; ++rr) {
-        const int k1 = fp.r0 + 8 * rr;
+        const int k1 = fp.row[rr];
 #pragma unroll
         for (int i = 0; i < 8; ++i) {
           const int k2 = 8 * i + 2 * fp.q, e = 4 * i + 2 * rr;

@@ -2,7 +2,8 @@
 // complex-rows mode of the composite sizes.
 //
 // Same algorithm and stage list as r128_common.cuh.  A pipeline owns one unit (a sequence pair of one channel) at a
-// time; its two warpgroups hold rows 0..63 / 64..127 of every stage's accumulator in registers.  The two pipelines of
+// time; its two warpgroups hold 32 conjugate row pairs each (fragment rows 0..63 / 64..127 of the radix-128 stages;
+// FragPos maps a thread's two slots to natural rows) of every stage's accumulator in registers.  The two pipelines of
 // a CTA share the tensor cores: while one runs a CUDA-core pass the other's MMAs execute.  Shared memory (227 KB per
 // block): 2 pipelines x 2 slots of (re, im) tiles, the DFT-128 operand image, the DFT-64 tiles and the stage-1 twiddle
 // table (loop-invariant per-thread state kept out of the 128 registers a thread has).  A slot holds the
@@ -31,7 +32,8 @@ constexpr int kSmemData3 = kPipes3 * 2 * kSlotBytes;
 constexpr int kSmemBars3 = 128;
 constexpr int kSmemTwSt3 = 128 * 8;             // (stc, sts) of every row (RowTw::store); the (bc, bs) part of the
                                                 // table takes the fourth DFT-64 plane, which no stage reads
-constexpr int kSmemTotal3 = kSmemData3 + kSmemF + kSmemG + kSmemBars3 + kSmemTwSt3 + 1024;
+constexpr int kSmemRows3 = kPipeThreads * 4;    // FragPos::packed() of every thread of a pipeline
+constexpr int kSmemTotal3 = kSmemData3 + kSmemF + kSmemG + kSmemBars3 + kSmemTwSt3 + kSmemRows3 + 1024;
 static_assert(kSmemTotal3 <= 227 * 1024, "shared memory per block");
 
 struct GateMaps { CUtensorMap pre, post, post2, y2, xg; };
@@ -107,6 +109,7 @@ fwd3_kernel(const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CU
   const uint32_t s_bars = s_g + kSmemG;
   const uint32_t s_twb = s_g + 3 * kGTileBytes;    // stage-1 twiddle table (RowTw::store)
   const uint32_t s_tws = s_bars + kSmemBars3;
+  const uint32_t s_rows = s_tws + kSmemTwSt3;
 
   const int tid = threadIdx.x;
   // warp-uniform by construction, so that the addresses and wgmma descriptors built from them live in uniform registers
@@ -114,7 +117,9 @@ fwd3_kernel(const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CU
   const int hf = __shfl_sync(0xffffffffu, (tid >> 7) & 1, 0);   // row half of the unit
   const int ptid = tid & 255;
   const bool leader = ptid == 0;       // issues this pipeline's TMA loads / stores (bulk groups are per thread)
-  const FragPos fp(tid);
+  // the thread's row map (FragPos) is read from a shared-memory table where it is used, like the twiddles: it holds no
+  // registers across the unit loop
+  auto frag = [&]() { return FragPos::unpack(tid, ld_shared_u32(s_rows + 4u * uint32_t(ptid))); };
 
   const uint32_t bar_tma0 = s_bars + pipe * 16;
   const uint32_t bar_g = s_bars + 32;
@@ -185,21 +190,24 @@ fwd3_kernel(const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CU
     for (int c = 0; c < 3 * kGTileBytes; c += 8192)
       bulk_load(s_g + c, reinterpret_cast<const uint8_t*>(p.gtiles) + c, 8192, bar_g);
   }
-  load_dft128(gen_base + kSmemData3, p.dftC, p.dftS, tid, kThreads3);
+  load_dft128(gen_base + kSmemData3, p.dft, tid, kThreads3);
   // stage-1 twiddles W_{tw_n}^{(k1 & tw_mask) j} of every row (small sizes: N/64-point blocks); the threads of pipeline
-  // 0 cover each (row, column pair) once
+  // 0 cover each (row, column pair) once, and write the row-map table (the same for both pipelines)
   if (pipe == 0) {
+    const FragPos fp(tid, kPlanes ? 128 : p.seg_bytes >> 7);   // rblk = the rows of one segment
+    st_shared_u32(s_rows + 4u * uint32_t(ptid), fp.packed());
     const float tw_inv = 1.0f / float(p.tw_n);
 #pragma unroll
     for (int rr = 0; rr < 2; ++rr) {
       RowTw t;
-      t.init((fp.r0 + 8 * rr) & p.tw_mask, fp.q, tw_inv);
-      t.store(s_twb, s_tws, fp.r0 + 8 * rr, fp.q);
+      t.init(fp.row[rr] & p.tw_mask, fp.q, tw_inv);
+      t.store(s_twb, s_tws, fp.row[rr], fp.q);
     }
   }
   auto row_tw = [&](RowTw (&tw)[2]) {
-    tw[0].load(s_twb, s_tws, fp.r0, fp.q);
-    tw[1].load(s_twb, s_tws, fp.r0 + 8, fp.q);
+    const FragPos fp = frag();
+    tw[0].load(s_twb, s_tws, fp.row[0], fp.q);
+    tw[1].load(s_twb, s_tws, fp.row[1], fp.q);
   };
   fence_proxy_async_smem();             // DFT-128 image: generic stores -> wgmma operand reads
   __syncthreads();
@@ -266,8 +274,8 @@ fwd3_kernel(const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CU
     }
 
     // ---------------- stage 1: D1 = F128 * X
-    f128_stage<kFmt, false>(d, s_f, hf, sX, p.kmask);
-    wgmma_wait_regs(d);
+    f128_stage<kFmt>(d, s_f, hf, sX, p.kmask);
+    f128_wait<false>(d, frag());
     if (leader) {
       if (kGated) {
         if (emit_xg) tma_store_wait_read0();   // pass 5 overwrites slot 0 after the barrier below
@@ -291,11 +299,12 @@ fwd3_kernel(const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CU
     // ---------------- pass 3: * k_f -> A operand of stage 3.  k_f engine vector (c, k1), c = k2 / 4, holds words
     // (kr, kr)(ki, ki) of k2 = 4c, 4c+1 then of 4c+2, 4c+3; this thread's k2 = 8 i + 2 q + {0, 1}.
     {
+      const FragPos fp = frag();
       const uint2* kfp = reinterpret_cast<const uint2*>(p.kf) + size_t(h) * 16 * 128 * 2 + (fp.q & 1);
       const f32x2 kfs2 = pk2(p.kf_scale, p.kf_scale);
 #pragma unroll
       for (int rr = 0; rr < 2; ++rr) {
-        const int k1 = fp.r0 + 8 * rr;
+        const int k1 = fp.row[rr];
         uint2 kv[8];
 #pragma unroll
         for (int i = 0; i < 8; ++i) kv[i] = __ldg(kfp + ((2 * i + (fp.q >> 1)) * 128 + k1) * 2);
@@ -323,23 +332,31 @@ fwd3_kernel(const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CU
       twiddle_frag<true>(d, tw, p.tw_scale);
     }
     pipe_sync();                          // both halves' stage 1 has read X (and the xg store has left the slot)
-    frag_store_tile<kFmt>(sX, fp, d);
+    frag_store_tile<kFmt>(sX, frag(), d);
     publish_smem();
-    // ---------------- stage 4: conj F128 * Y
-    f128_stage<kFmt, true>(d, s_f, hf, sX, 0xff);
+    // ---------------- stage 4: conj F128 * Y (its pair butterfly runs in pass 6)
+    f128_stage<kFmt>(d, s_f, hf, sX, 0xff);
     wgmma_wait_regs(d);
     pipe_sync();                          // both halves' stage 4 has read Y: the slot takes the output
 
-    // ---------------- pass 6: fp32 -> 16 bit output tiles (x output gate), TMA store
+    // ---------------- pass 6: pair butterfly, fp32 -> 16 bit output tiles (x output gate), TMA store.  The butterfly
+    // works on copies of the accumulator on their way to 16 bit: rewriting the accumulator in place (f128_wait) costs
+    // this kernel about 1 KB of local memory per thread at the register cap.
     auto pass6 = [&](bool gate) {
+      const FragPos fp = frag();
 #pragma unroll
-      for (int rr = 0; rr < 2; ++rr) {
-        const int r = fp.r0 + 8 * rr;
+      for (int i = 0; i < 8; ++i) {
+        float o[2][2][2];                 // [slot][re, im][column 2 q + e]
 #pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          const uint32_t off = frag_off(r, i, fp.q);
-          const int e = 4 * i + 2 * rr;
-          uint32_t vr = NT::pack(d.r[e], d.r[e + 1]), vi = NT::pack(d.i[e], d.i[e + 1]);
+        for (int e = 0; e < 2; ++e) {
+          float pr = d.r[4 * i + e], pi = d.i[4 * i + e], qr = d.r[4 * i + 2 + e], qi = d.i[4 * i + 2 + e];
+          pair_butterfly<true>(fp.mix, pr, pi, qr, qi);
+          o[0][0][e] = pr; o[0][1][e] = pi; o[1][0][e] = qr; o[1][1][e] = qi;
+        }
+#pragma unroll
+        for (int rr = 0; rr < 2; ++rr) {
+          const uint32_t off = frag_off(fp.row[rr], i, fp.q);
+          uint32_t vr = NT::pack(o[rr][0][0], o[rr][0][1]), vi = NT::pack(o[rr][1][0], o[rr][1][1]);
           if (kGated && gate) {
             vr = NT::hmul2(vr, ld_shared_u32(sGate + off));
             vi = NT::hmul2(vi, ld_shared_u32(sGate + kTileBytes + off));

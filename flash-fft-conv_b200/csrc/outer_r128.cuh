@@ -10,8 +10,9 @@
 //   inv_tc : z'[i, j] = sum_k0 conj F128[i,k0] * ( conj W_N^{k0 j} * T[k0, j] )
 //
 // Machine mapping: the unit is one 64-column chunk of one sequence pair: a (128 x 64) tile per member, TMA
-// loaded with a 5-D map (col, chunk, row, channel, batch member: any batch stride); DFT-128 cos / sin planes resident in shared memory as the A
-// operand (exactly stage 1 / stage 4 of r128_common.cuh); the twiddle is applied by the CUDA cores on the accumulator
+// loaded with a 5-D map (col, chunk, row, channel, batch member: any batch stride); the DFT-128 conjugate-pair image
+// resident in shared memory as the A operand (exactly stage 1 / stage 4 of r128_common.cuh: the accumulator rows a
+// thread holds are FragPos::row after f128_wait); the twiddle is applied by the CUDA cores on the accumulator
 // (forward) or on the tile in shared memory before the MMA (inverse).  Two pipelines x two warpgroups (row halves)
 // per CTA.
 #pragma once
@@ -20,8 +21,7 @@
 namespace bffc {
 
 struct OuterTcParams {
-  const __nv_bfloat16* dftC;
-  const __nv_bfloat16* dftS;
+  const __nv_bfloat16* dft;   // DFT-128 conjugate-pair image, see FwdParams
   const uint32_t* postgate;   // inverse only, (B,H,L) bf16 or null
   const uint32_t* postgate2;  // inverse only: optional second gated output y2 = postgate2 * z' (gated backward)
   uint32_t* y2;
@@ -64,7 +64,7 @@ outer_tc_kernel(const __grid_constant__ CUtensorMap tm_x,    // real endpoint: u
   const int hf = (tid >> 7) & 1;
   const int lane = tid & 127;          // shared-memory passes: row `lane`, columns 32 hf .. 32 hf + 31
   const bool leader = (tid & 255) == 0;
-  const FragPos fp(tid);
+  const FragPos fp(tid, 128);
 
   const uint32_t bar_tma0 = s_bars + pipe * 16;       // one TMA barrier per slot
 
@@ -79,7 +79,7 @@ outer_tc_kernel(const __grid_constant__ CUtensorMap tm_x,    // real endpoint: u
   }
   fence_barrier_init();
   __syncthreads();
-  load_dft128(gen_base + kSmemOuterData, p.dftC, p.dftS, tid, kThreadsOuter);
+  load_dft128(gen_base + kSmemOuterData, p.dft, tid, kThreadsOuter);
   // inverse: in-chunk twiddles W_N^{k0 * t}, t = 32*half + 2q + {0,1} (k0 = lane), applied in shared memory; the chunk
   // base W_N^{k0*64*cj} is computed per unit in fp32
   __half2 twc[16], tws[16];
@@ -96,8 +96,8 @@ outer_tc_kernel(const __grid_constant__ CUtensorMap tm_x,    // real endpoint: u
   }
   // forward: W_N^{k0 t} of the accumulator fragment's rows, t = 8 i + 2 q + {0, 1}
   RowTw tw[2];
-  tw[0].init(fp.r0, fp.q, 1.0f / float(p.N));
-  tw[1].init(fp.r0 + 8, fp.q, 1.0f / float(p.N));
+  tw[0].init(fp.row[0], fp.q, 1.0f / float(p.N));
+  tw[1].init(fp.row[1], fp.q, 1.0f / float(p.N));
   fence_proxy_async_smem();
   __syncthreads();
 
@@ -199,19 +199,19 @@ outer_tc_kernel(const __grid_constant__ CUtensorMap tm_x,    // real endpoint: u
     // ---------------- radix-128 MMA: forward F = C - iS; inverse conj F
     {
       const int ks = kInverse ? 8 : p.ksteps;
-      f128_stage<kFmt, kInverse>(d, s_f, hf, sX, (1 << ks) - 1);
+      f128_stage<kFmt>(d, s_f, hf, sX, (1 << ks) - 1);
     }
     // next unit -> the other slot (ungated: its last reader was the previous unit's TMA store)
     if (leader && nslots == 2 && unit + 1 < u_end) {
       tma_store_wait_read0();
       issue_load(unit + 1, (n + 1) % nslots);
     }
-    wgmma_wait_regs(d);
+    f128_wait<kInverse>(d, fp);
     if (!kInverse) {     // * W_N^{k0 (64 cj + t)}: chunk base per row times the in-chunk twiddles
       float c0[2], s0[2];
 #pragma unroll
       for (int rr = 0; rr < 2; ++rr) {
-        sincospif(-float(((fp.r0 + 8 * rr) * 64 * x.cj) & (p.N - 1)) * invN2, &s0[rr], &c0[rr]);
+        sincospif(-float((fp.row[rr] * 64 * x.cj) & (p.N - 1)) * invN2, &s0[rr], &c0[rr]);
         c0[rr] *= p.tw_scale; s0[rr] *= p.tw_scale;
       }
       twiddle_frag<false>(d, tw, c0, s0);

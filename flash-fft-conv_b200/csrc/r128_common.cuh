@@ -7,12 +7,19 @@
 // (monarch_cuda_interface_fwd_bf16.cu:656-760).  Same math, different machine mapping:
 //  * two real sequences (b, b+1) of one channel h are packed as ONE complex sequence z = u_b + i u_{b+1};
 //    conv(z, k) = conv(u_b,k) + i conv(u_{b+1},k) because k is real, so no Hermitian split is needed.
-//  * N = 128 * 64, n = i*64 + j.  Stage 1 contracts i: the 128x128 DFT matrix (cos / sin planes) is the wgmma A
-//    operand, resident in shared memory for the whole kernel; the TMA-loaded (128 x 64) input tile is the MN-major B
-//    operand.  The 128 rows k1 are split between two warpgroups (m64 each); D1[k1, j] lands in registers.  Stages 2 / 3
-//    are radix-64 transforms over j against DFT-64 tiles resident in shared memory, with the A operand taken straight
-//    from the registers of the previous stage; stage 4 contracts k1 again.  The CUDA-core passes between the MMAs apply
-//    the twiddles and k_f ("engine order", frequency k = k1 + 128*k2).  No intermediate touches HBM.
+//  * N = 128 * 64, n = i*64 + j.  Stage 1 contracts i: a 128x128 image of the DFT matrix is the wgmma A operand,
+//    resident in shared memory for the whole kernel; the TMA-loaded (128 x 64) input tile is the MN-major B operand.
+//    The 128 rows k1 are split between two warpgroups (m64 each); D1[k1, j] lands in registers.  Stages 2 / 3 are
+//    radix-64 transforms over j against DFT-64 tiles resident in shared memory, with the A operand taken straight from
+//    the registers of the previous stage; stage 4 contracts k1 again.  The CUDA-core passes between the MMAs apply the
+//    twiddles and k_f ("engine order", frequency k = k1 + 128*k2).  No intermediate touches HBM.
+//  * Conjugate-pair rows (stages 1 and 4).  F = C - iS with C even and S odd in the row: row m - k of the DFT is the
+//    conjugate of row k.  With P = C X and Q = S X for one row k of each pair (both complex), D[k] = P - iQ and
+//    D[m - k] = P + iQ (inverse, conj F: the signs swap); m = 128, or the block size rblk of the block-diagonal matrix
+//    of the small sizes.  The A image holds, per pair, the cos row and the sin row of k in the two fragment rows one
+//    thread owns (FragPos), so a stage is two real products (A Xr, A Xi) instead of four, and a thread-local butterfly
+//    (f128_wait) turns them into the pair's two natural rows.  From then on fragment slot rr holds natural row
+//    FragPos::row[rr]; the tiles in shared memory and the engine order stay in natural row order.
 #pragma once
 #include "ptx.cuh"
 #include "short_filter.cuh"
@@ -23,8 +30,7 @@ namespace bffc {
 
 struct FwdParams {
   const uint32_t* kf;        // [rows][16][128][4] bf16x2 words (kr0,kr1)(ki0,ki1)(kr2,kr3)(ki2,ki3), engine order, /N
-  const __nv_bfloat16* dftC; // [128][128] cos(2*pi*m*k/128)
-  const __nv_bfloat16* dftS; // [128][128] sin(2*pi*m*k/128)
+  const __nv_bfloat16* dft;  // [128][128] conjugate-pair rows of the DFT-128 (cos / sin, see FragPos), K-major
   const uint8_t* gtiles;     // DFT-64 tiles Gr, Gi, -Gi, Gr: each 64 rows x 128 B, 128B-swizzled image
   float kf_scale;            // fp16 only: k_f is stored unscaled (1/N would underflow fp16) and scaled here in fp32
   float tw_scale;            // folded into the twiddles (fp16: 1/sqrt(128) keeps every stage near the input level)
@@ -54,13 +60,13 @@ constexpr int kTileBytes = 128 * 128;          // one (128 rows x 64 bf16) tile
 constexpr int kSlotBytes = 2 * kTileBytes;     // re tile + im tile
 constexpr int kGTileBytes = 64 * 128;          // one DFT-64 plane
 constexpr int kSmemG = 4 * kGTileBytes;        // Gr, Gi, -Gi, Gr planes (r64_stage uses the first three)
-constexpr int kSmemF = 4 * kTileBytes;         // DFT-128: cos k 0..63, cos k 64..127, sin k 0..63, sin k 64..127
+constexpr int kSmemF = 2 * kTileBytes;         // DFT-128 conjugate-pair image: columns k 0..63, k 64..127
 
 // MN-major B operand (N = 64) of one tile; a 16-row K step = +(2048 >> 4)
 DEVINL uint64_t tile_desc(uint32_t saddr) { return make_sdesc(saddr, kTileBytes, 1024); }
-// K-major A operand: DFT-128 plane `plane` (0 = cos, 1 = sin), rows 64 hf .. 64 hf + 63, K step s (16 columns)
-DEVINL uint64_t f_desc(uint32_t s_f, int plane, int hf, int s) {
-  return make_sdesc(s_f + plane * 2 * kTileBytes + (s >> 2) * kTileBytes + hf * 64 * 128 + (s & 3) * 32, 16, 1024);
+// K-major A operand: DFT-128 image rows 64 hf .. 64 hf + 63, K step s (16 columns)
+DEVINL uint64_t f_desc(uint32_t s_f, int hf, int s) {
+  return make_sdesc(s_f + (s >> 2) * kTileBytes + hf * 64 * 128 + (s & 3) * 32, 16, 1024);
 }
 
 // One (128 x 64) input tile = nseg segments of 128/nseg rows; segment s holds batch member b = (g*nseg + s)*2 + which
@@ -98,23 +104,47 @@ DEVINL uint2 ld_shared_v2(uint32_t addr) {
 }
 DEVINL void st_shared_u32(uint32_t addr, uint32_t v) { asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(v) : "memory"); }
 
-// DFT-128 cos / sin planes (row-major 128 x 128 in global memory) -> the K-major, 128B-swizzled operand image at `dst`
-DEVINL void load_dft128(uint8_t* dst, const __nv_bfloat16* dftC, const __nv_bfloat16* dftS, int tid, int nthreads) {
-  for (int idx = tid; idx < 2 * 128 * 16; idx += nthreads) {
-    const int plane = idx >> 11, m = (idx >> 4) & 127, c16 = idx & 15;
-    const uint4 v = __ldg(reinterpret_cast<const uint4*>((plane ? dftS : dftC) + m * 128) + c16);
-    *reinterpret_cast<uint4*>(dst + plane * 2 * kTileBytes + (c16 >> 3) * kTileBytes + m * 128 +
-                              (((c16 & 7) ^ (m & 7)) << 4)) = v;
+// DFT-128 image (row-major 128 x 128 in global memory) -> the K-major, 128B-swizzled operand image at `dst`
+DEVINL void load_dft128(uint8_t* dst, const __nv_bfloat16* dft, int tid, int nthreads) {
+  for (int idx = tid; idx < 128 * 16; idx += nthreads) {
+    const int m = idx >> 4, c16 = idx & 15;
+    const uint4 v = __ldg(reinterpret_cast<const uint4*>(dft + m * 128) + c16);
+    *reinterpret_cast<uint4*>(dst + (c16 >> 3) * kTileBytes + m * 128 + (((c16 & 7) ^ (m & 7)) << 4)) = v;
   }
 }
 
-// This thread's place in the m64 accumulator fragment of its warpgroup: rows r0 and r0 + 8 of the 128, column pair 2 q.
+// This thread's place in the m64 accumulator fragment of its warpgroup: fragment rows f = 64 hf + 16 w + lane / 4 and
+// f + 8 of the 128 (slots rr = 0, 1), column pair 2 q.  The two slots carry conjugate pair p = 32 hf + 8 w + lane / 4
+// (0..63) of the stage-1 DFT, whose blocks are rblk rows (128, or N/64 for the small sizes): with half = rblk / 2,
+// b = p / half and kk = p % half, the pair's natural rows are
+//   row[0] = b rblk + kk,   row[1] = b rblk + (kk ? rblk - kk : half).
+// A image row f is the cos row of row[0] (within block b); row f + 8 is the sin row of row[0], except for kk = 0, whose
+// sin row is all zero: the cos row of row[1] (+-1 within the block) sits there instead, and no butterfly is needed
+// (mix = false).  After f128_wait, slot rr holds natural row row[rr] in every stage.
 struct FragPos {
-  int r0, q;
-  DEVINL explicit FragPos(int tid) : r0(((tid >> 7) & 1) * 64 + ((tid >> 5) & 3) * 16 + ((tid & 31) >> 2)), q(tid & 3) {}
+  int row[2], q;
+  bool mix;
+  DEVINL FragPos(int tid, int rblk) : q(tid & 3) {
+    const int p = ((tid >> 7) & 1) * 32 + ((tid >> 5) & 3) * 8 + ((tid & 31) >> 2);
+    const int half = rblk >> 1, kk = p & (half - 1), base = 2 * (p - kk);   // base = b rblk (rblk: a power of two)
+    row[0] = base + kk;
+    row[1] = base + (kk ? rblk - kk : half);
+    mix = kk != 0;
+  }
+  // the row map in one word (row[0] | row[1] << 8 | mix << 16), for a shared-memory table, and back
+  DEVINL uint32_t packed() const { return uint32_t(row[0]) | uint32_t(row[1]) << 8 | uint32_t(mix) << 16; }
+  DEVINL static FragPos unpack(int tid, uint32_t w) {
+    FragPos f;
+    f.q = tid & 3;
+    f.row[0] = w & 255; f.row[1] = (w >> 8) & 255; f.mix = (w >> 16) != 0;
+    return f;
+  }
+
+ private:
+  FragPos() = default;
 };
 
-// Accumulator of one warpgroup's 64 rows x 64 complex columns: element (row r0 + 8 rr, column 8 i + 2 q + e) has its
+// Accumulator of one warpgroup's 64 rows x 64 complex columns: element (fragment slot rr, column 8 i + 2 q + e) has its
 // real part at r[4 i + 2 rr + e] and its imaginary part at i[4 i + 2 rr + e].  The two halves are separate m64n64
 // accumulators, so every wgmma owns one whole register array.
 struct Acc {
@@ -125,18 +155,16 @@ struct Acc {
   }
 };
 
-// Issue (no wait) the radix-128 stage on this warpgroup's 64 rows: D = F128 X (kInv: conj F128 X), F = C - iS,
-// X = the (re, im) tile pair at sX.  Only the K steps set in kmask are issued (all-zero rows of X are skipped).
-//   D_re = C Xr + S Xi,  D_im = C Xi - S Xr     (kInv: D_re = C Xr - S Xi,  D_im = C Xi + S Xr)
-template <int kFmt, bool kInv>
+// Issue (no wait) the radix-128 stage on this warpgroup's 64 fragment rows: d.r = A Xr, d.i = A Xi, A = the
+// conjugate-pair image (FragPos), X = the (re, im) tile pair at sX.  Only the K steps set in kmask are issued (all-zero
+// rows of X are skipped).  The direction is chosen by f128_wait, which completes the stage.
+template <int kFmt>
 DEVINL void f128_stage(Acc& d, uint32_t s_f, int hf, uint32_t sX, int kmask) {
   const uint64_t dXr = tile_desc(sX), dXi = tile_desc(sX + kTileBytes);
   auto step = [&](int s, uint32_t acc) {
-    const uint64_t c = f_desc(s_f, 0, hf, s), sn = f_desc(s_f, 1, hf, s);
-    wgmma_ss_n64<kFmt, 1, 0>(d.r, c, dXr + 128 * s, acc);
-    wgmma_ss_n64<kFmt, 1, 0>(d.i, c, dXi + 128 * s, acc);
-    wgmma_ss_n64<kFmt, kInv ? -1 : 1, 0>(d.r, sn, dXi + 128 * s, 1);
-    wgmma_ss_n64<kFmt, kInv ? 1 : -1, 0>(d.i, sn, dXr + 128 * s, 1);
+    const uint64_t a = f_desc(s_f, hf, s);
+    wgmma_ss_n64<kFmt, 1, 0>(d.r, a, dXr + 128 * s, acc);
+    wgmma_ss_n64<kFmt, 1, 0>(d.i, a, dXi + 128 * s, acc);
   };
   wgmma_fence();
   if (kmask == 0xff) {
@@ -176,6 +204,29 @@ DEVINL void wgmma_wait_regs(Acc& d) {
 #pragma unroll
   for (int k = 0; k < 32; ++k) asm volatile("" : "+f"(d.r[k]), "+f"(d.i[k]));
 }
+// The radix-128 stage's pair butterfly on one column: P = C x (slot 0) and Q = S x (slot 1) in, the pair's natural
+// rows FragPos::row out (in place: P <- row[0], Q <- row[1]):
+//   forward, F = C - iS:        row[0] = P - iQ,  row[1] = P + iQ
+//   kInv, conj F = C + iS:      row[0] = P + iQ,  row[1] = P - iQ
+// A kk = 0 pair (mix = false) already holds its two rows.
+template <bool kInv>
+DEVINL void pair_butterfly(bool mix, float& pr, float& pi, float& qr, float& qi) {
+  const float sr = kInv ? -qi : qi, si = kInv ? qr : -qr;   // -iQ (kInv: +iQ)
+  if (mix) {
+    const float ar = pr + sr, ai = pi + si;
+    qr = pr - sr; qi = pi - si; pr = ar; pi = ai;
+  }
+}
+// Wait for the radix-128 stage and apply the pair butterfly to the whole fragment: slot rr then holds row[rr].
+template <bool kInv>
+DEVINL void f128_wait(Acc& d, const FragPos& fp) {
+  wgmma_wait_regs(d);
+#pragma unroll
+  for (int i = 0; i < 8; ++i)
+#pragma unroll
+    for (int e = 0; e < 2; ++e)
+      pair_butterfly<kInv>(fp.mix, d.r[4 * i + e], d.i[4 * i + e], d.r[4 * i + 2 + e], d.i[4 * i + 2 + e]);
+}
 
 // Rounded 16-bit A fragments of the next stage (K = the 64 columns, four k steps).
 template <int kFmt>
@@ -198,10 +249,10 @@ DEVINL uint32_t frag_off(int r, int i, int q) { return uint32_t(r) * 128u + (uin
 template <int kFmt>
 DEVINL void frag_store_tile(uint32_t sT, const FragPos& fp, const Acc& d) {
 #pragma unroll
-  for (int rr = 0; rr < 2; ++rr)
+  for (int i = 0; i < 8; ++i)
 #pragma unroll
-    for (int i = 0; i < 8; ++i) {
-      const uint32_t off = frag_off(fp.r0 + 8 * rr, i, fp.q);
+    for (int rr = 0; rr < 2; ++rr) {
+      const uint32_t off = frag_off(fp.row[rr], i, fp.q);
       const int e = 4 * i + 2 * rr;
       st_shared_u32(sT + off, Num<kFmt>::pack(d.r[e], d.r[e + 1]));
       st_shared_u32(sT + kTileBytes + off, Num<kFmt>::pack(d.i[e], d.i[e + 1]));

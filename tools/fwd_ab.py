@@ -5,7 +5,10 @@
 Each library gets its own plan; k_f is packed once (by library A) and both time bffc_fwd on the same seeded tensors.
 A sample is CUDA events around --launches back-to-back calls after warm-up; the two libraries alternate for --rounds
 rounds, so that clock and neighbour drift falls on both.  Per shape: the median and range (ms per call) of each library,
-and whether the two outputs are bit-identical.  The card's name and power limit are read in the same run.
+whether the two outputs are bit-identical, and each library's accuracy against the fp64 reference
+(oracle/spectral_oracle.py) on a sample of channels: rel-L2, and the spectral_error statistic (max and median over the
+sampled rows), which the two builds can differ in when they order their fp32 sums differently.  The card's name and
+power limit are read in the same run.
 Shapes (N, B, H, L, gated), bf16: c2 (the bench.py headline), r8k and r1k (the reference's published table; r1k puts 8
 sequences in one 8192-point unit), c3 (32K, implicitly padded: outer stages around the complex-rows kernel).
 """
@@ -20,9 +23,13 @@ import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.join(ROOT, 'flash-fft-conv_b200'))
+sys.path.insert(0, ROOT)
 
 import torch  # noqa: E402
 from flashfftconv import _lib  # noqa: E402
+from oracle import spectral_oracle as so  # noqa: E402
+
+SAMPLED_CHANNELS = 32
 
 SHAPES = {
     'c2': (8192, 16, 768, 8192, False),
@@ -59,6 +66,21 @@ def ptr(t):
     return ctypes.c_void_p(t.data_ptr() if t is not None else 0)
 
 
+def accuracy(y, u, k, gates, N):
+    """rel-L2 and spectral_error of y against y = postgate * conv(u * pregate, k) in fp64, on evenly spaced channels"""
+    H = u.shape[1]
+    ch = torch.linspace(0, H - 1, min(SAMPLED_CHANNELS, H), device=u.device).long()
+    x = u[:, ch].double()
+    if gates[0] is not None:
+        x = x * gates[0][:, ch].double()
+    ref = so.conv(x, k[ch], N)
+    if gates[1] is not None:
+        ref = ref * gates[1][:, ch].double()
+    got = y[:, ch]
+    se = so.spectral_error(got, ref, N)
+    return {'rel_l2': so.rel_l2(got, ref), 'spectral_max': se.max().item(), 'spectral_median': se.median().item()}
+
+
 def run_shape(libs, name, rounds, launches, warmup):
     N, B, H, L, gated = SHAPES[name]
     dev = torch.device('cuda')
@@ -90,6 +112,7 @@ def run_shape(libs, name, rounds, launches, warmup):
             call(i)
     torch.cuda.synchronize()
     identical = bool(torch.equal(ys[0], ys[1]))
+    acc = [accuracy(y, u, k, gates, N) for y in ys]
     samples = [[] for _ in libs]
     for _ in range(rounds):
         for i in range(len(libs)):
@@ -105,8 +128,8 @@ def run_shape(libs, name, rounds, launches, warmup):
     for lib, p in zip(libs, plans):
         lib.bffc_plan_destroy(p)
     res = {'shape': {'N': N, 'B': B, 'H': H, 'L': L, 'gated': gated}, 'bit_identical': identical}
-    for tag, s in zip(('a', 'b'), samples):
-        res[tag] = {'median_ms': statistics.median(s), 'min_ms': min(s), 'max_ms': max(s)}
+    for tag, s, a in zip(('a', 'b'), samples, acc):
+        res[tag] = {'median_ms': statistics.median(s), 'min_ms': min(s), 'max_ms': max(s), 'accuracy_fp64': a}
     res['b_over_a'] = res['b']['median_ms'] / res['a']['median_ms']
     res['ranges_overlap'] = not (res['b']['max_ms'] < res['a']['min_ms'] or res['a']['max_ms'] < res['b']['min_ms'])
     return res
