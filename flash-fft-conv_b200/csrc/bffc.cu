@@ -1057,13 +1057,13 @@ int bffc_fwd(const bffc_plan* p, const void* u, const void* kf, const void* preg
   return bffc_fwd_strided(p, u, s, kf, pregate, s, postgate, s, y, s, B, H, L, workspace, workspace_bytes, stream);
 }
 
-int bffc_fwd_short_strided(const bffc_plan* p, const void* u_, int64_t u_bs, const void* kf, const void* pregate_,
-                           int64_t pregate_bs, const void* postgate_, int64_t postgate_bs, void* y_, int64_t y_bs, int B,
-                           int H, int L, const void* u_w, const void* u_bias, const void* pregate_w,
-                           const void* pregate_bias, const void* postgate_w, const void* postgate_bias, int w_dtype, int K,
-                           int padding, void* workspace, size_t workspace_bytes, void* stream) {
-  const char* fn = "bffc_fwd_short_strided";
-  // arguments first, the device last (as the depthwise entry points): a bad argument is BFFC_ERR_INVALID on any machine
+}  // extern "C"
+
+// The short filter arguments of bffc_fwd_short_strided / bffc_bwd_short_strided, checked before anything else (as the
+// depthwise entry points: a bad argument is BFFC_ERR_INVALID on any machine) and gathered into *sf.
+static int short_args(const char* fn, const void* pregate, const void* postgate, const void* u_w, const void* u_bias,
+                      const void* pregate_w, const void* pregate_bias, const void* postgate_w, const void* postgate_bias,
+                      int w_dtype, int K, int padding, bffc::ShortParams* sf) {
   if (K < 1 || K > 4) return fail(BFFC_ERR_INVALID, "%s: K=%d outside [1, 4]", fn, K);
   if (padding < 0 || padding > K - 1 || 2 * padding < K - 1)
     return fail(BFFC_ERR_INVALID, "%s: padding %d outside [(K-1)/2, K-1] for K=%d", fn, padding, K);
@@ -1071,17 +1071,43 @@ int bffc_fwd_short_strided(const bffc_plan* p, const void* u_, int64_t u_bs, con
     return fail(BFFC_ERR_INVALID, "%s: w_dtype %d (BF16 0, FP16 1, FP32 2)", fn, w_dtype);
   if ((u_bias && !u_w) || (pregate_bias && !pregate_w) || (postgate_bias && !postgate_w))
     return fail(BFFC_ERR_INVALID, "%s: a bias needs the taps of its tensor", fn);
-  if ((pregate_w && !pregate_) || (postgate_w && !postgate_))
+  if ((pregate_w && !pregate) || (postgate_w && !postgate))
     return fail(BFFC_ERR_INVALID, "%s: taps for an absent gate", fn);
   const size_t ew = w_dtype == BFFC_DTYPE_FP32 ? 4 : 2;
   for (const void* t : {u_w, u_bias, pregate_w, pregate_bias, postgate_w, postgate_bias})
     if (reinterpret_cast<uintptr_t>(t) % ew) return fail(BFFC_ERR_INVALID, "%s: taps not aligned to their element", fn);
-  if (B <= 0 || H <= 0 || L <= 0) return fail(BFFC_ERR_INVALID, "%s: bad shape B=%d H=%d L=%d", fn, B, H, L);
-  if (int rc = check_strides(fn, H, L, {seq(u_, u_bs), seq(pregate_, pregate_bs), seq(postgate_, postgate_bs), seq(y_, y_bs)}))
-    return rc;
+  *sf = bffc::ShortParams{};
+  sf->u = {u_w, u_bias};
+  sf->pre = {pregate_w, pregate_bias};
+  sf->post = {postgate_w, postgate_bias};
+  sf->wdt = w_dtype; sf->K = K; sf->P = padding;
+  return 0;
+}
+
+// the plan checks of the short filter entry points, after the arguments
+static int short_plan(const char* fn, const bffc_plan* p) {
   if (!p) return fail(BFFC_ERR_INVALID, "%s: null plan", fn);
   if (p->nlev > 0 && p->lev[0].tc)
     return fail(BFFC_ERR_UNSUPPORTED, "%s: seqlen %d (tensor-core outer stage) does not take the short filter", fn, p->N);
+  return 0;
+}
+
+extern "C" {
+
+int bffc_fwd_short_strided(const bffc_plan* p, const void* u_, int64_t u_bs, const void* kf, const void* pregate_,
+                           int64_t pregate_bs, const void* postgate_, int64_t postgate_bs, void* y_, int64_t y_bs, int B,
+                           int H, int L, const void* u_w, const void* u_bias, const void* pregate_w,
+                           const void* pregate_bias, const void* postgate_w, const void* postgate_bias, int w_dtype, int K,
+                           int padding, void* workspace, size_t workspace_bytes, void* stream) {
+  const char* fn = "bffc_fwd_short_strided";
+  bffc::ShortParams sf;
+  if (int rc = short_args(fn, pregate_, postgate_, u_w, u_bias, pregate_w, pregate_bias, postgate_w, postgate_bias,
+                          w_dtype, K, padding, &sf))
+    return rc;
+  if (B <= 0 || H <= 0 || L <= 0) return fail(BFFC_ERR_INVALID, "%s: bad shape B=%d H=%d L=%d", fn, B, H, L);
+  if (int rc = check_strides(fn, H, L, {seq(u_, u_bs), seq(pregate_, pregate_bs), seq(postgate_, postgate_bs), seq(y_, y_bs)}))
+    return rc;
+  if (int rc = short_plan(fn, p)) return rc;
   if ((pregate_ == nullptr) != (postgate_ == nullptr))
     return fail(BFFC_ERR_INVALID, "%s: pregate and postgate must both be given or both be null", fn);
   if (!u_ || !kf || !y_) return fail(BFFC_ERR_INVALID, "%s: null pointer", fn);
@@ -1092,11 +1118,6 @@ int bffc_fwd_short_strided(const bffc_plan* p, const void* u_, int64_t u_bs, con
     if (need && (!workspace || workspace_bytes < need))
       return fail(BFFC_ERR_INVALID, "%s: workspace of %zu bytes required", fn, need);
   }
-  bffc::ShortParams sf{};
-  sf.u = {u_w, u_bias};
-  sf.pre = {pregate_w, pregate_bias};
-  sf.post = {postgate_w, postgate_bias};
-  sf.wdt = w_dtype; sf.K = K; sf.P = padding;
   PassOpts po;
   po.sf = &sf;
   g_launches = 0;
@@ -1104,30 +1125,52 @@ int bffc_fwd_short_strided(const bffc_plan* p, const void* u_, int64_t u_bs, con
                       workspace, static_cast<cudaStream_t>(stream), po);
 }
 
-int bffc_bwd_strided(const bffc_plan* p, const void* dout_, int64_t dout_bs, const void* u_, int64_t u_bs, const void* kf,
-                     const void* kf_conj, const void* pregate_, int64_t pregate_bs, const void* postgate_,
-                     int64_t postgate_bs, void* du_, int64_t du_bs, void* dkf, void* dpregate_, int64_t dpregate_bs,
-                     void* dpostgate_, int64_t dpostgate_bs, int B, int H, int L, void* workspace, size_t workspace_bytes,
-                     void* stream) {
+}  // extern "C"
+
+// the taps of an entry point's u, pregate and postgate (sf) in the roles one backward pass gives its tensors
+static bffc::ShortParams short_roles(const bffc::ShortParams& sf, bffc::ShortTensor u, bffc::ShortTensor pre,
+                                     bffc::ShortTensor post = {}, bffc::ShortTensor post2 = {}) {
+  bffc::ShortParams r = sf;
+  r.u = u; r.pre = pre; r.post = post; r.post2 = post2;
+  return r;
+}
+
+// bffc_bwd_strided, and bffc_bwd_short_strided when sf (the short filter taps of u, pregate and postgate) is given: the
+// same passes, each of which filters the raw tensors it loads.  fn names the entry point in error messages.
+static int conv_backward(const char* fn, const bffc_plan* p, const void* dout_, int64_t dout_bs, const void* u_,
+                         int64_t u_bs, const void* kf, const void* kf_conj, const void* pregate_, int64_t pregate_bs,
+                         const void* postgate_, int64_t postgate_bs, void* du_, int64_t du_bs, void* dkf, void* dpregate_,
+                         int64_t dpregate_bs, void* dpostgate_, int64_t dpostgate_bs, int B, int H, int L, void* workspace,
+                         size_t workspace_bytes, void* stream, const bffc::ShortParams* sf) {
   if ((pregate_ == nullptr) != (postgate_ == nullptr))
-    return fail(BFFC_ERR_INVALID, "bffc_bwd: pregate and postgate must both be given or both be null");
+    return fail(BFFC_ERR_INVALID, "%s: pregate and postgate must both be given or both be null", fn);
   const bool gated = pregate_ != nullptr;
-  if (!dout_ || !u_ || (!kf && !kf_conj) || !du_ || !dkf) return fail(BFFC_ERR_INVALID, "bffc_bwd: null pointer");
-  if (gated && (!kf || !dpregate_ || !dpostgate_)) return fail(BFFC_ERR_INVALID, "bffc_bwd: gated backward needs kf, dpregate, dpostgate");
+  if (!dout_ || !u_ || (!kf && !kf_conj) || !du_ || !dkf) return fail(BFFC_ERR_INVALID, "%s: null pointer", fn);
+  if (gated && (!kf || !dpregate_ || !dpostgate_)) return fail(BFFC_ERR_INVALID, "%s: gated backward needs kf, dpregate, dpostgate", fn);
   if (!aligned16(pregate_, postgate_, dpregate_, dpostgate_, kf))
-    return fail(BFFC_ERR_INVALID, "bffc_bwd: gate pointers must be 16-byte aligned");
+    return fail(BFFC_ERR_INVALID, "%s: gate pointers must be 16-byte aligned", fn);
   if (int rc = check_common(p, B, H, L, u_, du_, dout_)) return rc;
   if (!aligned16(dkf, kf_conj, workspace))
-    return fail(BFFC_ERR_INVALID, "bffc_bwd: dkf / kf / workspace must be 16-byte aligned");
+    return fail(BFFC_ERR_INVALID, "%s: dkf / kf / workspace must be 16-byte aligned", fn);
   // an ungated call has no gate gradients: whatever it passes there is ignored
   const Seq dout = seq(dout_, dout_bs), u = seq(u_, u_bs), pregate = seq(pregate_, pregate_bs);
   const Seq postgate = seq(postgate_, postgate_bs), du = seq(du_, du_bs);
   const Seq dpregate = gated ? seq(dpregate_, dpregate_bs) : Seq(), dpostgate = gated ? seq(dpostgate_, dpostgate_bs) : Seq();
-  if (int rc = check_strides("bffc_bwd", H, L, {dout, u, pregate, postgate, du, dpregate, dpostgate})) return rc;
+  if (int rc = check_strides(fn, H, L, {dout, u, pregate, postgate, du, dpregate, dpostgate})) return rc;
   {
     const size_t need = bffc_workspace_bytes_ex(p, B, H, L, gated, 1);
     if (need && (!workspace || workspace_bytes < need))
-      return fail(BFFC_ERR_INVALID, "bffc_bwd: workspace of %zu bytes required", need);
+      return fail(BFFC_ERR_INVALID, "%s: workspace of %zu bytes required", fn, need);
+  }
+  // short filter roles (x1 = pregate, x2 = postgate, v = u of the mixer): the pass on u loads s(u) and s(pregate), its
+  // output gate dout is raw; the pass on dout loads raw dout and s(postgate), its output gates are s(pregate) and s(u)
+  bffc::ShortParams sf_u, sf_d;
+  const bffc::ShortParams *sfu = nullptr, *sfd = nullptr;
+  if (sf) {
+    sf_u = short_roles(*sf, sf->u, sf->pre);
+    sf_d = short_roles(*sf, {}, sf->post, sf->pre, sf->u);
+    sfu = &sf_u;
+    sfd = gated ? &sf_d : nullptr;        // ungated, dout and du are not filtered
   }
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   g_launches = 0;
@@ -1154,6 +1197,8 @@ int bffc_bwd_strided(const bffc_plan* p, const void* dout_, int64_t dout_bs, con
     gate_d = gate_x + gate_scratch_bytes(B, H, L) / 2;
     p1.xg_out = gate_x;
     dx.xg_out = gate_d;
+    p1.sf = sfu;
+    dx.sf = sfd;
     if (int rc = conv_forward(p, u, kf, pregate, dout, dpostgate, B, H, L, workspace, st, p1)) return rc;
     dx.postgate2 = u;
     dx.y2 = dpregate;
@@ -1173,6 +1218,7 @@ int bffc_bwd_strided(const bffc_plan* p, const void* dout_, int64_t dout_bs, con
     if (int rc = make_seq_map(p, &tm_u, xu, B, H, L, p->rblk)) return rc;
     if (int rc = make_seq_map(p, &tm_d, xd, B, H, L, p->rblk)) return rc;
     fill_seq_tiles(p, prm, B, H, L);
+    if (sfu && !gated) prm.sf = *sfu;     // ungated: the kernel filters raw u; gated: the passes stored filtered products
     return launch_dkf(p, false, tm_u, tm_d, tm_u, tm_d, prm, st);
   }
   // chunk by chunk: the outer stages turn u (* pregate) and dout (* postgate) into complex 8192-point rows ONCE
@@ -1186,8 +1232,8 @@ int bffc_bwd_strided(const bffc_plan* p, const void* dout_, int64_t dout_bs, con
     const PlaneSet sU = p->nlev == 2 ? set(1) : s0;
     const PlaneSet sD = set(p->nlev == 2 ? 2 : 1);
     PlaneSet ru, rd;
-    if (int rc = transform_fwd(p, at(u), at(pregate), v, L, s0, sU, &ru, st)) return rc;
-    if (int rc = transform_fwd(p, at(dout), at(postgate), v, L, p->nlev == 2 ? s0 : sD, sD, &rd, st)) return rc;
+    if (int rc = transform_fwd(p, at(u), at(pregate), v, L, s0, sU, &ru, st, sfu)) return rc;
+    if (int rc = transform_fwd(p, at(dout), at(postgate), v, L, p->nlev == 2 ? s0 : sD, sD, &rd, st, sfd)) return rc;
     CUtensorMap tur, tui, tdr, tdi;
     if (int rc = make_map(p, &tur, ru.re, vpairs * rows, kInner)) return rc;
     if (int rc = make_map(p, &tui, ru.im, vpairs * rows, kInner)) return rc;
@@ -1203,8 +1249,45 @@ int bffc_bwd_strided(const bffc_plan* p, const void* dout_, int64_t dout_bs, con
     }
     if (int rc = launch_planes(p, rd.re, rd.im, static_cast<const uint8_t*>(kfc) + kf_off, vpairs, rows, st, dx.conj)) return rc;
     return transform_inv(p, at(du), at(pregate), v, L, p->nlev == 2 ? s0 : sD, sD, st,
-                         gated ? at(u) : Seq(), gated ? at(dpregate) : Seq());
+                         gated ? at(u) : Seq(), gated ? at(dpregate) : Seq(), sfd);
   });
+}
+
+extern "C" {
+
+int bffc_bwd_strided(const bffc_plan* p, const void* dout, int64_t dout_bs, const void* u, int64_t u_bs, const void* kf,
+                     const void* kf_conj, const void* pregate, int64_t pregate_bs, const void* postgate,
+                     int64_t postgate_bs, void* du, int64_t du_bs, void* dkf, void* dpregate, int64_t dpregate_bs,
+                     void* dpostgate, int64_t dpostgate_bs, int B, int H, int L, void* workspace, size_t workspace_bytes,
+                     void* stream) {
+  return conv_backward("bffc_bwd", p, dout, dout_bs, u, u_bs, kf, kf_conj, pregate, pregate_bs, postgate, postgate_bs, du,
+                       du_bs, dkf, dpregate, dpregate_bs, dpostgate, dpostgate_bs, B, H, L, workspace, workspace_bytes,
+                       stream, nullptr);
+}
+
+int bffc_bwd_short_strided(const bffc_plan* p, const void* dout, int64_t dout_bs, const void* u, int64_t u_bs,
+                           const void* kf, const void* kf_conj, const void* pregate, int64_t pregate_bs,
+                           const void* postgate, int64_t postgate_bs, void* du, int64_t du_bs, void* dkf, void* dpregate,
+                           int64_t dpregate_bs, void* dpostgate, int64_t dpostgate_bs, int B, int H, int L,
+                           const void* u_w, const void* u_bias, const void* pregate_w, const void* pregate_bias,
+                           const void* postgate_w, const void* postgate_bias, int w_dtype, int K, int padding,
+                           void* workspace, size_t workspace_bytes, void* stream) {
+  const char* fn = "bffc_bwd_short_strided";
+  bffc::ShortParams sf;
+  if (int rc = short_args(fn, pregate, postgate, u_w, u_bias, pregate_w, pregate_bias, postgate_w, postgate_bias,
+                          w_dtype, K, padding, &sf))
+    return rc;
+  if (B <= 0 || H <= 0 || L <= 0) return fail(BFFC_ERR_INVALID, "%s: bad shape B=%d H=%d L=%d", fn, B, H, L);
+  const bool gated = pregate != nullptr;
+  if (int rc = check_strides(fn, H, L, {seq(dout, dout_bs), seq(u, u_bs), seq(pregate, pregate_bs),
+                                        seq(postgate, postgate_bs), seq(du, du_bs),
+                                        gated ? seq(dpregate, dpregate_bs) : Seq(),
+                                        gated ? seq(dpostgate, dpostgate_bs) : Seq()}))
+    return rc;
+  if (int rc = short_plan(fn, p)) return rc;
+  return conv_backward(fn, p, dout, dout_bs, u, u_bs, kf, kf_conj, pregate, pregate_bs, postgate, postgate_bs, du, du_bs,
+                       dkf, dpregate, dpregate_bs, dpostgate, dpostgate_bs, B, H, L, workspace, workspace_bytes, stream,
+                       &sf);
 }
 
 int bffc_bwd(const bffc_plan* p, const void* dout, const void* u, const void* kf, const void* kf_conj,

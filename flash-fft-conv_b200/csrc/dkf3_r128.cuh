@@ -19,7 +19,9 @@
 // spectrum is parked in a thread-private shared-memory area; the same for dout, then the product is accumulated in
 // registers.  The TMA loads of the next pair are issued as soon as stage 1 has consumed an input slot.  Gated
 // backward: the caller hands in u*pregate and dout*postgate (composite sizes: the outer stage applies the gates on
-// load; seqlen <= 8192: the two fused passes of bffc_bwd store those products through FwdParams::xg_out).
+// load; seqlen <= 8192: the two fused passes of bffc_bwd store those products through FwdParams::xg_out).  An ungated
+// backward on the raw projection (bffc_bwd_short_strided, seqlen <= 8192) hands in raw u tiles and DkfParams::sf: the
+// kernel filters them in shared memory before stage 1.
 #pragma once
 #include "fwd3_r128.cuh"
 
@@ -33,6 +35,7 @@ struct DkfParams {
   int nseg, seg_bytes;        // segmented tiles (small sizes), see load_tile()
   float tw_scale;            // see FwdParams::tw_scale; dkf_unpack compensates
   int tw_n, tw_mask;         // see FwdParams
+  ShortParams sf;            // tiles: sf.u = short filter taps of u (ungated bffc_bwd_short_strided), else sf.u.w null
 };
 
 namespace r128 {
@@ -120,6 +123,14 @@ dkf3_kernel(const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CU
   // both warpgroups has read it
   auto spectrum = [&](int n, int which) {
     mbar_wait(which ? bar_tma_d : bar_tma_u, n & 1);
+    if (!kPlanes && which == 0 && p.sf.u.w) {
+      // the raw u tiles of an ungated backward on the projection: s(u) in place, one tile row per thread (short_slot)
+      const Taps t = load_taps(p.sf.u, p.sf, unit_h(n));
+      short_slot<kFmt>(sbase, 0u, t, t, true, false, tid, ShortRow(p, unit_pr(n), tid),
+                       [&] { named_bar_sync(1, kThreadsDkf3); });
+      fence_proxy_async_smem();           // filtered tiles visible to the tensor cores
+      named_bar_sync(1, kThreadsDkf3);
+    }
     f128_stage<kFmt>(d, s_f, hf, sbase + which * kSlotBytes, p.kmask);
     f128_wait<false>(d, fp);
     named_bar_sync(1, kThreadsDkf3);

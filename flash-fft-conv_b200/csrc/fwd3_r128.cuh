@@ -41,10 +41,11 @@ struct GateMaps { CUtensorMap pre, post, post2, y2, xg; };
 // Where a row of a slot sits in its sequence (kShort).  The slot's 256 tile rows are the two pair members' tiles; tile
 // row r belongs to segment r / rblk, i.e. batch member b = (g * nseg + r / rblk) * 2 + tile, at rows (r % rblk) * 64 ..
 // + 63 of it.  A row is `valid` when that member exists and the row lies inside [0, L); its left / right neighbour row
-// is part of the same sequence when `lvalid` / `rvalid`.
+// is part of the same sequence when `lvalid` / `rvalid`.  P: FwdParams, or DkfParams (the same tile geometry).
 struct ShortRow {
   bool valid, lvalid, rvalid;
-  DEVINL ShortRow(const FwdParams& p, int g, int row) {
+  template <class P>
+  DEVINL ShortRow(const P& p, int g, int row) {
     const int r = row & 127, rblk = p.seg_bytes >> 7, sg = r / rblk, ris = r - sg * rblk, used = p.L >> 6;
     valid = (g * p.nseg + sg) * 2 + (row >> 7) < p.B && ris < used;
     lvalid = ris > 0;
@@ -91,8 +92,9 @@ DEVINL void short_slot(uint32_t sA, uint32_t sB, const Taps& ta, const Taps& tb,
   }
 }
 
-// kShort (with kGated): the gated pipeline on the raw projection — u and pregate filtered in pass 0, the postgate after
-// it lands in slot 1 (bffc_fwd_short_strided).  With no gates it is the residual filter's call: s(u) alone.
+// kShort (with kGated): the gated pipeline on the raw projection — u and pregate filtered in pass 0, the postgate and
+// the second output gate after each lands in slot 1 (bffc_fwd_short_strided, bffc_bwd_short_strided).  Each of them is
+// filtered only when it has taps.  With no gates it is the residual filter's call: s(u) alone.
 template <bool kPlanes, bool kGated, int kFmt, bool kShort = false>
 __global__ void __launch_bounds__(kThreads3, 1)
 fwd3_kernel(const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CUtensorMap tm_y,
@@ -398,6 +400,13 @@ fwd3_kernel(const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CU
     if (has_post2) {
       pipe_sync();
       mbar_wait(bar_gate, gate_phase); gate_phase ^= 1;
+      if constexpr (kShort) {
+        if (p.sf.post2.w) {               // s(postgate2) in place in slot 1, as the postgate above
+          const Taps tq = load_taps(p.sf.post2, p.sf, h);
+          short_slot<kFmt>(sGate, 0u, tq, tq, true, false, ptid, ShortRow(p, unit - h * p.pairs, ptid), pipe_sync);
+          pipe_sync();
+        }
+      }
       pass6(true);
       publish_smem();
       if (leader) store_out(&gm.y2);

@@ -45,7 +45,7 @@ struct OuterParams {
   float2 step[8];        // exp(-2 pi i t / (R*M)), t = 0..7: neighbour twiddle steps (host computed, double precision)
   int lookahead;         // blocks: a block pulls the input lines of block (its linear id + lookahead) into L2 (0 = off)
   float scale;           // applied to this stage's output (fp16: 1/sqrt(R) per direction; bf16: 1, 1/N lives in k_f)
-  ShortParams sf;        // kShort kernels: short filter taps of u, pregate (forward) and postgate (inverse)
+  ShortParams sf;        // kShort kernels: short filter taps of u, pregate (forward), postgate and postgate2 (inverse)
 };
 
 // kShort: s (short_filter.cuh) of vector i of the raw row x of nv vectors, or the raw vector when `on` is false.  The
@@ -250,7 +250,8 @@ __global__ void __launch_bounds__(128, (R <= 4) ? 4 : 2) fwd_kernel(const OuterP
 }
 
 // inverse: same grid
-// kShort (level 0, gated): the postgate is the raw tensor, filtered where the output is multiplied by it
+// kShort (level 0, gated): the postgate (and postgate2) are raw tensors, each filtered where the output is multiplied by
+// it when it has taps
 template <int R, bool kGated, bool kPlanes, int kFmt, bool kShort = false>
 __global__ void __launch_bounds__(128, (R <= 4) ? 4 : 2) inv_kernel(const OuterParams p) {
   static_assert(!kShort || (kGated && !kPlanes), "the short filter applies to the gated real endpoint");
@@ -277,13 +278,15 @@ __global__ void __launch_bounds__(128, (R <= 4) ? 4 : 2) inv_kernel(const OuterP
     }
     __syncthreads();
   }
-  __shared__ Taps s_tq[1];                    // kShort: the block's channel's postgate taps
-  const bool fq = kShort && p.sf.post.w;
+  __shared__ Taps s_tq[kShort ? 2 : 1];       // kShort: the block's channel's postgate and postgate2 taps
+  const bool fq = kShort && p.sf.post.w, fq2 = kShort && p.sf.post2.w;
   if constexpr (kShort) {
     if (threadIdx.x == 0 && fq) s_tq[0] = load_taps(p.sf.post, p.sf, p.h0 + h);
+    if (threadIdx.x == 1 && fq2) s_tq[1] = load_taps(p.sf.post2, p.sf, p.h0 + h);
     __syncthreads();
   }
   const Taps& tq = s_tq[0];
+  const Taps& tq2 = s_tq[kShort ? 1 : 0];
   f32x2 w1c[4], w1s[4];                      // conj twiddle: exp(+2 pi i (n'+t) / N)
   float2 stepc[8];
 #pragma unroll
@@ -334,15 +337,20 @@ __global__ void __launch_bounds__(128, (R <= 4) ? 4 : 2) inv_kernel(const OuterP
         if (b1 < p.B) y0[p.y_bs + o] = pack8v<kFmt>(yi);
         continue;
       }
-      if (p.y2) rows[2][o] = hmul8<kFmt>(v0, __ldg(rows[3] + o));
       if constexpr (kShort) {
+        if (p.y2) rows[2][o] = hmul8<kFmt>(v0, short_vec<kFmt>(rows[3], o, p.L / kVec, tq2, fq2));
         rows[0][o] = hmul8<kFmt>(v0, short_vec<kFmt>(rows[1], o, p.L / kVec, tq, fq));
       } else {
+        if (p.y2) rows[2][o] = hmul8<kFmt>(v0, __ldg(rows[3] + o));
         rows[0][o] = hmul8<kFmt>(v0, __ldg(rows[1] + o));
       }
       if (b1 < p.B) {
         const uint4 v1 = pack8v<kFmt>(yi);
-        if (p.y2) rows[6][o] = hmul8<kFmt>(v1, __ldg(rows[7] + o));
+        if constexpr (kShort) {
+          if (p.y2) rows[6][o] = hmul8<kFmt>(v1, short_vec<kFmt>(rows[7], o, p.L / kVec, tq2, fq2));
+        } else {
+          if (p.y2) rows[6][o] = hmul8<kFmt>(v1, __ldg(rows[7] + o));
+        }
         if constexpr (kShort) {
           rows[4][o] = hmul8<kFmt>(v1, short_vec<kFmt>(rows[5], o, p.L / kVec, tq, fq));
         } else {

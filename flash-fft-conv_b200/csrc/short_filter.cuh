@@ -1,5 +1,5 @@
 // short_filter.cuh — the Hyena / M2 short filter applied where the long-convolution kernels load their inputs and gates
-// (bffc_fwd_short_strided).
+// (bffc_fwd_short_strided, bffc_bwd_short_strided).
 //
 //   s[b, h, l] = bias[h] + sum_{j<K} w[h, j] * x[b, h, l - P + j]      (x = 0 outside [0, L)),  0 <= l < L
 //
@@ -22,8 +22,9 @@ struct ShortTensor {
   const void* w;
   const void* bias;   // may be null (bias 0) when w is given
 };
+// post2: the second output gate of a pass (FwdParams::postgate2 / OuterParams::postgate2), which the backward filters
 struct ShortParams {
-  ShortTensor u, pre, post;
+  ShortTensor u, pre, post, post2;
   int wdt;            // BFFC_DTYPE_BF16 (0), FP16 (1), FP32 (2)
   int K, P;
 };

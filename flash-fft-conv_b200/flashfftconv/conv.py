@@ -347,15 +347,19 @@ def _fwd(mod, u, k, pregate, postgate, band=None, use_cache=None, kf_engine=None
     return y, kf_engine
 
 
-def _bwd(mod, dout, u, kf_engine, k_len, pregate, postgate, band=None, out=None):
+def _bwd(mod, dout, u, kf_engine, k_len, pregate, postgate, band=None, out=None, taps=None):
     """du, dk[, dpregate, dpostgate] — reference: FlashFFTConvFunc.backward, conv.py:1737-1822.  band: the forward's
     band limit (None: full spectrum); kf_engine is then the band-limited spectrum and dk gets the same mask.  Inputs:
     any (B, H, L) layout, as for _fwd.  out: optional (du, dpregate, dpostgate) tensors to write the gradients into
-    (channel slices of one buffer are written in place) and return; otherwise they are new contiguous tensors."""
+    (channel slices of one buffer are written in place) and return; otherwise they are new contiguous tensors.
+    taps: the short filter of the forward, as _fwd takes it (bffc_bwd_short_strided): u and the gates are the raw
+    tensors, and du, dpregate, dpostgate the gradients with respect to their filtered versions."""
     B, H, L = u.shape
     plan = mod.plan(u.device)
     Lp = _pad_len(plan, L)
     if Lp != L:
+        if taps is not None:
+            raise RuntimeError(f'L={L} must be a multiple of bffc_length_multiple() to fuse a short filter')
         r = _bwd(mod, _padded(dout, Lp), _padded(u, Lp), kf_engine, k_len, _padded(pregate, Lp), _padded(postgate, Lp),
                  band)
         cut = lambda t: None if t is None else t[..., :L].contiguous()
@@ -382,10 +386,18 @@ def _bwd(mod, dout, u, kf_engine, k_len, pregate, postgate, band=None, out=None)
         dkf_engine = torch.empty((H, N, 2), dtype=torch.float32, device=u.device)
         ws, ws_bytes = _workspace(plan, B, H, L, gated, True, u.device)
         # kf_engine_conj = NULL: the kernels conjugate the forward's spectrum in their pointwise multiply
-        _launched(mod, _lib.lib().bffc_bwd_strided(plan.handle, _ptr(dout), dout_bs, _ptr(u), u_bs, _ptr(kf_engine),
+        if taps is None:
+            rc = _lib.lib().bffc_bwd_strided(plan.handle, _ptr(dout), dout_bs, _ptr(u), u_bs, _ptr(kf_engine), None,
+                                             _ptr(pre), pre_bs, _ptr(post), post_bs, _ptr(du), du_bs, _ptr(dkf_engine),
+                                             _ptr(dpre), dpre_bs, _ptr(dpost), dpost_bs, B, H, L, _ptr(ws), ws_bytes,
+                                             _stream())
+        else:
+            rows, w_dtype, K, P = taps
+            rc = _lib.lib().bffc_bwd_short_strided(plan.handle, _ptr(dout), dout_bs, _ptr(u), u_bs, _ptr(kf_engine),
                                                    None, _ptr(pre), pre_bs, _ptr(post), post_bs, _ptr(du), du_bs,
-                                                   _ptr(dkf_engine), _ptr(dpre), dpre_bs, _ptr(dpost), dpost_bs,
-                                                   B, H, L, _ptr(ws), ws_bytes, _stream()))
+                                                   _ptr(dkf_engine), _ptr(dpre), dpre_bs, _ptr(dpost), dpost_bs, B, H,
+                                                   L, *rows, w_dtype, K, P, _ptr(ws), ws_bytes, _stream())
+        _launched(mod, rc)
         for t, _, o in dst:
             if o is not None:
                 o.copy_(t)

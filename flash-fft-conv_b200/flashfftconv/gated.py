@@ -19,11 +19,12 @@ to a contiguous tensor first, with the same result.  `hyena_mixer` also writes t
 straight into one (B, 3H, L) gradient of the projection, so its backward does not concatenate them either.
 
 `hyena_operator` also runs the short depthwise filter that produces the projection's three slices
-(x1x2v = short_filter(in_proj(u))) inside the engine's loads, so the filtered (B, 3H, L) tensor is neither written nor
-read back in the forward, nor kept for the backward.
+(x1x2v = short_filter(in_proj(u))) inside the engine's loads, forward and backward, so the filtered (B, 3H, L) tensor
+is never written, read back or kept for the backward.
 """
 import torch
 
+from . import _lib
 from . import conv as _conv
 from . import depthwise_1d as _dw
 
@@ -63,21 +64,26 @@ class HyenaMixerFunc(torch.autograd.Function):
         return grad, dk, dk2, None, None
 
 
+def _short_taps(D, short):
+    """(taps, taps2) as _conv._fwd / _conv._bwd take them for the gated call and the residual call (v only), or
+    (None, None).  short: (weights (3D, K), bias (3D), padding) of the short depthwise filter on [x1 | x2 | v]."""
+    if short is None:
+        return None, None
+    w, b, P = short
+    K = w.shape[1]
+    # the rows of x1, x2, v in the contiguous (3D, K) weight and (3D) bias: plain pointer offsets (a split would cost
+    # several microseconds of host time per call)
+    w1, w2, wv = (w.data_ptr() + i * D * K * w.element_size() for i in range(3))
+    b1, b2, bv = (b.data_ptr() + i * D * b.element_size() for i in range(3))
+    wdt = _dw._DT[w.dtype]
+    return ((wv, bv, w1, b1, w2, b2), wdt, K, P), ((wv, bv, None, None, None, None), wdt, K, P)
+
+
 def _mixer_forward(mod, x1, x2, v, k, k2, short=None):
     """(y, kf, kf2) of y = x2 * conv(x1 * v, k) [+ conv(v, k2)] on the slices x1, x2, v of one (B, 3D, L) projection.
     short: (weights (3D, K), bias (3D), padding) of a short depthwise filter the engine applies to the three slices as
     it loads them (bffc_fwd_short_strided); the residual call filters only v."""
-    taps = taps2 = None
-    if short is not None:
-        w, b, P = short
-        D, K = v.shape[1], w.shape[1]
-        # the rows of x1, x2, v in the contiguous (3D, K) weight and (3D) bias: plain pointer offsets (a split would
-        # cost several microseconds of host time per call)
-        w1, w2, wv = (w.data_ptr() + i * D * K * w.element_size() for i in range(3))
-        b1, b2, bv = (b.data_ptr() + i * D * b.element_size() for i in range(3))
-        wdt = _dw._DT[w.dtype]
-        taps = ((wv, bv, w1, b1, w2, b2), wdt, K, P)
-        taps2 = ((wv, bv, None, None, None, None), wdt, K, P)
+    taps, taps2 = _short_taps(v.shape[1], short)
     y, kf = _conv._fwd(mod, v, k, x1, x2, taps=taps)
     kf2 = None
     if k2 is not None:
@@ -86,16 +92,19 @@ def _mixer_forward(mod, x1, x2, v, k, k2, short=None):
     return y, kf, kf2
 
 
-def _mixer_backward(mod, D, dout, x1x2v, kf, k_len, kf2, k2_len):
-    """(d x1x2v, dk, dk2) of y = x2 * conv(x1 * v, k) [+ conv(v, k2)]; d x1x2v is one contiguous (B, 3D, L) tensor."""
+def _mixer_backward(mod, D, dout, x1x2v, kf, k_len, kf2, k2_len, short=None):
+    """(d x1x2v, dk, dk2) of y = x2 * conv(x1 * v, k) [+ conv(v, k2)]; d x1x2v is one contiguous (B, 3D, L) tensor.
+    short: as for _mixer_forward; x1x2v is then the raw projection, the engine filters its slices as it loads them
+    (bffc_bwd_short_strided), and d x1x2v is the gradient of the filtered projection."""
     x1, x2, v = x1x2v.split(D, dim=1)
+    taps, taps2 = _short_taps(D, short)
     grad = torch.empty_like(x1x2v, memory_format=torch.contiguous_format)
     dx1, dx2, dv = grad.split(D, dim=1)
     # u = v, pregate = x1, postgate = x2: du -> [:, 2D:], dpregate -> [:, :D], dpostgate -> [:, D:2D]
-    _, dk, _, _ = _conv._bwd(mod, dout, v, kf, k_len, x1, x2, out=(dv, dx1, dx2))
+    _, dk, _, _ = _conv._bwd(mod, dout, v, kf, k_len, x1, x2, out=(dv, dx1, dx2), taps=taps)
     dk2 = None
     if kf2 is not None:
-        dv2, dk2, _, _ = _conv._bwd(mod, dout, v, kf2, k2_len, None, None)
+        dv2, dk2, _, _ = _conv._bwd(mod, dout, v, kf2, k2_len, None, None, taps=taps2)
         dv.add_(dv2)
     return grad, dk, dk2
 
@@ -130,9 +139,9 @@ class ShortHyenaFunc(torch.autograd.Function):
     """y = s_x2 * conv(s_x1 * s_v, k) [+ conv(s_v, k2)] with s = short(x), s_x1, s_x2, s_v = s.split(D, dim=1).
 
     Forward: one bffc_fwd_short_strided call (one more for k2) on the raw projection; s is never materialised.  Saved for
-    backward: x, the filter spectra and the short filter's parameters.  Backward: s is recomputed (bffc_dwconv1d_fwd),
-    the mixer's backward runs on it into one (B, 3D, L) gradient of s, and bffc_dwconv1d_bwd turns that into the
-    gradients of x, the taps and the bias."""
+    backward: x, the filter spectra and the short filter's parameters.  Backward: one bffc_bwd_short_strided call (one
+    more for k2) on the raw slices of x writes one (B, 3D, L) gradient of s, and bffc_dwconv1d_bwd turns that into the
+    gradients of x, the taps and the bias; s is not materialised there either."""
 
     @staticmethod
     def forward(ctx, x, weights, bias, k, k2, mod, d_model, padding):
@@ -151,17 +160,16 @@ class ShortHyenaFunc(torch.autograd.Function):
     def backward(ctx, dout):
         x, weights, bias, kf, kf2 = ctx.saved_tensors
         ctx.mod.__dict__['last_launches'] = 0
-        L = x.shape[-1]
-        s, shape = _dw._forward(x, weights, bias, ctx.padding, True)
-        Lout = s.shape[-1]
-        # padding = K - 1 (the original models): nn.Conv1d gives L + K - 1 outputs, of which the mixer uses the first L.
-        # Those slices do not qualify for in-place use and are copied, and the gradient of s is zero-extended: both
-        # costs fall on the backward only.
-        grad, dk, dk2 = _mixer_backward(ctx.mod, ctx.d_model, dout, s if Lout == L else s[..., :L], kf, ctx.k_len, kf2,
-                                        ctx.k2_len)
+        B, C, L = x.shape
+        K, P = weights.shape[1], ctx.padding
+        grad, dk, dk2 = _mixer_backward(ctx.mod, ctx.d_model, dout, x, kf, ctx.k_len, kf2, ctx.k2_len,
+                                        (weights, bias, P))
+        # padding = K - 1 (the original models): nn.Conv1d gives L + K - 1 outputs, of which the mixer uses the first L;
+        # the gradient of the others is zero
+        Lout = L + 2 * P - K + 1
         if Lout != L:
             grad = torch.nn.functional.pad(grad, (0, Lout - L))
-        dx, dw, dbias = _dw._backward(grad, x, weights, bias, shape)
+        dx, dw, dbias = _dw._backward(grad, x, weights, bias, (B, C, L, K, P, _lib.BFFC_LAYOUT_BHL))
         return dx, dw, dbias, dk, dk2, None, None, None
 
 
@@ -176,10 +184,10 @@ def hyena_operator(conv, short_filter, x, k, d_model, residual_filter=None):
     models); its `weights` and `bias` receive gradients, as do x, k and the residual filter k2.
 
     For K <= 4, seqlen < 1M and L a multiple of bffc_length_multiple, the forward is one engine call (two with k2) that
-    applies the short filter where the kernels load x1, x2 and v: s is not written to memory, and not kept for the
-    backward, which recomputes it.  Results are bit for bit those of short_filter followed by hyena_mixer, which is what
-    every other call runs.  Like hyena_mixer, the call goes to the engine directly: forward hooks on `conv` and
-    `short_filter` do not run for it."""
+    applies the short filter where the kernels load x1, x2 and v, and so is the mixer part of the backward: s is neither
+    written to memory nor kept between them.  Results are bit for bit those of short_filter followed by hyena_mixer,
+    which is what every other call runs.  Like hyena_mixer, the call goes to the engine directly: forward hooks on
+    `conv` and `short_filter` do not run for it."""
     if not isinstance(short_filter, _dw.FlashDepthWiseConv1d) or not short_filter.is_bhl:
         raise RuntimeError('short_filter must be a BHL FlashDepthWiseConv1d')
     if short_filter.d != 3 * d_model:

@@ -215,6 +215,24 @@ int bffc_fwd_short_strided(const bffc_plan* plan, const void* u, int64_t u_bstri
                            size_t workspace_bytes, void* stream);
 
 /*
+ * The backward of bffc_fwd_short_strided: bffc_bwd_strided with u, pregate and postgate replaced by their filtered
+ * versions s(.) (same definition, rounding and zero padding beyond L as the forward).  The inputs are the raw tensors;
+ * du, dpregate and dpostgate are the gradients with respect to s(u), s(pregate) and s(postgate) — bffc_dwconv1d_bwd
+ * turns each into the gradients of the raw tensor, the taps and the bias.  dkf_engine is that of the filtered operator.
+ * The result is bit for bit bffc_dwconv1d_fwd followed by bffc_bwd_strided; s is never written.  Taps, K, padding,
+ * w_dtype and their checks (done before the device is looked at) are those of bffc_fwd_short_strided; strides,
+ * workspace and launch count those of bffc_bwd_strided.  1M, 2M and 4M return BFFC_ERR_UNSUPPORTED.
+ */
+int bffc_bwd_short_strided(const bffc_plan* plan, const void* dout, int64_t dout_bstride, const void* u,
+                           int64_t u_bstride, const void* kf_engine, const void* kf_engine_conj,
+                           const void* pregate, int64_t pregate_bstride, const void* postgate, int64_t postgate_bstride,
+                           void* du, int64_t du_bstride, void* dkf_engine, void* dpregate, int64_t dpregate_bstride,
+                           void* dpostgate, int64_t dpostgate_bstride, int B, int H, int L,
+                           const void* u_w, const void* u_bias, const void* pregate_w, const void* pregate_bias,
+                           const void* postgate_w, const void* postgate_bias, int w_dtype, int K, int padding,
+                           void* workspace, size_t workspace_bytes, void* stream);
+
+/*
  * Forward on HOST buffers (the reference has no counterpart: its user writes u.cuda() -> conv -> y.cpu(),
  * README.md:108-149, three serial steps on one stream).  u_host, pregate_host, postgate_host, y_host: (B, H, L)
  * contiguous host memory of the plan dtype — page-locked for the copies to overlap; kf_engine: DEVICE, from
