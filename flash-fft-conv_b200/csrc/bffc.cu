@@ -697,6 +697,24 @@ static void fill_stage1(const bffc_plan* p, P& prm) {
   prm.tw_scale = p->tw_scale;
   prm.tw_n = p->rblk * 64;
   prm.tw_mask = p->rblk - 1;
+  prm.nblk = 1;
+  prm.srows = 0;
+  prm.win = 0;
+}
+
+// Overlap-save blocks (bffc_fwd_blocked / bffc_bwd_blocked, seqlen 8192), after fill_seq_tiles: blocks of S = 8192 - halo
+// new samples, ceil(L / S) per sequence, become the items i = b * nblk + j of the batch (load_tile).  win: the window's
+// tile row offset, halo/64 for a convolution pass (window [jS - halo, jS + S)), 0 for a correlation pass (window
+// [jS, jS + 8192)).  Every tile row of a window can be non-zero.
+template <class P>
+static void fill_blocks(P& prm, int B, int L, int halo, int win) {
+  const int S = kInner - halo;
+  prm.nblk = (L + S - 1) / S;
+  prm.srows = S / 64;
+  prm.win = win;
+  prm.B = B * prm.nblk;
+  prm.pairs = (prm.B + 1) / 2;
+  prm.kmask = 0xff;
 }
 
 // Tile geometry of (B, H, L) real sequences, seqlen <= 8192: S = 128/rblk batch members share one 8192-point unit
@@ -739,6 +757,8 @@ struct PassOpts {
   void* xg_out = nullptr;           // seqlen <= 8192, gated: the pass also stores its gated input u * pregate here
                                     // (contiguous (B, H, L) workspace)
   const bffc::ShortParams* sf = nullptr;   // short filter on u / pregate / postgate (bffc_fwd_short_strided)
+  int halo = -1;                    // >= 0: overlap-save blocks with this halo (bffc_fwd_blocked / bffc_bwd_blocked)
+  bool corr = false;                // blocked: the pass is a correlation (du), its windows start at the block
 };
 
 // fused 8192-point kernel on (B, H, L) real sequences (seqlen <= 8192)
@@ -747,6 +767,7 @@ static int launch_fused(const bffc_plan* p, Seq u, const void* kf, Seq pregate, 
   if (L % 64 != 0) return fail(BFFC_ERR_UNSUPPORTED, "L=%d must be a multiple of 64 for seqlen <= 8192 in this build", L);
   bffc::FwdParams prm = fwd_params(p, kf, po.conj);
   fill_seq_tiles(p, prm, B, H, L);
+  if (po.halo >= 0) fill_blocks(prm, B, L, po.halo, po.corr ? 0 : po.halo / 64);
   prm.pregate = static_cast<const uint32_t*>(pregate.p);
   prm.postgate = static_cast<const uint32_t*>(postgate.p);
   prm.postgate2 = static_cast<const uint32_t*>(po.postgate2.p);
@@ -754,20 +775,22 @@ static int launch_fused(const bffc_plan* p, Seq u, const void* kf, Seq pregate, 
   prm.xg_out = pregate.p ? po.xg_out : nullptr;
   prm.units = H * prm.pairs;
   const int seg_rows = p->rblk;
+  const int out_rows = po.halo >= 0 ? prm.srows : seg_rows;   // overlap-save blocks store their S new samples only
   auto map = [&](CUtensorMap* m, Seq t) { return make_seq_map(p, m, t, B, H, L, seg_rows); };
+  auto out_map = [&](CUtensorMap* m, Seq t) { return make_seq_map(p, m, t, B, H, L, out_rows); };
   CUtensorMap tm_u, tm_y, tm_g;
   if (int rc = map(&tm_u, u)) return rc;
-  if (int rc = map(&tm_y, y)) return rc;
+  if (int rc = out_map(&tm_y, y)) return rc;
   if (int rc = map(&tm_g, pregate.p ? pregate : u)) return rc;
   using namespace bffc::r128;
   const bool gated = pregate.p || postgate.p || prm.y2;
   // gate tiles travel by TMA like the inputs: pregate with the (segmented) geometry of u, output gates with that of y
   GateMaps gm{tm_g, tm_u, tm_u, tm_u, tm_u};
-  if (prm.xg_out) { if (int rc = map(&gm.xg, seq(prm.xg_out, int64_t(H) * L))) return rc; }
+  if (prm.xg_out) { if (int rc = out_map(&gm.xg, seq(prm.xg_out, int64_t(H) * L))) return rc; }
   if (postgate.p) { if (int rc = map(&gm.post, postgate)) return rc; }
   if (prm.y2) {
     if (int rc = map(&gm.post2, po.postgate2)) return rc;
-    if (int rc = map(&gm.y2, po.y2)) return rc;
+    if (int rc = out_map(&gm.y2, po.y2)) return rc;
   }
   const int g3 = persistent_grid(p, prm.units, kPipes3);
   bffc::FwdShortParams sprm;
@@ -993,13 +1016,16 @@ static int for_each_chunk(const bffc_plan* p, int B, int H, int L, void* ws, int
   return BFFC_OK;
 }
 
-static int check_common(const bffc_plan* p, int B, int H, int L, const void* a, const void* b, const void* c) {
+// blocked: overlap-save blocks (bffc_fwd_blocked / bffc_bwd_blocked), where L may exceed the seqlen
+static int check_common(const bffc_plan* p, int B, int H, int L, const void* a, const void* b, const void* c,
+                        bool blocked = false) {
   if (!p) return fail(BFFC_ERR_INVALID, "null plan");
   // Tensor maps are encoded through the driver API, which needs a current context in the CALLING thread.  A thread that
   // has made no runtime call yet (PyTorch's autograd worker entering bffc_bwd) has none: this runtime no-op binds the
   // device's primary context (cuTensorMapEncodeTiled otherwise fails with CUDA_ERROR_INVALID_CONTEXT).
   CUDA_TRY(cudaFree(nullptr));
-  if (B <= 0 || H <= 0 || L <= 0 || L > p->N) return fail(BFFC_ERR_INVALID, "bad shape B=%d H=%d L=%d (seqlen %d)", B, H, L, p->N);
+  if (B <= 0 || H <= 0 || L <= 0 || (L > p->N && !blocked))
+    return fail(BFFC_ERR_INVALID, "bad shape B=%d H=%d L=%d (seqlen %d)", B, H, L, p->N);
   if (L % 8 != 0) return fail(BFFC_ERR_UNSUPPORTED, "L=%d must be a multiple of 8 in this build", L);
   if (!aligned16(a, b, c)) return fail(BFFC_ERR_INVALID, "device pointers must be 16-byte aligned");
   return 0;
@@ -1029,26 +1055,56 @@ static int conv_forward(const bffc_plan* p, Seq u, const void* kf, Seq pregate, 
   });
 }
 
-extern "C" {
+// The checks of bffc_fwd_blocked / bffc_bwd_blocked beyond those of the strided calls, made first
+static int blocked_args(const char* fn, const bffc_plan* p, int L, int halo) {
+  if (!p) return fail(BFFC_ERR_INVALID, "%s: null plan", fn);
+  if (p->N != kInner)
+    return fail(BFFC_ERR_UNSUPPORTED, "%s: overlap-save blocks run on the seqlen 8192 plan, not seqlen %d", fn, p->N);
+  if (halo < 0 || halo > 4096 || halo % 512)
+    return fail(BFFC_ERR_INVALID, "%s: halo=%d is not a multiple of 512 in [0, 4096]", fn, halo);
+  if (L % 64) return fail(BFFC_ERR_INVALID, "%s: L=%d is not a multiple of 64", fn, L);
+  return 0;
+}
 
-int bffc_fwd_strided(const bffc_plan* p, const void* u_, int64_t u_bs, const void* kf, const void* pregate_,
-                     int64_t pregate_bs, const void* postgate_, int64_t postgate_bs, void* y_, int64_t y_bs, int B, int H,
-                     int L, void* workspace, size_t workspace_bytes, void* stream) {
+// bffc_fwd_strided, and bffc_fwd_blocked when po.halo >= 0
+static int forward_entry(const char* fn, const bffc_plan* p, const void* u_, int64_t u_bs, const void* kf,
+                         const void* pregate_, int64_t pregate_bs, const void* postgate_, int64_t postgate_bs, void* y_,
+                         int64_t y_bs, int B, int H, int L, void* workspace, size_t workspace_bytes, void* stream,
+                         const PassOpts& po) {
   if ((pregate_ == nullptr) != (postgate_ == nullptr))
-    return fail(BFFC_ERR_INVALID, "bffc_fwd: pregate and postgate must both be given or both be null");
-  if (!u_ || !kf || !y_) return fail(BFFC_ERR_INVALID, "bffc_fwd: null pointer");
-  if (int rc = check_common(p, B, H, L, u_, y_, kf)) return rc;
+    return fail(BFFC_ERR_INVALID, "%s: pregate and postgate must both be given or both be null", fn);
+  if (!u_ || !kf || !y_) return fail(BFFC_ERR_INVALID, "%s: null pointer", fn);
+  if (int rc = check_common(p, B, H, L, u_, y_, kf, po.halo >= 0)) return rc;
   if (!aligned16(pregate_, postgate_, workspace))
-    return fail(BFFC_ERR_INVALID, "bffc_fwd: gates / workspace must be 16-byte aligned");
+    return fail(BFFC_ERR_INVALID, "%s: gates / workspace must be 16-byte aligned", fn);
   const Seq u = seq(u_, u_bs), pregate = seq(pregate_, pregate_bs), postgate = seq(postgate_, postgate_bs), y = seq(y_, y_bs);
-  if (int rc = check_strides("bffc_fwd", H, L, {u, pregate, postgate, y})) return rc;
+  if (int rc = check_strides(fn, H, L, {u, pregate, postgate, y})) return rc;
   {
     const size_t need = bffc_workspace_bytes_ex(p, B, H, L, pregate.p != nullptr, 0);
     if (need && (!workspace || workspace_bytes < need))
-      return fail(BFFC_ERR_INVALID, "bffc_fwd: workspace of %zu bytes required", need);
+      return fail(BFFC_ERR_INVALID, "%s: workspace of %zu bytes required", fn, need);
   }
   g_launches = 0;
-  return conv_forward(p, u, kf, pregate, postgate, y, B, H, L, workspace, static_cast<cudaStream_t>(stream));
+  return conv_forward(p, u, kf, pregate, postgate, y, B, H, L, workspace, static_cast<cudaStream_t>(stream), po);
+}
+
+extern "C" {
+
+int bffc_fwd_strided(const bffc_plan* p, const void* u, int64_t u_bs, const void* kf, const void* pregate,
+                     int64_t pregate_bs, const void* postgate, int64_t postgate_bs, void* y, int64_t y_bs, int B, int H,
+                     int L, void* workspace, size_t workspace_bytes, void* stream) {
+  return forward_entry("bffc_fwd", p, u, u_bs, kf, pregate, pregate_bs, postgate, postgate_bs, y, y_bs, B, H, L,
+                       workspace, workspace_bytes, stream, PassOpts());
+}
+
+int bffc_fwd_blocked(const bffc_plan* p, const void* u, int64_t u_bs, const void* kf, const void* pregate,
+                     int64_t pregate_bs, const void* postgate, int64_t postgate_bs, void* y, int64_t y_bs, int B, int H,
+                     int L, int halo, void* workspace, size_t workspace_bytes, void* stream) {
+  if (int rc = blocked_args("bffc_fwd_blocked", p, L, halo)) return rc;
+  PassOpts po;
+  po.halo = halo;
+  return forward_entry("bffc_fwd_blocked", p, u, u_bs, kf, pregate, pregate_bs, postgate, postgate_bs, y, y_bs, B, H, L,
+                       workspace, workspace_bytes, stream, po);
 }
 
 int bffc_fwd(const bffc_plan* p, const void* u, const void* kf, const void* pregate, const void* postgate, void* y,
@@ -1136,12 +1192,13 @@ static bffc::ShortParams short_roles(const bffc::ShortParams& sf, bffc::ShortTen
 }
 
 // bffc_bwd_strided, and bffc_bwd_short_strided when sf (the short filter taps of u, pregate and postgate) is given: the
-// same passes, each of which filters the raw tensors it loads.  fn names the entry point in error messages.
+// same passes, each of which filters the raw tensors it loads.  halo >= 0: bffc_bwd_blocked, the same passes on
+// overlap-save blocks.  fn names the entry point in error messages.
 static int conv_backward(const char* fn, const bffc_plan* p, const void* dout_, int64_t dout_bs, const void* u_,
                          int64_t u_bs, const void* kf, const void* kf_conj, const void* pregate_, int64_t pregate_bs,
                          const void* postgate_, int64_t postgate_bs, void* du_, int64_t du_bs, void* dkf, void* dpregate_,
                          int64_t dpregate_bs, void* dpostgate_, int64_t dpostgate_bs, int B, int H, int L, void* workspace,
-                         size_t workspace_bytes, void* stream, const bffc::ShortParams* sf) {
+                         size_t workspace_bytes, void* stream, const bffc::ShortParams* sf, int halo = -1) {
   if ((pregate_ == nullptr) != (postgate_ == nullptr))
     return fail(BFFC_ERR_INVALID, "%s: pregate and postgate must both be given or both be null", fn);
   const bool gated = pregate_ != nullptr;
@@ -1149,7 +1206,7 @@ static int conv_backward(const char* fn, const bffc_plan* p, const void* dout_, 
   if (gated && (!kf || !dpregate_ || !dpostgate_)) return fail(BFFC_ERR_INVALID, "%s: gated backward needs kf, dpregate, dpostgate", fn);
   if (!aligned16(pregate_, postgate_, dpregate_, dpostgate_, kf))
     return fail(BFFC_ERR_INVALID, "%s: gate pointers must be 16-byte aligned", fn);
-  if (int rc = check_common(p, B, H, L, u_, du_, dout_)) return rc;
+  if (int rc = check_common(p, B, H, L, u_, du_, dout_, halo >= 0)) return rc;
   if (!aligned16(dkf, kf_conj, workspace))
     return fail(BFFC_ERR_INVALID, "%s: dkf / kf / workspace must be 16-byte aligned", fn);
   // an ungated call has no gate gradients: whatever it passes there is ignored
@@ -1179,6 +1236,8 @@ static int conv_backward(const char* fn, const bffc_plan* p, const void* dout_, 
   // (reference: kernels_bf16/monarch_cuda_32_16_16_bwd_kernel_bf16.h:740-815)
   PassOpts dx;
   dx.conj = kf_conj ? 0 : 1;
+  dx.halo = halo;
+  dx.corr = true;
   const void* kfc = kf_conj ? kf_conj : kf;
   uint8_t *gate_x = nullptr, *gate_d = nullptr;
   if (p->nlev > 0) {
@@ -1191,8 +1250,9 @@ static int conv_backward(const char* fn, const bffc_plan* p, const void* dout_, 
     //   dpostgate = dout * conv(u*p, k)                        — one pass of the forward path
     //   du = p * dx  and  dpregate = u * dx                    — ONE more pass with two gated outputs
     // the dk_f kernel below needs u*p and dout*q — the gated inputs of these two passes, which store them into the
-    // tail of the workspace on the way
+    // tail of the workspace on the way (overlap-save blocks: each block its own S samples, together the whole tensor)
     PassOpts p1;
+    p1.halo = halo;
     gate_x = static_cast<uint8_t*>(workspace);
     gate_d = gate_x + gate_scratch_bytes(B, H, L) / 2;
     p1.xg_out = gate_x;
@@ -1214,10 +1274,13 @@ static int conv_backward(const char* fn, const bffc_plan* p, const void* dout_, 
     // gated loads (reference: ..._bwd_kernel_bf16.h:505-509,571-581): the products stored by the two passes above
     // (contiguous workspace), else u and dout themselves
     const Seq xu = gated ? seq(gate_x, int64_t(H) * L) : u, xd = gated ? seq(gate_d, int64_t(H) * L) : dout;
+    fill_seq_tiles(p, prm, B, H, L);
+    // overlap-save blocks: u on the convolution window, dout on the block's own S samples (the last srows tile rows; the
+    // halo rows before them are zero, so no term of the correlation wraps around for lags m <= halo)
+    if (halo >= 0) fill_blocks(prm, B, L, halo, halo / 64);
     CUtensorMap tm_u, tm_d;
     if (int rc = make_seq_map(p, &tm_u, xu, B, H, L, p->rblk)) return rc;
-    if (int rc = make_seq_map(p, &tm_d, xd, B, H, L, p->rblk)) return rc;
-    fill_seq_tiles(p, prm, B, H, L);
+    if (int rc = make_seq_map(p, &tm_d, xd, B, H, L, p->rblk - prm.win)) return rc;
     if (sfu && !gated) prm.sf = *sfu;     // ungated: the kernel filters raw u; gated: the passes stored filtered products
     return launch_dkf(p, false, tm_u, tm_d, tm_u, tm_d, prm, st);
   }
@@ -1263,6 +1326,18 @@ int bffc_bwd_strided(const bffc_plan* p, const void* dout, int64_t dout_bs, cons
   return conv_backward("bffc_bwd", p, dout, dout_bs, u, u_bs, kf, kf_conj, pregate, pregate_bs, postgate, postgate_bs, du,
                        du_bs, dkf, dpregate, dpregate_bs, dpostgate, dpostgate_bs, B, H, L, workspace, workspace_bytes,
                        stream, nullptr);
+}
+
+int bffc_bwd_blocked(const bffc_plan* p, const void* dout, int64_t dout_bs, const void* u, int64_t u_bs, const void* kf,
+                     const void* kf_conj, const void* pregate, int64_t pregate_bs, const void* postgate,
+                     int64_t postgate_bs, void* du, int64_t du_bs, void* dkf, void* dpregate, int64_t dpregate_bs,
+                     void* dpostgate, int64_t dpostgate_bs, int B, int H, int L, int halo, void* workspace,
+                     size_t workspace_bytes, void* stream) {
+  const char* fn = "bffc_bwd_blocked";
+  if (int rc = blocked_args(fn, p, L, halo)) return rc;
+  return conv_backward(fn, p, dout, dout_bs, u, u_bs, kf, kf_conj, pregate, pregate_bs, postgate, postgate_bs, du, du_bs,
+                       dkf, dpregate, dpregate_bs, dpostgate, dpostgate_bs, B, H, L, workspace, workspace_bytes, stream,
+                       nullptr, halo);
 }
 
 int bffc_bwd_short_strided(const bffc_plan* p, const void* dout, int64_t dout_bs, const void* u, int64_t u_bs,

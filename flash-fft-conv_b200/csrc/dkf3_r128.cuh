@@ -36,6 +36,8 @@ struct DkfParams {
   float tw_scale;            // see FwdParams::tw_scale; dkf_unpack compensates
   int tw_n, tw_mask;         // see FwdParams
   ShortParams sf;            // tiles: sf.u = short filter taps of u (ungated bffc_bwd_short_strided), else sf.u.w null
+  int nblk, srows, win;      // overlap-save blocks (bffc_bwd_blocked, see load_tile): u on the convolution window, dout
+                             // on its last srows rows only (rows [0, win) of the dout slot stay zero); else 1, 0, 0
 };
 
 namespace r128 {
@@ -87,13 +89,16 @@ dkf3_kernel(const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CU
     const uint32_t bar = which ? bar_tma_d : bar_tma_u;
     const uint32_t dst = sbase + which * kSlotBytes;
     const CUtensorMap* tm = which ? &tm_d : &tm_u;
-    mbar_expect_tx(bar, kSlotBytes);
     if (kPlanes) {
+      mbar_expect_tx(bar, kSlotBytes);
       tma_load_3d(dst, tm, bar, 0, 0, pr * p.H + h);
       tma_load_3d(dst + kTileBytes, which ? &tm_di : &tm_ui, bar, 0, 0, pr * p.H + h);
     } else {
-      load_tile<true>(dst, tm, bar, h, pr, 0, p.nseg, p.seg_bytes);              // members beyond the batch: zeros
-      load_tile<true>(dst + kTileBytes, tm, bar, h, pr, 1, p.nseg, p.seg_bytes);
+      // overlap-save blocks: dout lands below its zero rows (tm_d's box is the srows-row sub-box), u on its window
+      const int skip = which ? p.win * 128 : 0;
+      mbar_expect_tx(bar, kSlotBytes - 2 * skip);
+      load_tile<true>(dst + skip, tm, bar, h, pr, 0, p, which ? 0 : p.win);      // members beyond the batch: zeros
+      load_tile<true>(dst + kTileBytes + skip, tm, bar, h, pr, 1, p, which ? 0 : p.win);
     }
   };
   // everything stage 1 needs from global memory is requested up front
@@ -103,6 +108,11 @@ dkf3_kernel(const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CU
     for (int c = 0; c < kSmemG; c += 8192) bulk_load(s_g + c, reinterpret_cast<const uint8_t*>(p.gtiles) + c, 8192, bar_g);
   }
   load_dft128(gen_base + kSmemDkf3Slots, p.dft, tid, kThreadsDkf3);
+  if (!kPlanes)       // overlap-save blocks: the first win rows of both dout tiles, which no TMA load writes, are zero
+    for (int c = tid; c < p.win * 8; c += kThreadsDkf3) {
+      *reinterpret_cast<uint4*>(gen_base + kSlotBytes + c * 16) = make_uint4(0u, 0u, 0u, 0u);
+      *reinterpret_cast<uint4*>(gen_base + kSlotBytes + kTileBytes + c * 16) = make_uint4(0u, 0u, 0u, 0u);
+    }
   RowTw tw[2];
   const float tw_inv = 1.0f / float(p.tw_n);
   tw[0].init(fp.row[0] & p.tw_mask, fp.q, tw_inv);

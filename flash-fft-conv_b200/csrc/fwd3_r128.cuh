@@ -102,6 +102,7 @@ fwd3_kernel(const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CU
             const std::conditional_t<kShort, FwdShortParams, FwdParams> p) {
   static_assert(!(kPlanes && kGated), "composite sizes apply their gates in the outer stages");
   static_assert(!kShort || kGated, "the short filter runs in the gated pipeline");
+  constexpr bool kBlocks = !kShort;     // overlap-save blocks (FwdParams::nblk) run in the plain and gated instantiations
   using NT = Num<kFmt>;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t sbase = (smem_u32(smem_raw) + 1023u) & ~1023u;
@@ -165,11 +166,11 @@ fwd3_kernel(const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CU
     if (kGated) {                        // input tiles -> slot 0, pregate tiles -> slot 1, one barrier
       const int uh = unit / p.pairs, ug = unit - uh * p.pairs;
       mbar_expect_tx(bar_tma0, has_pre ? 2 * kSlotBytes : kSlotBytes);
-      load_tile(s_slot0, &tm_u, bar_tma0, uh, ug, 0, p.nseg, p.seg_bytes);
-      load_tile(s_slot0 + kTileBytes, &tm_u, bar_tma0, uh, ug, 1, p.nseg, p.seg_bytes);
+      load_tile<false, kBlocks>(s_slot0, &tm_u, bar_tma0, uh, ug, 0, p, p.win);
+      load_tile<false, kBlocks>(s_slot0 + kTileBytes, &tm_u, bar_tma0, uh, ug, 1, p, p.win);
       if (has_pre) {
-        load_tile(s_slot0 + kSlotBytes, &gm.pre, bar_tma0, uh, ug, 0, p.nseg, p.seg_bytes);
-        load_tile(s_slot0 + kSlotBytes + kTileBytes, &gm.pre, bar_tma0, uh, ug, 1, p.nseg, p.seg_bytes);
+        load_tile<false, kBlocks>(s_slot0 + kSlotBytes, &gm.pre, bar_tma0, uh, ug, 0, p, p.win);
+        load_tile<false, kBlocks>(s_slot0 + kSlotBytes + kTileBytes, &gm.pre, bar_tma0, uh, ug, 1, p, p.win);
       }
       return;
     }
@@ -179,8 +180,8 @@ fwd3_kernel(const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CU
       tma_load_3d(dst + kTileBytes, &tm_g, bar, 0, 0, seq_index(unit));
     } else {
       const int uh = unit / p.pairs, ug = unit - uh * p.pairs;
-      load_tile(dst, &tm_u, bar, uh, ug, 0, p.nseg, p.seg_bytes);
-      load_tile(dst + kTileBytes, &tm_u, bar, uh, ug, 1, p.nseg, p.seg_bytes);
+      load_tile<false, kBlocks>(dst, &tm_u, bar, uh, ug, 0, p, p.win);
+      load_tile<false, kBlocks>(dst + kTileBytes, &tm_u, bar, uh, ug, 1, p, p.win);
     }
   };
   // Everything the first stage needs from global memory is requested up front and lands while the tables below are
@@ -221,14 +222,27 @@ fwd3_kernel(const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CU
   auto publish_smem = [&]() { fence_proxy_async_smem(); pipe_sync(); };
 
   // mirror of load_tile: the (up to two) tiles of a unit go back segment by segment, existing batch members only; rows
-  // beyond L/64 of a segment are outside the tensor map and dropped
+  // beyond L/64 of a segment are outside the tensor map and dropped.  Overlap-save blocks store the sub-box of their S new
+  // samples: tile rows [win, win + srows), the box of the output maps, to rows j * srows of the sequence.
   auto store_tiles = [&](const CUtensorMap* my, uint32_t sT, int unit) {
     const int uh = unit / p.pairs, ug = unit - uh * p.pairs;
-    for (int w = 0; w < 2; ++w)
-      for (int sg = 0; sg < p.nseg; ++sg) {
-        const int b = (ug * p.nseg + sg) * 2 + w;
-        if (b < p.B) tma_store_4d(my, sT + w * kTileBytes + sg * p.seg_bytes, 0, 0, uh, b);
+    for (int w = 0; w < 2; ++w) {
+      if constexpr (!kBlocks) {
+        for (int sg = 0; sg < p.nseg; ++sg) {
+          const int i = (ug * p.nseg + sg) * 2 + w;
+          if (i < p.B) {
+            const ItemPos<kBlocks> it(p, i, 0);
+            tma_store_4d(my, sT + w * kTileBytes + sg * p.seg_bytes + (kBlocks ? p.win * 128 : 0), 0, it.row, uh,
+                         it.b);
+          }
+        }
+      } else {
+        const ItemPos<kBlocks> it(p, ug * p.nseg * 2 + w, 0);
+        for (int sg = 0; sg < p.nseg; ++sg)
+          if ((ug * p.nseg + sg) * 2 + w < p.B)
+            tma_store_4d(my, sT + w * kTileBytes + sg * p.seg_bytes + p.win * 128, 0, it.row, uh, it.b + 2 * sg);
       }
+    }
     tma_store_commit();
   };
 
@@ -269,8 +283,8 @@ fwd3_kernel(const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CU
         if (has_post) {
           const int ug = unit - h * p.pairs;
           mbar_expect_tx(bar_gate, kSlotBytes);
-          load_tile(sGate, &gm.post, bar_gate, h, ug, 0, p.nseg, p.seg_bytes);
-          load_tile(sGate + kTileBytes, &gm.post, bar_gate, h, ug, 1, p.nseg, p.seg_bytes);
+          load_tile<false, kBlocks>(sGate, &gm.post, bar_gate, h, ug, 0, p, p.win);
+          load_tile<false, kBlocks>(sGate + kTileBytes, &gm.post, bar_gate, h, ug, 1, p, p.win);
         }
       }
     }
@@ -392,8 +406,8 @@ fwd3_kernel(const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CU
       if (has_post2) {                    // slot 1 has been read by every thread (barrier above): second gate -> slot 1
         const int ug = unit - h * p.pairs;
         mbar_expect_tx(bar_gate, kSlotBytes);
-        load_tile(sGate, &gm.post2, bar_gate, h, ug, 0, p.nseg, p.seg_bytes);
-        load_tile(sGate + kTileBytes, &gm.post2, bar_gate, h, ug, 1, p.nseg, p.seg_bytes);
+        load_tile<false, kBlocks>(sGate, &gm.post2, bar_gate, h, ug, 0, p, p.win);
+        load_tile<false, kBlocks>(sGate + kTileBytes, &gm.post2, bar_gate, h, ug, 1, p, p.win);
         tma_store_wait_read0();           // the first output has left slot 0
       }
     }

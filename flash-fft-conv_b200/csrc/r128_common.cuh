@@ -47,6 +47,7 @@ struct FwdParams {
   int tw_n, tw_mask;         // stage-1 twiddles W_{tw_n}^{(k1 & tw_mask) j}: 8192 / 127, small sizes N / (N/64 - 1)
   int units;                 // H * pairs
   uint32_t kf_conj_mask;     // 0x80008000: multiply by conj(k_f) (du path of the backward: correlation), else 0
+  int nblk, srows, win;      // overlap-save blocks, see load_tile (1, 0, 0 outside bffc_fwd_blocked / bffc_bwd_blocked)
 };
 // parameters of the fused kernel's kShort instantiations: the short filter taps of u, pregate, postgate (short_filter.cuh)
 struct FwdShortParams : FwdParams {
@@ -77,13 +78,42 @@ DEVINL uint64_t f_desc(uint32_t s_f, int hf, int s) {
 // member beyond the batch (b >= B) is out of bounds for the map: an all-zero tile.
 // kRolled: keep the segment loop rolled (the dk_f kernel: unrolled copies cost it spill slots; the fused forward kernel
 // spills less with the compiler's choice).
-template <bool kRolled = false>
-DEVINL void load_tile(uint32_t dst, const void* map, uint32_t bar, int h, int g, int which, int nseg, int seg_bytes) {
-  if (kRolled) {
-#pragma unroll 1
-    for (int s = 0; s < nseg; ++s) tma_load_4d(dst + s * seg_bytes, map, bar, 0, 0, h, (g * nseg + s) * 2 + which);
+//
+// Overlap-save blocks (bffc_fwd_blocked / bffc_bwd_blocked, seqlen 8192, nseg = 1): the batch is made of items
+// i = b * nblk + j, block j of sequence b, whose window starts at tile row j * srows - win of the sequence (srows = S/64,
+// S = 8192 - halo new samples per block; win = halo/64 for the convolution passes, 0 for the correlation passes).  Rows
+// before 0 and from L/64 on are zero-filled.  Outside blocked mode nblk = 1 and srows = win = 0: item = b, row 0.
+// The division is done once per call, for the first segment (blocked mode has one; the other segments are the members
+// 2, 4, ... after it).  kBlocks = false: an instantiation that never runs blocked keeps the plain batch loop.
+template <bool kBlocks = true>
+struct ItemPos {
+  int row, b;
+  template <class P>
+  DEVINL ItemPos(const P& p, int i, int win) {
+    if (kBlocks) {
+      b = i / p.nblk;
+      row = (i - b * p.nblk) * p.srows - win;
+    } else {
+      b = i;
+      row = 0;
+    }
+  }
+};
+template <bool kRolled = false, bool kBlocks = true, class P>
+DEVINL void load_tile(uint32_t dst, const void* map, uint32_t bar, int h, int g, int which, const P& p, int win) {
+  if constexpr (!kBlocks) {
+    for (int s = 0; s < p.nseg; ++s) {
+      const ItemPos<kBlocks> it(p, (g * p.nseg + s) * 2 + which, win);
+      tma_load_4d(dst + s * p.seg_bytes, map, bar, 0, it.row, h, it.b);
+    }
   } else {
-    for (int s = 0; s < nseg; ++s) tma_load_4d(dst + s * seg_bytes, map, bar, 0, 0, h, (g * nseg + s) * 2 + which);
+    const ItemPos<kBlocks> it(p, g * p.nseg * 2 + which, win);
+    if (kRolled) {
+#pragma unroll 1
+      for (int s = 0; s < p.nseg; ++s) tma_load_4d(dst + s * p.seg_bytes, map, bar, 0, it.row, h, it.b + 2 * s);
+    } else {
+      for (int s = 0; s < p.nseg; ++s) tma_load_4d(dst + s * p.seg_bytes, map, bar, 0, it.row, h, it.b + 2 * s);
+    }
   }
 }
 

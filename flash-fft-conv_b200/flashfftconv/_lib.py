@@ -49,6 +49,13 @@ SYMBOLS = {
                                     _c.c_void_p, _c.c_void_p, _c.c_int64, _c.c_void_p, _c.c_int64, _c.c_void_p,
                                     _c.c_int64, _c.c_void_p, _c.c_void_p, _c.c_int64, _c.c_void_p, _c.c_int64]
                          + [_c.c_int] * 3 + [_c.c_void_p, _c.c_size_t, _c.c_void_p]),
+    'bffc_fwd_blocked': (_c.c_int, [_c.c_void_p, _c.c_void_p, _c.c_int64, _c.c_void_p, _c.c_void_p, _c.c_int64,
+                                    _c.c_void_p, _c.c_int64, _c.c_void_p, _c.c_int64] + [_c.c_int] * 4
+                         + [_c.c_void_p, _c.c_size_t, _c.c_void_p]),
+    'bffc_bwd_blocked': (_c.c_int, [_c.c_void_p, _c.c_void_p, _c.c_int64, _c.c_void_p, _c.c_int64, _c.c_void_p,
+                                    _c.c_void_p, _c.c_void_p, _c.c_int64, _c.c_void_p, _c.c_int64, _c.c_void_p,
+                                    _c.c_int64, _c.c_void_p, _c.c_void_p, _c.c_int64, _c.c_void_p, _c.c_int64]
+                         + [_c.c_int] * 4 + [_c.c_void_p, _c.c_size_t, _c.c_void_p]),
     'bffc_fwd_short_strided': (_c.c_int, [_c.c_void_p, _c.c_void_p, _c.c_int64, _c.c_void_p, _c.c_void_p, _c.c_int64,
                                           _c.c_void_p, _c.c_int64, _c.c_void_p, _c.c_int64] + [_c.c_int] * 3
                                + [_c.c_void_p] * 6 + [_c.c_int] * 3 + [_c.c_void_p, _c.c_size_t, _c.c_void_p]),

@@ -209,8 +209,9 @@ def _engine_view(t, dtype):
     return t, s
 
 
-def _check_inputs(u, k, mod, gates=(), views=False):
-    """views: u and the gates may be any (B, H, L) layout (channel slices are used in place, others copied)."""
+def _check_inputs(u, k, mod, gates=(), views=False, blocked=False):
+    """views: u and the gates may be any (B, H, L) layout (channel slices are used in place, others copied).  blocked:
+    overlap-save blocks (blocked_long_conv), where L may exceed the seqlen."""
     if not u.is_cuda:
         raise RuntimeError('u must be a CUDA tensor (bffc has no CPU path)')          # monarch_fwd.h:7-13
     if u.dtype != mod.dtype:
@@ -220,7 +221,7 @@ def _check_inputs(u, k, mod, gates=(), views=False):
     B, H, L = u.shape
     if k.dim() != 2 or k.shape[0] != H or k.shape[1] > mod.seqlen:
         raise RuntimeError(f'k must be (H={H}, Lk<={mod.seqlen}), got {tuple(k.shape)}')
-    if L > mod.seqlen:
+    if L > mod.seqlen and not blocked:
         raise RuntimeError(f'L={L} exceeds seqlen={mod.seqlen}')
     for g in gates:
         if g.shape != u.shape or g.dtype != u.dtype or not (views or g.is_contiguous()) or not g.is_cuda:
@@ -314,12 +315,13 @@ class _on_device:
             self.ctx.__exit__(*a)
 
 
-def _fwd(mod, u, k, pregate, postgate, band=None, use_cache=None, kf_engine=None, taps=None):
+def _fwd(mod, u, k, pregate, postgate, band=None, use_cache=None, kf_engine=None, taps=None, halo=None):
     """y (contiguous) and the engine-order filter spectrum it used.  u and the gates: any (B, H, L) layout; those that
     qualify (batch_stride) are read in place, others copied.  band / use_cache: see _kf_engine_for; kf_engine: a
     spectrum of k already at hand.  taps: ((u_w, u_bias, pregate_w, pregate_bias, postgate_w, postgate_bias), w_dtype,
     K, padding), a short depthwise filter bffc_fwd_short_strided applies to u and the gates as it loads them; the rows
-    are device addresses of (H, K) taps and (H) biases, None for a tensor that is not filtered."""
+    are device addresses of (H, K) taps and (H) biases, None for a tensor that is not filtered.  halo: overlap-save
+    blocks with this halo (bffc_fwd_blocked, blocked_long_conv), else None."""
     B, H, L = u.shape
     dev = u.device
     plan = mod.plan(dev)
@@ -327,7 +329,8 @@ def _fwd(mod, u, k, pregate, postgate, band=None, use_cache=None, kf_engine=None
     if Lp != L:
         if taps is not None:       # the filter's bias would reach past L: padding the input is not padding its output
             raise RuntimeError(f'L={L} must be a multiple of bffc_length_multiple() to fuse a short filter')
-        y, kf = _fwd(mod, _padded(u, Lp), k, _padded(pregate, Lp), _padded(postgate, Lp), band, use_cache, kf_engine)
+        y, kf = _fwd(mod, _padded(u, Lp), k, _padded(pregate, Lp), _padded(postgate, Lp), band, use_cache, kf_engine,
+                     halo=halo)
         return y[..., :L].contiguous(), kf
     (u, u_bs), (pre, pre_bs), (post, post_bs) = [_engine_view(t, mod.dtype) for t in (u, pregate, postgate)]
     with _on_device(dev):
@@ -335,7 +338,10 @@ def _fwd(mod, u, k, pregate, postgate, band=None, use_cache=None, kf_engine=None
             kf_engine = _kf_engine_for(mod, plan, k, band=band, use_cache=use_cache)
         y = torch.empty((B, H, L), dtype=u.dtype, device=dev)
         ws, ws_bytes = _workspace(plan, B, H, L, pre is not None, False, dev)
-        if taps is None:
+        if halo is not None:
+            rc = _lib.lib().bffc_fwd_blocked(plan.handle, _ptr(u), u_bs, _ptr(kf_engine), _ptr(pre), pre_bs, _ptr(post),
+                                             post_bs, _ptr(y), H * L, B, H, L, int(halo), _ptr(ws), ws_bytes, _stream())
+        elif taps is None:
             rc = _lib.lib().bffc_fwd_strided(plan.handle, _ptr(u), u_bs, _ptr(kf_engine), _ptr(pre), pre_bs, _ptr(post),
                                              post_bs, _ptr(y), H * L, B, H, L, _ptr(ws), ws_bytes, _stream())
         else:
@@ -347,13 +353,14 @@ def _fwd(mod, u, k, pregate, postgate, band=None, use_cache=None, kf_engine=None
     return y, kf_engine
 
 
-def _bwd(mod, dout, u, kf_engine, k_len, pregate, postgate, band=None, out=None, taps=None):
+def _bwd(mod, dout, u, kf_engine, k_len, pregate, postgate, band=None, out=None, taps=None, halo=None):
     """du, dk[, dpregate, dpostgate] — reference: FlashFFTConvFunc.backward, conv.py:1737-1822.  band: the forward's
     band limit (None: full spectrum); kf_engine is then the band-limited spectrum and dk gets the same mask.  Inputs:
     any (B, H, L) layout, as for _fwd.  out: optional (du, dpregate, dpostgate) tensors to write the gradients into
     (channel slices of one buffer are written in place) and return; otherwise they are new contiguous tensors.
     taps: the short filter of the forward, as _fwd takes it (bffc_bwd_short_strided): u and the gates are the raw
-    tensors, and du, dpregate, dpostgate the gradients with respect to their filtered versions."""
+    tensors, and du, dpregate, dpostgate the gradients with respect to their filtered versions.  halo: the forward's
+    overlap-save blocks (bffc_bwd_blocked), else None."""
     B, H, L = u.shape
     plan = mod.plan(u.device)
     Lp = _pad_len(plan, L)
@@ -361,7 +368,7 @@ def _bwd(mod, dout, u, kf_engine, k_len, pregate, postgate, band=None, out=None,
         if taps is not None:
             raise RuntimeError(f'L={L} must be a multiple of bffc_length_multiple() to fuse a short filter')
         r = _bwd(mod, _padded(dout, Lp), _padded(u, Lp), kf_engine, k_len, _padded(pregate, Lp), _padded(postgate, Lp),
-                 band)
+                 band, halo=halo)
         cut = lambda t: None if t is None else t[..., :L].contiguous()
         res = [cut(r[0]), r[1], cut(r[2]), cut(r[3])]
         for i, o in zip((0, 2, 3), out or ()):
@@ -386,7 +393,12 @@ def _bwd(mod, dout, u, kf_engine, k_len, pregate, postgate, band=None, out=None,
         dkf_engine = torch.empty((H, N, 2), dtype=torch.float32, device=u.device)
         ws, ws_bytes = _workspace(plan, B, H, L, gated, True, u.device)
         # kf_engine_conj = NULL: the kernels conjugate the forward's spectrum in their pointwise multiply
-        if taps is None:
+        if halo is not None:
+            rc = _lib.lib().bffc_bwd_blocked(plan.handle, _ptr(dout), dout_bs, _ptr(u), u_bs, _ptr(kf_engine), None,
+                                             _ptr(pre), pre_bs, _ptr(post), post_bs, _ptr(du), du_bs, _ptr(dkf_engine),
+                                             _ptr(dpre), dpre_bs, _ptr(dpost), dpost_bs, B, H, L, int(halo), _ptr(ws),
+                                             ws_bytes, _stream())
+        elif taps is None:
             rc = _lib.lib().bffc_bwd_strided(plan.handle, _ptr(dout), dout_bs, _ptr(u), u_bs, _ptr(kf_engine), None,
                                              _ptr(pre), pre_bs, _ptr(post), post_bs, _ptr(du), du_bs, _ptr(dkf_engine),
                                              _ptr(dpre), dpre_bs, _ptr(dpost), dpost_bs, B, H, L, _ptr(ws), ws_bytes,
@@ -416,14 +428,15 @@ def _bwd(mod, dout, u, kf_engine, k_len, pregate, postgate, band=None, out=None,
 class FlashFFTConvFunc(torch.autograd.Function):
     """y = postgate * conv(u * pregate, k), the gates both given or both None.  save: keep what backward reads (the
     caller's rule: the module's training mode, or whether a gradient is wanted).  band / use_cache: see _kf_engine_for.
-    views: u and the gates may be channel slices or other non-contiguous (B, H, L) layouts (gated_long_conv)."""
+    views: u and the gates may be channel slices or other non-contiguous (B, H, L) layouts (gated_long_conv).
+    halo: overlap-save blocks of any length L on the seqlen-8192 module (blocked_long_conv), else None."""
 
     @staticmethod
-    def forward(ctx, u, k, mod, save, pregate=None, postgate=None, band=None, use_cache=None, views=False):
-        _check_inputs(u, k, mod, () if pregate is None else (pregate, postgate), views)
+    def forward(ctx, u, k, mod, save, pregate=None, postgate=None, band=None, use_cache=None, views=False, halo=None):
+        _check_inputs(u, k, mod, () if pregate is None else (pregate, postgate), views, halo is not None)
         mod.__dict__['last_launches'] = 0
-        y, kf_engine = _fwd(mod, u, k, pregate, postgate, band, use_cache)
-        ctx.mod, ctx.k_len, ctx.band = mod, k.shape[-1], band
+        y, kf_engine = _fwd(mod, u, k, pregate, postgate, band, use_cache, halo=halo)
+        ctx.mod, ctx.k_len, ctx.band, ctx.halo = mod, k.shape[-1], band, halo
         if save:                                                      # conv.py:587-588
             ctx.save_for_backward(u, kf_engine, pregate, postgate)
         return y
@@ -432,5 +445,5 @@ class FlashFFTConvFunc(torch.autograd.Function):
     def backward(ctx, dout):
         u, kf_engine, pregate, postgate = ctx.saved_tensors
         ctx.mod.__dict__['last_launches'] = 0
-        du, dk, dpre, dpost = _bwd(ctx.mod, dout, u, kf_engine, ctx.k_len, pregate, postgate, ctx.band)
-        return du, dk, None, None, dpre, dpost, None, None, None      # conv.py:1822, :3939
+        du, dk, dpre, dpost = _bwd(ctx.mod, dout, u, kf_engine, ctx.k_len, pregate, postgate, ctx.band, halo=ctx.halo)
+        return du, dk, None, None, dpre, dpost, None, None, None, None      # conv.py:1822, :3939

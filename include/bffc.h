@@ -192,6 +192,37 @@ int bffc_bwd_strided(const bffc_plan* plan, const void* dout, int64_t dout_bstri
                      void* workspace, size_t workspace_bytes, void* stream);
 
 /*
+ * Causal convolution of sequences of any length with a filter of at most halo + 1 taps, by overlap-save blocks on the
+ * seqlen-8192 plan:
+ *
+ *     y[b,h,t] = postgate[b,h,t] * sum_{m=0}^{halo} k[h,m] * (u*pregate)[b,h,t-m],  (u*pregate)[t < 0] = 0,  0 <= t < L
+ *
+ * which is what bffc_fwd_strided computes on a plan of any seqlen >= L + halo.  Each sequence is cut into blocks of
+ * S = 8192 - halo new samples; block j is convolved, with the halo samples before it, by one 8192-point transform of the
+ * fused kernel and keeps its last S outputs.  The backward runs the same passes as bffc_bwd_strided on the same blocks
+ * (du from windows that start at the block), and dkf_engine is what bffc_dk_from_dkf of the same plan turns into dk for
+ * any Lk <= halo + 1.
+ *   - The plan's seqlen is 8192, else BFFC_ERR_UNSUPPORTED.  halo is a multiple of 512 in [0, 4096] and L a multiple of
+ *     64, else BFFC_ERR_INVALID; L has no upper bound beyond int.
+ *   - The CALLER guarantees k[h, m] = 0 for m > halo: kf_engine is bffc_kf_from_filter of a filter of at most halo + 1
+ *     taps.  A longer filter wraps around the blocks and gives a wrong result (not detected).
+ *   - Arguments, strides and gates as for bffc_fwd_strided / bffc_bwd_strided.  No output may overlap an input: the
+ *     windows of neighbouring blocks read the same samples.
+ *   - Workspace: bffc_workspace_bytes_ex of the same plan at (B, H, L).  Launch counts are those of bffc_fwd / bffc_bwd
+ *     at seqlen 8192.
+ */
+int bffc_fwd_blocked(const bffc_plan* plan, const void* u, int64_t u_bstride, const void* kf_engine,
+                     const void* pregate, int64_t pregate_bstride, const void* postgate, int64_t postgate_bstride,
+                     void* y, int64_t y_bstride, int B, int H, int L, int halo, void* workspace, size_t workspace_bytes,
+                     void* stream);
+int bffc_bwd_blocked(const bffc_plan* plan, const void* dout, int64_t dout_bstride, const void* u, int64_t u_bstride,
+                     const void* kf_engine, const void* kf_engine_conj,
+                     const void* pregate, int64_t pregate_bstride, const void* postgate, int64_t postgate_bstride,
+                     void* du, int64_t du_bstride, void* dkf_engine, void* dpregate, int64_t dpregate_bstride,
+                     void* dpostgate, int64_t dpostgate_bstride, int B, int H, int L, int halo,
+                     void* workspace, size_t workspace_bytes, void* stream);
+
+/*
  * bffc_fwd_strided with the Hyena / M2 short filter applied to its tensors as the kernels load them: each of u, pregate
  * and postgate is replaced by
  *

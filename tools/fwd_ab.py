@@ -52,6 +52,8 @@ def _card():
 def load(path):
     lib = ctypes.CDLL(os.path.abspath(path))
     for name, (res, args) in _lib.SYMBOLS.items():
+        if not hasattr(lib, name):        # a build from before the symbol was added: this tool does not call it
+            continue
         fn = getattr(lib, name)
         fn.restype, fn.argtypes = res, args
     return lib
