@@ -221,6 +221,15 @@ struct bffc_plan {
   // 1/64 with the (unscaled) k_f in pass 3, 1/sqrt(R) per direction in the outer stages (lev[i].scale; the
   // tensor-core level folds it into its twiddles).  The two spectra multiplied into dk_f then both carry
   // 1/sqrt(rblk) and 1/sqrt(R) per outer level: the gradient transforms undo the product.
+  // Range (tests/test_dynamic_range_gpu.py).  fp16: a coherent component of amplitude A (one bin) is rounded to fp16 as
+  // sqrt(N)/8 * A in passes 1 and 3 and after stage 1 of the dk_f kernel, so outputs, du and either input of dk overflow
+  // to inf past C(N) = 65504 * 8 / sqrt(N) (5790 at 8192, 512 at 1M, 256 at 4M; measured: the first power of two above
+  // C(N) or the one below).  White signals keep rel-L2 <= 1e-2 down to an output rms of 2^-14 (1.2-2.1e-2 at 2^-16): the pass-3 value
+  // of a flat spectrum is rms/8 and reaches fp16's subnormals there.  kf_scale sets both edges: moving it moves the
+  // ceiling and the floor by the same factor, and fp16's ~2^40 (subnormals included) cannot hold both at 4M.
+  // bf16: exact power-of-two scaling of every input by 2^-60 .. 2^60 (bit for bit).  A NaN or inf reaches the unit of
+  // its (batch member, channel): the pair b, b ^ 1, below 8192 all 2 * 8192/N members of the 8192-point unit; the
+  // filter-side transforms pair channels 2j, 2j + 1 (every kf_from_filter, the composite sizes' dk_from_dkf).
   float kf_pack_scale;   // k_f: 1/N (bf16), 1 (fp16)
   float tw_scale;        // stage-1 twiddles: 1 (bf16), 1/sqrt(rblk) (fp16)
   float dk_scale;        // dk_f: 1 (bf16), rblk * R (fp16)

@@ -25,6 +25,14 @@
  * legacy default stream).  The caller owns every buffer.  Return value 0 = success, non-zero =
  * error; bffc_last_error() gives a message (thread-local).  No CPU fallback exists: on a machine
  * without an sm_90 GPU every compute entry point fails with BFFC_ERR_NO_DEVICE.
+ *
+ * Range.  FP16 plans: a coherent component (one frequency) of amplitude A in u, dout, or y overflows to inf past
+ * C(N) = 65504 * 8 / sqrt(N) (5790 at N = 8192, 512 at 1M, 256 at 4M; measured on an H100: the first power of two
+ * above C(N), or the one below); white signals keep rel-L2 <= 1e-2 down to an output rms of 2^-14 (1.2-2.1e-2 at 2^-16).  BF16 plans
+ * scale exactly: inputs multiplied by 2^e, |e| <= 60, give outputs multiplied by 2^e bit for bit.  A NaN or inf in one
+ * (batch member, channel) row reaches the rows that share its transform: members b and b ^ 1, and below seqlen 8192 all
+ * 2 * 8192/seqlen members b' with b' / (2 * 8192/seqlen) == b / (2 * 8192/seqlen); in k, or in dk at seqlen > 8192,
+ * channels h and h ^ 1 (the filter-side transforms pack two channels into one complex FFT).  No other row changes.
  */
 #ifndef BFFC_H_
 #define BFFC_H_

@@ -6,7 +6,10 @@ Test infrastructure only.  It mirrors, stage by stage, the accumulator images th
 layouts and the k_f "engine order" are right before any GPU time is spent.
 
 `quant=True` rounds every tensor-core operand to bf16 exactly where the kernel does, which gives the
-expected rel-L2 error of the real kernel.
+expected rel-L2 error of the real kernel.  `fp16=True` is the fp16 plan instead (bffc.cu, normalisation note at bffc_plan):
+operands rounded to fp16, the stage-1 twiddles scaled 1/sqrt(stage-1 radix) (passes 1 and 5), k_f unscaled with 1/64 in
+pass 3, and the output stored as fp16.  A value past 65504 becomes inf where it is rounded, as the kernel's fp16
+conversions do, and 0 * inf = NaN spreads it through the tensor-core stages.
 
 Round 2 additions: `model_fwd_small` / `model_dk_small` (8192/N batch members per tile as independent N-point circular
 convolutions through a block-diagonal stage 1) and `model_filter_composite` (the column + row decomposition of the
@@ -30,15 +33,26 @@ def bf16_round(x):
 
 
 def half_round(x):
-    return np.asarray(x, dtype=np.float16).astype(np.float64)
+    with np.errstate(over='ignore', invalid='ignore'):
+        return np.asarray(x, dtype=np.float16).astype(np.float64)
 
 
-def model_fwd(x0, x1, kf_nat, quant=False, ksteps=8):
+def _rounding(quant, fp16):
+    """(operand rounding, twiddle rounding) of the bf16 plan (quant), the fp16 plan, or exact arithmetic"""
+    if fp16:
+        return half_round, half_round
+    exact = lambda v: np.asarray(v, dtype=np.float64)
+    return (bf16_round, half_round) if quant else (exact, exact)
+
+
+@np.errstate(over='ignore', invalid='ignore')        # fp16: inf and NaN are results, see the module docstring
+def model_fwd(x0, x1, kf_nat, quant=False, ksteps=8, fp16=False):
     """x0, x1: real sequences (length L <= N, zero padded here); kf_nat: FFT_N(k) natural order (complex).
     Returns (y0, y1, stages) with stages = list of four (128,128) float64 accumulator images
-    (cols [0,64) real part, [64,128) imaginary part): D1 outer DFT, D2 spectrum, D3 after inverse radix-64, D4."""
-    q = bf16_round if quant else (lambda v: np.asarray(v, dtype=np.float64))
-    qh = half_round if quant else (lambda v: np.asarray(v, dtype=np.float64))
+    (cols [0,64) real part, [64,128) imaginary part): D1 outer DFT, D2 spectrum, D3 after inverse radix-64, D4.
+    fp16: the fp16 plan's scaling and rounding points (module docstring)."""
+    q, qh = _rounding(quant, fp16)
+    ts = 1 / np.sqrt(R) if fp16 else 1.0
     xr = np.zeros(N); xr[: len(x0)] = x0
     xi = np.zeros(N); xi[: len(x1)] = x1
     Xr = q(xr.reshape(R, M)); Xi = q(xi.reshape(R, M))       # tiles [i][j]
@@ -54,7 +68,7 @@ def model_fwd(x0, x1, kf_nat, quant=False, ksteps=8):
     Y = Dre + 1j * Dim                                         # [k1][j]
     k1 = np.arange(R)[:, None]
     j = np.arange(M)[None, :]
-    tw = np.exp(-2j * np.pi * ((k1 * j) % N) / N)
+    tw = np.exp(-2j * np.pi * ((k1 * j) % N) / N) * ts
     tw = qh(tw.real) + 1j * qh(tw.imag)                        # kernel keeps the twiddles as half2
     # pass 1
     Y1 = Y * tw
@@ -65,10 +79,10 @@ def model_fwd(x0, x1, kf_nat, quant=False, ksteps=8):
     G = q(np.cos(angg)) + 1j * q(np.sin(angg))
     Z = Y1 @ G                                                  # [k1][k2]
     stages.append(np.concatenate([Z.real, Z.imag], axis=1))
-    # pass 3: * k_f[k1 + 128*k2] / N, bf16
-    kfe = (np.asarray(kf_nat).reshape(M, R).T) / N             # [k1][k2]
+    # pass 3: * k_f[k1 + 128*k2] / N (bf16); fp16: * k_f[k1 + 128*k2] / 64
+    kfe = np.asarray(kf_nat).reshape(M, R).T / (1 if fp16 else N)     # [k1][k2]
     kfe = q(kfe.real) + 1j * q(kfe.imag)
-    V = Z * kfe
+    V = Z * kfe / (M if fp16 else 1)
     V = q(V.real) + 1j * q(V.imag)
     # stage 3: inverse radix-64
     Yi = V @ np.conj(G)                                         # [k1][j]
@@ -80,6 +94,8 @@ def model_fwd(x0, x1, kf_nat, quant=False, ksteps=8):
     Ore = C @ Yr - S @ Yim
     Oim = C @ Yim + S @ Yr
     stages.append(np.concatenate([Ore, Oim], axis=1))
+    if fp16:                                                   # the output is stored as fp16
+        Ore, Oim = qh(Ore), qh(Oim)
     return Ore.reshape(-1), Oim.reshape(-1), stages
 
 
@@ -89,17 +105,19 @@ def ref_conv(x, k, n=N):
     return np.fft.ifft(np.fft.fft(x, n) * np.fft.fft(k, n)).real[:L]
 
 
-def model_fwd_small(xs0, xs1, k, Nsmall, quant=False):
+@np.errstate(over='ignore', invalid='ignore')
+def model_fwd_small(xs0, xs1, k, Nsmall, quant=False, fp16=False):
     """Small sizes (fwd3_r128.cuh with the block-diagonal stage 1, r128_common.cuh): Q = 8192/Nsmall batch members per
     tile, member m in tile rows [m r, (m+1) r), r = Nsmall/64.  xs0 / xs1: (Q, L <= Nsmall) real members of the two
     tiles; k: real filter (Lk <= Nsmall).  Every member is an independent Nsmall-point CIRCULAR convolution:
         stage 1  = I_Q (x) F_r            (DFT-128 table replaced by a block-diagonal one)
         twiddle  = W_Nsmall^{(k1 mod r) j}
         k_f      = K_Nsmall[(k1 mod r) + r k2]  = K_8192[((k1 mod r) + r k2) * Q], replicated over the Q blocks
-    everything else is model_fwd().  Returns (y0, y1): (Q, Nsmall) each."""
-    q = bf16_round if quant else (lambda v: np.asarray(v, dtype=np.float64))
-    qh = half_round if quant else (lambda v: np.asarray(v, dtype=np.float64))
+    everything else is model_fwd().  Returns (y0, y1): (Q, Nsmall) each.  fp16: as for model_fwd, with the twiddles
+    scaled 1/sqrt(r)."""
+    q, qh = _rounding(quant, fp16)
     Q, r = N // Nsmall, Nsmall // M
+    ts = 1 / np.sqrt(r) if fp16 else 1.0
     def tile(xs):
         t = np.zeros((Q, Nsmall))
         t[:, : xs.shape[1]] = xs
@@ -112,7 +130,7 @@ def model_fwd_small(xs0, xs1, k, Nsmall, quant=False):
     Y = (C @ Xr + S @ Xi) + 1j * (C @ Xi - S @ Xr)             # [k1][j], k1 = m r + k1'
     k1p = (np.arange(R) % r)[:, None]
     j = np.arange(M)[None, :]
-    tw = np.exp(-2j * np.pi * ((k1p * j) % Nsmall) / Nsmall)
+    tw = np.exp(-2j * np.pi * ((k1p * j) % Nsmall) / Nsmall) * ts
     tw = qh(tw.real) + 1j * qh(tw.imag)
     Y1 = Y * tw
     Y1 = q(Y1.real) + 1j * q(Y1.imag)
@@ -122,14 +140,16 @@ def model_fwd_small(xs0, xs1, k, Nsmall, quant=False):
     Z = Y1 @ G                                                  # [k1][k2]: frequency k1' + r k2 of member k1 // r
     kf8192 = np.fft.fft(k, N)                                   # what the filter-side kernel computes (zero-extended k)
     f_small = k1p + r * np.arange(M)[None, :]
-    kfe = kf8192[f_small * Q] / Nsmall                          # sampled at multiples of Q = the Nsmall-point spectrum
+    kfe = kf8192[f_small * Q] / (1 if fp16 else Nsmall)        # sampled at multiples of Q = the Nsmall-point spectrum
     kfe = q(kfe.real) + 1j * q(kfe.imag)
-    V = Z * kfe
+    V = Z * kfe / (M if fp16 else 1)
     V = q(V.real) + 1j * q(V.imag)
     Yi = (V @ np.conj(G)) * np.conj(tw)
     Yr, Yim = q(Yi.real), q(Yi.imag)
     Ore = C @ Yr - S @ Yim
     Oim = C @ Yim + S @ Yr
+    if fp16:
+        Ore, Oim = qh(Ore), qh(Oim)
     return Ore.reshape(Q, Nsmall), Oim.reshape(Q, Nsmall)
 
 

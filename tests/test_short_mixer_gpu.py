@@ -13,7 +13,7 @@
    fp32 atomics, so with three or more pairs its bits depend on the order in which they land, in both paths alike.
 3. fp64 reference (test_short_mixer.ref_operator) with the spectral statistic and thresholds of test_spectral_gpu.py.
 4. Negative control: perturbing one tap of x1, x2 or v alone changes y.
-5. Fusion: no depthwise kernel in the forward (torch.profiler); forward peak memory above the inputs at least 6*B*D*L
+5. Fusion: no depthwise kernel in the forward (torch.profiler, in a child process); forward peak memory above the inputs at least 6*B*D*L
    bytes (the s tensor) below the composition's; no s-sized tensor saved for backward.
 6. Launch counts: forward and backward with a residual filter count both engine calls.
 """
@@ -199,8 +199,43 @@ def _fwd_peak(fn):
     return peak
 
 
+# The profiled forward runs in a child process of its own, as the profiled backward of test_short_mixer_bwd_gpu.py does:
+# a second profiler session in one process (the next size, or a later test) can come back without any CUDA event.
+_PROFILE_FORWARD = r'''
+import sys
+sys.path.insert(0, 'tests')
+import torch
+import __graft_entry__ as ge
+ge.build()
+import flashfftconv as ffc
+from test_short_mixer_gpu import _make
+N, B, D = int(sys.argv[1]), 8, 64
+conv, sf, x, k, _, _ = _make(ffc, N, N, B, D, 3, 1, torch.bfloat16, torch.float32, seed=1, residual=False)
+conv.eval()
+with torch.no_grad():
+    ffc.hyena_operator(conv, sf, x, k, D), ffc.hyena_mixer(conv, sf(x)[..., :N], k, D)   # warm-up: plans, cached k_f
+    torch.cuda.synchronize()
+    with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
+        ffc.hyena_operator(conv, sf, x, k, D)
+        torch.cuda.synchronize()
+for e in prof.events():
+    if e.device_type == torch.autograd.DeviceType.CUDA:
+        print('KERNEL', e.name)
+'''
+
+
 @pytest.mark.parametrize('N', [8192, 32 * KI])
 def test_fusion_happened(ffc, N):
+    import os
+    import subprocess
+    import sys
+    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+    cmd = [sys.executable] + (['-s'] if sys.flags.no_user_site else []) + ['-c', _PROFILE_FORWARD, str(N)]
+    r = subprocess.run(cmd, cwd=root, capture_output=True, text=True, timeout=600)
+    assert r.returncode == 0, r.stderr[-3000:]
+    names = [ln[len('KERNEL '):] for ln in r.stdout.splitlines() if ln.startswith('KERNEL ')]
+    assert names, 'profiler saw no kernels'
+    assert not [n for n in names if 'dw::' in n or 'dwconv' in n], names
     B, D, L = 8, 64, N
     conv, sf, x, k, _, _ = _make(ffc, N, L, B, D, 3, 1, torch.bfloat16, torch.float32, seed=1, residual=False)
     conv.eval()
@@ -208,12 +243,6 @@ def test_fusion_happened(ffc, N):
     comp = lambda: ffc.hyena_mixer(conv, sf(x)[..., :L], k, D)
     with torch.no_grad():
         fused(), comp()                # warm-up: plans, cached filter spectrum
-        with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
-            fused()
-            torch.cuda.synchronize()
-        names = [e.name for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA]
-        assert names, 'profiler saw no kernels'
-        assert not [n for n in names if 'dw::' in n or 'dwconv' in n], names
         peak_b, peak_a = _fwd_peak(fused), _fwd_peak(comp)
     assert peak_a - peak_b >= 6 * B * D * L, f'peak above inputs: composition {peak_a} B, fused {peak_b} B'
     # training: nothing s-sized is saved apart from x itself
