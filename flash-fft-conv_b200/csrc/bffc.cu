@@ -63,6 +63,11 @@ bool aligned16(T*... q) {
 
 constexpr double kPi = 3.14159265358979323846;
 
+// CUDA's largest gridDim.y / gridDim.z.  Every launch that puts channels, batch pairs or channel pairs there walks them
+// in groups of at most this many (chunk_view, kf_pack, dkf_unpack, the filter-side channel groups), so no shape within
+// `int` range is refused for its grid.
+constexpr int kMaxGridYZ = 65535;
+
 typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
                                     const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
                                     CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
@@ -252,17 +257,22 @@ template <bool kHalf>
 static int kf_pack(const bffc_plan* p, const void* src, void* kf_engine, int H, int conj, void* stream, const char* name) {
   if (!p || !src || !kf_engine || H <= 0) return fail(BFFC_ERR_INVALID, "%s: bad argument", name);
   const cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const float2* s = static_cast<const float2*>(src);
-  if (p->R0 >= 32) {
-    const dim3 grid(kInner / 2 / 32, (p->R0 / 32) * p->R1, H);
-    FMT_SWITCH(p->dtype, (kf_pack_tiled_kernel<kHalf, F><<<grid, dim3(32, 8), 0, st>>>(
-        s, static_cast<uint2*>(kf_engine), p->NE, p->R0, p->R1, p->kf_pack_scale, conj)););
-  } else {
-    const dim3 grid(std::min((p->NE / 4 + 255) / 256, 32), H);
-    FMT_SWITCH(p->dtype, (kf_pack_kernel<kHalf, F><<<grid, 256, 0, st>>>(
-        s, static_cast<uint4*>(kf_engine), p->NE, p->R0, p->R1, p->kf_pack_scale, conj, p->rblk)););
+  const size_t src_row = kHalf ? p->NE / 2 + 1 : p->NE;       // float2 per channel of the source
+  for (int h0 = 0; h0 < H; h0 += kMaxGridYZ) {                 // channels go to gridDim.y / z
+    const int Hc = std::min(kMaxGridYZ, H - h0);
+    const float2* s = static_cast<const float2*>(src) + size_t(h0) * src_row;
+    uint32_t* dst = static_cast<uint32_t*>(kf_engine) + size_t(h0) * p->NE;
+    if (p->R0 >= 32) {
+      const dim3 grid(kInner / 2 / 32, (p->R0 / 32) * p->R1, Hc);
+      FMT_SWITCH(p->dtype, (kf_pack_tiled_kernel<kHalf, F><<<grid, dim3(32, 8), 0, st>>>(
+          s, reinterpret_cast<uint2*>(dst), p->NE, p->R0, p->R1, p->kf_pack_scale, conj)););
+    } else {
+      const dim3 grid(std::min((p->NE / 4 + 255) / 256, 32), Hc);
+      FMT_SWITCH(p->dtype, (kf_pack_kernel<kHalf, F><<<grid, 256, 0, st>>>(
+          s, reinterpret_cast<uint4*>(dst), p->NE, p->R0, p->R1, p->kf_pack_scale, conj, p->rblk)););
+    }
+    CUDA_TRY(cudaGetLastError());
   }
-  CUDA_TRY(cudaGetLastError());
   return BFFC_OK;
 }
 
@@ -271,18 +281,22 @@ static int dkf_unpack(const bffc_plan* p, bool half, const void* dkf_engine, voi
                       const char* name) {
   if (!p || !dkf_engine || !dst || H <= 0) return fail(BFFC_ERR_INVALID, "%s: bad argument", name);
   const cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const float2* src = static_cast<const float2*>(dkf_engine);
-  float2* out = static_cast<float2*>(dst);
+  const size_t out_row = half ? p->NE / 2 + 1 : p->NE;         // float2 per channel of the output
   using namespace bffc::r128;
-  if (p->N < kInner)
-    dkf_unpack_small_kernel<<<dim3(half ? kInner / 2 / 256 + 1 : kInner / 256, H), 256, 0, st>>>(
-        src, out, p->N, p->dk_scale, half ? 1 : 0);
-  else if (half)
-    dkf_unpack_half_kernel<<<dim3(p->R < 32 ? 1 : p->R / 32, 128 * 2, H), 256, 0, st>>>(src, out, p->NE, p->R0, p->R1,
-                                                                                        p->dk_scale);
-  else
-    dkf_unpack_kernel<<<dim3(64, H), 256, 0, st>>>(src, out, p->NE, p->R0, p->R1, p->dk_scale);
-  CUDA_TRY(cudaGetLastError());
+  for (int h0 = 0; h0 < H; h0 += kMaxGridYZ) {                 // channels go to gridDim.y / z
+    const int Hc = std::min(kMaxGridYZ, H - h0);
+    const float2* src = static_cast<const float2*>(dkf_engine) + size_t(h0) * p->NE;
+    float2* out = static_cast<float2*>(dst) + size_t(h0) * out_row;
+    if (p->N < kInner)
+      dkf_unpack_small_kernel<<<dim3(half ? kInner / 2 / 256 + 1 : kInner / 256, Hc), 256, 0, st>>>(
+          src, out, p->N, p->dk_scale, half ? 1 : 0);
+    else if (half)
+      dkf_unpack_half_kernel<<<dim3(p->R < 32 ? 1 : p->R / 32, 128 * 2, Hc), 256, 0, st>>>(src, out, p->NE, p->R0, p->R1,
+                                                                                           p->dk_scale);
+    else
+      dkf_unpack_kernel<<<dim3(64, Hc), 256, 0, st>>>(src, out, p->NE, p->R0, p->R1, p->dk_scale);
+    CUDA_TRY(cudaGetLastError());
+  }
   return BFFC_OK;
 }
 
@@ -486,6 +500,14 @@ size_t bffc_filter_workspace_bytes(const bffc_plan* p, int H) {
   return (pairs < group ? pairs : group) * per;
 }
 
+// channels per group of the composite filter-side transforms, given room for `pairs` channel pairs: the grids put the
+// channel pairs (column launch) and the channels (row launch) in gridDim.y, so a group is at most kMaxGridYZ - 1
+// channels (even: a pair never straddles two groups)
+static int filter_group(size_t pairs, int H) {
+  const size_t cap = std::min<size_t>(size_t(H + 1) / 2, (kMaxGridYZ - 1) / 2);
+  return int(std::min(pairs, cap)) * 2;
+}
+
 // band that keeps every frequency of the plan's seqlen grid (min(f, N - f) <= N/2 < band)
 static int full_band(const bffc_plan* p) { return p->N / 2 + 1; }
 
@@ -507,7 +529,7 @@ static int kf_from_filter(const bffc_plan* p, const void* k, int Lk, void* kf_en
   const size_t per = filter_pair_bytes(p);
   if (!workspace || workspace_bytes < per)
     return fail(BFFC_ERR_INVALID, "%s: workspace %zu B < %zu B (one channel pair; see bffc_filter_workspace_bytes)", name, workspace_bytes, per);
-  const int group = int(std::min<size_t>(workspace_bytes / per, size_t(H + 1) / 2)) * 2;   // channels per group
+  const int group = filter_group(workspace_bytes / per, H);
   float2* T = static_cast<float2*>(workspace);
   for (int h0 = 0; h0 < H; h0 += group) {
     const int Hc = std::min(group, H - h0);
@@ -540,7 +562,7 @@ static int dk_from_dkf(const bffc_plan* p, const void* dkf_engine, void* dk, int
   const size_t per = filter_pair_bytes(p);
   if (!workspace || workspace_bytes < per)
     return fail(BFFC_ERR_INVALID, "%s: workspace %zu B < %zu B (one channel pair; see bffc_filter_workspace_bytes)", name, workspace_bytes, per);
-  const int group = int(std::min<size_t>(workspace_bytes / per, size_t(H + 1) / 2)) * 2;
+  const int group = filter_group(workspace_bytes / per, H);
   float2* T = static_cast<float2*>(workspace);
   for (int h0 = 0; h0 < H; h0 += group) {
     const int Hc = std::min(group, H - h0);
@@ -597,20 +619,23 @@ struct View { int B, H, Hs, h0; };
 // first (the k_f rows of a channel are then shared by its batch pairs inside one chunk); a single channel that is too
 // large is cut over batch pairs.  Every chunk pays the launch gaps, prologues and tails of 3-5 persistent launches, so
 // chunks are not cut to L2 size; the budget only bounds the workspace (and with it the peak memory of a call): 4 GB of
-// plane sets per chunk.
+// plane sets per chunk.  The CUDA-core outer stages launch (.., channels, pairs) grids, so a chunk also holds at most
+// kMaxGridYZ channels and kMaxGridYZ batch pairs; only 16K forward chunks reach that (65536 items), and only from
+// H >= 65536 or B >= 131071 on.
 constexpr size_t kPlaneBudget = size_t(4) << 30;
 static View chunk_view(const bffc_plan* p, int B, int H, int sets) {
   const size_t item = size_t(sets) * p->N * 4;                     // one (pair, channel) in all plane sets
   size_t items = kPlaneBudget / item;
   if (items < 1) items = 1;
+  const size_t cap = kMaxGridYZ;
   const int pairs = (B + 1) / 2;
   View v{B, H, H, 0};
-  if (items >= size_t(pairs)) {
-    const size_t hc = items / pairs;
+  if (items >= size_t(pairs) && size_t(pairs) <= cap) {
+    const size_t hc = std::min(items / pairs, cap);
     v.H = hc < size_t(H) ? int(hc) : H;
   } else {
     v.H = 1;
-    v.B = 2 * int(items);
+    v.B = 2 * int(std::min(items, cap));
     if (v.B > B) v.B = B;
   }
   return v;

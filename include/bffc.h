@@ -33,6 +33,16 @@
  * (batch member, channel) row reaches the rows that share its transform: members b and b ^ 1, and below seqlen 8192 all
  * 2 * 8192/seqlen members b' with b' / (2 * 8192/seqlen) == b / (2 * 8192/seqlen); in k, or in dk at seqlen > 8192,
  * channels h and h ^ 1 (the filter-side transforms pack two channels into one complex FFT).  No other row changes.
+ *
+ * Extents.  For the FFT convolution entry points (bffc_fwd*, bffc_bwd*, the filter-side transforms, the packs) B, H
+ * and L are limited only by `int` and device memory, and offsets are 64-bit.  The depthwise entry points also refuse a
+ * shape that needs more than 2^31 - 1 CTAs (bffc_dwconv1d_*: BHL B * D * ceil(L / tile), BLH B * ceil(L / tile) *
+ * ceil(D / chunk)), which can fit in device memory at a small L.  Launches that
+ * put channels, batch pairs or channel pairs in gridDim.y / z walk them in groups of at most 65535 (CUDA's limit), so
+ * launch counts grow past it: seqlen 16384 forward calls run one more chunk per 65535 channels (B <= 2) or 65535 batch
+ * pairs (B >= 131071); bffc_kf_pack*, bffc_dkf_unpack* launch once per 65535 channels; the composite filter-side
+ * transforms use at most 65534 channels per group whatever the workspace (tests/test_extents.py,
+ * tests/test_extents_gpu.py).
  */
 #ifndef BFFC_H_
 #define BFFC_H_

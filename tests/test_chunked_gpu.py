@@ -105,19 +105,22 @@ def ffc():
 
 # ----------------------------------------------------------------------------- mirror of bffc.cu's chunking
 PLANE_BUDGET = 4 << 30         # kPlaneBudget
+GRID_YZ = 65535                # kMaxGridYZ: CUDA's largest gridDim.y / gridDim.z
 
 
 def _nlev(N):
     return sum(r > 1 for r in so.OUTER[N])
 
 
-def _chunk_view(N, B, H, sets):
-    """chunk_view: (batch members, channels) of a full chunk; `sets` plane sets of N-point rows, 4 bytes per element"""
+def _chunk_view(N, B, H, sets, cap=GRID_YZ):
+    """chunk_view: (batch members, channels) of a full chunk; `sets` plane sets of N-point rows, 4 bytes per element.
+    A chunk holds at most `cap` channels and `cap` batch pairs (the outer stages' gridDim.y / z); cap=None: no cap."""
     items = max(PLANE_BUDGET // (sets * N * 4), 1)
     pairs = (B + 1) // 2
-    if items >= pairs:
-        return B, min(items // pairs, H)
-    return min(2 * items, B), 1
+    cap = cap or float('inf')
+    if items >= pairs and pairs <= cap:
+        return B, min(items // pairs, H, cap)
+    return min(2 * min(items, cap), B), 1
 
 
 def _chunks(N, B, H, sets):
