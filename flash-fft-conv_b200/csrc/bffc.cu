@@ -16,6 +16,7 @@
 #include "outer_r128.cuh"
 #include "filter_fft.cuh"
 #include "dwconv1d.cuh"
+#include "decode_step.cuh"
 
 #include <algorithm>
 #include <cmath>
@@ -1660,6 +1661,191 @@ int bffc_dwconv1d_bwd(const void* dout, const void* u, int u_dtype, const void* 
   else if (w_dtype == BFFC_DTYPE_FP16) reduce(Tag<__half>());
   else reduce(Tag<__nv_bfloat16>());
   return launched();
+}
+
+}  // extern "C"
+
+// ------------------------------------------------------------------------------ decoding state and step (no plan)
+namespace {
+
+namespace dec = bffc::decode;
+
+// byte offsets of the parts of a decoding state (include/bffc.h): tail, z cache, s_u cache
+struct StateLayout {
+  size_t tail, zc, vc, total;
+};
+StateLayout state_layout(int B, int H, int max_len, int K, int residual) {
+  const size_t rows = size_t(B) * size_t(H), cache = align256(rows * size_t(max_len) * 2);
+  StateLayout s;
+  s.tail = 0;
+  s.zc = align256(3 * rows * size_t(K - 1) * 2);
+  s.vc = s.zc + cache;
+  s.total = s.vc + (residual ? cache : 0);
+  return s;
+}
+
+size_t step_workspace_bytes(int B, int H, int T, int Lk, int Lk2) {
+  const size_t nck = (size_t(Lk) + dec::kChunk - 1) / dec::kChunk, nck2 = (size_t(Lk2) + dec::kChunk - 1) / dec::kChunk;
+  return (dec::kHeaderFloats + size_t(B) * H * T * (1 + nck + nck2)) * sizeof(float);
+}
+
+// The arguments the fill and the step share, checked before the device is looked at.  x / bs: the raw inputs of the
+// roles u, pregate, postgate with their batch strides; len: their row length (L of the prompt, T of a step).
+int decode_args(const char* fn, int dtype, int B, int H, int len, int max_len, int K, int padding, int w_dtype,
+                const void* const (&x)[3], const int64_t (&bs)[3], const void* const (&w)[3],
+                const void* const (&bias)[3], int residual, const void* state, size_t state_bytes, const int64_t* pos) {
+  if (dtype != BFFC_DTYPE_BF16 && dtype != BFFC_DTYPE_FP16) return fail(BFFC_ERR_INVALID, "%s: dtype %d (BF16 0, FP16 1)", fn, dtype);
+  if (K < 1 || K > dec::kMaxK) return fail(BFFC_ERR_INVALID, "%s: K=%d outside [1, %d]", fn, K, dec::kMaxK);
+  if (padding != K - 1)
+    return fail(BFFC_ERR_INVALID, "%s: padding %d is not the causal padding K - 1 = %d (a smaller padding reads "
+                "inputs after the position it filters)", fn, padding, K - 1);
+  if (w_dtype != BFFC_DTYPE_BF16 && w_dtype != BFFC_DTYPE_FP16 && w_dtype != BFFC_DTYPE_FP32)
+    return fail(BFFC_ERR_INVALID, "%s: w_dtype %d (BF16 0, FP16 1, FP32 2)", fn, w_dtype);
+  if (B < 1 || H < 1 || max_len < 1 || len < 0 || len > max_len)
+    return fail(BFFC_ERR_INVALID, "%s: bad shape B=%d H=%d length %d max_len=%d", fn, B, H, len, max_len);
+  const size_t ew = w_dtype == BFFC_DTYPE_FP32 ? 4 : 2;
+  for (int r = 0; r < 3; ++r) {
+    if (bias[r] && !w[r]) return fail(BFFC_ERR_INVALID, "%s: a bias needs the taps of its tensor", fn);
+    if (w[r] && !x[r] && len > 0) return fail(BFFC_ERR_INVALID, "%s: taps for an absent input", fn);
+    if (reinterpret_cast<uintptr_t>(w[r]) % ew || reinterpret_cast<uintptr_t>(bias[r]) % ew)
+      return fail(BFFC_ERR_INVALID, "%s: taps not aligned to their element", fn);
+    if (!x[r]) continue;
+    if (reinterpret_cast<uintptr_t>(x[r]) % 2) return fail(BFFC_ERR_INVALID, "%s: input not aligned to its element", fn);
+    if (bs[r] < int64_t(H) * len)
+      return fail(BFFC_ERR_INVALID, "%s: batch stride %lld below H * length = %lld", fn, (long long)bs[r],
+                  (long long)H * len);
+  }
+  if (!x[0] && len > 0) return fail(BFFC_ERR_INVALID, "%s: null u", fn);
+  if (!state || reinterpret_cast<uintptr_t>(state) % 16) return fail(BFFC_ERR_INVALID, "%s: state null or not 16-byte aligned", fn);
+  const size_t need = state_layout(B, H, max_len, K, residual).total;
+  if (state_bytes < need) return fail(BFFC_ERR_INVALID, "%s: state of %zu bytes required", fn, need);
+  if (!pos || reinterpret_cast<uintptr_t>(pos) % 8) return fail(BFFC_ERR_INVALID, "%s: pos null or not 8-byte aligned", fn);
+  return 0;
+}
+
+dec::Params decode_params(int B, int H, int max_len, int K, int residual, void* state, int64_t* pos,
+                          const void* const (&x)[3], const int64_t (&bs)[3], const void* const (&w)[3],
+                          const void* const (&bias)[3]) {
+  const StateLayout lay = state_layout(B, H, max_len, K, residual);
+  uint8_t* st = static_cast<uint8_t*>(state);
+  dec::Params p{};
+  for (int r = 0; r < 3; ++r) p.r[r] = dec::Role{x[r], bs[r], w[r], bias[r]};
+  p.tail = st + lay.tail;
+  p.zc = st + lay.zc;
+  p.vc = residual ? st + lay.vc : nullptr;
+  p.pos = reinterpret_cast<long long*>(pos);
+  p.B = B; p.H = H; p.K = K; p.max_len = max_len;
+  return p;
+}
+
+template <class Fn>
+void decode_dispatch(int dtype, int w_dtype, Fn&& fn) {
+  auto with_w = [&](auto tt) {
+    if (w_dtype == BFFC_DTYPE_FP32) fn(tt, Tag<float>());
+    else if (w_dtype == BFFC_DTYPE_FP16) fn(tt, Tag<__half>());
+    else fn(tt, Tag<__nv_bfloat16>());
+  };
+  if (dtype == BFFC_DTYPE_FP16) with_w(Tag<__half>());
+  else with_w(Tag<__nv_bfloat16>());
+}
+
+}  // namespace
+
+extern "C" {
+
+size_t bffc_conv_state_bytes(int B, int H, int max_len, int K, int has_residual, int dtype) {
+  if (B < 1 || H < 1 || max_len < 1 || K < 1 || K > dec::kMaxK || (dtype != BFFC_DTYPE_BF16 && dtype != BFFC_DTYPE_FP16))
+    return 0;
+  return state_layout(B, H, max_len, K, has_residual != 0).total;
+}
+
+size_t bffc_conv_step_workspace_bytes(int B, int H, int T, int Lk, int Lk2) {
+  if (B < 1 || H < 1 || T < 1 || T > dec::kMaxT || Lk < 1 || Lk2 < 0) return 0;
+  return step_workspace_bytes(B, H, T, Lk, Lk2);
+}
+
+int bffc_conv_state_fill(const void* u, int64_t u_bstride, const void* pregate, int64_t pregate_bstride,
+                         const void* postgate, int64_t postgate_bstride, const void* u_w, const void* u_bias,
+                         const void* pregate_w, const void* pregate_bias, const void* postgate_w,
+                         const void* postgate_bias, int w_dtype, int K, int padding, int dtype, int B, int H, int L,
+                         int max_len, int has_residual, void* state, size_t state_bytes, int64_t* pos, void* stream) {
+  const char* fn = "bffc_conv_state_fill";
+  const void* const x[3] = {u, pregate, postgate};
+  const int64_t bs[3] = {u_bstride, pregate_bstride, postgate_bstride};
+  const void* const w[3] = {u_w, pregate_w, postgate_w};
+  const void* const bias[3] = {u_bias, pregate_bias, postgate_bias};
+  const int residual = has_residual != 0;
+  if (int rc = decode_args(fn, dtype, B, H, L, max_len, K, padding, w_dtype, x, bs, w, bias, residual, state,
+                           state_bytes, pos))
+    return rc;
+  if (int rc = check_device()) return rc;
+  dec::Params p = decode_params(B, H, max_len, K, residual, state, pos, x, bs, w, bias);
+  if (L == 0)
+    for (auto& r : p.r) r = dec::Role{};
+  const dim3 grid(unsigned((std::max(L, 1) + dec::kThreads - 1) / dec::kThreads), unsigned(std::min(H, kMaxGridYZ)),
+                  unsigned(std::min(B, kMaxGridYZ)));
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  g_launches = 0;
+  decode_dispatch(dtype, w_dtype, [&](auto tt, auto tw) {
+    using T = typename decltype(tt)::type;
+    using W = typename decltype(tw)::type;
+    dec::state_fill<T, W><<<grid, dec::kThreads, 0, st>>>(p, L);
+  });
+  return launched();
+}
+
+int bffc_conv_step(const void* u, int64_t u_bstride, const void* pregate, int64_t pregate_bstride, const void* postgate,
+                   int64_t postgate_bstride, const void* k, int Lk, const void* k2, int Lk2, const void* u_w,
+                   const void* u_bias, const void* pregate_w, const void* pregate_bias, const void* postgate_w,
+                   const void* postgate_bias, int w_dtype, int K, int padding, int dtype, void* state,
+                   size_t state_bytes, int64_t* pos, void* y, int64_t y_bstride, int B, int H, int T, int max_len,
+                   void* workspace, size_t workspace_bytes, void* stream) {
+  const char* fn = "bffc_conv_step";
+  const void* const x[3] = {u, pregate, postgate};
+  const int64_t bs[3] = {u_bstride, pregate_bstride, postgate_bstride};
+  const void* const w[3] = {u_w, pregate_w, postgate_w};
+  const void* const bias[3] = {u_bias, pregate_bias, postgate_bias};
+  const int residual = k2 != nullptr;
+  if (T < 1 || T > dec::kMaxT) return fail(BFFC_ERR_INVALID, "%s: T=%d outside [1, %d]", fn, T, dec::kMaxT);
+  if (int rc = decode_args(fn, dtype, B, H, T, max_len, K, padding, w_dtype, x, bs, w, bias, residual, state,
+                           state_bytes, pos))
+    return rc;
+  if (!k || reinterpret_cast<uintptr_t>(k) % 4 || reinterpret_cast<uintptr_t>(k2) % 4)
+    return fail(BFFC_ERR_INVALID, "%s: k null, or k / k2 not 4-byte aligned", fn);
+  if (Lk < 1 || Lk > max_len) return fail(BFFC_ERR_INVALID, "%s: Lk=%d outside [1, max_len=%d]", fn, Lk, max_len);
+  if (k2 && (Lk2 < 1 || Lk2 > max_len))
+    return fail(BFFC_ERR_INVALID, "%s: Lk2=%d outside [1, max_len=%d]", fn, Lk2, max_len);
+  if (!k2) Lk2 = 0;
+  if (!y || reinterpret_cast<uintptr_t>(y) % 2) return fail(BFFC_ERR_INVALID, "%s: y null or not aligned to its element", fn);
+  if (y_bstride < int64_t(H) * T)
+    return fail(BFFC_ERR_INVALID, "%s: batch stride %lld below H * length = %lld", fn, (long long)y_bstride, (long long)H * T);
+  const size_t need = step_workspace_bytes(B, H, T, Lk, Lk2);
+  if (!workspace || reinterpret_cast<uintptr_t>(workspace) % 16 || workspace_bytes < need)
+    return fail(BFFC_ERR_INVALID, "%s: a 16-byte aligned workspace of %zu bytes required", fn, need);
+  if (int rc = check_device()) return rc;
+  dec::Params p = decode_params(B, H, max_len, K, residual, state, pos, x, bs, w, bias);
+  p.k = static_cast<const float*>(k);
+  p.k2 = static_cast<const float*>(k2);
+  p.Lk = Lk; p.Lk2 = Lk2;
+  p.nck = (Lk + dec::kChunk - 1) / dec::kChunk;
+  p.nck2 = (Lk2 + dec::kChunk - 1) / dec::kChunk;
+  p.y = y; p.y_bs = y_bstride; p.T = T;
+  p.ws = static_cast<float*>(workspace);
+  const dim3 grid1(unsigned(std::max(p.nck, p.nck2)), unsigned(std::min(H, kMaxGridYZ)));
+  const long long outs = dec::outputs(p);
+  const unsigned grid2 = unsigned(std::min<long long>((outs + dec::kThreads - 1) / dec::kThreads, kMaxGridYZ));
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  g_launches = 0;
+  int rc = 0;
+  decode_dispatch(dtype, w_dtype, [&](auto tt, auto tw) {
+    using T_ = typename decltype(tt)::type;
+    using W = typename decltype(tw)::type;
+    dec::step_lags<T_, W><<<grid1, dec::kThreads, 0, st>>>(p);
+    if ((rc = launched())) return;
+    dec::step_finish<T_><<<grid2, dec::kThreads, 0, st>>>(p);
+    rc = launched();
+  });
+  return rc;
 }
 
 }  // extern "C"

@@ -3,3 +3,4 @@ from .depthwise_1d import FlashDepthWiseConv1d  # noqa: F401  (reference flashff
 from .gated import gated_long_conv, hyena_mixer, hyena_operator  # noqa: F401
 from .sparse_conv import PartialFFTConv, FrequencySparseFFTConv  # noqa: F401  (reference flashfftconv/sparse_conv.py)
 from .block_conv import blocked_long_conv  # noqa: F401
+from .decode import HyenaDecoder, LongConvDecoder  # noqa: F401

@@ -1,0 +1,339 @@
+"""Token-by-token decoding of the causal long convolution: generation after the prompt.
+
+Each new output of y = postgate * conv(u * pregate, k) needs one dot product per channel over the cached past,
+y_t = postgate_t * sum_m k[m] z[t - m] with z = u * pregate, so a step streams k and a cache of z once instead of
+convolving the whole prefix again.  Both decoders keep that cache on the device (bffc_conv_state_fill /
+bffc_conv_step, include/bffc.h):
+
+    dec = HyenaDecoder(short_filter, k, d_model, batch, max_len, residual_filter=None, dtype=torch.bfloat16)
+    y_prompt = dec.prefill(x_prompt)     # (B, 3D, L) -> (B, D, L); L may be 0
+    y_new = dec.step(x_new)              # (B, 3D, T) -> (B, D, T), 1 <= T <= 64
+
+    lc = LongConvDecoder(k, batch, max_len, dtype)
+    y = lc.prefill(u, pregate, postgate); y_t = lc.step(u_t, pregate_t, postgate_t)     # gates optional
+
+HyenaDecoder is hyena_operator(conv, short_filter, x, k, d_model, residual_filter) position by position, for a causal
+short filter (padding = K - 1, the original Hyena / HyenaDNA models); LongConvDecoder is FlashFFTConv's gated
+convolution.  prefill computes y of the prompt with the FFT engine and fills the caches; each step appends T tokens.
+A step's outputs do not depend on how the tokens are grouped into steps or on the other batch members, bit for bit.
+
+Limits: inference only (the decoders run under torch.no_grad(); nothing is differentiated); causal short filters only;
+T <= 64 tokens per step (a longer chunk is a prefill); caches in (B, H, max_len) layout.
+
+`step` is capturable in a CUDA graph: the position lives on the device and the step neither allocates in the library
+nor synchronises.  Run one eager step with the same T first (it sizes the workspace), then:
+
+    x_static = x_new.clone()
+    dec.step(x_static)                                  # warm-up: sizes the workspace for this T
+    g = torch.cuda.CUDAGraph()
+    with torch.cuda.graph(g):
+        y_static = dec.step(x_static)
+    for _ in range(n):
+        x_static.copy_(next_tokens())                   # (B, 3D, T)
+        g.replay()                                      # y_static holds the outputs, dec.pos advanced by T
+
+A graph replay past max_len writes nothing and sets a device flag that reading `dec.pos` reports.
+"""
+import ctypes
+
+import torch
+
+from . import _lib
+from . import depthwise_1d as _dw
+from .conv import FlashFFTConv, _DT, _on_device, _ptr, _stream
+from .gated import gated_long_conv, hyena_operator
+
+MAX_STEP_TOKENS = 64
+MAX_KERNEL_SIZE = 32
+
+
+def prefill_seqlen(L, Lk):
+    """FFT size of a prefill of L positions with an Lk-tap filter: the next power of two >= max(256, L + min(Lk, L) - 1),
+    so the circular convolution of the first min(Lk, L) taps does not wrap."""
+    need = max(256, L + min(Lk, L) - 1)
+    return 1 << (need - 1).bit_length()
+
+
+def state_layout(B, H, max_len, K, residual):
+    """(z cache offset, s_u cache offset, total bytes) of a decoding state, the layout include/bffc.h documents and
+    state_layout in bffc.cu computes (tests/test_decode.py checks the total against bffc_conv_state_bytes)."""
+    a256 = lambda n: (n + 255) // 256 * 256
+    zc = a256(6 * B * H * (K - 1))
+    vc = zc + a256(2 * B * H * max_len)
+    return zc, vc, vc + (vc - zc if residual else 0)
+
+
+def _rows(t, H, T):
+    """(tensor, batch stride) of a (B, H, T) view with contiguous rows (element (b, h, t) at b * stride + h * T + t),
+    copying `t` when its layout does not qualify."""
+    _, sh, st = t.stride()
+    if (H > 1 and sh != T) or (T > 1 and st != 1):
+        t = t.contiguous()
+    return t, t.stride(0)
+
+
+def _filter(k, H, max_len, name):
+    """k as the step reads it: contiguous fp32 (the tensor itself when it already is, else a converted copy)"""
+    if k.dim() != 2 or k.shape[0] != H or not 1 <= k.shape[1] <= max_len:
+        raise ValueError(f'{name} must be ({H}, Lk) with 1 <= Lk <= max_len = {max_len}, got {tuple(k.shape)}')
+    if not k.is_cuda:
+        raise ValueError(f'{name} must be a CUDA tensor')
+    return k.detach().to(torch.float32).contiguous()
+
+
+class _Decoder:
+    """The state of one batch of sequences and the two library calls; the subclasses name the roles."""
+
+    def __init__(self, k, k2, H, batch, max_len, dtype, K):
+        if dtype not in _DT:
+            raise ValueError(f'dtype must be torch.bfloat16 or torch.float16, got {dtype}')
+        if batch < 1 or max_len < 1:
+            raise ValueError(f'batch {batch} and max_len {max_len} must be >= 1')
+        self.H, self.batch, self.max_len, self.dtype, self.K = H, int(batch), int(max_len), dtype, K
+        self.k = _filter(k, H, self.max_len, 'k')
+        self.k2 = None if k2 is None else _filter(k2, H, self.max_len, 'residual_filter')
+        self.device = self.k.device
+        dt = _DT[dtype]
+        nbytes = _lib.lib().bffc_conv_state_bytes(self.batch, H, self.max_len, K, int(self.k2 is not None), dt)
+        self.state = torch.zeros(nbytes, dtype=torch.uint8, device=self.device)
+        self._pos = torch.zeros(2, dtype=torch.int64, device=self.device)       # position, status
+        self._host_pos = 0                 # known position, or None after a graph capture
+        self._ws = None
+        # workspaces outgrown by a larger T: a graph captured earlier still writes to the address it was given
+        self._ws_outgrown = []
+        self._convs = {}
+        self.reset()
+
+    # ---- views of the state (include/bffc.h: tail, z cache, s_u cache)
+    def _caches(self):
+        B, H, n, K = self.batch, self.H, self.max_len, self.K
+        zc, vc, _ = state_layout(B, H, n, K, self.k2 is not None)
+        as_dt = lambda off, count: self.state[off:off + 2 * count].view(self.dtype)
+        tail = as_dt(0, 3 * B * H * (K - 1)).view(3, B, H, K - 1)
+        z = as_dt(zc, B * H * n).view(B, H, n)
+        v = as_dt(vc, B * H * n).view(B, H, n) if self.k2 is not None else None
+        return tail, z, v
+
+    @property
+    def z_cache(self):
+        """(B, H, max_len) cache of z = s_u * s_pregate; slots [0, pos) are valid."""
+        return self._caches()[1]
+
+    @property
+    def v_cache(self):
+        """(B, H, max_len) cache of s_u (kept when there is a residual filter), else None."""
+        return self._caches()[2]
+
+    @property
+    def tail(self):
+        """(3, B, H, K - 1) raw inputs of the last K - 1 positions of u, pregate and postgate."""
+        return self._caches()[0]
+
+    @property
+    def pos(self):
+        """Number of positions decoded so far, read from the device (a synchronisation).  Raises when a step ran past
+        max_len (it then wrote nothing)."""
+        pos, status = self._pos.tolist()
+        if status:
+            raise RuntimeError(f'a decoding step would have run past max_len = {self.max_len} and did nothing; '
+                               f'the position is still {pos}')
+        self._host_pos = pos
+        return pos
+
+    def reset(self):
+        """Start over with an empty prompt."""
+        self._fill(None, None, None, 0)
+
+    def _conv(self, L):
+        n = prefill_seqlen(L, max(self.k.shape[1], 0 if self.k2 is None else self.k2.shape[1]))
+        conv = self._convs.get(n)
+        if conv is None:
+            conv = self._convs[n] = FlashFFTConv(n, dtype=self.dtype).eval()
+        return conv
+
+    def _check(self, t, name, T):
+        if t.dim() != 3 or t.shape[0] != self.batch or t.shape[1] != self.H or t.shape[2] != T:
+            raise ValueError(f'{name} must be ({self.batch}, {self.H}, {T}), got {tuple(t.shape)}')
+        if t.dtype != self.dtype or t.device != self.device:
+            raise ValueError(f'{name} must be {self.dtype} on {self.device}, got {t.dtype} on {t.device}')
+
+    def _roles(self, u, pregate, postgate, T):
+        out = []
+        for name, t in (('u', u), ('pregate', pregate), ('postgate', postgate)):
+            if t is None:
+                out.append((None, 0))
+            else:
+                self._check(t, name, T)
+                out.append(_rows(t, self.H, T))
+        return out
+
+    def _tap_args(self):
+        """(rows of the u, pregate, postgate taps and biases, w_dtype) of the short filter; none here"""
+        return [None] * 6, _lib.BFFC_DTYPE_FP32
+
+    def _fill(self, u, pregate, postgate, L):
+        roles = self._roles(u, pregate, postgate, L) if L else [(None, 0)] * 3
+        rows, wdt = self._tap_args() if L else ([None] * 6, _lib.BFFC_DTYPE_FP32)
+        args = [a for t, s in roles for a in (_ptr(t), s)]
+        with _on_device(self.device):
+            _lib.check(_lib.lib().bffc_conv_state_fill(*args, *rows, wdt, self.K, self.K - 1, _DT[self.dtype],
+                                                       self.batch, self.H, L, self.max_len, int(self.k2 is not None),
+                                                       _ptr(self.state), self.state.numel(), _ptr(self._pos),
+                                                       _stream()))
+        self._host_pos = L
+
+    def _step(self, u, pregate, postgate):
+        T = u.shape[-1]
+        if not 1 <= T <= MAX_STEP_TOKENS:
+            raise ValueError(f'a step takes 1 to {MAX_STEP_TOKENS} tokens, got {T} (a longer chunk is a prefill)')
+        capturing = torch.cuda.is_current_stream_capturing()
+        if self._host_pos is not None and not capturing and self._host_pos + T > self.max_len:
+            raise ValueError(f'position {self._host_pos} + {T} tokens exceeds max_len = {self.max_len}')
+        roles = self._roles(u, pregate, postgate, T)
+        rows, wdt = self._tap_args()
+        Lk = self.k.shape[1]
+        Lk2 = 0 if self.k2 is None else self.k2.shape[1]
+        nws = _lib.lib().bffc_conv_step_workspace_bytes(self.batch, self.H, T, Lk, Lk2)
+        if self._ws is None or self._ws.numel() < nws:
+            if capturing:
+                raise RuntimeError(f'run one eager step with T = {T} before capturing it (it sizes the workspace)')
+            if self._ws is not None:
+                self._ws_outgrown.append(self._ws)
+            self._ws = torch.empty(nws, dtype=torch.uint8, device=self.device)
+        y = torch.empty((self.batch, self.H, T), dtype=self.dtype, device=self.device)
+        args = [a for t, s in roles for a in (_ptr(t), s)]
+        with _on_device(self.device):
+            _lib.check(_lib.lib().bffc_conv_step(*args, _ptr(self.k), Lk, _ptr(self.k2), Lk2, *rows, wdt, self.K,
+                                                 self.K - 1, _DT[self.dtype], _ptr(self.state), self.state.numel(),
+                                                 _ptr(self._pos), _ptr(y), self.H * T, self.batch, self.H, T,
+                                                 self.max_len, _ptr(self._ws), self._ws.numel(), _stream()))
+        self._host_pos = None if capturing or self._host_pos is None else self._host_pos + T
+        return y
+
+
+class HyenaDecoder(_Decoder):
+    """hyena_operator(conv, short_filter, x, k, d_model, residual_filter) decoded position by position.
+
+    short_filter: a BHL FlashDepthWiseConv1d(3 * d_model, K, padding=K - 1) (K <= 32); the flash examples' padding
+    (K - 1) / 2 reads one input past the position it filters and cannot be decoded.  k: (d_model, Lk) and
+    residual_filter: (d_model, Lk2), Lk, Lk2 <= max_len; both are taken at construction as contiguous fp32 (the tensors
+    themselves when they already are, so later in-place changes to them are seen; otherwise converted copies).  The
+    short filter's current weights and bias are read at every call.  x: the raw (B, 3 * d_model, T) projection [x1 | x2 | v]:
+
+        s = short_filter(x)[..., :L];  x1, x2, v = s.split(d_model, dim=1)
+        y = x2 * causal_conv(x1 * v, k) [+ causal_conv(v, k2)]
+    """
+
+    def __init__(self, short_filter, k, d_model, batch, max_len, residual_filter=None, dtype=torch.bfloat16):
+        if not isinstance(short_filter, _dw.FlashDepthWiseConv1d) or not short_filter.is_bhl:
+            raise ValueError('short_filter must be a BHL FlashDepthWiseConv1d')
+        if short_filter.d != 3 * d_model:
+            raise ValueError(f'short_filter has {short_filter.d} channels, the projection needs 3 * d_model = '
+                             f'{3 * d_model}')
+        K, P = short_filter.k, int(short_filter.padding)
+        if not 1 <= K <= MAX_KERNEL_SIZE:
+            raise ValueError(f'short filter kernel size {K} outside [1, {MAX_KERNEL_SIZE}]')
+        if P != K - 1:
+            raise ValueError(f'short filter padding {P}: decoding needs the causal padding K - 1 = {K - 1} (padding '
+                             f'{P} makes each output read {K - 1 - P} input(s) after its position)')
+        self.short_filter, self.d_model = short_filter, d_model
+        super().__init__(k, residual_filter, d_model, batch, max_len, dtype, K)
+        self._tap_args()
+
+    def _tap_args(self):
+        """the taps of the short filter's parameters as they are now (a .to(), .half() or load_state_dict(assign=True)
+        replaces their storage)"""
+        w, b, D, K = self.short_filter.weights, self.short_filter.bias, self.d_model, self.K
+        if w.dtype != b.dtype or w.dtype not in _dw._DT or not (w.is_contiguous() and b.is_contiguous()):
+            raise ValueError('short filter weights and bias must be contiguous and of one dtype')
+        if w.device != self.device or b.device != self.device:
+            raise ValueError(f'short filter on {w.device}, k on {self.device}')
+        es = w.element_size()
+        # rows of x1, x2, v in the (3D, K) weight and (3D) bias; roles u = v, pregate = x1, postgate = x2
+        w1, w2, wv = (w.data_ptr() + i * D * K * es for i in range(3))
+        b1, b2, bv = (b.data_ptr() + i * D * es for i in range(3))
+        return [ctypes.c_void_p(a) for a in (wv, bv, w1, b1, w2, b2)], _dw._DT[w.dtype]
+
+    def _split(self, x):
+        if x.dim() != 3 or x.shape[1] != 3 * self.d_model:
+            raise ValueError(f'x must be (B, 3 * d_model = {3 * self.d_model}, T), got {tuple(x.shape)}')
+        x1, x2, v = x.split(self.d_model, dim=1)
+        return v, x1, x2
+
+    @torch.no_grad()
+    def prefill(self, x):
+        """y (B, d_model, L) of the prompt x (B, 3 * d_model, L) by the FFT engine, and the caches filled from it; starts
+        a new sequence.  L may be 0."""
+        L = x.shape[-1]
+        if L > self.max_len:
+            raise ValueError(f'prompt of {L} positions exceeds max_len = {self.max_len}')
+        x = x.contiguous()                 # the short filter takes a contiguous projection
+        v, x1, x2 = self._split(x)
+        if L == 0:
+            self.reset()
+            return x.new_empty((x.shape[0], self.d_model, 0))
+        k = self.k[:, :min(self.k.shape[1], L)]
+        k2 = None if self.k2 is None else self.k2[:, :min(self.k2.shape[1], L)]
+        y = hyena_operator(self._conv(L), self.short_filter, x, k, self.d_model, residual_filter=k2)
+        self._fill(v, x1, x2, L)
+        return y
+
+    @torch.no_grad()
+    def step(self, x):
+        """y (B, d_model, T) of the next T <= 64 positions of the projection x (B, 3 * d_model, T); the three slices are
+        read in place when their rows are contiguous."""
+        v, x1, x2 = self._split(x)
+        return self._step(v, x1, x2)
+
+
+class LongConvDecoder(_Decoder):
+    """y = postgate * causal_conv(u * pregate, k) (FlashFFTConv's gated convolution; either gate may be absent)
+    decoded position by position.  k: (H, Lk), Lk <= max_len, taken at construction as contiguous fp32 (k itself when
+    it already is, else a converted copy).  The gates given to prefill are the gates every step takes: z = u * pregate
+    and z = u must not mix in one cache, so a step with another set of gates is refused."""
+
+    def __init__(self, k, batch, max_len, dtype=torch.bfloat16):
+        self._gates = None                 # (pregate given, postgate given) of this sequence, once known
+        super().__init__(k, None, k.shape[0], batch, max_len, dtype, 1)
+
+    def _same_gates(self, pregate, postgate):
+        gates = (pregate is not None, postgate is not None)
+        if self._gates is not None and gates != self._gates:
+            name = lambda g: {(False, False): 'no gates', (True, False): 'a pregate', (False, True): 'a postgate',
+                              (True, True): 'both gates'}[g]
+            raise ValueError(f'this sequence was started with {name(self._gates)}; a step with {name(gates)} would mix '
+                             'two operators in one cache')
+        self._gates = gates
+
+    def reset(self):
+        """Start over with an empty prompt; the first step sets the gates of the sequence."""
+        self._gates = None
+        super().reset()
+
+    @torch.no_grad()
+    def prefill(self, u, pregate=None, postgate=None):
+        """y (B, H, L) of the prompt by the FFT engine, and the cache filled from it; starts a new sequence."""
+        L = u.shape[-1]
+        if L > self.max_len:
+            raise ValueError(f'prompt of {L} positions exceeds max_len = {self.max_len}')
+        self._roles(u, pregate, postgate, L)
+        if L == 0:
+            self.reset()
+            return torch.empty_like(u)
+        self._gates = None
+        self._same_gates(pregate, postgate)
+        conv = self._conv(L)
+        k = self.k[:, :min(self.k.shape[1], L)]
+        if pregate is None and postgate is None:
+            y = conv(u.contiguous(), k)
+        else:                              # a missing gate is 1: the products with it are exact
+            ones = torch.ones_like(u)
+            y = gated_long_conv(conv, u, k, ones if pregate is None else pregate, ones if postgate is None else postgate)
+        self._fill(u, pregate, postgate, L)
+        return y
+
+    @torch.no_grad()
+    def step(self, u, pregate=None, postgate=None):
+        """y (B, H, T) of the next T <= 64 positions, with the gates the sequence was started with."""
+        self._same_gates(pregate, postgate)
+        return self._step(u, pregate, postgate)

@@ -326,8 +326,64 @@ int bffc_dwconv1d_bwd(const void* dout, const void* u, int u_dtype, const void* 
                       void* dbias, int B, int D, int L, int K, int padding, int layout, void* workspace,
                       size_t workspace_bytes, void* stream);
 
+/*
+ * Decoding: the causal gated long convolution one step at a time, for generation after a prompt (no plan; inference
+ * only).  Per batch member b, channel h and absolute position t < max_len, with the roles c in {u, pregate, postgate}:
+ *
+ *     s_c[t] = round( bias_c[h] + sum_{j<K} w_c[h, j] * x_c[t - (K-1) + j] )     (x_c[< 0] = 0; no taps: s_c = x_c)
+ *     z[t]   = round( s_u[t] * s_pregate[t] )                                   (s_u[t] without a pregate)
+ *     y[t]   = round( s_postgate[t] * sum_{m=0}^{min(t, Lk-1)} k[h, m] z[t-m]  +  sum_{m=0}^{min(t, Lk2-1)} k2[h, m] s_u[t-m] )
+ *
+ * round: to dtype.  s is bffc_dwconv1d_fwd (BHL) with padding K - 1, the only causal padding (padding != K - 1 is
+ * BFFC_ERR_INVALID); z is the 16-bit product the fused forward forms on load.  The sums are fp32; an absent postgate is
+ * 1, an absent k2 drops the second sum.  The Hyena / M2 mixer is u = v, pregate = x1, postgate = x2 with the taps of
+ * its short filter and k2 its residual filter; FlashFFTConv's gated convolution is the same with no taps.
+ *
+ * State (bffc_conv_state_bytes, one device buffer, 16-byte aligned), byte offsets:
+ *   0:                                    tail  (3, B, H, K - 1) dtype: the raw inputs of the last K - 1 positions per role
+ *   zc = align256(6 * B * H * (K - 1)):   z cache (B, H, max_len) dtype
+ *   zc + align256(2 * B * H * max_len):   s_u cache (B, H, max_len) dtype, only with has_residual
+ * pos: device int64[2]: pos[0] the number of positions filled, pos[1] a status word (0 ok, 1: a step would have run past
+ * max_len; it then wrote nothing, neither y nor the state, and pos[0] is unchanged).  The caller reads it outside graph
+ * capture.
+ *
+ * bffc_conv_state_fill: from a raw prompt u / pregate / postgate (B, H, L), element (b, h, t) at x + b * x_bstride +
+ *   h * L + t, writes z (and s_u) into slots [0, L), the tail, pos = {L, 0}.  One launch, bit-identical to the state L
+ *   single steps leave.  0 <= L <= max_len; L = 0 (inputs unread, may be NULL) resets the state to an empty prompt.
+ * bffc_conv_step: T new raw tokens (B, H, T) (x + b * x_bstride + h * T + t), 1 <= T <= 64, at the device position:
+ *   writes their z (and s_u) into slots [pos, pos + T), the tail, y (B, H, T) (y + b * y_bstride + h * T + t) and
+ *   advances pos by T.  k: (H, Lk) fp32, 1 <= Lk <= max_len; k2: (H, Lk2) fp32 or NULL (then Lk2 is ignored; a state
+ *   filled with has_residual is stepped with k2 at every step).  Two launches (bffc_last_launch_count): per 2048 lags
+ *   of each channel one block that reads those k lags once for every batch member and only the cache slots they reach,
+ *   then a fixed-order sum of the per-block partials.  Each output's summation order depends on its position and Lk
+ *   only: T tokens in one step or in T steps, a member alone or in a batch, and repeated runs give the same bits; no
+ *   atomics.  The grid depends on Lk, not on pos, and the step neither allocates nor synchronises, so it can be
+ *   captured in a CUDA graph.  workspace: bffc_conv_step_workspace_bytes(B, H, T, Lk, Lk2) bytes (Lk2 = 0 without k2),
+ *   16-byte aligned.
+ * Taps and NULL conventions as bffc_fwd_short_strided: *_w (H, K), *_bias (H) of w_dtype (BF16, FP16, FP32); NULL taps:
+ * that role is not filtered; NULL bias: 0; a bias without taps, or taps of an absent input, is BFFC_ERR_INVALID.  Either
+ * gate may be absent.  Arguments are validated before the device is looked at: dtype, 1 <= K <= 32, padding = K - 1,
+ * w_dtype, shapes, element alignment of every pointer, batch strides >= H * (row length), T, Lk, Lk2 <= max_len, the
+ * state and workspace sizes give BFFC_ERR_INVALID on any machine.  Offsets are 64-bit; channels and batch members in
+ * gridDim.y / z are walked in groups of at most 65535.
+ */
+size_t bffc_conv_state_bytes(int B, int H, int max_len, int K, int has_residual, int dtype);
+size_t bffc_conv_step_workspace_bytes(int B, int H, int T, int Lk, int Lk2);
+int bffc_conv_state_fill(const void* u, int64_t u_bstride, const void* pregate, int64_t pregate_bstride,
+                         const void* postgate, int64_t postgate_bstride, const void* u_w, const void* u_bias,
+                         const void* pregate_w, const void* pregate_bias, const void* postgate_w,
+                         const void* postgate_bias, int w_dtype, int K, int padding, int dtype, int B, int H, int L,
+                         int max_len, int has_residual, void* state, size_t state_bytes, int64_t* pos, void* stream);
+int bffc_conv_step(const void* u, int64_t u_bstride, const void* pregate, int64_t pregate_bstride, const void* postgate,
+                   int64_t postgate_bstride, const void* k, int Lk, const void* k2, int Lk2, const void* u_w,
+                   const void* u_bias, const void* pregate_w, const void* pregate_bias, const void* postgate_w,
+                   const void* postgate_bias, int w_dtype, int K, int padding, int dtype, void* state,
+                   size_t state_bytes, int64_t* pos, void* y, int64_t y_bstride, int B, int H, int T, int max_len,
+                   void* workspace, size_t workspace_bytes, void* stream);
+
 /* Number of kernel launches the last bffc_fwd / bffc_bwd / bffc_fwd_host / filter-side transform /
- * bffc_dwconv1d_fwd (1) / bffc_dwconv1d_bwd (2) on this thread enqueued (bench.py). */
+ * bffc_dwconv1d_fwd (1) / bffc_dwconv1d_bwd (2) / bffc_conv_state_fill (1) / bffc_conv_step (2) on this thread
+ * enqueued (bench.py). */
 int bffc_last_launch_count(void);
 
 #ifdef __cplusplus
