@@ -1541,16 +1541,19 @@ void dw_dispatch(int u_dtype, int w_dtype, int K, Fn&& fn) {
 
 size_t dw_elem(int dtype) { return dtype == BFFC_DTYPE_FP32 ? 4 : 2; }
 
-// Shape checks shared by the three entry points; fills the launch geometry (backward: its tiles cover du positions
-// [0, L) and dout positions [0, Lout), and `tiles` is the number of parts per batch member).
+// Shape checks shared by the entry points; fills the launch geometry (backward: its tiles cover du positions
+// [0, L) and dout positions [0, Lout), and `tiles` is the number of parts per batch member).  docs: the varlen entry
+// points, whose outputs are the first L of each document's (Lout = L, which needs 2P >= K - 1).
 int dw_geometry(const char* fn, int B, int D, int L, int K, int P, int layout, bool backward, bffc::dw::Shape* sh,
-                long long* ctas) {
+                long long* ctas, bool docs = false) {
   using namespace bffc::dw;
   if (layout != BFFC_LAYOUT_BHL && layout != BFFC_LAYOUT_BLH) return fail(BFFC_ERR_INVALID, "%s: layout %d is not BHL (0) or BLH (1)", fn, layout);
   if (K < 1 || K > kMaxK) return fail(BFFC_ERR_INVALID, "%s: K=%d outside [1, %d]", fn, K, kMaxK);
   if (P < 0 || P > K - 1) return fail(BFFC_ERR_INVALID, "%s: padding %d outside [0, K-1=%d]", fn, P, K - 1);
+  if (docs && 2 * P < K - 1)
+    return fail(BFFC_ERR_INVALID, "%s: padding %d < (K-1)/2: a document's output would be shorter than it", fn, P);
   if (B < 1 || D < 1 || L < 1 || L > (1 << 30)) return fail(BFFC_ERR_INVALID, "%s: bad shape B=%d D=%d L=%d", fn, B, D, L);
-  const int Lout = L + 2 * P - K + 1;
+  const int Lout = docs ? L : L + 2 * P - K + 1;
   if (Lout < 1) return fail(BFFC_ERR_INVALID, "%s: output length L + 2P - K + 1 = %d < 1", fn, Lout);
   const long long span = backward ? std::max(L, Lout) : Lout;
   long long n;
@@ -1587,6 +1590,89 @@ int dw_pointers(const char* fn, std::initializer_list<std::pair<const void*, siz
   return 0;
 }
 
+// the document arguments of the varlen entry points (host side only: the offsets live on the device)
+int dw_docs(const char* fn, const int* cu_seqlens, int n_docs, int B, int L) {
+  if (!cu_seqlens || reinterpret_cast<uintptr_t>(cu_seqlens) % 4)
+    return fail(BFFC_ERR_INVALID, "%s: cu_seqlens is null or not 4-byte aligned", fn);
+  if (n_docs < B) return fail(BFFC_ERR_INVALID, "%s: n_docs=%d < B=%d (every row start is a document offset)", fn, n_docs, B);
+  if (static_cast<long long>(B) * L > 0x7fffffffLL)
+    return fail(BFFC_ERR_INVALID, "%s: B * L = %lld positions exceed the int32 offsets of cu_seqlens", fn,
+                static_cast<long long>(B) * L);
+  return 0;
+}
+
+// bffc_dwconv1d_fwd / bffc_dwconv1d_fwd_varlen (cu_seqlens non-null: the kDoc kernels)
+int dw_fwd(const char* fn, const void* u, int u_dtype, const void* w, const void* bias, int w_dtype, void* y, int B,
+           int D, int L, int K, int padding, int layout, const int* cu_seqlens, int n_docs, void* stream) {
+  const bool docs = cu_seqlens != nullptr;
+  bffc::dw::Shape sh;
+  long long ctas;
+  if (int rc = dw_dtypes(fn, u_dtype, w_dtype)) return rc;
+  if (int rc = dw_geometry(fn, B, D, L, K, padding, layout, false, &sh, &ctas, docs)) return rc;
+  const size_t eu = dw_elem(u_dtype), ew = dw_elem(w_dtype);
+  if (int rc = dw_pointers(fn, {{u, eu}, {w, ew}, {bias, ew}, {y, eu}})) return rc;
+  sh.cu = cu_seqlens;
+  sh.ndocs = n_docs;
+  if (int rc = check_device()) return rc;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  g_launches = 0;
+  dw_dispatch(u_dtype, w_dtype, K, [&](auto tu, auto tw, auto km) {
+    using T = typename decltype(tu)::type;
+    using W = typename decltype(tw)::type;
+    constexpr int KM = decltype(km)::value;
+    using namespace bffc::dw;
+    auto kernel = layout == BFFC_LAYOUT_BHL ? (docs ? fwd_bhl<T, W, KM, true> : fwd_bhl<T, W, KM>)
+                                            : (docs ? fwd_blh<T, W, KM, true> : fwd_blh<T, W, KM>);
+    kernel<<<unsigned(ctas), kThreads, 0, st>>>(static_cast<const T*>(u), static_cast<const W*>(w),
+                                                static_cast<const W*>(bias), static_cast<T*>(y), sh);
+  });
+  return launched();
+}
+
+// bffc_dwconv1d_bwd / bffc_dwconv1d_bwd_varlen; the workspace is bffc_dwconv1d_workspace_bytes of the shape in both
+// (documents need no more parts: their tiles cover L positions, the plain backward's max(L, Lout))
+int dw_bwd(const char* fn, const void* dout, const void* u, int u_dtype, const void* w, int w_dtype, void* du, void* dw,
+           void* dbias, int B, int D, int L, int K, int padding, int layout, const int* cu_seqlens, int n_docs,
+           void* workspace, size_t workspace_bytes, void* stream) {
+  const bool docs = cu_seqlens != nullptr;
+  bffc::dw::Shape sh;
+  long long ctas;
+  if (int rc = dw_dtypes(fn, u_dtype, w_dtype)) return rc;
+  if (int rc = dw_geometry(fn, B, D, L, K, padding, layout, true, &sh, &ctas, docs)) return rc;
+  const size_t eu = dw_elem(u_dtype), ew = dw_elem(w_dtype);
+  if (int rc = dw_pointers(fn, {{dout, eu}, {u, eu}, {w, ew}, {du, eu}, {dw, ew}, {dbias, ew}, {workspace, 4}})) return rc;
+  const size_t need = bffc_dwconv1d_workspace_bytes(B, D, L, K, padding, layout);
+  if (workspace_bytes < need) return fail(BFFC_ERR_INVALID, "%s: workspace of %zu bytes required", fn, need);
+  sh.cu = cu_seqlens;
+  sh.ndocs = n_docs;
+  if (int rc = check_device()) return rc;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  float* part = static_cast<float*>(workspace);
+  g_launches = 0;
+  dw_dispatch(u_dtype, w_dtype, K, [&](auto tu, auto tw, auto km) {
+    using T = typename decltype(tu)::type;
+    using W = typename decltype(tw)::type;
+    constexpr int KM = decltype(km)::value;
+    using namespace bffc::dw;
+    auto kernel = layout == BFFC_LAYOUT_BHL ? (docs ? bwd_bhl<T, W, KM, true> : bwd_bhl<T, W, KM>)
+                                            : (docs ? bwd_blh<T, W, KM, true> : bwd_blh<T, W, KM>);
+    kernel<<<unsigned(ctas), kThreads, 0, st>>>(static_cast<const T*>(dout), static_cast<const T*>(u),
+                                                static_cast<const W*>(w), static_cast<T*>(du), part, sh);
+  });
+  if (int rc = launched()) return rc;
+  const long long rows = static_cast<long long>(K + 1) * D, per_cta = bffc::dw::kThreads / 32;
+  const long long parts = static_cast<long long>(B) * sh.tiles;
+  auto reduce = [&](auto tw) {
+    using W = typename decltype(tw)::type;
+    bffc::dw::reduce_parts<W><<<unsigned((rows + per_cta - 1) / per_cta), bffc::dw::kThreads, 0, st>>>(
+        part, static_cast<W*>(dw), static_cast<W*>(dbias), D, K, parts, layout == BFFC_LAYOUT_BLH);
+  };
+  if (w_dtype == BFFC_DTYPE_FP32) reduce(Tag<float>());
+  else if (w_dtype == BFFC_DTYPE_FP16) reduce(Tag<__half>());
+  else reduce(Tag<__nv_bfloat16>());
+  return launched();
+}
+
 }  // namespace
 
 extern "C" {
@@ -1604,63 +1690,31 @@ size_t bffc_dwconv1d_workspace_bytes(int B, int D, int L, int K, int padding, in
 
 int bffc_dwconv1d_fwd(const void* u, int u_dtype, const void* w, const void* bias, int w_dtype, void* y, int B, int D,
                       int L, int K, int padding, int layout, void* stream) {
-  const char* fn = "bffc_dwconv1d_fwd";
-  bffc::dw::Shape sh;
-  long long ctas;
-  if (int rc = dw_dtypes(fn, u_dtype, w_dtype)) return rc;
-  if (int rc = dw_geometry(fn, B, D, L, K, padding, layout, false, &sh, &ctas)) return rc;
-  const size_t eu = dw_elem(u_dtype), ew = dw_elem(w_dtype);
-  if (int rc = dw_pointers(fn, {{u, eu}, {w, ew}, {bias, ew}, {y, eu}})) return rc;
-  if (int rc = check_device()) return rc;
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  g_launches = 0;
-  dw_dispatch(u_dtype, w_dtype, K, [&](auto tu, auto tw, auto km) {
-    using T = typename decltype(tu)::type;
-    using W = typename decltype(tw)::type;
-    constexpr int KM = decltype(km)::value;
-    auto kernel = layout == BFFC_LAYOUT_BHL ? bffc::dw::fwd_bhl<T, W, KM> : bffc::dw::fwd_blh<T, W, KM>;
-    kernel<<<unsigned(ctas), bffc::dw::kThreads, 0, st>>>(static_cast<const T*>(u), static_cast<const W*>(w),
-                                                         static_cast<const W*>(bias), static_cast<T*>(y), sh);
-  });
-  return launched();
+  return dw_fwd("bffc_dwconv1d_fwd", u, u_dtype, w, bias, w_dtype, y, B, D, L, K, padding, layout, nullptr, 0, stream);
 }
 
 int bffc_dwconv1d_bwd(const void* dout, const void* u, int u_dtype, const void* w, int w_dtype, void* du, void* dw,
                       void* dbias, int B, int D, int L, int K, int padding, int layout, void* workspace,
                       size_t workspace_bytes, void* stream) {
-  const char* fn = "bffc_dwconv1d_bwd";
-  bffc::dw::Shape sh;
-  long long ctas;
-  if (int rc = dw_dtypes(fn, u_dtype, w_dtype)) return rc;
-  if (int rc = dw_geometry(fn, B, D, L, K, padding, layout, true, &sh, &ctas)) return rc;
-  const size_t eu = dw_elem(u_dtype), ew = dw_elem(w_dtype);
-  if (int rc = dw_pointers(fn, {{dout, eu}, {u, eu}, {w, ew}, {du, eu}, {dw, ew}, {dbias, ew}, {workspace, 4}})) return rc;
-  const size_t need = bffc_dwconv1d_workspace_bytes(B, D, L, K, padding, layout);
-  if (workspace_bytes < need) return fail(BFFC_ERR_INVALID, "%s: workspace of %zu bytes required", fn, need);
-  if (int rc = check_device()) return rc;
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  float* part = static_cast<float*>(workspace);
-  g_launches = 0;
-  dw_dispatch(u_dtype, w_dtype, K, [&](auto tu, auto tw, auto km) {
-    using T = typename decltype(tu)::type;
-    using W = typename decltype(tw)::type;
-    constexpr int KM = decltype(km)::value;
-    auto kernel = layout == BFFC_LAYOUT_BHL ? bffc::dw::bwd_bhl<T, W, KM> : bffc::dw::bwd_blh<T, W, KM>;
-    kernel<<<unsigned(ctas), bffc::dw::kThreads, 0, st>>>(static_cast<const T*>(dout), static_cast<const T*>(u),
-                                                         static_cast<const W*>(w), static_cast<T*>(du), part, sh);
-  });
-  if (int rc = launched()) return rc;
-  const long long rows = static_cast<long long>(K + 1) * D, per_cta = bffc::dw::kThreads / 32;
-  const long long parts = static_cast<long long>(B) * sh.tiles;
-  auto reduce = [&](auto tw) {
-    using W = typename decltype(tw)::type;
-    bffc::dw::reduce_parts<W><<<unsigned((rows + per_cta - 1) / per_cta), bffc::dw::kThreads, 0, st>>>(
-        part, static_cast<W*>(dw), static_cast<W*>(dbias), D, K, parts, layout == BFFC_LAYOUT_BLH);
-  };
-  if (w_dtype == BFFC_DTYPE_FP32) reduce(Tag<float>());
-  else if (w_dtype == BFFC_DTYPE_FP16) reduce(Tag<__half>());
-  else reduce(Tag<__nv_bfloat16>());
-  return launched();
+  return dw_bwd("bffc_dwconv1d_bwd", dout, u, u_dtype, w, w_dtype, du, dw, dbias, B, D, L, K, padding, layout, nullptr, 0,
+                workspace, workspace_bytes, stream);
+}
+
+int bffc_dwconv1d_fwd_varlen(const void* u, int u_dtype, const void* w, const void* bias, int w_dtype, void* y, int B,
+                             int D, int L, int K, int padding, int layout, const int* cu_seqlens, int n_docs,
+                             void* stream) {
+  const char* fn = "bffc_dwconv1d_fwd_varlen";
+  if (int rc = dw_docs(fn, cu_seqlens, n_docs, B, L)) return rc;
+  return dw_fwd(fn, u, u_dtype, w, bias, w_dtype, y, B, D, L, K, padding, layout, cu_seqlens, n_docs, stream);
+}
+
+int bffc_dwconv1d_bwd_varlen(const void* dout, const void* u, int u_dtype, const void* w, int w_dtype, void* du,
+                             void* dw, void* dbias, int B, int D, int L, int K, int padding, int layout,
+                             const int* cu_seqlens, int n_docs, void* workspace, size_t workspace_bytes, void* stream) {
+  const char* fn = "bffc_dwconv1d_bwd_varlen";
+  if (int rc = dw_docs(fn, cu_seqlens, n_docs, B, L)) return rc;
+  return dw_bwd(fn, dout, u, u_dtype, w, w_dtype, du, dw, dbias, B, D, L, K, padding, layout, cu_seqlens, n_docs,
+                workspace, workspace_bytes, stream);
 }
 
 }  // extern "C"

@@ -16,6 +16,9 @@
 // from the same shared-memory tiles, per-CTA fp32 partial sums of dw[d, k] = sum dout * shifted u and dbias[d] = sum dout,
 // written to the workspace as [(K + 1) * D][parts].  Pass 2 sums each row of partials in a fixed order.  The split of
 // (B, L) into parts depends on the shape only, so results are bit-identical across runs and devices.
+//
+// Packed documents (the kDoc instantiations, bffc_dwconv1d_*_varlen): each row holds several documents, and every sum
+// above runs over the output's document only (DocCursor below), with the same tiles, loads and summation order.
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
@@ -186,7 +189,69 @@ struct Shape {
   int B, D, L, K, P, Lout;
   int tiles;    // BHL: CTAs per row; BLH forward: tiles along L; BLH backward: strips along L
   int dchunks;  // BLH: channel chunks of kChunkD
+  const int* cu = nullptr;   // documents (kDoc kernels): offsets cu[0 .. ndocs] into the flattened (B, L) positions
+  int ndocs = 0;
 };
+
+// Documents.  Position p of row b is the flattened position b * L + p; cu is non-decreasing from 0 to B * L and holds
+// every row start, so a document never crosses a row (Lout = L).  With the document [o, e) of position p, input
+// p - P + k lies in it iff klo <= k < khi, klo = P - (p - o), khi = P + (e - p): the taps of output p, and of the
+// weight-gradient partials of dout[p]; dout[p + P - k] lies in it iff klo <= 2P - k < khi: the taps of du[p].  Taps
+// outside are dropped by select, so a NaN or inf in another document never reaches p.  The contents of cu are not
+// validated; the searches stay inside cu[0 .. ndocs] whatever they hold.
+//
+// A thread keeps its taps as bit masks (bit k: tap k kept), one word per position: the forward's, or in the backward
+// the partials' in bits [0, KMAX) and du's in bits [KMAX, 2 KMAX).
+//
+// index d in [lo, hi) with cu[d] <= f < cu[d + 1], given cu[lo] <= f < cu[hi]
+__device__ __forceinline__ int find_doc(const int* __restrict__ cu, int lo, int hi, int f) {
+  while (hi - lo > 1) {
+    const int mid = (lo + hi) >> 1;
+    if (__ldg(cu + mid) <= f) lo = mid;
+    else hi = mid;
+  }
+  return lo;
+}
+
+// bits [a, b) of a 32-bit word (a, b clamped to [0, 32])
+__device__ __forceinline__ uint32_t bit_range(int a, int b) {
+  a = min(max(a, 0), 32);
+  b = min(max(b, a), 32);
+  const uint32_t below_b = b == 32 ? 0xffffffffu : (1u << b) - 1u, below_a = a == 32 ? 0xffffffffu : (1u << a) - 1u;
+  return below_b & ~below_a;
+}
+
+// The document of a thread's positions in row b, for positions visited in non-decreasing order: a position inside the
+// current document costs a compare; crossing a boundary searches from the current document on.
+struct DocCursor {
+  const int* cu;
+  int base, L, P, ndocs, d, o, e;     // [o, e): the current document, row coordinates (empty before the first search)
+  __device__ __forceinline__ DocCursor(const Shape& sh, int b)
+      : cu(sh.cu), base(b * sh.L), L(sh.L), P(sh.P), ndocs(sh.ndocs), d(0), o(0), e(0) {}
+  // (klo, khi) of position p; no taps past the row
+  __device__ __forceinline__ int2 taps(int p) {
+    if (p >= L) return make_int2(0, 0);
+    if (p >= e) {
+      d = find_doc(cu, d, ndocs, base + p);
+      o = __ldg(cu + d) - base;
+      e = __ldg(cu + d + 1) - base;
+    }
+    return make_int2(P - (p - o), P + (e - p));
+  }
+  __device__ __forceinline__ uint32_t fwd_mask(int p) {
+    const int2 t = taps(p);
+    return bit_range(t.x, t.y);
+  }
+  template <int KMAX>
+  __device__ __forceinline__ auto bwd_mask(int p) {
+    using M = std::conditional_t<(2 * KMAX <= 32), uint32_t, uint64_t>;
+    const int2 t = taps(p);
+    // both ranges cut at KMAX: the partials' bits must not reach the du half
+    return M(bit_range(t.x, min(t.y, KMAX))) | (M(bit_range(2 * P - t.y + 1, min(2 * P - t.x + 1, KMAX))) << KMAX);
+  }
+};
+template <class M>
+__device__ __forceinline__ float tap_in(float x, M mask, int bit) { return ((mask >> bit) & 1) ? x : 0.f; }
 
 // taps of channel d (0 when d >= D); w is (D, K) for BHL, (K, D) for BLH
 template <int KMAX, bool BLH, class W>
@@ -196,7 +261,8 @@ __device__ __forceinline__ void load_taps(float (&wr)[KMAX], const W* w, int d, 
 }
 
 // ------------------------------------------------------------------------------------------------------------- forward
-template <class T, class W, int KMAX>
+// kDoc: taps stop at document boundaries (DocCursor); the same fmaf chain, with the dropped taps' inputs 0
+template <class T, class W, int KMAX, bool kDoc = false>
 __global__ void __launch_bounds__(kThreads) fwd_bhl(const T* __restrict__ u, const W* __restrict__ w,
                                                      const W* __restrict__ bias, T* __restrict__ y, Shape sh) {
   constexpr int J = kTileL / kThreads;
@@ -206,6 +272,12 @@ __global__ void __launch_bounds__(kThreads) fwd_bhl(const T* __restrict__ u, con
   float wr[KMAX];
   load_taps<KMAX, false>(wr, w, d, sh.D, K);
   const float b0 = to_f(bias[d]);
+  uint32_t tm[J];
+  if constexpr (kDoc) {
+    DocCursor docs(sh, static_cast<int>(row / sh.D));
+#pragma unroll
+    for (int j = 0; j < J; ++j) tm[j] = docs.fwd_mask(l0 + threadIdx.x + j * kThreads);
+  }
   const int m = load_row(s, u + row * sh.L, static_cast<long long>(l0) - sh.P, kTileL + K - 1, sh.L);
   __syncthreads();
   float acc[J];
@@ -215,7 +287,11 @@ __global__ void __launch_bounds__(kThreads) fwd_bhl(const T* __restrict__ u, con
   for (int k = 0; k < KMAX; ++k) {
     if (k >= K) break;
 #pragma unroll
-    for (int j = 0; j < J; ++j) acc[j] = fmaf(wr[k], s[m + threadIdx.x + j * kThreads + k], acc[j]);
+    for (int j = 0; j < J; ++j) {
+      float x = s[m + threadIdx.x + j * kThreads + k];
+      if constexpr (kDoc) x = tap_in(x, tm[j], k);
+      acc[j] = fmaf(wr[k], x, acc[j]);
+    }
   }
   __syncthreads();
   T* yr = y + row * sh.Lout;
@@ -226,7 +302,7 @@ __global__ void __launch_bounds__(kThreads) fwd_bhl(const T* __restrict__ u, con
   store_row(yr, s, l0, kTileL, sh.Lout);
 }
 
-template <class T, class W, int KMAX>
+template <class T, class W, int KMAX, bool kDoc = false>
 __global__ void __launch_bounds__(kThreads) fwd_blh(const T* __restrict__ u, const W* __restrict__ w,
                                                      const W* __restrict__ bias, T* __restrict__ y, Shape sh) {
   constexpr int TLB = blh_tile(KMAX), RUN = TLB * kChunkD / kThreads;
@@ -238,6 +314,12 @@ __global__ void __launch_bounds__(kThreads) fwd_blh(const T* __restrict__ u, con
   float wr[KMAX];
   load_taps<KMAX, true>(wr, w, c0 + c, sh.D, K);
   const float b0 = c0 + c < sh.D ? to_f(bias[c0 + c]) : 0.f;
+  uint32_t tm[RUN];
+  if constexpr (kDoc) {
+    DocCursor docs(sh, b);
+#pragma unroll
+    for (int v = 0; v < RUN; ++v) tm[v] = docs.fwd_mask(l0 + g * RUN + v);
+  }
   const T* ub = u + size_t(b) * sh.L * sh.D;
   const long long r0 = static_cast<long long>(l0) - sh.P;
   load_rows(s, ub, r0, TLB + K - 1, sh.L, sh.D, c0);
@@ -252,7 +334,9 @@ __global__ void __launch_bounds__(kThreads) fwd_blh(const T* __restrict__ u, con
 #pragma unroll
     for (int v = 0; v < RUN; ++v) {
       const int r = g * RUN + v + k;
-      acc[v] = fmaf(wr[k], s[r * kRowStride + off(r) + c], acc[v]);
+      float x = s[r * kRowStride + off(r) + c];
+      if constexpr (kDoc) x = tap_in(x, tm[v], k);
+      acc[v] = fmaf(wr[k], x, acc[v]);
     }
   }
   __syncthreads();
@@ -272,7 +356,7 @@ __global__ void __launch_bounds__(kThreads) fwd_blh(const T* __restrict__ u, con
 // [i0, i0 + T) for the partials: dw[k] += dout[o] * u[o - P + k], dbias += dout[o].  With the dout window starting at
 // i0 + P - (K - 1) and the u window at i0 - P, local position t reads dout at t + K - 1 - k (du) and t + K - 1 - P
 // (partials), u at t + k.
-template <class T, class W, int KMAX>
+template <class T, class W, int KMAX, bool kDoc = false>
 __global__ void __launch_bounds__(kThreads, 1) bwd_bhl(const T* __restrict__ dout, const T* __restrict__ u,
                                                      const W* __restrict__ w, T* __restrict__ du,
                                                      float* __restrict__ part, Shape sh) {
@@ -285,6 +369,12 @@ __global__ void __launch_bounds__(kThreads, 1) bwd_bhl(const T* __restrict__ dou
   const int b = static_cast<int>(row / sh.D), K = sh.K, P = sh.P;
   float wr[KMAX];
   load_taps<KMAX, false>(wr, w, d, sh.D, K);
+  decltype(DocCursor(sh, 0).bwd_mask<KMAX>(0)) tm[J];
+  if constexpr (kDoc) {
+    DocCursor docs(sh, b);
+#pragma unroll
+    for (int j = 0; j < J; ++j) tm[j] = docs.bwd_mask<KMAX>(i0 + threadIdx.x + j * kThreads);
+  }
   const int md = load_row(sd, dout + row * sh.Lout, static_cast<long long>(i0) + P - (K - 1), kTileL + K - 1, sh.Lout);
   const int mu = load_row(su, u + row * sh.L, static_cast<long long>(i0) - P, kTileL + K - 1, sh.L);
   __syncthreads();
@@ -295,7 +385,11 @@ __global__ void __launch_bounds__(kThreads, 1) bwd_bhl(const T* __restrict__ dou
   for (int k = 0; k < KMAX; ++k) {
     if (k >= K) break;
 #pragma unroll
-    for (int j = 0; j < J; ++j) acc[j] = fmaf(wr[k], sd[md + threadIdx.x + j * kThreads + K - 1 - k], acc[j]);
+    for (int j = 0; j < J; ++j) {
+      float x = sd[md + threadIdx.x + j * kThreads + K - 1 - k];
+      if constexpr (kDoc) x = tap_in(x, tm[j], KMAX + k);
+      acc[j] = fmaf(wr[k], x, acc[j]);
+    }
   }
   // partials (pk[KMAX] is dbias): per-thread sums over its positions, then a warp butterfly per tap
   float pk[KMAX + 1];
@@ -309,7 +403,9 @@ __global__ void __launch_bounds__(kThreads, 1) bwd_bhl(const T* __restrict__ dou
 #pragma unroll
     for (int k = 0; k < KMAX; ++k) {
       if (k >= K) break;
-      pk[k] = fmaf(dv, su[mu + t + k], pk[k]);
+      float x = su[mu + t + k];
+      if constexpr (kDoc) x = tap_in(x, tm[j], k);
+      pk[k] = fmaf(dv, x, pk[k]);
     }
   }
   const int lane = threadIdx.x % 32, warp = threadIdx.x / 32;
@@ -337,8 +433,10 @@ __global__ void __launch_bounds__(kThreads, 1) bwd_bhl(const T* __restrict__ dou
   store_row(dur, sd, i0, kTileL, sh.L);
 }
 
-template <class T, class W, int KMAX>
-__global__ void __launch_bounds__(kThreads, KMAX <= 4 ? 3 : 1) bwd_blh(const T* __restrict__ dout, const T* __restrict__ u,
+// kDoc: the tap masks of a thread's RUN positions and its document cursor do not fit the 80 registers of three CTAs per
+// SM without spills (ptxas), so that instantiation asks for two
+template <class T, class W, int KMAX, bool kDoc = false>
+__global__ void __launch_bounds__(kThreads, KMAX <= 4 ? (kDoc ? 2 : 3) : 1) bwd_blh(const T* __restrict__ dout, const T* __restrict__ u,
                                                                        const W* __restrict__ w, T* __restrict__ du,
                                                                        float* __restrict__ part, Shape sh) {
   constexpr int TLB = blh_tile(KMAX), RUN = TLB * kChunkD / kThreads;
@@ -357,9 +455,16 @@ __global__ void __launch_bounds__(kThreads, KMAX <= 4 ? 3 : 1) bwd_blh(const T* 
   const T* dout_b = dout + size_t(b) * sh.Lout * sh.D;
   const T* u_b = u + size_t(b) * sh.L * sh.D;
   T* du_b = du + size_t(b) * sh.L * sh.D;
+  // kDoc: one cursor walks the thread's positions through the strip's tiles in order
+  DocCursor docs(sh, b);
   for (int tl = 0; tl < kStripL / TLB; ++tl) {
     const int i0 = strip * kStripL + tl * TLB;
     if (i0 >= Lmax) break;
+    decltype(docs.bwd_mask<KMAX>(0)) tm[RUN];
+    if constexpr (kDoc) {
+#pragma unroll
+      for (int v = 0; v < RUN; ++v) tm[v] = docs.bwd_mask<KMAX>(i0 + g * RUN + v);
+    }
     const long long rd = static_cast<long long>(i0) + P - (K - 1), ru = static_cast<long long>(i0) - P;
     load_rows(sd, dout_b, rd, TLB + K - 1, sh.Lout, sh.D, c0);
     load_rows(su, u_b, ru, TLB + K - 1, sh.L, sh.D, c0);
@@ -374,7 +479,9 @@ __global__ void __launch_bounds__(kThreads, KMAX <= 4 ? 3 : 1) bwd_blh(const T* 
 #pragma unroll
       for (int v = 0; v < RUN; ++v) {
         const int r = g * RUN + v + K - 1 - k;
-        acc[v] = fmaf(wr[k], sd[r * kRowStride + offd(r) + c], acc[v]);
+        float x = sd[r * kRowStride + offd(r) + c];
+        if constexpr (kDoc) x = tap_in(x, tm[v], KMAX + k);
+        acc[v] = fmaf(wr[k], x, acc[v]);
       }
     }
 #pragma unroll
@@ -385,7 +492,9 @@ __global__ void __launch_bounds__(kThreads, KMAX <= 4 ? 3 : 1) bwd_blh(const T* 
 #pragma unroll
       for (int k = 0; k < KMAX; ++k) {
         if (k >= K) break;
-        pk[k] = fmaf(dv, su[(t + k) * kRowStride + offu(t + k) + c], pk[k]);
+        float x = su[(t + k) * kRowStride + offu(t + k) + c];
+        if constexpr (kDoc) x = tap_in(x, tm[v], k);
+        pk[k] = fmaf(dv, x, pk[k]);
       }
     }
     __syncthreads();

@@ -73,6 +73,11 @@ SYMBOLS = {
     'bffc_dwconv1d_workspace_bytes': (_c.c_size_t, [_c.c_int] * 6),
     'bffc_dwconv1d_bwd': (_c.c_int, [_c.c_void_p, _c.c_void_p, _c.c_int, _c.c_void_p, _c.c_int, _c.c_void_p, _c.c_void_p,
                                      _c.c_void_p] + [_c.c_int] * 6 + [_c.c_void_p, _c.c_size_t, _c.c_void_p]),
+    'bffc_dwconv1d_fwd_varlen': (_c.c_int, [_c.c_void_p, _c.c_int, _c.c_void_p, _c.c_void_p, _c.c_int, _c.c_void_p]
+                                 + [_c.c_int] * 6 + [_c.c_void_p, _c.c_int, _c.c_void_p]),
+    'bffc_dwconv1d_bwd_varlen': (_c.c_int, [_c.c_void_p, _c.c_void_p, _c.c_int, _c.c_void_p, _c.c_int, _c.c_void_p,
+                                            _c.c_void_p, _c.c_void_p] + [_c.c_int] * 6
+                                 + [_c.c_void_p, _c.c_int, _c.c_void_p, _c.c_size_t, _c.c_void_p]),
     'bffc_conv_state_bytes': (_c.c_size_t, [_c.c_int] * 6),
     'bffc_conv_step_workspace_bytes': (_c.c_size_t, [_c.c_int] * 5),
     'bffc_conv_state_fill': (_c.c_int, [_c.c_void_p, _c.c_int64] * 3 + [_c.c_void_p] * 6 + [_c.c_int] * 9

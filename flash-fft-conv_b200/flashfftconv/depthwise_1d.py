@@ -4,7 +4,8 @@ The operator is exactly `torch.nn.Conv1d(D, D, K, groups=D, padding=P)` on `(B, 
 convolution along L of `(B, L, D)` input (`is_bhl=False`).  Both passes run in libbffc.so (bffc_dwconv1d_fwd /
 bffc_dwconv1d_bwd, include/bffc.h): the forward is one kernel, the backward two (du with per-CTA partial sums of the
 weight and bias gradients, then their fixed-order reduction).  All arithmetic is fp32 whatever the input and weight
-types.
+types.  With `cu_seqlens` (packed documents, `forward(u, cu_seqlens)`) the same passes run through
+bffc_dwconv1d_fwd_varlen / bffc_dwconv1d_bwd_varlen and keep the documents apart (INTEGRATION.md §10).
 
 Differences from the reference, each deliberate:
 - it accumulates in fp32 (the reference accumulates in the 16-bit input type);
@@ -62,21 +63,43 @@ def _check(u, weights, bias, padding, is_bhl):
     return B, D, L, K
 
 
-def _forward(u, weights, bias, padding, is_bhl=True):
-    """(y, shape) of one bffc_dwconv1d_fwd launch; shape = (B, D, L, K, padding, layout) is what _backward takes."""
+def _check_docs(cu_seqlens, u, B):
+    """n_docs of a cu_seqlens argument for a batch of B rows on u's device; RuntimeError otherwise.  Only what the host
+    can see is checked: the offsets stay on the device (as in flash-attn), so a call never synchronises."""
+    if not isinstance(cu_seqlens, torch.Tensor) or cu_seqlens.device != u.device:
+        raise RuntimeError(f'cu_seqlens must be a tensor on {u.device}')
+    if cu_seqlens.dtype != torch.int32 or cu_seqlens.dim() != 1 or not cu_seqlens.is_contiguous():
+        raise RuntimeError(f'cu_seqlens must be a contiguous 1-D int32 tensor, got {cu_seqlens.dtype} of shape '
+                           f'{tuple(cu_seqlens.shape)}')
+    n_docs = cu_seqlens.numel() - 1
+    if n_docs < B:
+        raise RuntimeError(f'cu_seqlens has {n_docs} documents for {B} rows: every row start must be an offset')
+    return n_docs
+
+
+def _forward(u, weights, bias, padding, is_bhl=True, cu_seqlens=None):
+    """(y, shape) of one bffc_dwconv1d_fwd launch (bffc_dwconv1d_fwd_varlen with cu_seqlens: y has u's shape);
+    shape = (B, D, L, K, padding, layout) is what _backward takes."""
     padding = int(padding)
     B, D, L, K = _check(u, weights, bias, padding, is_bhl)
-    Lout = L + 2 * padding - K + 1
     layout = _lib.BFFC_LAYOUT_BHL if is_bhl else _lib.BFFC_LAYOUT_BLH
+    args = (_ptr(u), _DT[u.dtype], _ptr(weights), _ptr(bias), _DT[weights.dtype])
     with _on_device(u.device):
-        y = torch.empty((B, D, Lout) if is_bhl else (B, Lout, D), dtype=u.dtype, device=u.device)
-        _lib.check(_lib.lib().bffc_dwconv1d_fwd(_ptr(u), _DT[u.dtype], _ptr(weights), _ptr(bias), _DT[weights.dtype],
-                                                _ptr(y), B, D, L, K, padding, layout, _stream()))
+        if cu_seqlens is None:
+            Lout = L + 2 * padding - K + 1
+            y = torch.empty((B, D, Lout) if is_bhl else (B, Lout, D), dtype=u.dtype, device=u.device)
+            _lib.check(_lib.lib().bffc_dwconv1d_fwd(*args, _ptr(y), B, D, L, K, padding, layout, _stream()))
+        else:
+            n_docs = _check_docs(cu_seqlens, u, B)
+            y = torch.empty_like(u)
+            _lib.check(_lib.lib().bffc_dwconv1d_fwd_varlen(*args, _ptr(y), B, D, L, K, padding, layout,
+                                                           _ptr(cu_seqlens), n_docs, _stream()))
     return y, (B, D, L, K, padding, layout)
 
 
-def _backward(dout, u, weights, bias, shape):
-    """(du, dw, dbias) of the bffc_dwconv1d_bwd launches; dout must be contiguous."""
+def _backward(dout, u, weights, bias, shape, cu_seqlens=None):
+    """(du, dw, dbias) of the bffc_dwconv1d_bwd launches (bffc_dwconv1d_bwd_varlen with cu_seqlens); dout must be
+    contiguous."""
     B, D, L, K, padding, layout = shape
     with _on_device(u.device):
         du = torch.empty_like(u)
@@ -84,25 +107,29 @@ def _backward(dout, u, weights, bias, shape):
         dbias = torch.empty_like(bias)
         nws = _lib.lib().bffc_dwconv1d_workspace_bytes(B, D, L, K, padding, layout)
         ws = torch.empty(nws, dtype=torch.uint8, device=u.device)
-        _lib.check(_lib.lib().bffc_dwconv1d_bwd(_ptr(dout), _ptr(u), _DT[u.dtype], _ptr(weights), _DT[weights.dtype],
-                                                _ptr(du), _ptr(dw), _ptr(dbias), B, D, L, K, padding, layout,
-                                                _ptr(ws), nws, _stream()))
+        args = (_ptr(dout), _ptr(u), _DT[u.dtype], _ptr(weights), _DT[weights.dtype], _ptr(du), _ptr(dw), _ptr(dbias),
+                B, D, L, K, padding, layout)
+        if cu_seqlens is None:
+            _lib.check(_lib.lib().bffc_dwconv1d_bwd(*args, _ptr(ws), nws, _stream()))
+        else:
+            _lib.check(_lib.lib().bffc_dwconv1d_bwd_varlen(*args, _ptr(cu_seqlens), cu_seqlens.numel() - 1, _ptr(ws),
+                                                           nws, _stream()))
     return du, dw, dbias
 
 
 class DepthWiseConv1dFunc(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, u, weights, bias, padding, is_bhl=True):
-        y, ctx.shape = _forward(u, weights, bias, padding, is_bhl)
-        ctx.save_for_backward(u, weights, bias)
+    def forward(ctx, u, weights, bias, padding, is_bhl=True, cu_seqlens=None):
+        y, ctx.shape = _forward(u, weights, bias, padding, is_bhl, cu_seqlens)
+        ctx.save_for_backward(u, weights, bias, cu_seqlens)
         return y
 
     @staticmethod
     def backward(ctx, dout):
-        u, weights, bias = ctx.saved_tensors
+        u, weights, bias, cu_seqlens = ctx.saved_tensors
         dout = dout.contiguous()                                      # reference depthwise_1d.py:19
-        du, dw, dbias = _backward(dout, u, weights, bias, ctx.shape)
-        return du, dw, dbias, None, None
+        du, dw, dbias = _backward(dout, u, weights, bias, ctx.shape, cu_seqlens)
+        return du, dw, dbias, None, None, None
 
 
 class FlashDepthWiseConv1d(torch.nn.Module):
@@ -127,5 +154,10 @@ class FlashDepthWiseConv1d(torch.nn.Module):
     def extra_repr(self):
         return f'channels={self.d}, kernel_size={self.k}, padding={self.padding}, is_bhl={self.is_bhl}'
 
-    def forward(self, input):
-        return DepthWiseConv1dFunc.apply(input, self.weights, self.bias, self.padding, self.is_bhl)
+    def forward(self, input, cu_seqlens=None):
+        """With `cu_seqlens` (packed documents, flash-attn's convention: a CUDA int32 tensor of n_docs + 1 offsets into
+        the flattened (B, L) positions, from 0 to B * L, every row start b * L among them), each document is convolved
+        alone: the output has the input's shape and holds, for each document, the first len(document) outputs of this
+        module run on that document, with inputs outside it counted as zero.  That needs (K - 1) / 2 <= padding; padding
+        K - 1 is the causal form.  The offsets are not read on the host."""
+        return DepthWiseConv1dFunc.apply(input, self.weights, self.bias, self.padding, self.is_bhl, cu_seqlens)

@@ -327,6 +327,29 @@ int bffc_dwconv1d_bwd(const void* dout, const void* u, int u_dtype, const void* 
                       size_t workspace_bytes, void* stream);
 
 /*
+ * Packed documents: the same convolution on rows that each hold several documents, as flash-attn gives them.
+ * cu_seqlens: device int32[n_docs + 1], offsets into the flattened (B, L) positions (position (b, l) is b * L + l),
+ * non-decreasing from 0 to B * L, with every row start b * L among them (no document crosses a row; zero-length
+ * documents are allowed).  For the document [o, e) holding l:
+ *
+ *     y[b, d, l] = bias[d] + sum_{k<K, o <= l-P+k < e} w[d, k] * u[b, d, l - P + k]
+ *
+ * the first e - o outputs of the convolution above run on the document alone, so y and dout have u's shape (Lout = L);
+ * that needs (K - 1) / 2 <= P <= K - 1 (P = K - 1: causal).  du, dw and dbias are the gradients of that y: no tap,
+ * du term or weight-gradient term crosses a boundary, and taps across one are dropped by select (a NaN or inf in one
+ * document reaches no other).  y and du are bit for bit the plain entry points run on each document alone with dout
+ * zero past e - o.  The workspace is bffc_dwconv1d_workspace_bytes of the shape; launches as the plain entry points.
+ * Host arguments, n_docs >= B and B * L < 2^31 included, are validated first (BFFC_ERR_INVALID); the contents of
+ * cu_seqlens are not (they stay on the device, so the calls can be captured in a CUDA graph).
+ */
+int bffc_dwconv1d_fwd_varlen(const void* u, int u_dtype, const void* w, const void* bias, int w_dtype, void* y, int B,
+                             int D, int L, int K, int padding, int layout, const int* cu_seqlens, int n_docs,
+                             void* stream);
+int bffc_dwconv1d_bwd_varlen(const void* dout, const void* u, int u_dtype, const void* w, int w_dtype, void* du,
+                             void* dw, void* dbias, int B, int D, int L, int K, int padding, int layout,
+                             const int* cu_seqlens, int n_docs, void* workspace, size_t workspace_bytes, void* stream);
+
+/*
  * Decoding: the causal gated long convolution one step at a time, for generation after a prompt (no plan; inference
  * only).  Per batch member b, channel h and absolute position t < max_len, with the roles c in {u, pregate, postgate}:
  *
