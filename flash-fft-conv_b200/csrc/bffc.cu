@@ -1057,8 +1057,14 @@ static int check_common(const bffc_plan* p, int B, int H, int L, const void* a, 
   if (!p) return fail(BFFC_ERR_INVALID, "null plan");
   // Tensor maps are encoded through the driver API, which needs a current context in the CALLING thread.  A thread that
   // has made no runtime call yet (PyTorch's autograd worker entering bffc_bwd) has none: this runtime no-op binds the
-  // device's primary context (cuTensorMapEncodeTiled otherwise fails with CUDA_ERROR_INVALID_CONTEXT).
-  CUDA_TRY(cudaFree(nullptr));
+  // device's primary context (cuTensorMapEncodeTiled otherwise fails with CUDA_ERROR_INVALID_CONTEXT).  Once per thread
+  // and device: cudaFree is not allowed while a stream is being captured into a CUDA graph, and a capture follows a
+  // warm-up call on the same thread.
+  thread_local int bound_device = -1;
+  if (bound_device != p->device) {
+    CUDA_TRY(cudaFree(nullptr));
+    bound_device = p->device;
+  }
   if (B <= 0 || H <= 0 || L <= 0 || (L > p->N && !blocked))
     return fail(BFFC_ERR_INVALID, "bad shape B=%d H=%d L=%d (seqlen %d)", B, H, L, p->N);
   if (L % 8 != 0) return fail(BFFC_ERR_UNSUPPORTED, "L=%d must be a multiple of 8 in this build", L);

@@ -29,13 +29,41 @@ def _ptr(t):
     return ctypes.c_void_p(t.data_ptr()) if t is not None else ctypes.c_void_p(0)
 
 
-def _stream():
-    """Raw handle of the current stream of the current device.  torch.cuda.current_stream() builds a Stream object
-    (~13 us per call, measured: tools/host_overhead.py); the raw query underneath it is what Triton's launcher uses too."""
+def _raw_stream():
+    """Raw handle (an int) of the current stream of the current device.  torch.cuda.current_stream() builds a Stream
+    object (~13 us per call, measured: tools/host_overhead.py); the raw query underneath it is what Triton's launcher
+    uses too."""
     try:
-        return ctypes.c_void_p(torch._C._cuda_getCurrentRawStream(torch.cuda.current_device()))
+        return torch._C._cuda_getCurrentRawStream(torch.cuda.current_device())
     except AttributeError:                                         # private API moved: fall back to the public path
-        return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
+        return torch.cuda.current_stream().cuda_stream
+
+
+def _stream():
+    return ctypes.c_void_p(_raw_stream())
+
+
+class _StreamOrder:
+    """Orders a device tensor that outlives a call (the cached spectrum, the staging buffer of forward_host) across
+    streams.  `mark()` records an event after the tensor's latest use on the current stream; `join(t)` makes the current
+    stream wait for it when it is another stream than the one marked, and tells the caching allocator that `t` is in use
+    there (record_stream), so dropping `t` does not hand its memory out while this stream still works on it.  On the
+    marked stream join() is one integer comparison."""
+
+    def __init__(self):
+        self.event = torch.cuda.Event()
+        self.streams = set()
+
+    def mark(self):
+        self.event.record()
+        self.streams = {_raw_stream()}
+
+    def join(self, t):
+        if _raw_stream() not in self.streams:
+            cur = torch.cuda.current_stream()
+            cur.wait_event(self.event)
+            t.record_stream(cur)
+            self.streams.add(cur.cuda_stream)
 
 
 class _Plan:
@@ -92,8 +120,8 @@ class FlashFFTConv(torch.nn.Module):
         # plain-dict writes: torch.nn.Module.__setattr__ costs ~4 us per assignment, the hot path makes several per call
         d = self.__dict__
         d['_plans'] = {}
-        d['_host_ws'] = {}
-        d['_kf_cache'] = None          # (weakref(k), k._version, device, kf_engine, band)
+        d['_host_ws'] = {}             # (device, bytes) -> (staging buffer, _StreamOrder of its latest call)
+        d['_kf_cache'] = None          # (weakref(k), k._version, device, kf_engine, band, _StreamOrder of its transform)
         d['last_launches'] = 0         # kernels enqueued by the most recent operator call (bench.py); see _launched
 
     def __getstate__(self):
@@ -136,7 +164,9 @@ class FlashFFTConv(torch.nn.Module):
         convolution and the device->host copy pipelined over batch chunks (bffc_fwd_host, include/bffc.h), so both
         PCIe directions are busy at once.  u / gates / out: (B, H, L) host tensors of the module dtype (pin them, or
         the copies serialise); k: (H, Lk) fp32, host or device.  The result is complete once the current CUDA stream
-        of `device` is (the call is asynchronous).  Inference only (no autograd)."""
+        of `device` is (the call is asynchronous).  Calls on one module run one after the other, also when they are
+        issued on different streams (they share one staging buffer).  Inference only (no autograd), and not capturable
+        in a CUDA graph."""
         device = torch.device('cuda', torch.cuda.current_device()) if device is None else torch.device(device)
         return _forward_host(self, u, k, pregate, postgate, out, device)
 
@@ -167,18 +197,28 @@ def _forward_host(mod, u, k, pregate, postgate, out, device):
         raise RuntimeError('forward_host: out must be a contiguous host tensor like u')
     plan = mod.plan(device)
     with torch.cuda.device(device):
+        if torch.cuda.is_current_stream_capturing():
+            raise RuntimeError('forward_host cannot be captured in a CUDA graph: it pipelines host copies over internal '
+                               'streams; capture forward() on device tensors instead')
         mod.__dict__['last_launches'] = 0
         kf_engine = _kf_engine_for(mod, plan, k if k.is_cuda else k.to(device, non_blocking=True), cache_key=k)
         nws = _lib.lib().bffc_host_workspace_bytes(plan.handle, B, H, L, 1 if gates else 0)
-        ws = mod._host_ws.get((device, nws))
-        if ws is None:
+        # one staging buffer and one set of internal streams per module: calls follow each other.  On one stream that is
+        # stream order; a call on another stream first waits for the latest call (and for the buffer it outgrows)
+        for (d, _), (old, order) in mod._host_ws.items():
+            if d == device:
+                order.join(old)
+        held = mod._host_ws.get((device, nws))
+        if held is None:
             mod._host_ws.clear()
-            ws = mod._host_ws[(device, nws)] = torch.empty(nws, dtype=torch.uint8, device=device)
+            held = mod._host_ws[(device, nws)] = (torch.empty(nws, dtype=torch.uint8, device=device), _StreamOrder())
+        ws, order = held
         rc = _lib.lib().bffc_fwd_host(plan.handle, _ptr(u), _ptr(kf_engine), _ptr(pregate), _ptr(postgate),
                                       _ptr(out), B, H, L, _ptr(ws), nws, _stream())
         if rc:
             torch.cuda.synchronize(device)     # nothing may still be copying into / out of buffers we are about to drop
         _launched(mod, rc)
+        order.mark()
         # the library joins its internal streams back into the current stream before returning, so the caching
         # allocator (stream-ordered on the current stream) may recycle kf_engine / ws after this point
     return out
@@ -269,16 +309,24 @@ def _pack_kf(mod, plan, k, conj=0, band=None):
 
 def _kf_engine_for(mod, plan, k, cache_key=None, band=None, use_cache=None):
     """Engine-order spectrum of `k` (band-limited unless band is None), cached in eval mode (use_cache=None: the
-    module's own mode) while the same tensor object is unmodified and the band is the same."""
+    module's own mode) while the same tensor object is unmodified and the band is the same.  A hit on another stream
+    than the one that transformed the filter waits for the transform (_StreamOrder); a spectrum made while a CUDA graph
+    is being captured exists only when the graph runs, and is not cached."""
     key = k if cache_key is None else cache_key
     if use_cache is None:
         use_cache = not mod.training
     if use_cache and mod._kf_cache is not None:
-        ref, ver, dev, kf, kf_band = mod._kf_cache
+        ref, ver, dev, kf, kf_band, order = mod._kf_cache
         if ref() is key and ver == key._version and dev == k.device and kf_band == band:
+            order.join(kf)
             return kf
     kf = _pack_kf(mod, plan, k, band=band)
-    mod.__dict__['_kf_cache'] = (weakref.ref(key), key._version, k.device, kf, band) if use_cache else None
+    if use_cache and not torch.cuda.is_current_stream_capturing():
+        order = _StreamOrder()
+        order.mark()
+        mod.__dict__['_kf_cache'] = (weakref.ref(key), key._version, k.device, kf, band, order)
+    else:
+        mod.__dict__['_kf_cache'] = None
     return kf
 
 

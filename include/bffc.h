@@ -182,6 +182,9 @@ int bffc_fwd(const bffc_plan* plan, const void* u, const void* kf_engine, const 
  * Outputs: du (B,H,L) plan dtype; dkf_engine (H, N) float2 fp32 summed over B inside the kernel (overwritten, not
  * accumulated across calls); dpregate/dpostgate (B,H,L) plan dtype when gated (else NULL).  Gated: kf_engine is
  * required (dpostgate = dout * conv(u*pregate, k) is one pass of the forward path; du and dpregate come from one more).
+ * dkf_engine is accumulated with fp32 reductions (red.global.add) whose order depends on scheduling and on the SM count:
+ * an address that receives more than two partial sums can differ in its last bits from run to run; every other output
+ * is bit-reproducible.
  */
 int bffc_bwd(const bffc_plan* plan, const void* dout, const void* u, const void* kf_engine,
              const void* kf_engine_conj, const void* pregate, const void* postgate, void* du,
