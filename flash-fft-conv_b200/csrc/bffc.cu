@@ -12,6 +12,7 @@
 #include "r128_common.cuh"
 #include "fwd3_r128.cuh"
 #include "dkf3_r128.cuh"
+#include "engine_convert.cuh"
 #include "outer_cuda.cuh"
 #include "outer_r128.cuh"
 #include "filter_fft.cuh"
@@ -137,72 +138,6 @@ uint16_t f2h16(double x, int dtype) {   // table entry in the plan's element typ
   return b;
 }
 
-// k_f -> engine order.  One thread produces one 16-byte engine vector = 4 consecutive inner frequencies k2 = 4cc..4cc+3
-// of one (row, k1): words (re k2, re k2+1) (im ..) (re k2+2, re k2+3) (im ..).  Reads are coalesced along k1
-// (stride R complex numbers), writes are fully coalesced.
-// kHalf: the source holds only frequencies 0..N/2 of a real filter (torch.fft.rfft); k > N/2 is conj(src[N-k]).
-template <bool kHalf, int kFmt>
-__global__ void kf_pack_kernel(const float2* __restrict__ kf_nat, uint4* __restrict__ kf_eng, int N, int R0, int R1,
-                               float scale, int conj, int rblk) {
-  const int h = blockIdx.y;
-  const float2* src = kf_nat + size_t(h) * (kHalf ? (N / 2 + 1) : N);
-  const int nvec = N / 4;                              // engine vectors per channel
-  for (int v = blockIdx.x * blockDim.x + threadIdx.x; v < nvec; v += gridDim.x * blockDim.x) {
-    const int row = v / 2048, rem = v % 2048;          // 2048 vectors per 8192-word row
-    const int cc = rem >> 7, k1 = rem & 127;
-    const int c0 = row / R1, c1 = row % R1;
-    float2 e[4];
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      // small sizes (rblk = seqlen/64 < 128): K_seqlen[f] = K_8192[f * 128/rblk] at f = (k1 mod rblk) + rblk k2
-      int k = c0 + R0 * (c1 + R1 * (((k1 & (rblk - 1)) + rblk * (4 * cc + i)) * (128 / rblk)));
-      float sg = conj ? -1.f : 1.f;
-      if (kHalf && k > N / 2) { k = N - k; sg = -sg; }
-      const float2 t = src[k];
-      e[i] = make_float2(t.x * scale, t.y * scale * sg);
-    }
-    using NT = bffc::Num<kFmt>;
-    kf_eng[size_t(h) * nvec + v] = make_uint4(NT::pack(e[0].x, e[1].x), NT::pack(e[0].y, e[1].y),
-                                              NT::pack(e[2].x, e[3].x), NT::pack(e[2].y, e[3].y));
-  }
-}
-
-// Tiled variant for a large outermost radix R0 (tensor-core outer stage, R0 = 128): consecutive c0 are adjacent in the
-// natural order, consecutive words are adjacent in the engine rows, so a (32 c0) x (32 word pairs) tile goes
-// through shared memory and both sides are accessed in 256-byte runs.
-// grid: (8192/2/32 word-pair tiles, R0/32 * R1, H)
-constexpr int kInnerWords = 8192;
-
-template <bool kHalf, int kFmt>
-__global__ void kf_pack_tiled_kernel(const float2* __restrict__ kf_nat, uint2* __restrict__ kf_eng, int N, int R0, int R1,
-                                     float scale, int conj) {
-  __shared__ uint2 tile[32][33];
-  const int h = blockIdx.z;
-  const int c0b = (blockIdx.y % (R0 / 32)) * 32, c1 = blockIdx.y / (R0 / 32);
-  const int wp0 = blockIdx.x * 32;
-  const float2* src = kf_nat + size_t(h) * (kHalf ? (N / 2 + 1) : N);
-  const int tx = threadIdx.x, ty = threadIdx.y;      // 32 x 8
-  for (int j = ty; j < 32; j += 8) {
-    const int wp = wp0 + j;                            // word pair index inside the row: (cc*128 + k1)*2 + pp
-    const int pp = wp & 1, k1 = (wp >> 1) & 127, cc = wp >> 8;
-    float2 v[2];
-#pragma unroll
-    for (int e = 0; e < 2; ++e) {
-      int k = (c0b + tx) + R0 * (c1 + R1 * (k1 + 128 * (4 * cc + 2 * pp + e)));
-      float sg = conj ? -1.f : 1.f;
-      if (kHalf && k > N / 2) { k = N - k; sg = -sg; }
-      float2 t = src[k];
-      v[e] = make_float2(t.x * scale, t.y * scale * sg);
-    }
-    tile[tx][j] = make_uint2(bffc::Num<kFmt>::pack(v[0].x, v[1].x), bffc::Num<kFmt>::pack(v[0].y, v[1].y));
-  }
-  __syncthreads();
-  for (int j = ty; j < 32; j += 8) {                   // j = c0 offset, tx = word pair
-    const size_t row = (size_t(h) * R0 + (c0b + j)) * R1 + c1;
-    kf_eng[row * (kInnerWords / 2) + wp0 + tx] = tile[j][tx];
-  }
-}
-
 constexpr int kInner = 8192;   // the fused tensor-core kernel's size
 
 }  // namespace
@@ -259,6 +194,7 @@ static int kf_pack(const bffc_plan* p, const void* src, void* kf_engine, int H, 
   if (!p || !src || !kf_engine || H <= 0) return fail(BFFC_ERR_INVALID, "%s: bad argument", name);
   const cudaStream_t st = static_cast<cudaStream_t>(stream);
   const size_t src_row = kHalf ? p->NE / 2 + 1 : p->NE;       // float2 per channel of the source
+  using namespace bffc::eng;
   for (int h0 = 0; h0 < H; h0 += kMaxGridYZ) {                 // channels go to gridDim.y / z
     const int Hc = std::min(kMaxGridYZ, H - h0);
     const float2* s = static_cast<const float2*>(src) + size_t(h0) * src_row;
@@ -283,7 +219,7 @@ static int dkf_unpack(const bffc_plan* p, bool half, const void* dkf_engine, voi
   if (!p || !dkf_engine || !dst || H <= 0) return fail(BFFC_ERR_INVALID, "%s: bad argument", name);
   const cudaStream_t st = static_cast<cudaStream_t>(stream);
   const size_t out_row = half ? p->NE / 2 + 1 : p->NE;         // float2 per channel of the output
-  using namespace bffc::r128;
+  using namespace bffc::eng;
   for (int h0 = 0; h0 < H; h0 += kMaxGridYZ) {                 // channels go to gridDim.y / z
     const int Hc = std::min(kMaxGridYZ, H - h0);
     const float2* src = static_cast<const float2*>(dkf_engine) + size_t(h0) * p->NE;
@@ -422,10 +358,6 @@ int bffc_plan_create(bffc_plan** out, int seqlen, int dtype) {
       PLAN_TRY(table(&p->tw_hi, p->NE / 2048, double(p->NE) / 2048.0));
     }
   }
-
-  // engine order of k_f (32-bit words), per channel h: R rows of 8192 words, row = c0*R1 + c1 (outer digits); inside a
-  // row  w = (cc*128 + k1)*4 + 2*pp + part  holds the 16-bit pair (part ? imag : real) of k_f at inner frequencies
-  // k'' = k1 + 128*k2 with k2 = 4cc + 2pp and k2 + 1; natural frequency k = c0 + R0*(c1 + R1*k'').  See kf_pack_kernel.
 
   using namespace bffc::r128;
   FMT_SWITCH(dtype,

@@ -30,7 +30,7 @@ namespace bffc {
 struct DkfParams {
   const __nv_bfloat16* dft;  // see FwdParams
   const uint8_t* gtiles;
-  float2* dkf;               // [H][4][128][16] complex fp32: k2 = 16*q + t, frequency k = k1 + 128*k2
+  float2* dkf;               // [H][8192] complex fp32, engine order (engine_order.cuh)
   int B, H, L, pairs, kmask;  // pairs = batch groups per channel; kmask as in FwdParams
   int nseg, seg_bytes;        // segmented tiles (small sizes), see load_tile()
   float tw_scale;            // see FwdParams::tw_scale; dkf_unpack compensates
@@ -181,6 +181,7 @@ dkf3_kernel(const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CU
 #pragma unroll
         for (int i = 0; i < 8; ++i) {
           const int k2 = 8 * i + 2 * fp.q, e = 4 * i + 2 * rr;
+          // = p.dkf + h * 8192 + eng::dkf_slot(k1, k2), spelled out: the helper changes this kernel's code
           float* out = reinterpret_cast<float*>(p.dkf + ((size_t(h) * 4 + (k2 >> 4)) * 128 + k1) * 16 + (k2 & 15));
           red_add_v4(out, acc[e], acc[32 + e], acc[e + 1], acc[32 + e + 1]);
         }
@@ -188,101 +189,6 @@ dkf3_kernel(const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CU
 #pragma unroll
       for (int i = 0; i < 64; ++i) acc[i] = 0.f;
     }
-  }
-}
-
-// dk_f engine order -> natural order complex64 (reference analogue: the inverse permutation at conv.py:1818).
-// Composite sizes: channel row (h*R0 + c0)*R1 + c1 holds frequencies k = c0 + R0*(c1 + R1*(k1 + 128*k2)).
-// One thread moves the 16 consecutive-k2 values of one (row, quarter, k1): 128 contiguous bytes in, 16 stores that are
-// contiguous across the k1 lanes of a warp.
-__global__ void dkf_unpack_kernel(const float2* __restrict__ eng, float2* __restrict__ nat, int N, int R0, int R1,
-                                  float scale) {
-  const int h = blockIdx.y;
-  const int R = R0 * R1;
-  const int ngroups = R * 4 * 128;                      // (row, quarter, k1) groups per channel
-  for (int g = blockIdx.x * blockDim.x + threadIdx.x; g < ngroups; g += gridDim.x * blockDim.x) {
-    const int k1 = g & 127, qd = (g >> 7) & 3, row = g >> 9;
-    const int c0 = row / R1, c1 = row % R1;
-    const float4* in = reinterpret_cast<const float4*>(eng + ((size_t(h) * R + row) * 4 + qd) * 128 * 16 + size_t(k1) * 16);
-#pragma unroll
-    for (int t2 = 0; t2 < 8; ++t2) {
-      const float4 v = in[t2];
-      const int k2 = 16 * qd + 2 * t2;
-      const size_t ka = size_t(c0) + size_t(R0) * (c1 + size_t(R1) * (k1 + 128 * k2));
-      const size_t kb = size_t(c0) + size_t(R0) * (c1 + size_t(R1) * (k1 + 128 * (k2 + 1)));
-      nat[size_t(h) * N + ka] = make_float2(v.x * scale, v.y * scale);
-      nat[size_t(h) * N + kb] = make_float2(v.z * scale, v.w * scale);
-    }
-  }
-}
-
-
-// dk_f engine order -> the N/2 + 1 non-redundant bins of its Hermitian part, natural order, complex64:
-//     Xh[k] = (X[k] + conj X[(N - k) mod N]) / 2,   k = 0 .. N/2,
-// so that dk = irfft(Xh, n = N)[:Lk] — the same real part as the reference's ifft(dk_f).real (conv.py:1817-1820; the
-// pair-packed spectrum is not Hermitian, its anti-Hermitian part is exactly what `.real` discards) at half the FFT work
-// and without the full-spectrum round trips (unpack, c2c FFT, .real / slice).
-// A block moves a tile of TR residues r (k = r + R kin, natural-fastest; engine row rho = (r % R0) R1 + r / R0) x the 16
-// consecutive k2 of one (k1, quarter): 128-byte runs on the engine side, TR x 8-byte runs on the natural side.
-// grid: (R / TR, 128 * 2, H), TR = min(32, R); 256 threads.
-DEVINL size_t dkf_engine_index(int h, int k, int R0, int R1) {
-  const int R = R0 * R1;
-  const int r = k % R, kin = k / R;
-  const int rho = (r % R0) * R1 + r / R0;
-  const int k1 = kin & 127, k2 = kin >> 7;
-  return ((size_t(h) * R + rho) * 4 + (k2 >> 4)) * 2048 + size_t(k1) * 16 + (k2 & 15);
-}
-__global__ void dkf_unpack_half_kernel(const float2* __restrict__ eng, float2* __restrict__ half, int N, int R0, int R1,
-                                       float scale) {
-  __shared__ float2 tile[16][33];
-  const int R = R0 * R1, TR = R < 32 ? R : 32;
-  const int r0 = blockIdx.x * TR, k1 = blockIdx.y & 127, qd = blockIdx.y >> 7, h = blockIdx.z;
-  const float sc = 0.5f * scale;
-  for (int idx = threadIdx.x; idx < TR * 16; idx += blockDim.x) {
-    const int rl = idx >> 4, t = idx & 15;
-    const int k = (r0 + rl) + R * (k1 + 128 * (16 * qd + t));
-    const float2 a = eng[dkf_engine_index(h, k, R0, R1)];
-    const float2 b = eng[dkf_engine_index(h, (N - k) & (N - 1), R0, R1)];
-    tile[t][rl] = make_float2((a.x + b.x) * sc, (a.y - b.y) * sc);
-  }
-  __syncthreads();
-  float2* out = half + size_t(h) * (N / 2 + 1);
-  for (int idx = threadIdx.x; idx < TR * 16; idx += blockDim.x) {
-    const int t = idx / TR, rl = idx - t * TR;
-    const int k = (r0 + rl) + R * (k1 + 128 * (16 * qd + t));
-    if (k < N / 2) out[k] = tile[t][rl];
-  }
-  if (blockIdx.x == 0 && blockIdx.y == 0 && threadIdx.x == 0) {        // the Nyquist bin (self-conjugate partner)
-    const float2 a = eng[dkf_engine_index(h, N / 2, R0, R1)];
-    out[N / 2] = make_float2(a.x * scale, 0.f);
-  }
-}
-
-
-// Small sizes (seqlen N < 8192, one engine row per channel): the 8192/N stage-1 blocks hold different batch members at the
-// same N-point frequency f = (k1 mod r) + r k2, r = N/64.  Natural-order output on the 8192-point grid the plan reports
-// as its fft size: X[f * 8192/N] = (8192/N) sum_blocks dk_f (zero elsewhere), so that ifft_8192(X).real[:Lk] = dk.
-// half = 0: all 8192 bins; half = 1: bins 0..4096 of the Hermitian part (X[k] + conj X[8192 - k]) / 2 (for irfft).
-__global__ void dkf_unpack_small_kernel(const float2* __restrict__ eng, float2* __restrict__ out, int N, float scale, int half) {
-  const int h = blockIdx.y, k = blockIdx.x * blockDim.x + threadIdx.x;
-  const int r = N >> 6, q8 = 8192 / N;
-  const float2* src = eng + size_t(h) * 8192;
-  auto X = [&](int kk) {
-    float2 acc = make_float2(0.f, 0.f);
-    if (kk % q8) return acc;
-    const int f = kk / q8, k1p = f & (r - 1), k2 = f / r;
-    for (int m = 0; m < q8; ++m) {
-      const float2 v = src[(((k2 >> 4) * 128 + k1p + r * m) << 4) + (k2 & 15)];
-      acc.x += v.x; acc.y += v.y;
-    }
-    const float sc = scale * float(q8);
-    return make_float2(acc.x * sc, acc.y * sc);
-  };
-  if (!half) {
-    if (k < 8192) out[size_t(h) * 8192 + k] = X(k);
-  } else if (k <= 4096) {
-    const float2 a = X(k), b = X((8192 - k) & 8191);
-    out[size_t(h) * 4097 + k] = make_float2(0.5f * (a.x + b.x), 0.5f * (a.y - b.y));
   }
 }
 

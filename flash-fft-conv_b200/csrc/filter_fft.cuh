@@ -15,6 +15,7 @@
 // limit there (in_band below): the frequency-sparse convolution's mask, free when it keeps everything.
 #pragma once
 #include "ptx.cuh"
+#include "engine_order.cuh"
 
 namespace bffc {
 namespace ffft {
@@ -137,8 +138,7 @@ DEVINL int pos_of_freq(int f) { return 512 * (f & 15) + 32 * ((f >> 4) & 15) + (
 DEVINL bool in_band(int f, int N, int band) { return min(f, N - f) < band; }
 
 // grid = ceil(H / 2): channels 2*blockIdx.x (real part) and 2*blockIdx.x + 1 (imaginary part)
-// N < 8192 (small sizes): the engine row holds the N-point spectrum K_N[f] = K_8192[f * 8192/N] (k has support < N) at
-// (lane k1, column k2) -> f = (k1 mod N/64) + (N/64) k2, i.e. replicated over the 8192/N stage-1 blocks of the kernel.
+// N < 8192 (small sizes): the engine row holds the N-point spectrum K_N[f] = K_8192[f * 8192/N] (k has support < N).
 template <int kFmt>
 __global__ void __launch_bounds__(kThreads, 3) kf_from_filter_kernel(const float* __restrict__ k, int Lk, uint4* __restrict__ kf_eng,
                                                                      int H, float scale, int conj, const float2* __restrict__ tw,
@@ -161,8 +161,7 @@ __global__ void __launch_bounds__(kThreads, 3) kf_from_filter_kernel(const float
   }
   __syncthreads();
   fft8192<-1>(fbuf, tid, tw);
-  // K_a[f] = (Z[f] + conj Z[-f]) / 2,  K_b[f] = (Z[f] - conj Z[-f]) / (2i); engine vector v = c*128 + k1 holds
-  // frequencies k1 + 128 (4c + j), j = 0..3, as (re01, im01, re23, im23)
+  // K_a[f] = (Z[f] + conj Z[-f]) / 2,  K_b[f] = (Z[f] - conj Z[-f]) / (2i)
   using NT = Num<kFmt>;
   const float sa = 0.5f * scale, sgn = conj ? -1.f : 1.f;
   const int r = N >> 6, q8 = kN / N;                  // stage-1 block size, spectrum stride
@@ -171,7 +170,7 @@ __global__ void __launch_bounds__(kThreads, 3) kf_from_filter_kernel(const float
     float2 A[4], Bv[4];
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
-      const int fn = (k1 & (r - 1)) + r * (4 * c + j), f = fn * q8;     // frequency on the N grid, on the 8192 grid
+      const int fn = eng::kf_freq(c, k1, j, r), f = fn * q8;           // frequency on the N grid, on the 8192 grid
       const float2 z = fbuf[slot(pos_of_freq(f))], zc = fbuf[slot(pos_of_freq((kN - f) & (kN - 1)))];
       const bool keep = in_band(fn, N, band);
       A[j] = keep ? make_float2((z.x + zc.x) * sa, (z.y - zc.y) * sa * sgn) : make_float2(0.f, 0.f);
@@ -186,10 +185,8 @@ __global__ void __launch_bounds__(kThreads, 3) kf_from_filter_kernel(const float
 }
 
 // grid = H.  dk[n] = scale/N * Re( sum_f D_N[f] e^{2 pi i f n / N} ), n < Lk.
-// Engine order of dk_f (dkf3_r128.cuh): index ((qd*128 + k1)*16 + k2l) holds (lane k1, column k2 = 16 qd + k2l).
-// N = 8192: frequency k1 + 128 k2.  N < 8192: the 8192/N stage-1 blocks hold different batch members at the same
-// N-point frequency f = (k1 mod r) + r k2, r = N/64; their sum D_N[f] goes to 8192-point frequency f * 8192/N (the rest
-// is zero), whose inverse transform is the N-periodic gradient.  The band limit masks D_N[f] as it is read (Re ifft of
+// N < 8192: the block sum D_N[f] (engine_order.cuh) goes to 8192-point frequency f * 8192/N (the rest is zero), whose
+// inverse transform is the N-periodic gradient.  The band limit masks D_N[f] as it is read (Re ifft of
 // the masked spectrum = ifft of the masked Hermitian part, the mask being symmetric).
 __global__ void __launch_bounds__(kThreads, 3) dk_from_dkf_kernel(const float2* __restrict__ dkf_eng, float* __restrict__ dk, int Lk,
                                                                   float scale, int N, const float2* __restrict__ tw, int band) {
@@ -199,8 +196,7 @@ __global__ void __launch_bounds__(kThreads, 3) dk_from_dkf_kernel(const float2* 
   if (N == kN) {
 #pragma unroll 16
     for (int e = tid; e < kN; e += kThreads) {
-      const int k2l = e & 15, k1 = (e >> 4) & 127, qd = e >> 11;
-      const int f = k1 + 128 * (16 * qd + k2l);
+      const int f = eng::dkf_freq(e);
       const float2 d = __ldg(src + e);
       fbuf[slot(f)] = in_band(f, kN, band) ? d : make_float2(0.f, 0.f);
     }
@@ -212,10 +208,7 @@ __global__ void __launch_bounds__(kThreads, 3) dk_from_dkf_kernel(const float2* 
     // task t -> (k2l fastest, then k1', then quarter): 16 consecutive threads read 128 contiguous bytes of every block
     for (int t = tid; t < N; t += kThreads) {
       const int k2l = t & 15, k1p = (t >> 4) & (r - 1), qd = t / (16 * r);
-      const float2* b0 = src + ((qd * 128 + k1p) << 4) + k2l;
-      float2 acc = make_float2(0.f, 0.f);
-#pragma unroll 4
-      for (int m = 0; m < q8; ++m) acc = cadd(acc, __ldg(b0 + ((r * m) << 4)));
+      const float2 acc = eng::small_block_sum<float2>(k1p, 16 * qd + k2l, r, q8, [&](int s) { return __ldg(src + s); });
       const int fn = k1p + r * (16 * qd + k2l);                       // frequency on the N grid
       fbuf[slot(fn * q8)] = in_band(fn, N, band) ? acc : make_float2(0.f, 0.f);
     }
@@ -380,8 +373,8 @@ DEVINL void load_row(float2* fbuf, const float2* __restrict__ src, int tid) {
   }
 }
 
-// engine vector v = c*128 + k1 holds the frequencies f_j = k1 + 128 (4c + j); with k1 fixed per thread (v = tid + 256 i)
-// pos_of_freq(f_j) = 512 (k1 & 15) + 32 ((k1 >> 4) + 8 (j & 1)) + 2c + (j >> 1); the mirrored row reads 8191 - f_j.
+// engine vector v = c*128 + k1 (v = tid + 256 i) holds the frequencies f_j = eng::kf_freq(c, k1, j); with k1 fixed per
+// thread pos_of_freq(f_j) = 512 (k1 & 15) + 32 ((k1 >> 4) + 8 (j & 1)) + 2c + (j >> 1); the mirrored row reads 8191 - f_j.
 // rho_w: residue of the row written, whose word f_j holds natural frequency rho_w + R f_j (band-limited there)
 template <int kFmt, bool kMirror>
 DEVINL void store_engine_row(const float2* fbuf, uint4* __restrict__ row, int tid, float sgn, int rho_w, int R, int band) {
@@ -399,14 +392,14 @@ DEVINL void store_engine_row(const float2* fbuf, uint4* __restrict__ row, int ti
         const int k1m = 127 - k1, jm = 3 - j, cm = 15 - c;
         p = 512 * (k1m & 15) + 32 * ((k1m >> 4) + 8 * (jm & 1)) + 2 * cm + (jm >> 1);
       }
-      A[j] = in_band(rho_w + R * (k1 + 128 * (4 * c + j)), N, band) ? fbuf[slot(p)] : make_float2(0.f, 0.f);
+      A[j] = in_band(rho_w + R * eng::kf_freq(c, k1, j), N, band) ? fbuf[slot(p)] : make_float2(0.f, 0.f);
     }
     row[tid + 256 * i] = make_uint4(NT::pack(A[0].x, A[1].x), NT::pack(sgn * A[0].y, sgn * A[1].y),
                                     NT::pack(A[2].x, A[3].x), NT::pack(sgn * A[2].y, sgn * A[3].y));
   }
 }
 
-// grid (R/2 + 1, Hc).  kf_eng: (Hc, R rows, 2048 vectors of 16 bytes); row of residue rho = (rho % R0) * R1 + rho / R0
+// grid (R/2 + 1, Hc).  kf_eng: (Hc, R rows, 2048 vectors of 16 bytes)
 template <int kFmt>
 __global__ void __launch_bounds__(kThreads, 3) filter_rows_kernel(const float2* __restrict__ T, uint4* __restrict__ kf_eng, int R, int R0,
                                                                   int R1, int conj, const float2* __restrict__ tw, int band) {
@@ -416,18 +409,16 @@ __global__ void __launch_bounds__(kThreads, 3) filter_rows_kernel(const float2* 
   __syncthreads();
   fft8192<-1>(fbuf, tid, tw);
   const float sgn = conj ? -1.f : 1.f;
-  store_engine_row<kFmt, false>(fbuf, kf_eng + (size_t(h) * R + (rho % R0) * R1 + rho / R0) * (kN / 4), tid, sgn, rho, R,
-                                band);
+  store_engine_row<kFmt, false>(fbuf, kf_eng + (size_t(h) * R + eng::row_of_residue(rho, R0, R1)) * (kN / 4), tid, sgn,
+                                rho, R, band);
   if (rho == 0 || 2 * rho == R) return;
   const int rm = R - rho;
-  store_engine_row<kFmt, true>(fbuf, kf_eng + (size_t(h) * R + (rm % R0) * R1 + rm / R0) * (kN / 4), tid, -sgn, rm, R,
-                               band);
+  store_engine_row<kFmt, true>(fbuf, kf_eng + (size_t(h) * R + eng::row_of_residue(rm, R0, R1)) * (kN / 4), tid, -sgn,
+                               rm, R, band);
 }
 
-// ---- inverse: dk (Hc, Lk) fp32 from dk_f engine rows (fp32 complex, row layout [quarter 4][k1 128][k2l 16], frequency
-// k'' = k1 + 128 (16 quarter + k2l) — dkf3_r128.cuh).  dk = Re ifft(dk_f): only the Hermitian part of the pair-packed
-// spectrum contributes, G[k] = (D[k] + conj D[N - k]) / 2; the partner of (rho, k'') is (R - rho, 8191 - k''), i.e. the
-// partner row read backwards (row 0: (0, (8192 - k'') mod 8192)).
+// ---- inverse: dk (Hc, Lk) fp32 from dk_f engine rows.  dk = Re ifft(dk_f): only the Hermitian part of the pair-packed
+// spectrum contributes, G[k] = (D[k] + conj D[N - k]) / 2 (partner: eng::dkf_partner_slot).
 // grid (R/2 + 1, Hc).  T: (Hc, R/2 + 1, 8192) = Y[rho][n2] = sum_{n1} W_R^{n1 rho} dk[n1*8192 + n2], unscaled.
 __global__ void __launch_bounds__(kThreads, 3) dk_rows_kernel(const float2* __restrict__ dkf_eng, float2* __restrict__ T, int R, int R0,
                                                               int R1, const float2* __restrict__ tw,
@@ -436,18 +427,12 @@ __global__ void __launch_bounds__(kThreads, 3) dk_rows_kernel(const float2* __re
   extern __shared__ float2 fbuf[];
   const int tid = threadIdx.x, rho = blockIdx.x, h = blockIdx.y;
   const int rm = (R - rho) & (R - 1), N = R * kN;
-  const float2* row = dkf_eng + (size_t(h) * R + (rho % R0) * R1 + rho / R0) * kN;
-  const float2* mrow = dkf_eng + (size_t(h) * R + (rm % R0) * R1 + rm / R0) * kN;
+  const float2* row = dkf_eng + (size_t(h) * R + eng::row_of_residue(rho, R0, R1)) * kN;
+  const float2* mrow = dkf_eng + (size_t(h) * R + eng::row_of_residue(rm, R0, R1)) * kN;
 #pragma unroll 8
   for (int e = tid; e < kN; e += kThreads) {
-    const int k2l = e & 15, k1 = (e >> 4) & 127, qd = e >> 11;
-    const int f = k1 + 128 * (16 * qd + k2l);
-    int em = kN - 1 - e;
-    if (rho == 0) {
-      const int fm = (kN - f) & (kN - 1), k2m = fm >> 7;
-      em = ((k2m >> 4) * 128 + (fm & 127)) * 16 + (k2m & 15);
-    }
-    const float2 a = row[e], b = mrow[em];
+    const int f = eng::dkf_freq(e);
+    const float2 a = row[e], b = mrow[eng::dkf_partner_slot(e, rho == 0)];
     fbuf[slot(f)] = in_band(rho + R * f, N, band) ? make_float2(0.5f * (a.x + b.x), 0.5f * (a.y - b.y)) : make_float2(0.f, 0.f);
   }
   __syncthreads();

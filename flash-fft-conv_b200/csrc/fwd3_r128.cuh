@@ -312,8 +312,8 @@ fwd3_kernel(const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CU
     r64_stage<kFmt>(d, are, aim, s_g, s_g + 2 * kGTileBytes, s_g + kGTileBytes, s_g);
     wgmma_wait_regs(d);
 
-    // ---------------- pass 3: * k_f -> A operand of stage 3.  k_f engine vector (c, k1), c = k2 / 4, holds words
-    // (kr, kr)(ki, ki) of k2 = 4c, 4c+1 then of 4c+2, 4c+3; this thread's k2 = 8 i + 2 q + {0, 1}.
+    // ---------------- pass 3: * k_f -> A operand of stage 3.  This thread's k2 = 8 i + 2 q + {0, 1}: one word pair
+    // (re, im) of k_f per i, at eng::kf_pair(k1, 8 i + 2 q) — spelled out below: the helper changes this kernel's code.
     {
       const FragPos fp = frag();
       const uint2* kfp = reinterpret_cast<const uint2*>(p.kf) + size_t(h) * 16 * 128 * 2 + (fp.q & 1);

@@ -22,6 +22,7 @@
 //    FragPos::row[rr]; the tiles in shared memory and the engine order stay in natural row order.
 #pragma once
 #include "ptx.cuh"
+#include "engine_order.cuh"
 #include "short_filter.cuh"
 #include <cuda.h>
 #include <cuda_fp16.h>
@@ -29,7 +30,7 @@
 namespace bffc {
 
 struct FwdParams {
-  const uint32_t* kf;        // [rows][16][128][4] bf16x2 words (kr0,kr1)(ki0,ki1)(kr2,kr3)(ki2,ki3), engine order, /N
+  const uint32_t* kf;        // [rows][2048][4] words of two 16-bit values, engine order (engine_order.cuh), /N
   const __nv_bfloat16* dft;  // [128][128] conjugate-pair rows of the DFT-128 (cos / sin, see FragPos), K-major
   const uint8_t* gtiles;     // DFT-64 tiles Gr, Gi, -Gi, Gr: each 64 rows x 128 B, 128B-swizzled image
   float kf_scale;            // fp16 only: k_f is stored unscaled (1/N would underflow fp16) and scaled here in fp32
