@@ -18,6 +18,7 @@
 #include "filter_fft.cuh"
 #include "dwconv1d.cuh"
 #include "decode_step.cuh"
+#include "docs.cuh"
 
 #include <algorithm>
 #include <cmath>
@@ -1838,6 +1839,83 @@ int bffc_conv_step(const void* u, int64_t u_bstride, const void* pregate, int64_
     rc = launched();
   });
   return rc;
+}
+
+}  // extern "C"
+
+// ------------------------------------------------------------------------------ packed documents by length class
+namespace {
+
+// The arguments gather and scatter share, checked before the device is looked at.  rows / bs: the row-side tensors
+// (B, H, L) with their batch strides; gathered: the class-batch buffers of H * positions elements.
+int docs_args(const char* fn, const void* items, int n_items, long long positions, int B, int H, int L,
+              const void* const* rows, const int64_t* bs, const void* const* gathered, int n_tensors,
+              bffc::docs::Params* prm) {
+  if (B < 1 || H < 1 || L < 1) return fail(BFFC_ERR_INVALID, "%s: bad shape B=%d H=%d L=%d", fn, B, H, L);
+  if (n_items < 0) return fail(BFFC_ERR_INVALID, "%s: n_items=%d is negative", fn, n_items);
+  if (positions < 128LL * n_items || positions % 128 ||
+      positions > 2LL * B * L + 128LL * n_items)
+    return fail(BFFC_ERR_INVALID, "%s: positions=%lld is not a multiple of 128 in [128 * n_items, 2 * B * L + 128 * "
+                "n_items] (n_items=%d)", fn, positions, n_items);
+  if (n_items > 0 && (!items || reinterpret_cast<uintptr_t>(items) % 8))
+    return fail(BFFC_ERR_INVALID, "%s: item table is null or not 8-byte aligned", fn);
+  if (n_tensors < 1 || n_tensors > bffc::docs::kMaxTensors)
+    return fail(BFFC_ERR_INVALID, "%s: n_tensors=%d outside [1, %d]", fn, n_tensors, bffc::docs::kMaxTensors);
+  if (!rows || !bs || !gathered) return fail(BFFC_ERR_INVALID, "%s: null tensor array", fn);
+  *prm = bffc::docs::Params{};
+  for (int k = 0; k < n_tensors; ++k) {
+    if (!rows[k] || reinterpret_cast<uintptr_t>(rows[k]) % 2)
+      return fail(BFFC_ERR_INVALID, "%s: row tensor %d is null or not 2-byte aligned", fn, k);
+    if (!gathered[k] || reinterpret_cast<uintptr_t>(gathered[k]) % 16)
+      return fail(BFFC_ERR_INVALID, "%s: gathered tensor %d is null or not 16-byte aligned", fn, k);
+    if (bs[k] < int64_t(H) * L)
+      return fail(BFFC_ERR_INVALID, "%s: batch stride %lld of tensor %d below H * L = %lld", fn, (long long)bs[k], k,
+                  (long long)H * L);
+    prm->rows[k] = static_cast<uint16_t*>(const_cast<void*>(rows[k]));
+    prm->bs[k] = bs[k];
+    prm->gathered[k] = static_cast<uint16_t*>(const_cast<void*>(gathered[k]));
+  }
+  prm->items = static_cast<const bffc::docs::DocItem*>(items);
+  prm->n_items = n_items;
+  prm->positions = positions;
+  prm->B = B; prm->H = H; prm->L = L;
+  prm->nt = n_tensors;
+  return 0;
+}
+
+int docs_launch(const bffc::docs::Params& prm, bool scatter, void* stream) {
+  if (int rc = check_device()) return rc;
+  g_launches = 0;
+  const long long nvec = prm.positions * prm.H / bffc::docs::kVec;
+  if (nvec == 0) return 0;                        // no documents: nothing to move
+  const long long blocks = std::min<long long>((nvec + bffc::docs::kThreads - 1) / bffc::docs::kThreads, 1LL << 22);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (scatter) bffc::docs::scatter_kernel<<<unsigned(blocks), bffc::docs::kThreads, 0, st>>>(prm);
+  else bffc::docs::gather_kernel<<<unsigned(blocks), bffc::docs::kThreads, 0, st>>>(prm);
+  return launched();
+}
+
+}  // namespace
+
+extern "C" {
+
+int bffc_docs_gather(const void* items, int n_items, int64_t positions, int B, int H, int L, const void* const* src,
+                     const int64_t* src_bstride, void* const* gathered, int n_tensors, void* stream) {
+  bffc::docs::Params prm;
+  if (int rc = docs_args("bffc_docs_gather", items, n_items, positions, B, H, L, src, src_bstride,
+                         const_cast<const void* const*>(gathered), n_tensors, &prm))
+    return rc;
+  return docs_launch(prm, false, stream);
+}
+
+int bffc_docs_scatter(const void* items, int n_items, int64_t positions, int B, int H, int L,
+                      const void* const* gathered, void* const* dst, const int64_t* dst_bstride, int n_tensors,
+                      void* stream) {
+  bffc::docs::Params prm;
+  if (int rc = docs_args("bffc_docs_scatter", items, n_items, positions, B, H, L, const_cast<const void* const*>(dst),
+                         dst_bstride, gathered, n_tensors, &prm))
+    return rc;
+  return docs_launch(prm, true, stream);
 }
 
 }  // extern "C"

@@ -4,3 +4,4 @@ from .gated import gated_long_conv, hyena_mixer, hyena_operator  # noqa: F401
 from .sparse_conv import PartialFFTConv, FrequencySparseFFTConv  # noqa: F401  (reference flashfftconv/sparse_conv.py)
 from .block_conv import blocked_long_conv  # noqa: F401
 from .decode import HyenaDecoder, LongConvDecoder  # noqa: F401
+from .docs import DocumentTable  # noqa: F401

@@ -12,6 +12,7 @@ returns what FlashFFTConv(n)(u, k, pregate, postgate) returns for any n >= L + L
 gates (bffc_fwd_blocked / bffc_bwd_blocked, include/bffc.h).
 """
 from . import conv as _conv
+from . import docs as _docs
 
 BLOCK = 8192                 # transform size of every block: the seqlen of the module the call takes
 MAX_TAPS = 4097              # filter taps a block can hold: halo <= 4096
@@ -25,12 +26,14 @@ def blocked_halo(Lk):
     return 512 * ((Lk - 1 + 511) // 512)
 
 
-def blocked_long_conv(conv, u, k, pregate=None, postgate=None):
+def blocked_long_conv(conv, u, k, pregate=None, postgate=None, docs=None):
     """y = postgate * causal_conv(u * pregate, k) of any length L, in overlap-save blocks of FlashFFTConv(8192).
 
     conv: a FlashFFTConv(8192, dtype) module; u, pregate, postgate: (B, H, L) tensors of conv.dtype (channel slices of a
     projection are read in place), the gates both given or both None; k: (H, Lk) fp32 filter, Lk <= 4097.  Gradients
-    flow to u, k and the gates.  A ragged L is zero-padded to a multiple of 64, which does not change a causal result."""
+    flow to u, k and the gates.  A ragged L is zero-padded to a multiple of 64, which does not change a causal result.
+    Packed documents (docs) are not kept apart by the blocks yet: a DocumentTable is refused."""
+    _docs.refuse(docs, 'blocked_long_conv')
     if not isinstance(conv, _conv.FlashFFTConv) or conv.seqlen != BLOCK:
         raise RuntimeError(f'blocked_long_conv needs a FlashFFTConv({BLOCK}, dtype) module, got '
                            f'{type(conv).__name__}({getattr(conv, "seqlen", "?")})')

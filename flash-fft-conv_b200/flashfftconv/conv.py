@@ -123,10 +123,11 @@ class FlashFFTConv(torch.nn.Module):
         d['_host_ws'] = {}             # (device, bytes) -> (staging buffer, _StreamOrder of its latest call)
         d['_kf_cache'] = None          # (weakref(k), k._version, device, kf_engine, band, _StreamOrder of its transform)
         d['last_launches'] = 0         # kernels enqueued by the most recent operator call (bench.py); see _launched
+        d['_class_mods'] = {}          # class length c -> FlashFFTConv(2c) of the packed-document path (docs.py)
 
     def __getstate__(self):
         state = self.__dict__.copy()
-        for key in ('_plans', '_host_ws', '_kf_cache'):
+        for key in ('_plans', '_host_ws', '_kf_cache', '_class_mods'):
             state.pop(key, None)
         return state
 
@@ -159,20 +160,31 @@ class FlashFFTConv(torch.nn.Module):
         """FFT size of the engine: seqlen, or 8192 for the small sizes (8192/seqlen batch members share one 8192-point unit)."""
         return self.plan(device).fft_size
 
-    def forward_host(self, u, k, pregate=None, postgate=None, out=None, device=None):
+    def forward_host(self, u, k, pregate=None, postgate=None, out=None, device=None, docs=None):
         """Forward on HOST tensors: y = forward(u.cuda(), k.cuda(), ...).cpu(), with the host->device copies, the
         convolution and the device->host copy pipelined over batch chunks (bffc_fwd_host, include/bffc.h), so both
         PCIe directions are busy at once.  u / gates / out: (B, H, L) host tensors of the module dtype (pin them, or
         the copies serialise); k: (H, Lk) fp32, host or device.  The result is complete once the current CUDA stream
         of `device` is (the call is asynchronous).  Calls on one module run one after the other, also when they are
         issued on different streams (they share one staging buffer).  Inference only (no autograd), and not capturable
-        in a CUDA graph."""
+        in a CUDA graph, and no packed documents (docs)."""
+        from . import docs as _docs
+        _docs.refuse(docs, 'forward_host')
         device = torch.device('cuda', torch.cuda.current_device()) if device is None else torch.device(device)
         return _forward_host(self, u, k, pregate, postgate, out, device)
 
-    def forward(self, u, k, pregate=None, postgate=None):
+    def forward(self, u, k, pregate=None, postgate=None, docs=None):
+        """y = postgate * conv(u * pregate, k), the gates both given or both None.  docs: a DocumentTable of packed
+        documents in the rows of u; each document is then convolved alone and causally (flashfftconv.docs,
+        INTEGRATION.md §11), with gradients to u, k and the gates."""
         if pregate is not None or postgate is not None:
             assert pregate is not None and postgate is not None       # conv.py:557-558
+        if docs is not None:
+            from . import docs as _docs
+            _check_inputs(u, k, self, () if pregate is None else (pregate, postgate), views=True)
+            _docs._check(docs, u)
+            return _docs.DocsConvFunc.apply(u, k, self, self.training, docs, pregate, postgate)
+        if pregate is not None:
             return FlashFFTConvFunc.apply(u, k, self, self.training, pregate, postgate)
         return FlashFFTConvFunc.apply(u, k, self, self.training)
 
@@ -363,13 +375,15 @@ class _on_device:
             self.ctx.__exit__(*a)
 
 
-def _fwd(mod, u, k, pregate, postgate, band=None, use_cache=None, kf_engine=None, taps=None, halo=None):
+def _fwd(mod, u, k, pregate, postgate, band=None, use_cache=None, kf_engine=None, taps=None, halo=None, out=None,
+         cache_key=None):
     """y (contiguous) and the engine-order filter spectrum it used.  u and the gates: any (B, H, L) layout; those that
     qualify (batch_stride) are read in place, others copied.  band / use_cache: see _kf_engine_for; kf_engine: a
     spectrum of k already at hand.  taps: ((u_w, u_bias, pregate_w, pregate_bias, postgate_w, postgate_bias), w_dtype,
     K, padding), a short depthwise filter bffc_fwd_short_strided applies to u and the gates as it loads them; the rows
     are device addresses of (H, K) taps and (H) biases, None for a tensor that is not filtered.  halo: overlap-save
-    blocks with this halo (bffc_fwd_blocked, blocked_long_conv), else None."""
+    blocks with this halo (bffc_fwd_blocked, blocked_long_conv), else None.  out: a contiguous (B, H, L) tensor to write y
+    into (L a multiple of bffc_length_multiple()).  cache_key: see _kf_engine_for."""
     B, H, L = u.shape
     dev = u.device
     plan = mod.plan(dev)
@@ -377,14 +391,16 @@ def _fwd(mod, u, k, pregate, postgate, band=None, use_cache=None, kf_engine=None
     if Lp != L:
         if taps is not None:       # the filter's bias would reach past L: padding the input is not padding its output
             raise RuntimeError(f'L={L} must be a multiple of bffc_length_multiple() to fuse a short filter')
+        if out is not None:
+            raise RuntimeError(f'L={L} must be a multiple of bffc_length_multiple() to write into `out`')
         y, kf = _fwd(mod, _padded(u, Lp), k, _padded(pregate, Lp), _padded(postgate, Lp), band, use_cache, kf_engine,
                      halo=halo)
         return y[..., :L].contiguous(), kf
     (u, u_bs), (pre, pre_bs), (post, post_bs) = [_engine_view(t, mod.dtype) for t in (u, pregate, postgate)]
     with _on_device(dev):
         if kf_engine is None:
-            kf_engine = _kf_engine_for(mod, plan, k, band=band, use_cache=use_cache)
-        y = torch.empty((B, H, L), dtype=u.dtype, device=dev)
+            kf_engine = _kf_engine_for(mod, plan, k, cache_key=cache_key, band=band, use_cache=use_cache)
+        y = torch.empty((B, H, L), dtype=u.dtype, device=dev) if out is None else out
         ws, ws_bytes = _workspace(plan, B, H, L, pre is not None, False, dev)
         if halo is not None:
             rc = _lib.lib().bffc_fwd_blocked(plan.handle, _ptr(u), u_bs, _ptr(kf_engine), _ptr(pre), pre_bs, _ptr(post),

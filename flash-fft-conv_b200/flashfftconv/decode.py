@@ -41,6 +41,7 @@ import torch
 from . import _lib
 from . import depthwise_1d as _dw
 from .conv import FlashFFTConv, _DT, _on_device, _ptr, _stream
+from .docs import refuse
 from .gated import gated_long_conv, hyena_operator
 
 MAX_STEP_TOKENS = 64
@@ -261,9 +262,10 @@ class HyenaDecoder(_Decoder):
         return v, x1, x2
 
     @torch.no_grad()
-    def prefill(self, x):
+    def prefill(self, x, docs=None):
         """y (B, d_model, L) of the prompt x (B, 3 * d_model, L) by the FFT engine, and the caches filled from it; starts
-        a new sequence.  L may be 0."""
+        a new sequence.  L may be 0.  Packed documents (docs) are refused: one decoder row is one sequence."""
+        refuse(docs, 'HyenaDecoder')
         L = x.shape[-1]
         if L > self.max_len:
             raise ValueError(f'prompt of {L} positions exceeds max_len = {self.max_len}')
@@ -279,9 +281,10 @@ class HyenaDecoder(_Decoder):
         return y
 
     @torch.no_grad()
-    def step(self, x):
+    def step(self, x, docs=None):
         """y (B, d_model, T) of the next T <= 64 positions of the projection x (B, 3 * d_model, T); the three slices are
         read in place when their rows are contiguous."""
+        refuse(docs, 'HyenaDecoder')
         v, x1, x2 = self._split(x)
         return self._step(v, x1, x2)
 
@@ -311,8 +314,10 @@ class LongConvDecoder(_Decoder):
         super().reset()
 
     @torch.no_grad()
-    def prefill(self, u, pregate=None, postgate=None):
-        """y (B, H, L) of the prompt by the FFT engine, and the cache filled from it; starts a new sequence."""
+    def prefill(self, u, pregate=None, postgate=None, docs=None):
+        """y (B, H, L) of the prompt by the FFT engine, and the cache filled from it; starts a new sequence.  Packed
+        documents (docs) are refused: one decoder row is one sequence."""
+        refuse(docs, 'LongConvDecoder')
         L = u.shape[-1]
         if L > self.max_len:
             raise ValueError(f'prompt of {L} positions exceeds max_len = {self.max_len}')
@@ -333,7 +338,8 @@ class LongConvDecoder(_Decoder):
         return y
 
     @torch.no_grad()
-    def step(self, u, pregate=None, postgate=None):
+    def step(self, u, pregate=None, postgate=None, docs=None):
         """y (B, H, T) of the next T <= 64 positions, with the gates the sequence was started with."""
+        refuse(docs, 'LongConvDecoder')
         self._same_gates(pregate, postgate)
         return self._step(u, pregate, postgate)

@@ -27,6 +27,7 @@ import torch
 from . import _lib
 from . import conv as _conv
 from . import depthwise_1d as _dw
+from . import docs as _docs
 
 
 def gated_long_conv(conv, v, k, x1, x2):
@@ -109,7 +110,7 @@ def _mixer_backward(mod, D, dout, x1x2v, kf, k_len, kf2, k2_len, short=None):
     return grad, dk, dk2
 
 
-def hyena_mixer(conv, x1x2v, k, d_model, residual_filter=None):
+def hyena_mixer(conv, x1x2v, k, d_model, residual_filter=None, docs=None):
     """The long-convolution part of the reference's Hyena / M2 sequence mixers on the (B, 3*d_model, L) projection
     (monarch_mixer_sequence_mixer_flashfftconv.py:131-177): y = conv(x1 * v, k) * x2 [+ conv(v, k2)], where
     x1, x2, v = x1x2v.split(d_model, dim=1).
@@ -118,7 +119,18 @@ def hyena_mixer(conv, x1x2v, k, d_model, residual_filter=None):
     qualify, see conv.batch_stride, is copied first).  The backward writes d x1, d x2 and d v into one (B, 3*d_model, L)
     gradient, which is returned as the projection's gradient.  residual_filter k2: one more ungated call on the v slice;
     its input gradient is added into the v slice of that gradient with one add.  Like gated_long_conv, this calls the
-    engine directly rather than conv(...): forward hooks registered on the module do not run for it."""
+    engine directly rather than conv(...): forward hooks registered on the module do not run for it.
+
+    docs: a DocumentTable of packed documents in the rows of x1x2v; each document is then mixed alone and causally
+    (flashfftconv.docs): one gather of the three slices, read in place, into class batches, hyena_mixer's engine calls
+    per class, one scatter of y; the backward scatters d x1, d x2 and d v into the slices of one gradient."""
+    if docs is not None:
+        x1, x2, v = x1x2v.split(d_model, dim=1)
+        _conv._check_inputs(v, k, conv, (x1, x2), views=True)
+        if residual_filter is not None:
+            _conv._check_inputs(v, residual_filter, conv, views=True)
+        _docs._check(docs, v)
+        return _docs.MixerDocsFunc.apply(x1x2v, k, residual_filter, conv, d_model, docs)
     return HyenaMixerFunc.apply(x1x2v, k, residual_filter, conv, d_model)
 
 
@@ -173,7 +185,7 @@ class ShortHyenaFunc(torch.autograd.Function):
         return dx, dw, dbias, dk, dk2, None, None, None
 
 
-def hyena_operator(conv, short_filter, x, k, d_model, residual_filter=None):
+def hyena_operator(conv, short_filter, x, k, d_model, residual_filter=None, docs=None):
     """The whole Hyena / M2 sequence mixer from the raw (B, 3*d_model, L) projection x (the output of in_proj):
 
         s = short_filter(x)[..., :L];  x1, x2, v = s.split(d_model, dim=1)
@@ -187,7 +199,10 @@ def hyena_operator(conv, short_filter, x, k, d_model, residual_filter=None):
     applies the short filter where the kernels load x1, x2 and v, and so is the mixer part of the backward: s is neither
     written to memory nor kept between them.  Results are bit for bit those of short_filter followed by hyena_mixer,
     which is what every other call runs.  Like hyena_mixer, the call goes to the engine directly: forward hooks on
-    `conv` and `short_filter` do not run for it."""
+    `conv` and `short_filter` do not run for it.
+
+    docs: a DocumentTable of packed documents in the rows of x.  The call is then short_filter(x, docs.cu_seqlens)
+    followed by hyena_mixer(..., docs=docs): both filters keep every document apart."""
     if not isinstance(short_filter, _dw.FlashDepthWiseConv1d) or not short_filter.is_bhl:
         raise RuntimeError('short_filter must be a BHL FlashDepthWiseConv1d')
     if short_filter.d != 3 * d_model:
@@ -198,6 +213,8 @@ def hyena_operator(conv, short_filter, x, k, d_model, residual_filter=None):
     if x.dim() != 3 or x.shape[1] != 3 * d_model:
         raise RuntimeError(f'x must be (B, 3 * d_model = {3 * d_model}, L), got {tuple(x.shape)}')
     L = x.shape[-1]
+    if docs is not None:
+        return hyena_mixer(conv, short_filter(x, docs.cu_seqlens), k, d_model, residual_filter, docs)
     if not _short_fused(conv, short_filter, x):
         return hyena_mixer(conv, short_filter(x)[..., :L], k, d_model, residual_filter)
     w, b = short_filter.weights, short_filter.bias

@@ -17,6 +17,7 @@ reach both `x` and `k` as they do through the reference's torch operations, but 
 import torch
 
 from .conv import FlashFFTConv, FlashFFTConvFunc
+from .docs import refuse
 
 
 class _EngineCache(torch.nn.Module):
@@ -38,7 +39,8 @@ class PartialFFTConv(_EngineCache):
         super().__init__()
         self.N_partial = N_partial
 
-    def forward(self, x, k):
+    def forward(self, x, k, docs=None):
+        refuse(docs, 'PartialFFTConv')
         L = x.shape[-1]
         return self.conv(2 * L, x.dtype, x.device)(x, k[..., : self.N_partial].contiguous())
 
@@ -57,7 +59,8 @@ class FrequencySparseFFTConv(_EngineCache):
         super().__init__()
         self.N_partial = N_partial
 
-    def forward(self, x, k):
+    def forward(self, x, k, docs=None):
+        refuse(docs, 'FrequencySparseFFTConv')
         L = x.shape[-1]
         mod = self.conv(2 * L, x.dtype, x.device)
         # the engines sit in a plain dict (no .train() / .eval() reaches them): this module's own mode and the grad

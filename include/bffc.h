@@ -407,9 +407,40 @@ int bffc_conv_step(const void* u, int64_t u_bstride, const void* pregate, int64_
                    size_t state_bytes, int64_t* pos, void* y, int64_t y_bstride, int B, int H, int T, int max_len,
                    void* workspace, size_t workspace_bytes, void* stream);
 
+/*
+ * Packed documents regrouped by length class for the long convolution (no plan; INTEGRATION.md §11).  Rows (B, H, L)
+ * hold several documents; a document of length l (1 <= l <= 2^21) belongs to the class c = max(128, next_pow2(l)) and is
+ * convolved as one member of a (n_c, H, c) class batch by the plan of seqlen 2c with the filter k[:, :min(Lk, c)],
+ * which is the causal convolution of the document alone.  The class batches of all classes lie one after the other in
+ * a "gathered" buffer of H * positions elements (16-byte aligned, plan dtype), positions = sum of n_c * c.
+ *
+ * items: device table of n_items entries of 24 bytes, 8-byte aligned, sorted by dst, each
+ *     { int32 row, int32 start, int32 length, int32 cls, int64 dst }
+ * the document [start, start + length) of row `row` in class cls, whose row of its class batch begins at position dst
+ * of the gathered buffer: element (h, t) of the item is gathered element H * dst + h * cls + t.  The items tile the
+ * buffer (dst of an item = dst + cls of the one before, the first at 0).  Zero-length documents have no item.
+ *
+ *   bffc_docs_gather:  gathered[H * dst + h * cls + t] = src[row * bs + h * L + start + t] for t < length, 0 for
+ *                      length <= t < cls
+ *   bffc_docs_scatter: dst[row * bs + h * L + start + t] = gathered[H * dst + h * cls + t] for t < length
+ *
+ * n_tensors (1..4) tensors move in one launch: src / dst, src_bstride / dst_bstride and gathered are host arrays of
+ * n_tensors entries.  Row-side tensors have contiguous rows and any batch stride >= H * L, and may start at any
+ * element (2-byte alignment).  Elements are copied as 16-bit words, so bf16 and fp16 take the same call.  Host
+ * arguments (shape, 0 <= n_items, positions a multiple of 128 in [128 n_items, 2 B L + 128 n_items], pointers,
+ * alignments, strides) are checked before the device is looked at (BFFC_ERR_INVALID).  The table is not read on the
+ * host, so the calls can be captured in a CUDA graph; an item whose fields do not fit the rows is treated as empty.
+ * One launch each (none when positions is 0); the grid is one-dimensional and grid-strided, offsets are 64-bit.
+ */
+int bffc_docs_gather(const void* items, int n_items, int64_t positions, int B, int H, int L, const void* const* src,
+                     const int64_t* src_bstride, void* const* gathered, int n_tensors, void* stream);
+int bffc_docs_scatter(const void* items, int n_items, int64_t positions, int B, int H, int L,
+                      const void* const* gathered, void* const* dst, const int64_t* dst_bstride, int n_tensors,
+                      void* stream);
+
 /* Number of kernel launches the last bffc_fwd / bffc_bwd / bffc_fwd_host / filter-side transform /
- * bffc_dwconv1d_fwd (1) / bffc_dwconv1d_bwd (2) / bffc_conv_state_fill (1) / bffc_conv_step (2) on this thread
- * enqueued (bench.py). */
+ * bffc_dwconv1d_fwd (1) / bffc_dwconv1d_bwd (2) / bffc_conv_state_fill (1) / bffc_conv_step (2) /
+ * bffc_docs_gather (1) / bffc_docs_scatter (1) on this thread enqueued (bench.py). */
 int bffc_last_launch_count(void);
 
 #ifdef __cplusplus
