@@ -183,7 +183,8 @@ struct bffc_plan {
   float2* tw512 = nullptr;    // composite sizes: e^{-2 pi i t / 512} (column FFTs), W_N^{j} j < 2048, W_N^{2048 i} i < N/2048
   float2* tw_lo = nullptr;
   float2* tw_hi = nullptr;
-  int num_sms = 0;
+  int num_sms = 0;               // CTAs of a persistent launch: the SM count, or the plan's max_ctas below it
+  bool deterministic = false;     // BFFC_PLAN_DETERMINISTIC: dk_f by the fixed slab partition (dkf_slabs.cuh)
   // bffc_fwd_host: copy-in / compute / copy-out streams and the per-slot events (created with the plan)
   cudaStream_t hs[3] = {nullptr, nullptr, nullptr};
   cudaEvent_t hev[7] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
@@ -269,10 +270,14 @@ int bffc_supported(int seqlen, int dtype) {
   return levels_for(seqlen, lev) >= 0 ? 1 : 0;
 }
 
-int bffc_plan_create(bffc_plan** out, int seqlen, int dtype) {
+int bffc_plan_create(bffc_plan** out, int seqlen, int dtype) { return bffc_plan_create_ex(out, seqlen, dtype, 0, 0); }
+
+int bffc_plan_create_ex(bffc_plan** out, int seqlen, int dtype, int flags, int max_ctas) {
   if (!out) return fail(BFFC_ERR_INVALID, "plan output pointer is null");
   *out = nullptr;
   if (dtype != BFFC_DTYPE_BF16 && dtype != BFFC_DTYPE_FP16) return fail(BFFC_ERR_INVALID, "unknown dtype %d", dtype);
+  if (flags & ~BFFC_PLAN_DETERMINISTIC) return fail(BFFC_ERR_INVALID, "unknown plan flags 0x%x", unsigned(flags));
+  if (max_ctas < 0) return fail(BFFC_ERR_INVALID, "max_ctas %d < 0", max_ctas);
   if (!bffc_supported(seqlen, dtype))
     return fail(BFFC_ERR_UNSUPPORTED, "seqlen %d / dtype %d not supported by this build", seqlen, dtype);
   if (int rc = check_device()) return rc;
@@ -303,6 +308,8 @@ int bffc_plan_create(bffc_plan** out, int seqlen, int dtype) {
   p->dtype = dtype;
   PLAN_TRY(cudaGetDevice(&p->device));
   PLAN_TRY(cudaDeviceGetAttribute(&p->num_sms, cudaDevAttrMultiProcessorCount, p->device));
+  if (max_ctas > 0 && max_ctas < p->num_sms) p->num_sms = max_ctas;
+  p->deterministic = (flags & BFFC_PLAN_DETERMINISTIC) != 0;
 
   // stage-1 DFT of the fused kernel (symmetric, K-major rows): F_128, or for the small sizes the block-diagonal
   // I_{8192/N} (x) F_r, r = N/64 (one block per batch member sharing the unit).  One conjugate-pair image: A row f holds
@@ -368,6 +375,8 @@ int bffc_plan_create(bffc_plan** out, int seqlen, int dtype) {
     PLAN_TRY(cudaFuncSetAttribute(fwd3_kernel<true, false, F>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemTotal3));
     PLAN_TRY(cudaFuncSetAttribute(dkf3_kernel<true, F>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemTotalDkf3));
     PLAN_TRY(cudaFuncSetAttribute(dkf3_kernel<false, F>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemTotalDkf3));
+    PLAN_TRY(cudaFuncSetAttribute(dkf3_fixed_kernel<true, F>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemTotalDkf3));
+    PLAN_TRY(cudaFuncSetAttribute(dkf3_fixed_kernel<false, F>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemTotalDkf3));
     PLAN_TRY(cudaFuncSetAttribute(outer_tc_kernel<false, F>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemOuter));
     PLAN_TRY(cudaFuncSetAttribute(outer_tc_kernel<true, F>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemOuter));
     PLAN_TRY(cudaFuncSetAttribute(bffc::ffft::kf_from_filter_kernel<F>, cudaFuncAttributeMaxDynamicSharedMemorySize, bffc::ffft::kSmemBytes));
@@ -546,8 +555,9 @@ int bffc_dkf_unpack_half(const bffc_plan* p, const void* dkf_engine, void* dkf_h
 // Composite sizes keep the outer stage's output as two bf16 planes (real, imaginary) of pairs*H*N elements.
 static size_t plane_bytes(const bffc_plan* p, int B, int H) { return size_t((B + 1) / 2) * H * p->N * 2; }
 // One launch group of a composite size works on batch members [0, B) (tensor pointers are pre-offset to the first one)
-// and channels [h0, h0 + H) of (.., Hs, L) tensors; its plane sets hold ceil(B/2) * H * N complex elements.
-struct View { int B, H, Hs, h0; };
+// and channels [h0, h0 + H) of (.., Hs, L) tensors; its plane sets hold ceil(B/2) * H * N complex elements.  b0: the
+// first batch member (a chunk with b0 > 0 adds into the dk_f rows of an earlier one).
+struct View { int B, H, Hs, h0, b0; };
 
 // Composite sizes can run chunk by chunk: `sets` plane sets of one chunk take at most ~kPlaneBudget bytes.  Channels
 // first (the k_f rows of a channel are then shared by its batch pairs inside one chunk); a single channel that is too
@@ -563,7 +573,7 @@ static View chunk_view(const bffc_plan* p, int B, int H, int sets) {
   if (items < 1) items = 1;
   const size_t cap = kMaxGridYZ;
   const int pairs = (B + 1) / 2;
-  View v{B, H, H, 0};
+  View v{B, H, H, 0, 0};
   if (items >= size_t(pairs) && size_t(pairs) <= cap) {
     const size_t hc = std::min(items / pairs, cap);
     v.H = hc < size_t(H) ? int(hc) : H;
@@ -579,8 +589,31 @@ static View chunk_view(const bffc_plan* p, int B, int H, int sets) {
 // u*pregate and dout*postgate for the dk_f kernel of a gated backward at seqlen <= 8192 (two (B,H,L) tensors)
 static size_t gate_scratch_bytes(int B, int H, int L) { return 2 * ((size_t(B) * H * L * 2 + 255) & ~size_t(255)); }
 
-extern "C" size_t bffc_workspace_bytes_ex(const bffc_plan* p, int B, int H, int L, int gated, int backward) {
-  if (!p) return 0;
+// Partial slots of a deterministic backward (dkf_slabs.cuh): the most any of its dk_f launches needs.  halo >= 0:
+// overlap-save blocks (bffc_bwd_blocked), whose items are the B * ceil(L / (8192 - halo)) blocks.
+static size_t dkf_partial_bytes(const bffc_plan* p, int B, int H, int L, int halo) {
+  long long slots = 0;
+  auto launch = [&](long long rows, long long pairs) {
+    const int r = int(std::min<long long>(rows, INT32_MAX)), q = int(std::min<long long>(pairs, INT32_MAX));
+    slots = std::max(slots, bffc::slab::partial_slots(r, q));
+  };
+  if (p->nlev == 0) {
+    const long long items = halo < 0 ? B : (long long)B * ((L + kInner - halo - 1) / (kInner - halo));
+    const long long members = 2LL * (kInner / std::min(p->N, kInner));
+    launch(H, (items + members - 1) / members);
+  } else {            // every chunk shape of for_each_chunk: full and ragged, over batch members and channels
+    const View c = chunk_view(p, B, H, p->nlev + 1);
+    for (int vb : {c.B, B % c.B})
+      for (int vh : {c.H, H % c.H})
+        if (vb && vh) launch((long long)vh * p->R, (vb + 1) / 2);
+  }
+  return size_t(slots) * bffc::slab::kSlotBytes;
+}
+
+// where the partial slots begin in the workspace of a deterministic backward
+static size_t dkf_partial_offset(size_t base) { return (base + 255) & ~size_t(255); }
+
+static size_t default_workspace_bytes(const bffc_plan* p, int B, int H, int L, int gated, int backward) {
   if (p->nlev == 0) return (gated && backward) ? gate_scratch_bytes(B, H, L) : 0;
   // plane sets (real + imaginary plane each) of ONE chunk: forward nlev sets; backward nlev + 1 (transformed u and dout)
   const View vf = chunk_view(p, B, H, p->nlev);
@@ -591,6 +624,23 @@ extern "C" size_t bffc_workspace_bytes_ex(const bffc_plan* p, int B, int H, int 
     if (nb > need) need = nb;
   }
   return need;
+}
+
+// the workspace of one call: a strided call (halo < 0) or overlap-save blocks
+static size_t workspace_need(const bffc_plan* p, int B, int H, int L, int gated, int backward, int halo) {
+  const size_t base = default_workspace_bytes(p, B, H, L, gated, backward);
+  const size_t part = (p->deterministic && backward) ? dkf_partial_bytes(p, B, H, L, halo) : 0;
+  return part ? dkf_partial_offset(base) + part : base;
+}
+
+extern "C" size_t bffc_workspace_bytes_ex(const bffc_plan* p, int B, int H, int L, int gated, int backward) {
+  return p ? workspace_need(p, B, H, L, gated, backward, -1) : 0;
+}
+
+extern "C" size_t bffc_workspace_bytes_blocked(const bffc_plan* p, int B, int H, int L, int halo, int gated,
+                                               int backward) {
+  if (!p || p->N != kInner || halo < 0 || halo > 4096 || halo % 512 || B <= 0 || H <= 0 || L <= 0 || L % 64) return 0;
+  return workspace_need(p, B, H, L, gated, backward, halo);
 }
 
 extern "C" size_t bffc_workspace_bytes(const bffc_plan* p, int B, int H, int L) {
@@ -793,10 +843,35 @@ static int launch_planes(const bffc_plan* p, void* pre, void* pim, const void* k
   return launched();
 }
 
-// dk_f kernel on real tiles (maps u, dout, u, dout) or on complex rows (planes: u re, dout re, u im, dout im)
+// dk_f kernel on real tiles (maps u, dout, u, dout) or on complex rows (planes: u re, dout re, u im, dout im).
+// Deterministic plans: dkf3_fixed_kernel on the slab partition (dkf_slabs.cuh), then, when a row has more than one slab,
+// dkf_slab_sum_kernel over the partial slots at `part`; accumulate: add into dk_f instead of overwriting it.
 static int launch_dkf(const bffc_plan* p, bool planes, const CUtensorMap& a, const CUtensorMap& b, const CUtensorMap& c,
-                      const CUtensorMap& d, const bffc::DkfParams& prm, cudaStream_t st) {
+                      const CUtensorMap& d, const bffc::DkfParams& prm, cudaStream_t st, void* part = nullptr,
+                      bool accumulate = false) {
   using namespace bffc::r128;
+  if (p->deterministic) {
+    bffc::DkfDetParams dp;
+    static_cast<bffc::DkfParams&>(dp) = prm;
+    dp.slabs = bffc::slab::slabs(prm.H, prm.pairs);
+    dp.accumulate = accumulate ? 1 : 0;
+    dp.part = dp.slabs > 1 ? static_cast<float2*>(part) : nullptr;
+    const int grid = persistent_grid(p, (long long)prm.H * dp.slabs, 1);
+    FMT_SWITCH(p->dtype,
+      if (planes)
+        dkf3_fixed_kernel<true, F><<<grid, kThreadsDkf3, kSmemTotalDkf3, st>>>(a, b, c, d, dp);
+      else
+        dkf3_fixed_kernel<false, F><<<grid, kThreadsDkf3, kSmemTotalDkf3, st>>>(a, b, c, d, dp);
+    );
+    if (int rc = launched()) return rc;
+    if (dp.slabs == 1) return 0;
+    const long long n = (long long)prm.H * (bffc::eng::kRowLen / 2);
+    const int sum_grid = int(std::min<long long>((n + kThreadsSlabSum - 1) / kThreadsSlabSum, 8LL * p->num_sms));
+    dkf_slab_sum_kernel<<<sum_grid, kThreadsSlabSum, 0, st>>>(static_cast<const float4*>(part),
+                                                              reinterpret_cast<float4*>(prm.dkf), prm.H, dp.slabs,
+                                                              dp.accumulate);
+    return launched();
+  }
   const int grid = persistent_grid(p, (long long)prm.H * prm.pairs, 1);
   FMT_SWITCH(p->dtype,
     if (planes)
@@ -975,7 +1050,7 @@ static int for_each_chunk(const bffc_plan* p, int B, int H, int L, void* ws, int
   auto set = [&](int i) { return plane_set(p, ws, i, c.B, c.H); };
   for (int b0 = 0; b0 < B; b0 += c.B)
     for (int h0 = 0; h0 < H; h0 += c.H) {
-      const View v{B - b0 < c.B ? B - b0 : c.B, H - h0 < c.H ? H - h0 : c.H, H, h0};
+      const View v{B - b0 < c.B ? B - b0 : c.B, H - h0 < c.H ? H - h0 : c.H, H, h0, b0};
       auto at = [&](Seq t) -> Seq {
         return t.p ? Seq{static_cast<uint8_t*>(t.p) + size_t(b0) * size_t(t.bs) * 2, t.bs} : Seq();
       };
@@ -1189,7 +1264,7 @@ static int conv_backward(const char* fn, const bffc_plan* p, const void* dout_, 
   const Seq dpregate = gated ? seq(dpregate_, dpregate_bs) : Seq(), dpostgate = gated ? seq(dpostgate_, dpostgate_bs) : Seq();
   if (int rc = check_strides(fn, H, L, {dout, u, pregate, postgate, du, dpregate, dpostgate})) return rc;
   {
-    const size_t need = bffc_workspace_bytes_ex(p, B, H, L, gated, 1);
+    const size_t need = workspace_need(p, B, H, L, gated, 1, halo);
     if (need && (!workspace || workspace_bytes < need))
       return fail(BFFC_ERR_INVALID, "%s: workspace of %zu bytes required", fn, need);
   }
@@ -1238,8 +1313,12 @@ static int conv_backward(const char* fn, const bffc_plan* p, const void* dout_, 
     dx.y2 = dpregate;
     if (int rc = conv_forward(p, dout, kfc, postgate, pregate, du, B, H, L, workspace, st, dx)) return rc;
   }
-  // dk_f = sum_b FFT(dout*q) * conj(FFT(u*p)), reduced with fp32 atomics into the zeroed gradient
-  CUDA_TRY(cudaMemsetAsync(dkf, 0, size_t(H) * p->NE * sizeof(float2), st));
+  // dk_f = sum_b FFT(dout*q) * conj(FFT(u*p)), reduced with fp32 atomics into the zeroed gradient; deterministic plans
+  // store every row in a fixed order instead (launch_dkf), the partial slots after the rest of the workspace
+  if (!p->deterministic) CUDA_TRY(cudaMemsetAsync(dkf, 0, size_t(H) * p->NE * sizeof(float2), st));
+  void* part = p->deterministic && workspace
+                   ? static_cast<uint8_t*>(workspace) + dkf_partial_offset(default_workspace_bytes(p, B, H, L, gated, 1))
+                   : nullptr;
   bffc::DkfParams prm{};
   fill_stage1(p, prm);
   prm.dkf = static_cast<float2*>(dkf);
@@ -1256,7 +1335,7 @@ static int conv_backward(const char* fn, const bffc_plan* p, const void* dout_, 
     if (int rc = make_seq_map(p, &tm_u, xu, B, H, L, p->rblk)) return rc;
     if (int rc = make_seq_map(p, &tm_d, xd, B, H, L, p->rblk - prm.win)) return rc;
     if (sfu && !gated) prm.sf = *sfu;     // ungated: the kernel filters raw u; gated: the passes stored filtered products
-    return launch_dkf(p, false, tm_u, tm_d, tm_u, tm_d, prm, st);
+    return launch_dkf(p, false, tm_u, tm_d, tm_u, tm_d, prm, st, part);
   }
   // chunk by chunk: the outer stages turn u (* pregate) and dout (* postgate) into complex 8192-point rows ONCE
   // (set U, set D; set 0 is the level-0 intermediate when nlev == 2).  The dk_f kernel reads both sets first; the
@@ -1278,7 +1357,7 @@ static int conv_backward(const char* fn, const bffc_plan* p, const void* dout_, 
     if (int rc = make_map(p, &tdi, rd.im, vpairs * rows, kInner)) return rc;
     fill_complex_rows(prm, vpairs, rows);
     prm.dkf = static_cast<float2*>(dkf) + size_t(v.h0) * p->NE;
-    if (int rc = launch_dkf(p, true, tur, tdr, tui, tdi, prm, st)) return rc;
+    if (int rc = launch_dkf(p, true, tur, tdr, tui, tdi, prm, st, part, v.b0 > 0)) return rc;
     const size_t kf_off = size_t(v.h0) * p->NE * 4;
     if (gated) {
       if (int rc = launch_planes(p, ru.re, ru.im, static_cast<const uint8_t*>(kf) + kf_off, vpairs, rows, st, 0)) return rc;

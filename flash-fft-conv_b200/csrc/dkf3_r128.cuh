@@ -5,8 +5,8 @@
 // (kernels_bf16/monarch_cuda_32_16_16_bwd_kernel_bf16.h:505-509,571-581,711-734: D = FFT(dout), X = FFT(u),
 // dk_f partial = sum over the CTA's batch tile of D * conj(X)) plus the host-side `dk_f_out.sum(0)` over the
 // (B/Bt, H, N, 2) bf16 partials (monarch_cuda_interface_bwd_bf16.cu:820,1107).  Here the sum over the batch is
-// accumulated in fp32 registers; nothing but the final (H, N) complex fp32 gradient is written (fp32 reductions into a
-// zeroed buffer, at most two CTAs per channel).
+// accumulated in fp32 registers; dkf3_kernel writes nothing but the final (H, N) complex fp32 gradient (fp32 reductions
+// into a zeroed buffer from the CTAs a channel's units fall into).  dkf3_fixed_kernel (below) stores instead of adding.
 //
 // Pair packing: z_u = u_b + i u_{b+1}, z_d = dout_b + i dout_{b+1}.  FFT(z_d) * conj(FFT(z_u)) is the spectrum
 // of corr(d_b,u_b) + corr(d_{b+1},u_{b+1}) + i (cross terms); the cross terms are purely imaginary in the time
@@ -22,8 +22,14 @@
 // load; seqlen <= 8192: the two fused passes of bffc_bwd store those products through FwdParams::xg_out).  An ungated
 // backward on the raw projection (bffc_bwd_short_strided, seqlen <= 8192) hands in raw u tiles and DkfParams::sf: the
 // kernel filters them in shared memory before stage 1.
+//
+// Deterministic plans (BFFC_PLAN_DETERMINISTIC) run the same body as dkf3_fixed_kernel: the work is cut at the slab
+// boundaries of dkf_slabs.cuh only, and each slab's sum is stored, not added (into dk_f when a slab is a whole row, else
+// into its partial slot, which dkf_slab_sum_kernel adds up in a fixed order).  No atomics: dk_f is a function of the
+// inputs and the shape.
 #pragma once
 #include "fwd3_r128.cuh"
+#include "dkf_slabs.cuh"
 
 namespace bffc {
 
@@ -40,6 +46,13 @@ struct DkfParams {
                              // on its last srows rows only (rows [0, win) of the dout slot stay zero); else 1, 0, 0
 };
 
+// dkf3_fixed_kernel: DkfParams and the slab partition of the launch (dkf_slabs.cuh)
+struct DkfDetParams : DkfParams {
+  int slabs;                 // S = slab::slabs(H, pairs)
+  int accumulate;            // S = 1: add each row's sum into dk_f (a later batch chunk of the same rows); else store it
+  float2* part;              // S > 1: the launch's partial slots [H * S][8192], engine order; S = 1: null
+};
+
 namespace r128 {
 
 constexpr int kThreadsDkf3 = kPipeThreads;
@@ -48,10 +61,19 @@ constexpr int kSmemDkf3Park = kThreadsDkf3 * 64 * 4;           // spectrum of u:
 constexpr int kSmemTotalDkf3 = kSmemDkf3Slots + kSmemF + kSmemG + kSmemDkf3Park + 64 + 1024;
 static_assert(kSmemTotalDkf3 <= 227 * 1024, "shared memory per block");
 
-template <bool kPlanes, int kFmt = 1>
-__global__ void __launch_bounds__(kThreadsDkf3, 1)
-dkf3_kernel(const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CUtensorMap tm_d,
-            const __grid_constant__ CUtensorMap tm_ui, const __grid_constant__ CUtensorMap tm_di, const DkfParams p) {
+// first unit of CTA i: the units cut evenly (atomics), or at slab boundaries (kDet)
+template <bool kDet, class P>
+__device__ __forceinline__ int first_unit(const P& p, long long total, unsigned i) {
+  if constexpr (kDet)
+    return int(slab::slab_unit(p.pairs, p.slabs, slab::cta_slab((long long)p.H * p.slabs, i, gridDim.x)));
+  else
+    return int(total * i / gridDim.x);
+}
+
+// the body of dkf3_kernel (kDet false) and dkf3_fixed_kernel (kDet true)
+template <bool kPlanes, int kFmt, bool kDet, class P>
+__device__ __forceinline__ void dkf3_body(const CUtensorMap& tm_u, const CUtensorMap& tm_d, const CUtensorMap& tm_ui,
+                                          const CUtensorMap& tm_di, const P& p) {
   extern __shared__ uint8_t smem_raw[];
   const uint32_t sbase = (smem_u32(smem_raw) + 1023u) & ~1023u;
   uint8_t* gen_base = smem_raw + (sbase - smem_u32(smem_raw));
@@ -78,9 +100,9 @@ dkf3_kernel(const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CU
   // work split: the H * pairs units (channel-major: g = h * pairs + pr) are cut into gridDim.x contiguous ranges, so the
   // grid is not limited by the channel count and no CTA carries a whole extra channel.  A channel that straddles two
   // CTAs is completed by both through fp32 reductions into the zero-initialised gradient (red.global.add), as is every
-  // other flush.
+  // other flush.  kDet: the ranges end at slab boundaries, and every slab end flushes.
   const long long total = (long long)p.H * p.pairs;
-  const int g_begin = int(total * blockIdx.x / gridDim.x), g_end = int(total * (blockIdx.x + 1) / gridDim.x);
+  const int g_begin = first_unit<kDet>(p, total, blockIdx.x), g_end = first_unit<kDet>(p, total, blockIdx.x + 1);
   const int n_units = g_end - g_begin;
   auto unit_h = [&](int n) { return (g_begin + n) / p.pairs; };
   auto unit_pr = [&](int n) { return (g_begin + n) % p.pairs; };
@@ -173,7 +195,32 @@ dkf3_kernel(const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CU
       }
     }
     // ---- channel (or this CTA's share of it) finished: add it to the gradient spectrum
-    if (unit_pr(n) == p.pairs - 1 || n == n_units - 1) {
+    const bool flush = unit_pr(n) == p.pairs - 1 || n == n_units - 1;
+    if constexpr (kDet) {
+      // a slab finished: its sum, stored into its partial slot, or as (or into, for a later batch chunk) the row of dk_f
+      if (!flush && slab::slab_of(p.pairs, p.slabs, unit_pr(n)) == slab::slab_of(p.pairs, p.slabs, unit_pr(n) + 1))
+        continue;
+      const int h = unit_h(n);
+      float2* row = p.part ? p.part + (size_t(h) * p.slabs + slab::slab_of(p.pairs, p.slabs, unit_pr(n))) * eng::kRowLen
+                           : p.dkf + size_t(h) * eng::kRowLen;
+      const bool add = p.accumulate && !p.part;
+#pragma unroll
+      for (int rr = 0; rr < 2; ++rr) {
+#pragma unroll
+        for (int i = 0; i < 8; ++i) {
+          const int k2 = 8 * i + 2 * fp.q, e = 4 * i + 2 * rr;
+          float4* out = reinterpret_cast<float4*>(row + eng::dkf_slot(fp.row[rr], k2));
+          float4 v = make_float4(acc[e], acc[32 + e], acc[e + 1], acc[32 + e + 1]);
+          if (add) {
+            const float4 o = *out;
+            v = make_float4(o.x + v.x, o.y + v.y, o.z + v.z, o.w + v.w);
+          }
+          *out = v;
+        }
+      }
+#pragma unroll
+      for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+    } else if (flush) {
       const int h = unit_h(n);
 #pragma unroll
       for (int rr = 0; rr < 2; ++rr) {
@@ -189,6 +236,40 @@ dkf3_kernel(const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CU
 #pragma unroll
       for (int i = 0; i < 64; ++i) acc[i] = 0.f;
     }
+  }
+}
+
+template <bool kPlanes, int kFmt = 1>
+__global__ void __launch_bounds__(kThreadsDkf3, 1)
+dkf3_kernel(const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CUtensorMap tm_d,
+            const __grid_constant__ CUtensorMap tm_ui, const __grid_constant__ CUtensorMap tm_di, const DkfParams p) {
+  dkf3_body<kPlanes, kFmt, false>(tm_u, tm_d, tm_ui, tm_di, p);
+}
+
+template <bool kPlanes, int kFmt = 1>
+__global__ void __launch_bounds__(kThreadsDkf3, 1)
+dkf3_fixed_kernel(const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CUtensorMap tm_d,
+                  const __grid_constant__ CUtensorMap tm_ui, const __grid_constant__ CUtensorMap tm_di,
+                  const DkfDetParams p) {
+  dkf3_body<kPlanes, kFmt, true>(tm_u, tm_d, tm_ui, tm_di, p);
+}
+
+// S > 1 (dkf_slabs.cuh): dk_f[r] = (dk_f[r] +) part[r * S] + part[r * S + 1] + ... + part[r * S + S - 1], r < rows, in
+// that order; one thread per 16 bytes of dk_f, grid-strided, 64-bit offsets
+constexpr int kThreadsSlabSum = 256;
+__global__ void __launch_bounds__(kThreadsSlabSum)
+dkf_slab_sum_kernel(const float4* __restrict__ part, float4* __restrict__ dkf, int rows, int S, int accumulate) {
+  constexpr long long kRow = eng::kRowLen / 2;          // float4 per row
+  const long long n = rows * kRow;
+  for (long long i = blockIdx.x * (long long)kThreadsSlabSum + threadIdx.x; i < n;
+       i += (long long)gridDim.x * kThreadsSlabSum) {
+    const float4* src = part + (i / kRow) * S * kRow + i % kRow;
+    float4 a = accumulate ? dkf[i] : src[0];
+    for (int s = accumulate ? 0 : 1; s < S; ++s) {
+      const float4 b = src[s * kRow];
+      a = make_float4(a.x + b.x, a.y + b.y, a.z + b.z, a.w + b.w);
+    }
+    dkf[i] = a;
   }
 }
 

@@ -12,6 +12,7 @@ BFFC_DTYPE_FP16 = 1
 BFFC_DTYPE_FP32 = 2          # depthwise convolution only
 BFFC_LAYOUT_BHL = 0
 BFFC_LAYOUT_BLH = 1
+BFFC_PLAN_DETERMINISTIC = 1      # bffc_plan_create_ex: dk_f summed in a fixed order
 
 _lib = None
 
@@ -22,6 +23,7 @@ SYMBOLS = {
     'bffc_last_error': (_c.c_char_p, []),
     'bffc_supported': (_c.c_int, [_c.c_int, _c.c_int]),
     'bffc_plan_create': (_c.c_int, [_c.POINTER(_c.c_void_p), _c.c_int, _c.c_int]),
+    'bffc_plan_create_ex': (_c.c_int, [_c.POINTER(_c.c_void_p), _c.c_int, _c.c_int, _c.c_int, _c.c_int]),
     'bffc_plan_destroy': (_c.c_int, [_c.c_void_p]),
     'bffc_fft_size': (_c.c_int, [_c.c_void_p]),
     'bffc_length_multiple': (_c.c_int, [_c.c_void_p]),
@@ -40,6 +42,7 @@ SYMBOLS = {
                                          _c.c_size_t, _c.c_void_p]),
     'bffc_workspace_bytes': (_c.c_size_t, [_c.c_void_p, _c.c_int, _c.c_int, _c.c_int]),
     'bffc_workspace_bytes_ex': (_c.c_size_t, [_c.c_void_p, _c.c_int, _c.c_int, _c.c_int, _c.c_int, _c.c_int]),
+    'bffc_workspace_bytes_blocked': (_c.c_size_t, [_c.c_void_p] + [_c.c_int] * 6),
     'bffc_fwd': (_c.c_int, [_c.c_void_p] * 6 + [_c.c_int] * 3 + [_c.c_void_p, _c.c_size_t, _c.c_void_p]),
     'bffc_bwd': (_c.c_int, [_c.c_void_p] * 11 + [_c.c_int] * 3 + [_c.c_void_p, _c.c_size_t, _c.c_void_p]),
     'bffc_fwd_strided': (_c.c_int, [_c.c_void_p, _c.c_void_p, _c.c_int64, _c.c_void_p, _c.c_void_p, _c.c_int64,

@@ -67,13 +67,17 @@ class _StreamOrder:
 
 
 class _Plan:
-    """Owns one bffc_plan per (seqlen, dtype, device)."""
+    """Owns one bffc_plan per (seqlen, dtype, device, deterministic).  deterministic: BFFC_PLAN_DETERMINISTIC, the
+    backward sums dk_f in a fixed order (include/bffc.h); max_ctas: see bffc_plan_create_ex."""
 
-    def __init__(self, seqlen, dtype, device):
+    def __init__(self, seqlen, dtype, device, deterministic=False, max_ctas=0):
         self.handle = ctypes.c_void_p(0)
         self.device = device
+        self.deterministic = bool(deterministic)
+        flags = _lib.BFFC_PLAN_DETERMINISTIC if deterministic else 0
         with torch.cuda.device(device):
-            _lib.check(_lib.lib().bffc_plan_create(ctypes.byref(self.handle), int(seqlen), _DT[dtype]))
+            _lib.check(_lib.lib().bffc_plan_create_ex(ctypes.byref(self.handle), int(seqlen), _DT[dtype], flags,
+                                                      int(max_ctas)))
         # constants of the plan and memoised size queries: the per-call host path is a handful of ctypes calls, and at
         # C2 a forward step is a fraction of a millisecond of GPU work — Python overhead shows up as launch gaps
         self.fft_size = _lib.lib().bffc_fft_size(self.handle)
@@ -81,11 +85,16 @@ class _Plan:
         self._ws_bytes = {}
         self._filter_ws_bytes = {}
 
-    def workspace_bytes(self, B, H, L, gated, backward):
-        key = (B, H, L, gated, backward)
+    def workspace_bytes(self, B, H, L, gated, backward, halo=None):
+        """bffc_workspace_bytes_ex, or bffc_workspace_bytes_blocked for overlap-save blocks with this halo"""
+        key = (B, H, L, gated, backward, halo)
         n = self._ws_bytes.get(key)
         if n is None:
-            n = self._ws_bytes[key] = _lib.lib().bffc_workspace_bytes_ex(self.handle, B, H, L, int(gated), int(backward))
+            if halo is None:
+                n = _lib.lib().bffc_workspace_bytes_ex(self.handle, B, H, L, int(gated), int(backward))
+            else:
+                n = _lib.lib().bffc_workspace_bytes_blocked(self.handle, B, H, L, int(halo), int(gated), int(backward))
+            self._ws_bytes[key] = n
         return n
 
     def filter_workspace_bytes(self, H):
@@ -150,10 +159,16 @@ class FlashFFTConv(torch.nn.Module):
             del state_dict[key]
         return super()._load_from_state_dict(state_dict, prefix, *args, **kwargs)
 
-    def plan(self, device):
-        key = (device.type, device.index)
+    def plan(self, device, deterministic=False):
+        """The native plan of `device`, made on first use.  deterministic: the plan whose backward sums dk in a fixed
+        order, which backward takes under torch.use_deterministic_algorithms(True).  Both plans read the same k_f."""
+        key = (device.type, device.index, bool(deterministic))
         if key not in self._plans:
-            self._plans[key] = _Plan(self.seqlen, self.dtype, device)
+            if torch.cuda.is_current_stream_capturing():
+                raise RuntimeError('FlashFFTConv: the plan for deterministic=%s is made on first use, which cannot happen '
+                                   'during CUDA-graph capture; run one eager call under the same '
+                                   'torch.use_deterministic_algorithms setting before capturing' % bool(deterministic))
+            self._plans[key] = _Plan(self.seqlen, self.dtype, device, deterministic)
         return self._plans[key]
 
     def fft_size(self, device):
@@ -355,8 +370,8 @@ def _padded(t, Lp):
     return torch.nn.functional.pad(t, (0, Lp - t.shape[-1]))          # one kernel: copy + zero tail
 
 
-def _workspace(plan, B, H, L, gated, backward, device):
-    n = plan.workspace_bytes(B, H, L, gated, backward)
+def _workspace(plan, B, H, L, gated, backward, device, halo=None):
+    n = plan.workspace_bytes(B, H, L, gated, backward, halo)
     return (torch.empty(n, dtype=torch.uint8, device=device) if n else None), n
 
 
@@ -401,7 +416,7 @@ def _fwd(mod, u, k, pregate, postgate, band=None, use_cache=None, kf_engine=None
         if kf_engine is None:
             kf_engine = _kf_engine_for(mod, plan, k, cache_key=cache_key, band=band, use_cache=use_cache)
         y = torch.empty((B, H, L), dtype=u.dtype, device=dev) if out is None else out
-        ws, ws_bytes = _workspace(plan, B, H, L, pre is not None, False, dev)
+        ws, ws_bytes = _workspace(plan, B, H, L, pre is not None, False, dev, halo)
         if halo is not None:
             rc = _lib.lib().bffc_fwd_blocked(plan.handle, _ptr(u), u_bs, _ptr(kf_engine), _ptr(pre), pre_bs, _ptr(post),
                                              post_bs, _ptr(y), H * L, B, H, L, int(halo), _ptr(ws), ws_bytes, _stream())
@@ -424,9 +439,11 @@ def _bwd(mod, dout, u, kf_engine, k_len, pregate, postgate, band=None, out=None,
     (channel slices of one buffer are written in place) and return; otherwise they are new contiguous tensors.
     taps: the short filter of the forward, as _fwd takes it (bffc_bwd_short_strided): u and the gates are the raw
     tensors, and du, dpregate, dpostgate the gradients with respect to their filtered versions.  halo: the forward's
-    overlap-save blocks (bffc_bwd_blocked), else None."""
+    overlap-save blocks (bffc_bwd_blocked), else None.  Under torch.use_deterministic_algorithms(True) dk is summed in
+    a fixed order (the module's deterministic plan): the same bits from run to run and on any GPU; du and the gate
+    gradients are the same in either mode."""
     B, H, L = u.shape
-    plan = mod.plan(u.device)
+    plan = mod.plan(u.device, torch.are_deterministic_algorithms_enabled())
     Lp = _pad_len(plan, L)
     if Lp != L:
         if taps is not None:
@@ -455,7 +472,7 @@ def _bwd(mod, dout, u, kf_engine, k_len, pregate, postgate, band=None, out=None,
     (du, du_bs, _), (dpre, dpre_bs, _), (dpost, dpost_bs, _) = dst
     with _on_device(u.device):
         dkf_engine = torch.empty((H, N, 2), dtype=torch.float32, device=u.device)
-        ws, ws_bytes = _workspace(plan, B, H, L, gated, True, u.device)
+        ws, ws_bytes = _workspace(plan, B, H, L, gated, True, u.device, halo)
         # kf_engine_conj = NULL: the kernels conjugate the forward's spectrum in their pointwise multiply
         if halo is not None:
             rc = _lib.lib().bffc_bwd_blocked(plan.handle, _ptr(dout), dout_bs, _ptr(u), u_bs, _ptr(kf_engine), None,

@@ -85,6 +85,28 @@ int bffc_supported(int seqlen, int dtype);
  */
 int bffc_plan_create(bffc_plan** plan, int seqlen, int dtype);
 int bffc_plan_destroy(bffc_plan* plan);
+/*
+ * bffc_plan_create with options; bffc_plan_create is bffc_plan_create_ex(plan, seqlen, dtype, 0, 0).
+ *   flags: 0 or BFFC_PLAN_DETERMINISTIC.  A deterministic plan sums dkf_engine in a fixed order in every backward entry
+ *     point (bffc_bwd*, no atomics): dkf_engine, and with it dk, is a function of the inputs and the shape only, the
+ *     same from run to run, on any stream, under other work, in a CUDA graph, at any max_ctas and on any SM count.
+ *     Every other output is produced by the same kernels as on a default plan, so it has the same bits.
+ *     Partition: one dk_f launch sums `pairs` batch pairs into each of `rows` rows of 8192 complex fp32 (rows = H up to
+ *     seqlen 8192, H * seqlen / 8192 per channel chunk above; pairs = the launch's 8192-point units per row).  A row's
+ *     pairs are cut into S = min(pairs, ceil(512 / rows)) contiguous slabs of near-equal size, each summed in ascending
+ *     order by one CTA, and the CTAs take whole slabs.  S = 1: the CTA stores the row (a later batch chunk of a composite
+ *     size adds into it, one writer at a time).  S > 1: each slab stores its sum into a 64 KB partial slot of the
+ *     workspace and one more kernel adds a row's slots in ascending order.  S > 1 only when rows < 512, so a launch
+ *     needs fewer than 1024 slots (64 MB).
+ *     Workspace: bffc_workspace_bytes_ex(..., backward = 1) of a deterministic plan adds the slots, after the default
+ *     need rounded up to 256 bytes, for the largest launch of the call; bffc_workspace_bytes_blocked does the same for
+ *     overlap-save blocks.  So a backward at seqlen <= 8192 may need a workspace where a default plan needs none.  Launches (bffc_last_launch_count): one more per dk_f launch with S > 1.
+ *   max_ctas: 0, or a cap below the device's SM count on the CTAs of every persistent launch of the plan (a property of
+ *     the plan, not of the device; results of a deterministic plan do not depend on it).
+ * Unknown flags or max_ctas < 0: BFFC_ERR_INVALID, before the device is looked at.
+ */
+#define BFFC_PLAN_DETERMINISTIC 1
+int bffc_plan_create_ex(bffc_plan** plan, int seqlen, int dtype, int flags, int max_ctas);
 /* FFT size n of the natural-order spectra at this boundary (k_f = rfft(k, n) handed to bffc_kf_pack*, the natural-order
  * dk_f bffc_dkf_unpack* return, the H x n engine buffers): seqlen for seqlen >= 8192; 8192 for the small sizes (256..4096).
  * A small size runs 8192/seqlen batch members per 8192-point unit as independent seqlen-point circular convolutions; its
@@ -165,6 +187,10 @@ int bffc_dk_from_dkf_band(const bffc_plan* plan, const void* dkf_engine, void* d
  * backward nlev + 1 (nlev = 1 for 16K..64K and 1M, 2 for 128K..512K, 2M, 4M). */
 size_t bffc_workspace_bytes(const bffc_plan* plan, int B, int H, int L);
 size_t bffc_workspace_bytes_ex(const bffc_plan* plan, int B, int H, int L, int gated, int backward);
+/* The exact need of bffc_fwd_blocked (backward = 0) / bffc_bwd_blocked (backward = 1) with this halo; 0 for arguments
+ * those calls refuse.  On a default plan it equals bffc_workspace_bytes_ex at (B, H, L); on a deterministic plan the
+ * backward's partial slots depend on the number of blocks, so they are sized from the halo. */
+size_t bffc_workspace_bytes_blocked(const bffc_plan* plan, int B, int H, int L, int halo, int gated, int backward);
 
 /*
  * Forward.  u, y, pregate, postgate: (B, H, L) contiguous, plan dtype, L <= N, L a multiple of
@@ -184,7 +210,7 @@ int bffc_fwd(const bffc_plan* plan, const void* u, const void* kf_engine, const 
  * required (dpostgate = dout * conv(u*pregate, k) is one pass of the forward path; du and dpregate come from one more).
  * dkf_engine is accumulated with fp32 reductions (red.global.add) whose order depends on scheduling and on the SM count:
  * an address that receives more than two partial sums can differ in its last bits from run to run; every other output
- * is bit-reproducible.
+ * is bit-reproducible.  A BFFC_PLAN_DETERMINISTIC plan (bffc_plan_create_ex) sums dkf_engine in a fixed order instead.
  */
 int bffc_bwd(const bffc_plan* plan, const void* dout, const void* u, const void* kf_engine,
              const void* kf_engine_conj, const void* pregate, const void* postgate, void* du,
@@ -229,8 +255,8 @@ int bffc_bwd_strided(const bffc_plan* plan, const void* dout, int64_t dout_bstri
  *     taps.  A longer filter wraps around the blocks and gives a wrong result (not detected).
  *   - Arguments, strides and gates as for bffc_fwd_strided / bffc_bwd_strided.  No output may overlap an input: the
  *     windows of neighbouring blocks read the same samples.
- *   - Workspace: bffc_workspace_bytes_ex of the same plan at (B, H, L).  Launch counts are those of bffc_fwd / bffc_bwd
- *     at seqlen 8192.
+ *   - Workspace: bffc_workspace_bytes_blocked of the same plan at (B, H, L, halo), which on a default plan is
+ *     bffc_workspace_bytes_ex at (B, H, L).  Launch counts are those of bffc_fwd / bffc_bwd at seqlen 8192.
  */
 int bffc_fwd_blocked(const bffc_plan* plan, const void* u, int64_t u_bstride, const void* kf_engine,
                      const void* pregate, int64_t pregate_bstride, const void* postgate, int64_t postgate_bstride,
@@ -440,7 +466,8 @@ int bffc_docs_scatter(const void* items, int n_items, int64_t positions, int B, 
 
 /* Number of kernel launches the last bffc_fwd / bffc_bwd / bffc_fwd_host / filter-side transform /
  * bffc_dwconv1d_fwd (1) / bffc_dwconv1d_bwd (2) / bffc_conv_state_fill (1) / bffc_conv_step (2) /
- * bffc_docs_gather (1) / bffc_docs_scatter (1) on this thread enqueued (bench.py). */
+ * bffc_docs_gather (1) / bffc_docs_scatter (1) on this thread enqueued (bench.py).  A bffc_bwd* on a deterministic plan
+ * counts the same launches as on a default plan, plus one slot sum per dk_f launch whose rows have S > 1 slabs. */
 int bffc_last_launch_count(void);
 
 #ifdef __cplusplus
