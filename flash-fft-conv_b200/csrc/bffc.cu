@@ -1741,6 +1741,8 @@ int bffc_dwconv1d_bwd_varlen(const void* dout, const void* u, int u_dtype, const
 namespace {
 
 namespace dec = bffc::decode;
+static_assert(dec::kTapsBF16 == BFFC_DTYPE_BF16 && dec::kTapsFP16 == BFFC_DTYPE_FP16 && dec::kTapsFP32 == BFFC_DTYPE_FP32,
+              "the step reads the taps' dtype as BFFC_DTYPE_*");
 
 // byte offsets of the parts of a decoding state (include/bffc.h): tail, z cache, s_u cache
 struct StateLayout {
@@ -1756,9 +1758,10 @@ StateLayout state_layout(int B, int H, int max_len, int K, int residual) {
   return s;
 }
 
-size_t step_workspace_bytes(int B, int H, int T, int Lk, int Lk2) {
+// P: columns of the position array, 1 (shared) or B (slots)
+size_t step_workspace_bytes(int B, int H, int T, int Lk, int Lk2, int P) {
   const size_t nck = (size_t(Lk) + dec::kChunk - 1) / dec::kChunk, nck2 = (size_t(Lk2) + dec::kChunk - 1) / dec::kChunk;
-  return (dec::kHeaderFloats + size_t(B) * H * T * (1 + nck + nck2)) * sizeof(float);
+  return (size_t(dec::header_floats(P)) + size_t(B) * H * T * (1 + nck + nck2)) * sizeof(float);
 }
 
 // The arguments the fill and the step share, checked before the device is looked at.  x / bs: the raw inputs of the
@@ -1833,50 +1836,55 @@ size_t bffc_conv_state_bytes(int B, int H, int max_len, int K, int has_residual,
 
 size_t bffc_conv_step_workspace_bytes(int B, int H, int T, int Lk, int Lk2) {
   if (B < 1 || H < 1 || T < 1 || T > dec::kMaxT || Lk < 1 || Lk2 < 0) return 0;
-  return step_workspace_bytes(B, H, T, Lk, Lk2);
+  return step_workspace_bytes(B, H, T, Lk, Lk2, 1);
 }
 
-int bffc_conv_state_fill(const void* u, int64_t u_bstride, const void* pregate, int64_t pregate_bstride,
-                         const void* postgate, int64_t postgate_bstride, const void* u_w, const void* u_bias,
-                         const void* pregate_w, const void* pregate_bias, const void* postgate_w,
-                         const void* postgate_bias, int w_dtype, int K, int padding, int dtype, int B, int H, int L,
-                         int max_len, int has_residual, void* state, size_t state_bytes, int64_t* pos, void* stream) {
-  const char* fn = "bffc_conv_state_fill";
-  const void* const x[3] = {u, pregate, postgate};
-  const int64_t bs[3] = {u_bstride, pregate_bstride, postgate_bstride};
-  const void* const w[3] = {u_w, pregate_w, postgate_w};
-  const void* const bias[3] = {u_bias, pregate_bias, postgate_bias};
+size_t bffc_conv_step_slots_workspace_bytes(int B, int H, int T, int Lk, int Lk2) {
+  if (B < 1 || H < 1 || T < 1 || T > dec::kMaxT || Lk < 1 || Lk2 < 0) return 0;
+  return step_workspace_bytes(B, H, T, Lk, Lk2, B);
+}
+
+}  // extern "C"
+
+namespace {
+
+// bffc_conv_state_fill (slot_map null: n = B rows, every one of length L) and bffc_conv_state_fill_slots
+int conv_fill(const char* fn, const void* const (&x)[3], const int64_t (&bs)[3], const void* const (&w)[3],
+              const void* const (&bias)[3], int w_dtype, int K, int padding, int dtype, int B, int H, int n, int L,
+              const int32_t* slot_map, const int32_t* lengths, bool slots, int max_len, int has_residual, void* state,
+              size_t state_bytes, int64_t* pos, void* stream) {
   const int residual = has_residual != 0;
   if (int rc = decode_args(fn, dtype, B, H, L, max_len, K, padding, w_dtype, x, bs, w, bias, residual, state,
                            state_bytes, pos))
     return rc;
+  if (slots) {
+    if (n < 1 || n > B) return fail(BFFC_ERR_INVALID, "%s: n=%d prompts outside [1, B=%d]", fn, n, B);
+    if (!slot_map || reinterpret_cast<uintptr_t>(slot_map) % 4 || !lengths || reinterpret_cast<uintptr_t>(lengths) % 4)
+      return fail(BFFC_ERR_INVALID, "%s: slots / lengths null or not 4-byte aligned", fn);
+  }
   if (int rc = check_device()) return rc;
   dec::Params p = decode_params(B, H, max_len, K, residual, state, pos, x, bs, w, bias);
   if (L == 0)
     for (auto& r : p.r) r = dec::Role{};
+  p.slots = slots;
+  p.fill_slots = slot_map;
+  p.fill_lengths = lengths;
+  p.n = n;
   const dim3 grid(unsigned((std::max(L, 1) + dec::kThreads - 1) / dec::kThreads), unsigned(std::min(H, kMaxGridYZ)),
-                  unsigned(std::min(B, kMaxGridYZ)));
+                  unsigned(std::min(n, kMaxGridYZ)));
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   g_launches = 0;
-  decode_dispatch(dtype, w_dtype, [&](auto tt, auto tw) {
-    using T = typename decltype(tt)::type;
-    using W = typename decltype(tw)::type;
-    dec::state_fill<T, W><<<grid, dec::kThreads, 0, st>>>(p, L);
-  });
+  p.w_dtype = w_dtype;                            // the fill reads the taps' dtype at run time
+  if (dtype == BFFC_DTYPE_FP16) dec::state_fill<__half, dec::TapsAtRunTime><<<grid, dec::kThreads, 0, st>>>(p, L);
+  else dec::state_fill<__nv_bfloat16, dec::TapsAtRunTime><<<grid, dec::kThreads, 0, st>>>(p, L);
   return launched();
 }
 
-int bffc_conv_step(const void* u, int64_t u_bstride, const void* pregate, int64_t pregate_bstride, const void* postgate,
-                   int64_t postgate_bstride, const void* k, int Lk, const void* k2, int Lk2, const void* u_w,
-                   const void* u_bias, const void* pregate_w, const void* pregate_bias, const void* postgate_w,
-                   const void* postgate_bias, int w_dtype, int K, int padding, int dtype, void* state,
-                   size_t state_bytes, int64_t* pos, void* y, int64_t y_bstride, int B, int H, int T, int max_len,
-                   void* workspace, size_t workspace_bytes, void* stream) {
-  const char* fn = "bffc_conv_step";
-  const void* const x[3] = {u, pregate, postgate};
-  const int64_t bs[3] = {u_bstride, pregate_bstride, postgate_bstride};
-  const void* const w[3] = {u_w, pregate_w, postgate_w};
-  const void* const bias[3] = {u_bias, pregate_bias, postgate_bias};
+// bffc_conv_step (slots false: pos is (2, 1)) and bffc_conv_step_slots (pos is (2, B))
+int conv_step(const char* fn, const void* const (&x)[3], const int64_t (&bs)[3], const void* k, int Lk, const void* k2,
+              int Lk2, const void* const (&w)[3], const void* const (&bias)[3], int w_dtype, int K, int padding,
+              int dtype, void* state, size_t state_bytes, int64_t* pos, bool slots, void* y, int64_t y_bstride, int B,
+              int H, int T, int max_len, void* workspace, size_t workspace_bytes, void* stream) {
   const int residual = k2 != nullptr;
   if (T < 1 || T > dec::kMaxT) return fail(BFFC_ERR_INVALID, "%s: T=%d outside [1, %d]", fn, T, dec::kMaxT);
   if (int rc = decode_args(fn, dtype, B, H, T, max_len, K, padding, w_dtype, x, bs, w, bias, residual, state,
@@ -1891,11 +1899,13 @@ int bffc_conv_step(const void* u, int64_t u_bstride, const void* pregate, int64_
   if (!y || reinterpret_cast<uintptr_t>(y) % 2) return fail(BFFC_ERR_INVALID, "%s: y null or not aligned to its element", fn);
   if (y_bstride < int64_t(H) * T)
     return fail(BFFC_ERR_INVALID, "%s: batch stride %lld below H * length = %lld", fn, (long long)y_bstride, (long long)H * T);
-  const size_t need = step_workspace_bytes(B, H, T, Lk, Lk2);
+  const size_t need = step_workspace_bytes(B, H, T, Lk, Lk2, slots ? B : 1);
   if (!workspace || reinterpret_cast<uintptr_t>(workspace) % 16 || workspace_bytes < need)
     return fail(BFFC_ERR_INVALID, "%s: a 16-byte aligned workspace of %zu bytes required", fn, need);
   if (int rc = check_device()) return rc;
   dec::Params p = decode_params(B, H, max_len, K, residual, state, pos, x, bs, w, bias);
+  p.slots = slots;
+  p.w_dtype = w_dtype;
   p.k = static_cast<const float*>(k);
   p.k2 = static_cast<const float*>(k2);
   p.Lk = Lk; p.Lk2 = Lk2;
@@ -1903,21 +1913,79 @@ int bffc_conv_step(const void* u, int64_t u_bstride, const void* pregate, int64_
   p.nck2 = (Lk2 + dec::kChunk - 1) / dec::kChunk;
   p.y = y; p.y_bs = y_bstride; p.T = T;
   p.ws = static_cast<float*>(workspace);
+  p.hdr = int(dec::header_floats(slots ? B : 1));
   const dim3 grid1(unsigned(std::max(p.nck, p.nck2)), unsigned(std::min(H, kMaxGridYZ)));
   const long long outs = dec::outputs(p);
   const unsigned grid2 = unsigned(std::min<long long>((outs + dec::kThreads - 1) / dec::kThreads, kMaxGridYZ));
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   g_launches = 0;
   int rc = 0;
-  decode_dispatch(dtype, w_dtype, [&](auto tt, auto tw) {
+  // the shared step per tap dtype; the slot step reads the taps' dtype at run time (decode_step.cuh, TapsAtRunTime)
+  auto launch = [&](auto tt, auto tw, auto mode) {
     using T_ = typename decltype(tt)::type;
     using W = typename decltype(tw)::type;
-    dec::step_lags<T_, W><<<grid1, dec::kThreads, 0, st>>>(p);
+    constexpr bool kSlots = decltype(mode)::value;
+    dec::step_lags<T_, W, kSlots><<<grid1, dec::kThreads, 0, st>>>(p);
     if ((rc = launched())) return;
-    dec::step_finish<T_><<<grid2, dec::kThreads, 0, st>>>(p);
+    dec::step_finish<T_, kSlots><<<grid2, dec::kThreads, 0, st>>>(p);
     rc = launched();
-  });
+  };
+  if (slots) {
+    if (dtype == BFFC_DTYPE_FP16) launch(Tag<__half>(), Tag<dec::TapsAtRunTime>(), std::true_type());
+    else launch(Tag<__nv_bfloat16>(), Tag<dec::TapsAtRunTime>(), std::true_type());
+  } else {
+    decode_dispatch(dtype, w_dtype, [&](auto tt, auto tw) { launch(tt, tw, std::false_type()); });
+  }
   return rc;
+}
+
+}  // namespace
+
+extern "C" {
+
+int bffc_conv_state_fill(const void* u, int64_t u_bstride, const void* pregate, int64_t pregate_bstride,
+                         const void* postgate, int64_t postgate_bstride, const void* u_w, const void* u_bias,
+                         const void* pregate_w, const void* pregate_bias, const void* postgate_w,
+                         const void* postgate_bias, int w_dtype, int K, int padding, int dtype, int B, int H, int L,
+                         int max_len, int has_residual, void* state, size_t state_bytes, int64_t* pos, void* stream) {
+  return conv_fill("bffc_conv_state_fill", {u, pregate, postgate}, {u_bstride, pregate_bstride, postgate_bstride},
+                   {u_w, pregate_w, postgate_w}, {u_bias, pregate_bias, postgate_bias}, w_dtype, K, padding, dtype, B,
+                   H, B, L, nullptr, nullptr, false, max_len, has_residual, state, state_bytes, pos, stream);
+}
+
+int bffc_conv_state_fill_slots(const void* u, int64_t u_bstride, const void* pregate, int64_t pregate_bstride,
+                               const void* postgate, int64_t postgate_bstride, const void* u_w, const void* u_bias,
+                               const void* pregate_w, const void* pregate_bias, const void* postgate_w,
+                               const void* postgate_bias, int w_dtype, int K, int padding, int dtype, int B, int H,
+                               int n, int L, const int32_t* slots, const int32_t* lengths, int max_len,
+                               int has_residual, void* state, size_t state_bytes, int64_t* pos, void* stream) {
+  return conv_fill("bffc_conv_state_fill_slots", {u, pregate, postgate}, {u_bstride, pregate_bstride, postgate_bstride},
+                   {u_w, pregate_w, postgate_w}, {u_bias, pregate_bias, postgate_bias}, w_dtype, K, padding, dtype, B,
+                   H, n, L, slots, lengths, true, max_len, has_residual, state, state_bytes, pos, stream);
+}
+
+int bffc_conv_step(const void* u, int64_t u_bstride, const void* pregate, int64_t pregate_bstride, const void* postgate,
+                   int64_t postgate_bstride, const void* k, int Lk, const void* k2, int Lk2, const void* u_w,
+                   const void* u_bias, const void* pregate_w, const void* pregate_bias, const void* postgate_w,
+                   const void* postgate_bias, int w_dtype, int K, int padding, int dtype, void* state,
+                   size_t state_bytes, int64_t* pos, void* y, int64_t y_bstride, int B, int H, int T, int max_len,
+                   void* workspace, size_t workspace_bytes, void* stream) {
+  return conv_step("bffc_conv_step", {u, pregate, postgate}, {u_bstride, pregate_bstride, postgate_bstride}, k, Lk, k2,
+                   Lk2, {u_w, pregate_w, postgate_w}, {u_bias, pregate_bias, postgate_bias}, w_dtype, K, padding,
+                   dtype, state, state_bytes, pos, false, y, y_bstride, B, H, T, max_len, workspace, workspace_bytes,
+                   stream);
+}
+
+int bffc_conv_step_slots(const void* u, int64_t u_bstride, const void* pregate, int64_t pregate_bstride,
+                         const void* postgate, int64_t postgate_bstride, const void* k, int Lk, const void* k2, int Lk2,
+                         const void* u_w, const void* u_bias, const void* pregate_w, const void* pregate_bias,
+                         const void* postgate_w, const void* postgate_bias, int w_dtype, int K, int padding, int dtype,
+                         void* state, size_t state_bytes, int64_t* pos, void* y, int64_t y_bstride, int B, int H, int T,
+                         int max_len, void* workspace, size_t workspace_bytes, void* stream) {
+  return conv_step("bffc_conv_step_slots", {u, pregate, postgate}, {u_bstride, pregate_bstride, postgate_bstride}, k,
+                   Lk, k2, Lk2, {u_w, pregate_w, postgate_w}, {u_bias, pregate_bias, postgate_bias}, w_dtype, K,
+                   padding, dtype, state, state_bytes, pos, true, y, y_bstride, B, H, T, max_len, workspace,
+                   workspace_bytes, stream);
 }
 
 }  // extern "C"

@@ -88,6 +88,13 @@ SYMBOLS = {
     'bffc_conv_step': (_c.c_int, [_c.c_void_p, _c.c_int64] * 3 + [_c.c_void_p, _c.c_int] * 2 + [_c.c_void_p] * 6
                        + [_c.c_int] * 4 + [_c.c_void_p, _c.c_size_t, _c.c_void_p, _c.c_void_p, _c.c_int64]
                        + [_c.c_int] * 4 + [_c.c_void_p, _c.c_size_t, _c.c_void_p]),
+    'bffc_conv_step_slots_workspace_bytes': (_c.c_size_t, [_c.c_int] * 5),
+    'bffc_conv_state_fill_slots': (_c.c_int, [_c.c_void_p, _c.c_int64] * 3 + [_c.c_void_p] * 6 + [_c.c_int] * 8
+                                   + [_c.c_void_p] * 2 + [_c.c_int] * 2
+                                   + [_c.c_void_p, _c.c_size_t, _c.c_void_p, _c.c_void_p]),
+    'bffc_conv_step_slots': (_c.c_int, [_c.c_void_p, _c.c_int64] * 3 + [_c.c_void_p, _c.c_int] * 2 + [_c.c_void_p] * 6
+                             + [_c.c_int] * 4 + [_c.c_void_p, _c.c_size_t, _c.c_void_p, _c.c_void_p, _c.c_int64]
+                             + [_c.c_int] * 4 + [_c.c_void_p, _c.c_size_t, _c.c_void_p]),
     'bffc_docs_gather': (_c.c_int, [_c.c_void_p, _c.c_int, _c.c_int64] + [_c.c_int] * 3
                          + [_c.POINTER(_c.c_void_p), _c.POINTER(_c.c_int64), _c.POINTER(_c.c_void_p), _c.c_int,
                             _c.c_void_p]),

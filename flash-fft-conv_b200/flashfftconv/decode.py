@@ -33,6 +33,19 @@ nor synchronises.  Run one eager step with the same T first (it sizes the worksp
         g.replay()                                      # y_static holds the outputs, dec.pos advanced by T
 
 A graph replay past max_len writes nothing and sets a device flag that reading `dec.pos` reports.
+
+Slots (continuous batching): a decoder made with slots=True keeps one position per batch row ("slot"), so prompts of
+different lengths share one batch and a freed row takes the next request while the others keep generating:
+
+    dec = HyenaDecoder(short_filter, k, d_model, batch, max_len, slots=True)     # every slot idle
+    y = dec.prefill(x, lengths=[30, 255, 0])     # x (3, 3D, L) right-padded; slots 0, 1, 2 restart... (n == batch)
+    y = dec.prefill(x2, lengths=[17], slots=[1]) # ...or fill chosen slots; the others are untouched
+    y_new = dec.step(x_new)                      # (B, 3D, T) -> (B, D, T); idle or overflowing rows are zero
+    dec.release([0])                             # slot 0 idle again; the host does not wait for the device
+    dec.positions                                # [-1, 18, 1]: per-slot positions read from the device
+
+Each slot's outputs and state are bit for bit those of a one-row decoder run on that slot's own sequence.  A captured
+step can be replayed after eager admissions and releases made on the stream the replays run on.
 """
 import ctypes
 
@@ -42,7 +55,7 @@ from . import _lib
 from . import depthwise_1d as _dw
 from .conv import FlashFFTConv, _DT, _on_device, _ptr, _stream
 from .docs import refuse
-from .gated import gated_long_conv, hyena_operator
+from .gated import gated_long_conv, hyena_mixer, hyena_operator
 
 MAX_STEP_TOKENS = 64
 MAX_KERNEL_SIZE = 32
@@ -62,6 +75,30 @@ def state_layout(B, H, max_len, K, residual):
     zc = a256(6 * B * H * (K - 1))
     vc = zc + a256(2 * B * H * max_len)
     return zc, vc, vc + (vc - zc if residual else 0)
+
+
+def _host_ints(v, name):
+    """a host sequence or CPU tensor of ints as a list"""
+    if isinstance(v, torch.Tensor):
+        if v.is_cuda or v.dim() != 1 or v.dtype.is_floating_point or v.dtype == torch.bool:
+            raise ValueError(f'{name} must be a host sequence or a 1-D CPU integer tensor')
+        return [int(i) for i in v.tolist()]
+    return [int(i) for i in v]
+
+
+def position_array(batch, slots, device):
+    """The device position array of a decoder (include/bffc.h): int64 (2, P), row 0 the positions, row 1 the status
+    words.  P = batch with slots, every slot idle (-1); P = 1 without, kept as the int64[2] {0, 0} of the shared calls."""
+    if not slots:
+        return torch.zeros(2, dtype=torch.int64, device=device)
+    pos = torch.zeros(2, batch, dtype=torch.int64, device=device)
+    pos[0].fill_(-1)
+    return pos
+
+
+def _device_ints(values, dtype, device):
+    """a host list as a device tensor, copied from pinned memory without waiting for the stream's work"""
+    return torch.tensor(values, dtype=dtype).pin_memory().to(device, non_blocking=True)
 
 
 def _rows(t, H, T):
@@ -85,7 +122,7 @@ def _filter(k, H, max_len, name):
 class _Decoder:
     """The state of one batch of sequences and the two library calls; the subclasses name the roles."""
 
-    def __init__(self, k, k2, H, batch, max_len, dtype, K):
+    def __init__(self, k, k2, H, batch, max_len, dtype, K, slots=False):
         if dtype not in _DT:
             raise ValueError(f'dtype must be torch.bfloat16 or torch.float16, got {dtype}')
         if batch < 1 or max_len < 1:
@@ -97,8 +134,11 @@ class _Decoder:
         dt = _DT[dtype]
         nbytes = _lib.lib().bffc_conv_state_bytes(self.batch, H, self.max_len, K, int(self.k2 is not None), dt)
         self.state = torch.zeros(nbytes, dtype=torch.uint8, device=self.device)
-        self._pos = torch.zeros(2, dtype=torch.int64, device=self.device)       # position, status
-        self._host_pos = 0                 # known position, or None after a graph capture
+        self.slots = bool(slots)
+        # (2, P) positions and status words (include/bffc.h): P = 1 shared, kept as int64[2]; P = batch with slots
+        self._pos = position_array(self.batch, self.slots, self.device)
+        # known position (a list per slot with slots), or None after a graph capture
+        self._host_pos = [-1] * self.batch if self.slots else 0
         self._ws = None
         # workspaces outgrown by a larger T: a graph captured earlier still writes to the address it was given
         self._ws_outgrown = []
@@ -134,6 +174,8 @@ class _Decoder:
     def pos(self):
         """Number of positions decoded so far, read from the device (a synchronisation).  Raises when a step ran past
         max_len (it then wrote nothing)."""
+        if self.slots:
+            raise RuntimeError('a slot decoder keeps one position per slot: read `positions`')
         pos, status = self._pos.tolist()
         if status:
             raise RuntimeError(f'a decoding step would have run past max_len = {self.max_len} and did nothing; '
@@ -141,8 +183,86 @@ class _Decoder:
         self._host_pos = pos
         return pos
 
+    @property
+    def positions(self):
+        """Per-slot positions read from the device (a synchronisation), -1 for an idle slot.  Raises naming every slot
+        whose status is set (a step would have taken it past max_len; it kept its state and position).  Admitting the
+        slot again clears its status."""
+        if not self.slots:
+            raise RuntimeError('positions is for a decoder made with slots=True; read `pos`')
+        pos, status = self._pos.tolist()
+        bad = [b for b, s in enumerate(status) if s]
+        if bad:
+            raise RuntimeError(f'slots {bad} would have run past max_len = {self.max_len} and kept their state; their '
+                               f'positions are {[pos[b] for b in bad]}')
+        self._host_pos = list(pos)
+        return pos
+
+    def release(self, slots):
+        """Idle the given slots on the device, with no synchronisation (the slot indices go to the device from pinned
+        memory, ordered on the current stream): their state is kept but no longer read, their rows of y are zero, and
+        a later prefill may admit a new prompt into them."""
+        self._need_slots('release')
+        if slots is None:
+            raise ValueError('release takes the slots to idle (reset() idles every slot)')
+        idx = self._slot_list(slots, None)
+        if not idx:
+            return
+        i = _device_ints(idx, torch.int64, self.device)
+        self._pos[0].index_fill_(0, i, -1)
+        self._pos[1].index_fill_(0, i, 0)
+        if self._host_pos is not None:
+            for b in idx:
+                self._host_pos[b] = -1
+
+    def _need_slots(self, what):
+        if not self.slots:
+            raise RuntimeError(f'{what} is for a decoder made with slots=True')
+
+    def _slot_list(self, slots, n):
+        """slots as a validated list: distinct, in [0, batch), n of them (n = batch and every slot for None)"""
+        idx = list(range(self.batch)) if slots is None else _host_ints(slots, 'slots')
+        if n is not None and len(idx) != n:
+            raise ValueError(f'{len(idx)} slots for {n} prompts' if slots is not None else
+                             f'slots=None admits every one of the {self.batch} slots, got {n} prompts')
+        bad = [b for b in idx if not 0 <= b < self.batch]
+        if bad:
+            raise ValueError(f'slots {bad} outside [0, {self.batch})')
+        if len(set(idx)) != len(idx):
+            raise ValueError(f'slots {idx} are not distinct')
+        return idx
+
+    def _admission(self, n, L, lengths, slots):
+        """(slots, lengths) of a slot prefill of n right-padded prompts of L positions, validated on the host"""
+        if L > self.max_len:
+            raise ValueError(f'prompt of {L} positions exceeds max_len = {self.max_len}')
+        if lengths is None:
+            raise ValueError('a slot decoder\'s prefill takes lengths=[...] (one per prompt row)')
+        if not 1 <= n <= self.batch:
+            raise ValueError(f'{n} prompts for {self.batch} slots')
+        lens = _host_ints(lengths, 'lengths')
+        if len(lens) != n:
+            raise ValueError(f'{len(lens)} lengths for {n} prompts')
+        bad = [l for l in lens if not 0 <= l <= L]
+        if bad:
+            raise ValueError(f'lengths {bad} outside [0, L = {L}]')
+        return self._slot_list(slots, n), lens
+
+    @staticmethod
+    def _mask(t, lens):
+        """t (n, C, L) zero at positions t >= lens[i] of row i (NaN and large values in the padding included)"""
+        if t is None:
+            return None
+        keep = torch.arange(t.shape[-1], device=t.device)[None] < _device_ints(lens, torch.int64, t.device)[:, None]
+        return torch.where(keep[:, None, :], t, torch.zeros((), dtype=t.dtype, device=t.device))
+
     def reset(self):
-        """Start over with an empty prompt."""
+        """Start over with an empty prompt (with slots: every slot idle)."""
+        if self.slots:
+            self._pos[0].fill_(-1)
+            self._pos[1].zero_()
+            self._host_pos = [-1] * self.batch
+            return
         self._fill(None, None, None, 0)
 
     def _conv(self, L):
@@ -152,19 +272,20 @@ class _Decoder:
             conv = self._convs[n] = FlashFFTConv(n, dtype=self.dtype).eval()
         return conv
 
-    def _check(self, t, name, T):
-        if t.dim() != 3 or t.shape[0] != self.batch or t.shape[1] != self.H or t.shape[2] != T:
-            raise ValueError(f'{name} must be ({self.batch}, {self.H}, {T}), got {tuple(t.shape)}')
+    def _check(self, t, name, T, n=None):
+        n = self.batch if n is None else n
+        if t.dim() != 3 or t.shape[0] != n or t.shape[1] != self.H or t.shape[2] != T:
+            raise ValueError(f'{name} must be ({n}, {self.H}, {T}), got {tuple(t.shape)}')
         if t.dtype != self.dtype or t.device != self.device:
             raise ValueError(f'{name} must be {self.dtype} on {self.device}, got {t.dtype} on {t.device}')
 
-    def _roles(self, u, pregate, postgate, T):
+    def _roles(self, u, pregate, postgate, T, n=None):
         out = []
         for name, t in (('u', u), ('pregate', pregate), ('postgate', postgate)):
             if t is None:
                 out.append((None, 0))
             else:
-                self._check(t, name, T)
+                self._check(t, name, T, n)
                 out.append(_rows(t, self.H, T))
         return out
 
@@ -183,18 +304,42 @@ class _Decoder:
                                                        _stream()))
         self._host_pos = L
 
+    def _fill_slots(self, u, pregate, postgate, L, slots, lengths):
+        """one bffc_conv_state_fill_slots call: prompt row i (already zero past lengths[i]) into slot slots[i]"""
+        n = len(slots)
+        roles = self._roles(u, pregate, postgate, L, n) if L else [(None, 0)] * 3
+        rows, wdt = self._tap_args() if L else ([None] * 6, _lib.BFFC_DTYPE_FP32)
+        args = [a for t, s in roles for a in (_ptr(t), s)]
+        meta = _device_ints(slots + lengths, torch.int32, self.device)
+        with _on_device(self.device):
+            _lib.check(_lib.lib().bffc_conv_state_fill_slots(*args, *rows, wdt, self.K, self.K - 1, _DT[self.dtype],
+                                                             self.batch, self.H, n, L, _ptr(meta),
+                                                             _ptr(meta[n:]), self.max_len, int(self.k2 is not None),
+                                                             _ptr(self.state), self.state.numel(), _ptr(self._pos),
+                                                             _stream()))
+        if self._host_pos is not None:
+            for b, l in zip(slots, lengths):
+                self._host_pos[b] = l
+
     def _step(self, u, pregate, postgate):
         T = u.shape[-1]
         if not 1 <= T <= MAX_STEP_TOKENS:
             raise ValueError(f'a step takes 1 to {MAX_STEP_TOKENS} tokens, got {T} (a longer chunk is a prefill)')
         capturing = torch.cuda.is_current_stream_capturing()
-        if self._host_pos is not None and not capturing and self._host_pos + T > self.max_len:
-            raise ValueError(f'position {self._host_pos} + {T} tokens exceeds max_len = {self.max_len}')
+        if self._host_pos is not None and not capturing:
+            if self.slots:
+                over = [b for b, p in enumerate(self._host_pos) if p >= 0 and p + T > self.max_len]
+                if over:
+                    raise ValueError(f'slots {over} at positions {[self._host_pos[b] for b in over]} + {T} tokens '
+                                     f'exceed max_len = {self.max_len}')
+            elif self._host_pos + T > self.max_len:
+                raise ValueError(f'position {self._host_pos} + {T} tokens exceeds max_len = {self.max_len}')
         roles = self._roles(u, pregate, postgate, T)
         rows, wdt = self._tap_args()
         Lk = self.k.shape[1]
         Lk2 = 0 if self.k2 is None else self.k2.shape[1]
-        nws = _lib.lib().bffc_conv_step_workspace_bytes(self.batch, self.H, T, Lk, Lk2)
+        nws = (_lib.lib().bffc_conv_step_slots_workspace_bytes if self.slots else
+               _lib.lib().bffc_conv_step_workspace_bytes)(self.batch, self.H, T, Lk, Lk2)
         if self._ws is None or self._ws.numel() < nws:
             if capturing:
                 raise RuntimeError(f'run one eager step with T = {T} before capturing it (it sizes the workspace)')
@@ -203,12 +348,18 @@ class _Decoder:
             self._ws = torch.empty(nws, dtype=torch.uint8, device=self.device)
         y = torch.empty((self.batch, self.H, T), dtype=self.dtype, device=self.device)
         args = [a for t, s in roles for a in (_ptr(t), s)]
+        fn = _lib.lib().bffc_conv_step_slots if self.slots else _lib.lib().bffc_conv_step
         with _on_device(self.device):
-            _lib.check(_lib.lib().bffc_conv_step(*args, _ptr(self.k), Lk, _ptr(self.k2), Lk2, *rows, wdt, self.K,
-                                                 self.K - 1, _DT[self.dtype], _ptr(self.state), self.state.numel(),
-                                                 _ptr(self._pos), _ptr(y), self.H * T, self.batch, self.H, T,
-                                                 self.max_len, _ptr(self._ws), self._ws.numel(), _stream()))
-        self._host_pos = None if capturing or self._host_pos is None else self._host_pos + T
+            _lib.check(fn(*args, _ptr(self.k), Lk, _ptr(self.k2), Lk2, *rows, wdt, self.K, self.K - 1,
+                          _DT[self.dtype], _ptr(self.state), self.state.numel(), _ptr(self._pos), _ptr(y),
+                          self.H * T, self.batch, self.H, T, self.max_len, _ptr(self._ws), self._ws.numel(),
+                          _stream()))
+        if capturing or self._host_pos is None:
+            self._host_pos = None
+        elif self.slots:
+            self._host_pos = [p + T if p >= 0 else p for p in self._host_pos]
+        else:
+            self._host_pos += T
         return y
 
 
@@ -223,9 +374,12 @@ class HyenaDecoder(_Decoder):
 
         s = short_filter(x)[..., :L];  x1, x2, v = s.split(d_model, dim=1)
         y = x2 * causal_conv(x1 * v, k) [+ causal_conv(v, k2)]
+
+    slots=True: one position per batch row (see the module docstring); every slot starts idle.
     """
 
-    def __init__(self, short_filter, k, d_model, batch, max_len, residual_filter=None, dtype=torch.bfloat16):
+    def __init__(self, short_filter, k, d_model, batch, max_len, residual_filter=None, dtype=torch.bfloat16,
+                 slots=False):
         if not isinstance(short_filter, _dw.FlashDepthWiseConv1d) or not short_filter.is_bhl:
             raise ValueError('short_filter must be a BHL FlashDepthWiseConv1d')
         if short_filter.d != 3 * d_model:
@@ -238,7 +392,7 @@ class HyenaDecoder(_Decoder):
             raise ValueError(f'short filter padding {P}: decoding needs the causal padding K - 1 = {K - 1} (padding '
                              f'{P} makes each output read {K - 1 - P} input(s) after its position)')
         self.short_filter, self.d_model = short_filter, d_model
-        super().__init__(k, residual_filter, d_model, batch, max_len, dtype, K)
+        super().__init__(k, residual_filter, d_model, batch, max_len, dtype, K, slots)
         self._tap_args()
 
     def _tap_args(self):
@@ -262,10 +416,18 @@ class HyenaDecoder(_Decoder):
         return v, x1, x2
 
     @torch.no_grad()
-    def prefill(self, x, docs=None):
+    def prefill(self, x, docs=None, *, lengths=None, slots=None):
         """y (B, d_model, L) of the prompt x (B, 3 * d_model, L) by the FFT engine, and the caches filled from it; starts
-        a new sequence.  L may be 0.  Packed documents (docs) are refused: one decoder row is one sequence."""
+        a new sequence.  L may be 0.  Packed documents (docs) are refused: one decoder row is one sequence.
+
+        With slots: x (n, 3 * d_model, L) right-padded, row i a prompt of lengths[i] <= L positions admitted into slot
+        slots[i] (slots=None: n = batch, every slot restarts); other slots are untouched.  Returns (n, d_model, L), zero
+        at t >= lengths[i]."""
         refuse(docs, 'HyenaDecoder')
+        if self.slots:
+            return self._prefill_slots(x, lengths, slots)
+        if lengths is not None or slots is not None:
+            raise ValueError('lengths and slots are for a decoder made with slots=True')
         L = x.shape[-1]
         if L > self.max_len:
             raise ValueError(f'prompt of {L} positions exceeds max_len = {self.max_len}')
@@ -278,6 +440,27 @@ class HyenaDecoder(_Decoder):
         k2 = None if self.k2 is None else self.k2[:, :min(self.k2.shape[1], L)]
         y = hyena_operator(self._conv(L), self.short_filter, x, k, self.d_model, residual_filter=k2)
         self._fill(v, x1, x2, L)
+        return y
+
+    def _prefill_slots(self, x, lengths, slots):
+        if x.dim() != 3:
+            raise ValueError(f'x must be (n, 3 * d_model = {3 * self.d_model}, L), got {tuple(x.shape)}')
+        n, L = x.shape[0], x.shape[-1]
+        slots, lens = self._admission(n, L, lengths, slots)
+        for name, t in zip(('v', 'x1', 'x2'), self._split(x)):   # shape, dtype and device before any work
+            self._check(t, name, L, n)
+        x = self._mask(x, lens)            # contiguous, zero past each length
+        v, x1, x2 = self._split(x)
+        if L == 0:
+            y = x.new_empty((n, self.d_model, 0))
+        else:
+            k = self.k[:, :min(self.k.shape[1], L)]
+            k2 = None if self.k2 is None else self.k2[:, :min(self.k2.shape[1], L)]
+            # the short filter's bias makes s non-zero past a prompt's end; zeroed there, the transform's rounding
+            # scales with each prompt alone rather than with its padded row
+            s = self._mask(self.short_filter(x)[..., :L], lens)
+            y = self._mask(hyena_mixer(self._conv(L), s, k, self.d_model, residual_filter=k2), lens)
+        self._fill_slots(v, x1, x2, L, slots, lens)
         return y
 
     @torch.no_grad()
@@ -293,11 +476,12 @@ class LongConvDecoder(_Decoder):
     """y = postgate * causal_conv(u * pregate, k) (FlashFFTConv's gated convolution; either gate may be absent)
     decoded position by position.  k: (H, Lk), Lk <= max_len, taken at construction as contiguous fp32 (k itself when
     it already is, else a converted copy).  The gates given to prefill are the gates every step takes: z = u * pregate
-    and z = u must not mix in one cache, so a step with another set of gates is refused."""
+    and z = u must not mix in one cache, so a step with another set of gates is refused.  With slots=True (one
+    position per batch row, see the module docstring) every slot shares the gate set of the first prefill or step."""
 
-    def __init__(self, k, batch, max_len, dtype=torch.bfloat16):
+    def __init__(self, k, batch, max_len, dtype=torch.bfloat16, slots=False):
         self._gates = None                 # (pregate given, postgate given) of this sequence, once known
-        super().__init__(k, None, k.shape[0], batch, max_len, dtype, 1)
+        super().__init__(k, None, k.shape[0], batch, max_len, dtype, 1, slots)
 
     def _same_gates(self, pregate, postgate):
         gates = (pregate is not None, postgate is not None)
@@ -314,10 +498,18 @@ class LongConvDecoder(_Decoder):
         super().reset()
 
     @torch.no_grad()
-    def prefill(self, u, pregate=None, postgate=None, docs=None):
+    def prefill(self, u, pregate=None, postgate=None, docs=None, *, lengths=None, slots=None):
         """y (B, H, L) of the prompt by the FFT engine, and the cache filled from it; starts a new sequence.  Packed
-        documents (docs) are refused: one decoder row is one sequence."""
+        documents (docs) are refused: one decoder row is one sequence.
+
+        With slots: u and the gates (n, H, L) right-padded, row i a prompt of lengths[i] <= L positions admitted into
+        slot slots[i] (slots=None: n = batch, every slot restarts); other slots are untouched.  Returns (n, H, L), zero
+        at t >= lengths[i]."""
         refuse(docs, 'LongConvDecoder')
+        if self.slots:
+            return self._prefill_slots(u, pregate, postgate, lengths, slots)
+        if lengths is not None or slots is not None:
+            raise ValueError('lengths and slots are for a decoder made with slots=True')
         L = u.shape[-1]
         if L > self.max_len:
             raise ValueError(f'prompt of {L} positions exceeds max_len = {self.max_len}')
@@ -335,6 +527,29 @@ class LongConvDecoder(_Decoder):
             ones = torch.ones_like(u)
             y = gated_long_conv(conv, u, k, ones if pregate is None else pregate, ones if postgate is None else postgate)
         self._fill(u, pregate, postgate, L)
+        return y
+
+    def _prefill_slots(self, u, pregate, postgate, lengths, slots):
+        if u.dim() != 3:
+            raise ValueError(f'u must be (n, {self.H}, L), got {tuple(u.shape)}')
+        n, L = u.shape[0], u.shape[-1]
+        slots, lens = self._admission(n, L, lengths, slots)
+        self._roles(u, pregate, postgate, L, n)
+        self._same_gates(pregate, postgate)
+        u, pregate, postgate = (self._mask(t, lens) for t in (u, pregate, postgate))
+        if L == 0:
+            y = torch.empty_like(u)
+        else:
+            conv = self._conv(L)
+            k = self.k[:, :min(self.k.shape[1], L)]
+            if pregate is None and postgate is None:
+                y = conv(u, k)
+            else:
+                ones = torch.ones_like(u)
+                y = gated_long_conv(conv, u, k, ones if pregate is None else pregate,
+                                    ones if postgate is None else postgate)
+            y = self._mask(y, lens)
+        self._fill_slots(u, pregate, postgate, L, slots, lens)
         return y
 
     @torch.no_grad()

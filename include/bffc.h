@@ -397,7 +397,7 @@ int bffc_dwconv1d_bwd_varlen(const void* dout, const void* u, int u_dtype, const
  *   zc + align256(2 * B * H * max_len):   s_u cache (B, H, max_len) dtype, only with has_residual
  * pos: device int64[2]: pos[0] the number of positions filled, pos[1] a status word (0 ok, 1: a step would have run past
  * max_len; it then wrote nothing, neither y nor the state, and pos[0] is unchanged).  The caller reads it outside graph
- * capture.
+ * capture.  It is the (2, P) position array of the slot calls below with P = 1.
  *
  * bffc_conv_state_fill: from a raw prompt u / pregate / postgate (B, H, L), element (b, h, t) at x + b * x_bstride +
  *   h * L + t, writes z (and s_u) into slots [0, L), the tail, pos = {L, 0}.  One launch, bit-identical to the state L
@@ -434,6 +434,47 @@ int bffc_conv_step(const void* u, int64_t u_bstride, const void* pregate, int64_
                    void* workspace, size_t workspace_bytes, void* stream);
 
 /*
+ * Slots: the same state with one position per batch row b (a "slot"), for sequences of different lengths in one batch
+ * and new prompts admitted between steps (continuous batching).  The formulas above hold per slot, with t counted from
+ * the slot's own start.  pos: device int64 (2, B), 8-byte aligned: pos[0][b] (at pos + b) the slot's position, -1 when
+ * idle; pos[1][b] (at pos + B + b) its sticky status word.
+ *   idle (pos[0][b] = -1): a step reads nothing of the slot, writes nothing to its state, writes its y row as zeros and
+ *     does not advance it.  Idling a slot needs no library call: write -1 to pos[0][b] and 0 to pos[1][b].
+ *   active (pos[0][b] >= 0): a step of T tokens writes z (and s_u) into slots [pos_b, pos_b + T) of row b, updates b's
+ *     tail, writes y[b] and advances pos_b by T.
+ *   overflow (pos_b + T > max_len): the slot's state and position are unchanged, its y row is zeros and pos[1][b] is
+ *     set to 1; the other slots proceed.
+ * bffc_conv_state_fill_slots: n prompts (1 <= n <= B), row i (H, L) at x + i * x_bstride (element (h, t) at
+ *   + h * L + t), 0 <= L <= max_len.  Slot slots[i] gets row i's first lengths[i] positions: z (and s_u) at
+ *   [0, lengths[i]), the tail from its last K - 1 positions (zeros before 0), pos[0][b] = lengths[i], pos[1][b] = 0.
+ *   lengths[i] = 0 is an empty prompt.  Slots not listed are untouched.  slots and lengths: device int32[n], 4-byte
+ *   aligned, never read on the host (a fill can be captured in a CUDA graph) and not validated: a slot outside [0, B) is
+ *   skipped and a length is clamped to [0, L]; duplicate slots give undefined values in those slots but no access out of
+ *   bounds.  One launch.
+ * bffc_conv_step_slots: bffc_conv_step with the (2, B) position array; every slot takes T tokens (idle and overflowing
+ *   rows of x are not read).  Two launches, with a grid that depends on Lk only, so one captured step can be replayed
+ *   after admissions and releases made between replays.  Each output's summation order depends on its slot's position
+ *   and Lk only, so a slot's outputs and state are bit-identical to a B = 1 bffc_conv_step run on that slot's sequence.
+ *   workspace: bffc_conv_step_slots_workspace_bytes(B, H, T, Lk, Lk2) bytes, 16-byte aligned (a per-slot snapshot of
+ *   the positions that the second launch reads).
+ * Both check their host arguments as the calls above, and n, and null or misaligned slots / lengths, before the device
+ * is looked at (BFFC_ERR_INVALID on any machine).
+ */
+size_t bffc_conv_step_slots_workspace_bytes(int B, int H, int T, int Lk, int Lk2);
+int bffc_conv_state_fill_slots(const void* u, int64_t u_bstride, const void* pregate, int64_t pregate_bstride,
+                               const void* postgate, int64_t postgate_bstride, const void* u_w, const void* u_bias,
+                               const void* pregate_w, const void* pregate_bias, const void* postgate_w,
+                               const void* postgate_bias, int w_dtype, int K, int padding, int dtype, int B, int H,
+                               int n, int L, const int32_t* slots, const int32_t* lengths, int max_len,
+                               int has_residual, void* state, size_t state_bytes, int64_t* pos, void* stream);
+int bffc_conv_step_slots(const void* u, int64_t u_bstride, const void* pregate, int64_t pregate_bstride,
+                         const void* postgate, int64_t postgate_bstride, const void* k, int Lk, const void* k2, int Lk2,
+                         const void* u_w, const void* u_bias, const void* pregate_w, const void* pregate_bias,
+                         const void* postgate_w, const void* postgate_bias, int w_dtype, int K, int padding, int dtype,
+                         void* state, size_t state_bytes, int64_t* pos, void* y, int64_t y_bstride, int B, int H, int T,
+                         int max_len, void* workspace, size_t workspace_bytes, void* stream);
+
+/*
  * Packed documents regrouped by length class for the long convolution (no plan; INTEGRATION.md §11).  Rows (B, H, L)
  * hold several documents; a document of length l (1 <= l <= 2^21) belongs to the class c = max(128, next_pow2(l)) and is
  * convolved as one member of a (n_c, H, c) class batch by the plan of seqlen 2c with the filter k[:, :min(Lk, c)],
@@ -465,7 +506,7 @@ int bffc_docs_scatter(const void* items, int n_items, int64_t positions, int B, 
                       void* stream);
 
 /* Number of kernel launches the last bffc_fwd / bffc_bwd / bffc_fwd_host / filter-side transform /
- * bffc_dwconv1d_fwd (1) / bffc_dwconv1d_bwd (2) / bffc_conv_state_fill (1) / bffc_conv_step (2) /
+ * bffc_dwconv1d_fwd (1) / bffc_dwconv1d_bwd (2) / bffc_conv_state_fill[_slots] (1) / bffc_conv_step[_slots] (2) /
  * bffc_docs_gather (1) / bffc_docs_scatter (1) on this thread enqueued (bench.py).  A bffc_bwd* on a deterministic plan
  * counts the same launches as on a default plan, plus one slot sum per dk_f launch whose rows have S > 1 slabs. */
 int bffc_last_launch_count(void);
