@@ -18,6 +18,7 @@
 #include "filter_fft.cuh"
 #include "dwconv1d.cuh"
 #include "decode_step.cuh"
+#include "decode_far.cuh"
 #include "docs.cuh"
 
 #include <algorithm>
@@ -1880,6 +1881,20 @@ int conv_fill(const char* fn, const void* const (&x)[3], const int64_t (&bs)[3],
   return launched();
 }
 
+// the filters and the output of a step (direct or far), checked before the device is looked at
+int step_args(const char* fn, const void* k, int Lk, const void* k2, int Lk2, const void* y, int64_t y_bstride, int H,
+              int T, int max_len) {
+  if (!k || reinterpret_cast<uintptr_t>(k) % 4 || reinterpret_cast<uintptr_t>(k2) % 4)
+    return fail(BFFC_ERR_INVALID, "%s: k null, or k / k2 not 4-byte aligned", fn);
+  if (Lk < 1 || Lk > max_len) return fail(BFFC_ERR_INVALID, "%s: Lk=%d outside [1, max_len=%d]", fn, Lk, max_len);
+  if (k2 && (Lk2 < 1 || Lk2 > max_len))
+    return fail(BFFC_ERR_INVALID, "%s: Lk2=%d outside [1, max_len=%d]", fn, Lk2, max_len);
+  if (!y || reinterpret_cast<uintptr_t>(y) % 2) return fail(BFFC_ERR_INVALID, "%s: y null or not aligned to its element", fn);
+  if (y_bstride < int64_t(H) * T)
+    return fail(BFFC_ERR_INVALID, "%s: batch stride %lld below H * length = %lld", fn, (long long)y_bstride, (long long)H * T);
+  return 0;
+}
+
 // bffc_conv_step (slots false: pos is (2, 1)) and bffc_conv_step_slots (pos is (2, B))
 int conv_step(const char* fn, const void* const (&x)[3], const int64_t (&bs)[3], const void* k, int Lk, const void* k2,
               int Lk2, const void* const (&w)[3], const void* const (&bias)[3], int w_dtype, int K, int padding,
@@ -1890,15 +1905,8 @@ int conv_step(const char* fn, const void* const (&x)[3], const int64_t (&bs)[3],
   if (int rc = decode_args(fn, dtype, B, H, T, max_len, K, padding, w_dtype, x, bs, w, bias, residual, state,
                            state_bytes, pos))
     return rc;
-  if (!k || reinterpret_cast<uintptr_t>(k) % 4 || reinterpret_cast<uintptr_t>(k2) % 4)
-    return fail(BFFC_ERR_INVALID, "%s: k null, or k / k2 not 4-byte aligned", fn);
-  if (Lk < 1 || Lk > max_len) return fail(BFFC_ERR_INVALID, "%s: Lk=%d outside [1, max_len=%d]", fn, Lk, max_len);
-  if (k2 && (Lk2 < 1 || Lk2 > max_len))
-    return fail(BFFC_ERR_INVALID, "%s: Lk2=%d outside [1, max_len=%d]", fn, Lk2, max_len);
+  if (int rc = step_args(fn, k, Lk, k2, Lk2, y, y_bstride, H, T, max_len)) return rc;
   if (!k2) Lk2 = 0;
-  if (!y || reinterpret_cast<uintptr_t>(y) % 2) return fail(BFFC_ERR_INVALID, "%s: y null or not aligned to its element", fn);
-  if (y_bstride < int64_t(H) * T)
-    return fail(BFFC_ERR_INVALID, "%s: batch stride %lld below H * length = %lld", fn, (long long)y_bstride, (long long)H * T);
   const size_t need = step_workspace_bytes(B, H, T, Lk, Lk2, slots ? B : 1);
   if (!workspace || reinterpret_cast<uintptr_t>(workspace) % 16 || workspace_bytes < need)
     return fail(BFFC_ERR_INVALID, "%s: a 16-byte aligned workspace of %zu bytes required", fn, need);
@@ -1986,6 +1994,185 @@ int bffc_conv_step_slots(const void* u, int64_t u_bstride, const void* pregate, 
                    Lk, k2, Lk2, {u_w, pregate_w, postgate_w}, {u_bias, pregate_bias, postgate_bias}, w_dtype, K,
                    padding, dtype, state, state_bytes, pos, true, y, y_bstride, B, H, T, max_len, workspace,
                    workspace_bytes, stream);
+}
+
+}  // extern "C"
+
+// ------------------------------------------------------------------------------ decoding with a far field (no plan)
+namespace {
+
+namespace far = bffc::decode_far;
+
+// engine length multiple of a supported FFT size (bffc_length_multiple of its plan)
+int length_multiple_for(int n) {
+  bffc_level lev[2];
+  const int nlev = levels_for(n, lev);
+  if (nlev == 0) return 64;
+  return lev[0].tc ? n / 128 : 8;
+}
+
+// W and n of the far field of filters of Lk and Lk2 taps (decode_far.cuh): n = max(256, next_pow2(roundup(L - 1, 64) +
+// P)) with L = max(Lk, Lk2), and W + P = L - 1 + P rounded up to max(64, the length multiple of n), which stays <= n
+// because n is a multiple of it.  0, or BFFC_ERR_INVALID when n would pass 4M.
+int far_geometry(const char* fn, int Lk, int Lk2, int* W, int* n) {
+  const long long L = std::max(Lk, Lk2), P = far::kBlockOutputs;
+  const long long need = (L - 1 + 63) / 64 * 64 + P;
+  long long nn = 256;
+  while (nn < need) nn <<= 1;
+  if (nn > (1LL << 22))
+    return fail(BFFC_ERR_INVALID, "%s: filters of %lld taps need a far-field FFT of %lld > 4194304 points", fn, L, nn);
+  const long long q = std::max(64, length_multiple_for(int(nn)));
+  *W = int((L - 1 + P + q - 1) / q * q - P);
+  *n = int(nn);
+  return 0;
+}
+
+int far_gather(const char* fn, const void* state, size_t state_bytes, const int64_t* pos, int64_t* far_pos,
+               const int32_t* slots, int n, bool slot_positions, int B, int H, int max_len, int K, int has_residual,
+               int Lk, int Lk2, int dtype, void* far_u, void* far_v, void* stream) {
+  const int residual = has_residual != 0;
+  if (dtype != BFFC_DTYPE_BF16 && dtype != BFFC_DTYPE_FP16) return fail(BFFC_ERR_INVALID, "%s: dtype %d (BF16 0, FP16 1)", fn, dtype);
+  if (K < 1 || K > dec::kMaxK) return fail(BFFC_ERR_INVALID, "%s: K=%d outside [1, %d]", fn, K, dec::kMaxK);
+  if (B < 1 || H < 1 || max_len < 1) return fail(BFFC_ERR_INVALID, "%s: bad shape B=%d H=%d max_len=%d", fn, B, H, max_len);
+  if (Lk < 1 || Lk > max_len) return fail(BFFC_ERR_INVALID, "%s: Lk=%d outside [1, max_len=%d]", fn, Lk, max_len);
+  if (residual ? (Lk2 < 1 || Lk2 > max_len) : Lk2 != 0)
+    return fail(BFFC_ERR_INVALID, "%s: Lk2=%d (1..max_len=%d with a residual cache, else 0)", fn, Lk2, max_len);
+  if (slots ? (n < 1 || n > B) : n != B) return fail(BFFC_ERR_INVALID, "%s: n=%d rows (B=%d)", fn, n, B);
+  if (slots && reinterpret_cast<uintptr_t>(slots) % 4) return fail(BFFC_ERR_INVALID, "%s: slots not 4-byte aligned", fn);
+  if (!state || reinterpret_cast<uintptr_t>(state) % 16) return fail(BFFC_ERR_INVALID, "%s: state null or not 16-byte aligned", fn);
+  const size_t need = state_layout(B, H, max_len, K, residual).total;
+  if (state_bytes < need) return fail(BFFC_ERR_INVALID, "%s: state of %zu bytes required", fn, need);
+  if (!pos || reinterpret_cast<uintptr_t>(pos) % 8 || !far_pos || reinterpret_cast<uintptr_t>(far_pos) % 8)
+    return fail(BFFC_ERR_INVALID, "%s: pos / far_pos null or not 8-byte aligned", fn);
+  if (!far_u || reinterpret_cast<uintptr_t>(far_u) % 16 || (residual && (!far_v || reinterpret_cast<uintptr_t>(far_v) % 16)))
+    return fail(BFFC_ERR_INVALID, "%s: far_u (and far_v with a residual cache) null or not 16-byte aligned", fn);
+  int W = 0, nfft = 0;
+  if (int rc = far_geometry(fn, Lk, Lk2, &W, &nfft)) return rc;
+  if (int rc = check_device()) return rc;
+  const StateLayout lay = state_layout(B, H, max_len, K, residual);
+  far::Params fp{};
+  fp.d.zc = static_cast<uint8_t*>(const_cast<void*>(state)) + lay.zc;
+  fp.d.vc = residual ? static_cast<uint8_t*>(const_cast<void*>(state)) + lay.vc : nullptr;
+  fp.d.pos = reinterpret_cast<long long*>(const_cast<int64_t*>(pos));
+  fp.d.B = B; fp.d.H = H; fp.d.max_len = max_len;
+  fp.r = reinterpret_cast<long long*>(far_pos);
+  fp.W = W;
+  fp.gu = far_u;
+  fp.gv = residual ? far_v : nullptr;
+  fp.rows = slots;
+  fp.n = n;
+  const long long WP = W + far::kBlockOutputs, per_block = 8LL * dec::kThreads;
+  const dim3 grid(unsigned((WP + per_block - 1) / per_block), unsigned(std::min<long long>(1LL * n * H, kMaxGridYZ)));
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  g_launches = 0;
+  if (slot_positions) far::gather<true><<<grid, dec::kThreads, 0, st>>>(fp);
+  else far::gather<false><<<grid, dec::kThreads, 0, st>>>(fp);
+  return launched();
+}
+
+int conv_step_far(const char* fn, const void* const (&x)[3], const int64_t (&bs)[3], const void* k, int Lk,
+                  const void* k2, int Lk2, const void* const (&w)[3], const void* const (&bias)[3], int w_dtype, int K,
+                  int padding, int dtype, void* state, size_t state_bytes, int64_t* pos, const int64_t* far_pos,
+                  const void* far_y, const void* far_y2, bool slots, void* y, int64_t y_bstride, int B, int H, int T,
+                  int max_len, void* stream) {
+  const int residual = k2 != nullptr;
+  if (T < 1 || T > dec::kMaxT) return fail(BFFC_ERR_INVALID, "%s: T=%d outside [1, %d]", fn, T, dec::kMaxT);
+  if (int rc = decode_args(fn, dtype, B, H, T, max_len, K, padding, w_dtype, x, bs, w, bias, residual, state,
+                           state_bytes, pos))
+    return rc;
+  if (int rc = step_args(fn, k, Lk, k2, Lk2, y, y_bstride, H, T, max_len)) return rc;
+  if (!k2) Lk2 = 0;
+  if (!far_pos || reinterpret_cast<uintptr_t>(far_pos) % 8)
+    return fail(BFFC_ERR_INVALID, "%s: far_pos null or not 8-byte aligned", fn);
+  if (!far_y || reinterpret_cast<uintptr_t>(far_y) % 2 || (k2 && (!far_y2 || reinterpret_cast<uintptr_t>(far_y2) % 2)))
+    return fail(BFFC_ERR_INVALID, "%s: far_y (and far_y2 with k2) null or not aligned to its element", fn);
+  int W = 0, nfft = 0;
+  if (int rc = far_geometry(fn, Lk, Lk2, &W, &nfft)) return rc;
+  if (int rc = check_device()) return rc;
+  far::Params fp{};
+  fp.d = decode_params(B, H, max_len, K, residual, state, pos, x, bs, w, bias);
+  fp.d.slots = slots;
+  fp.d.w_dtype = w_dtype;                         // the far step reads the taps' dtype at run time
+  fp.d.k = static_cast<const float*>(k);
+  fp.d.k2 = static_cast<const float*>(k2);
+  fp.d.Lk = Lk; fp.d.Lk2 = Lk2;
+  fp.d.y = y; fp.d.y_bs = y_bstride; fp.d.T = T;
+  fp.r = reinterpret_cast<long long*>(const_cast<int64_t*>(far_pos));
+  fp.W = W;
+  fp.fy = far_y;
+  fp.fy2 = k2 ? far_y2 : nullptr;
+  const dim3 grid1(unsigned(std::min(B, far::kMemberGroups)), unsigned(std::min(H, kMaxGridYZ)));
+  const int cols = slots ? B : 1;
+  const unsigned grid2 = unsigned(std::min((cols + dec::kThreads - 1) / dec::kThreads, kMaxGridYZ));
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  g_launches = 0;
+  if (slots) {
+    if (dtype == BFFC_DTYPE_FP16) far::step<__half, true><<<grid1, dec::kThreads, 0, st>>>(fp);
+    else far::step<__nv_bfloat16, true><<<grid1, dec::kThreads, 0, st>>>(fp);
+  } else {
+    if (dtype == BFFC_DTYPE_FP16) far::step<__half, false><<<grid1, dec::kThreads, 0, st>>>(fp);
+    else far::step<__nv_bfloat16, false><<<grid1, dec::kThreads, 0, st>>>(fp);
+  }
+  if (int rc = launched()) return rc;
+  if (slots) far::advance<true><<<grid2, dec::kThreads, 0, st>>>(fp);
+  else far::advance<false><<<grid2, dec::kThreads, 0, st>>>(fp);
+  return launched();
+}
+
+}  // namespace
+
+extern "C" {
+
+int bffc_conv_far_layout(int B, int H, int Lk, int Lk2, int dtype, int* window, int* fft_size, size_t* buffer_bytes) {
+  const char* fn = "bffc_conv_far_layout";
+  if (dtype != BFFC_DTYPE_BF16 && dtype != BFFC_DTYPE_FP16) return fail(BFFC_ERR_INVALID, "%s: dtype %d (BF16 0, FP16 1)", fn, dtype);
+  if (B < 1 || H < 1 || Lk < 1 || Lk2 < 0)
+    return fail(BFFC_ERR_INVALID, "%s: bad shape B=%d H=%d Lk=%d Lk2=%d", fn, B, H, Lk, Lk2);
+  int W = 0, n = 0;
+  if (int rc = far_geometry(fn, Lk, Lk2, &W, &n)) return rc;
+  if (window) *window = W;
+  if (fft_size) *fft_size = n;
+  if (buffer_bytes) *buffer_bytes = size_t(B) * size_t(H) * size_t(W + far::kBlockOutputs) * 2;
+  return 0;
+}
+
+int bffc_conv_far_gather(const void* state, size_t state_bytes, const int64_t* pos, int64_t* far_pos, int B, int H,
+                         int max_len, int K, int has_residual, int Lk, int Lk2, int dtype, void* far_u, void* far_v,
+                         void* stream) {
+  return far_gather("bffc_conv_far_gather", state, state_bytes, pos, far_pos, nullptr, B, false, B, H, max_len, K,
+                    has_residual, Lk, Lk2, dtype, far_u, far_v, stream);
+}
+
+int bffc_conv_far_gather_slots(const void* state, size_t state_bytes, const int64_t* pos, int64_t* far_pos,
+                               const int32_t* slots, int n, int B, int H, int max_len, int K, int has_residual, int Lk,
+                               int Lk2, int dtype, void* far_u, void* far_v, void* stream) {
+  return far_gather("bffc_conv_far_gather_slots", state, state_bytes, pos, far_pos, slots, slots ? n : B, true, B, H,
+                    max_len, K, has_residual, Lk, Lk2, dtype, far_u, far_v, stream);
+}
+
+int bffc_conv_step_far(const void* u, int64_t u_bstride, const void* pregate, int64_t pregate_bstride,
+                       const void* postgate, int64_t postgate_bstride, const void* k, int Lk, const void* k2, int Lk2,
+                       const void* u_w, const void* u_bias, const void* pregate_w, const void* pregate_bias,
+                       const void* postgate_w, const void* postgate_bias, int w_dtype, int K, int padding, int dtype,
+                       void* state, size_t state_bytes, int64_t* pos, const int64_t* far_pos, const void* far_y,
+                       const void* far_y2, void* y, int64_t y_bstride, int B, int H, int T, int max_len, void* stream) {
+  return conv_step_far("bffc_conv_step_far", {u, pregate, postgate}, {u_bstride, pregate_bstride, postgate_bstride}, k,
+                       Lk, k2, Lk2, {u_w, pregate_w, postgate_w}, {u_bias, pregate_bias, postgate_bias}, w_dtype, K,
+                       padding, dtype, state, state_bytes, pos, far_pos, far_y, far_y2, false, y, y_bstride, B, H, T,
+                       max_len, stream);
+}
+
+int bffc_conv_step_far_slots(const void* u, int64_t u_bstride, const void* pregate, int64_t pregate_bstride,
+                             const void* postgate, int64_t postgate_bstride, const void* k, int Lk, const void* k2,
+                             int Lk2, const void* u_w, const void* u_bias, const void* pregate_w,
+                             const void* pregate_bias, const void* postgate_w, const void* postgate_bias, int w_dtype,
+                             int K, int padding, int dtype, void* state, size_t state_bytes, int64_t* pos,
+                             const int64_t* far_pos, const void* far_y, const void* far_y2, void* y, int64_t y_bstride,
+                             int B, int H, int T, int max_len, void* stream) {
+  return conv_step_far("bffc_conv_step_far_slots", {u, pregate, postgate}, {u_bstride, pregate_bstride, postgate_bstride},
+                       k, Lk, k2, Lk2, {u_w, pregate_w, postgate_w}, {u_bias, pregate_bias, postgate_bias}, w_dtype, K,
+                       padding, dtype, state, state_bytes, pos, far_pos, far_y, far_y2, true, y, y_bstride, B, H, T,
+                       max_len, stream);
 }
 
 }  // extern "C"

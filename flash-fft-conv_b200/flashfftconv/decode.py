@@ -46,6 +46,22 @@ different lengths share one batch and a freed row takes the next request while t
 
 Each slot's outputs and state are bit for bit those of a one-row decoder run on that slot's own sequence.  A captured
 step can be replayed after eager admissions and releases made on the stream the replays run on.
+
+Far field (far_field=True, either decoder, with or without slots): a step's cost stops growing with the context.  At a
+refresh point r_b the contributions of positions j < r_b to the next FAR_BLOCK = 2048 outputs are computed at once by
+one FlashFFTConv(n) forward (the far field); the step then sums only the lags back to r_b (the near field), at most
+2048 of them (bffc_conv_far_gather / bffc_conv_step_far, include/bffc.h, INTEGRATION.md §9.4):
+
+    dec = HyenaDecoder(short_filter, k, d_model, batch, max_len, far_field=True)
+    y = dec.prefill(x)                           # fills the caches, then refreshes
+    y_new = dec.step(x_new)                      # refreshes first whenever a member would pass r_b + 2048
+
+A refresh costs about one FFT convolution of n = max(256, next_pow2(W + 2048)) points, W >= Lk - 1; filters that need
+n > 4M are refused at construction.  Outputs differ from the direct step by the engine's FFT error once a refresh has
+run (before it, the far field is zero and the outputs are the direct step's bits).  With the same refresh points,
+grouping tokens into steps changes no bit.  For graphs, capture a step and a refresh (after one eager refresh) and
+replay the refresh at least every floor(2048 / T) steps and after every admission; a replayed step past the far field
+does nothing for that member and sets a status that `pos` / `positions` report.
 """
 import ctypes
 
@@ -53,12 +69,13 @@ import torch
 
 from . import _lib
 from . import depthwise_1d as _dw
-from .conv import FlashFFTConv, _DT, _on_device, _ptr, _stream
+from .conv import FlashFFTConv, _DT, _fwd, _on_device, _ptr, _stream
 from .docs import refuse
 from .gated import gated_long_conv, hyena_mixer, hyena_operator
 
 MAX_STEP_TOKENS = 64
 MAX_KERNEL_SIZE = 32
+FAR_BLOCK = 2048            # outputs per far-field refresh (decode_far.cuh kBlockOutputs)
 
 
 def prefill_seqlen(L, Lk):
@@ -75,6 +92,17 @@ def state_layout(B, H, max_len, K, residual):
     zc = a256(6 * B * H * (K - 1))
     vc = zc + a256(2 * B * H * max_len)
     return zc, vc, vc + (vc - zc if residual else 0)
+
+
+def far_layout(batch, H, Lk, Lk2, dtype):
+    """(W, n, bytes of one (batch, H, W + FAR_BLOCK) buffer) of the far field of filters of Lk and Lk2 taps (Lk2 = 0
+    without a residual filter), from bffc_conv_far_layout.  ValueError when the filters need an FFT past 4M points."""
+    W, n, nbytes = ctypes.c_int(), ctypes.c_int(), ctypes.c_size_t()
+    rc = _lib.lib().bffc_conv_far_layout(int(batch), int(H), int(Lk), int(Lk2), _DT[dtype], ctypes.byref(W),
+                                         ctypes.byref(n), ctypes.byref(nbytes))
+    if rc:
+        raise ValueError(f'far_field=True: {_lib.lib().bffc_last_error().decode()}')
+    return W.value, n.value, nbytes.value
 
 
 def _host_ints(v, name):
@@ -122,12 +150,16 @@ def _filter(k, H, max_len, name):
 class _Decoder:
     """The state of one batch of sequences and the two library calls; the subclasses name the roles."""
 
-    def __init__(self, k, k2, H, batch, max_len, dtype, K, slots=False):
+    def __init__(self, k, k2, H, batch, max_len, dtype, K, slots=False, far_field=False):
         if dtype not in _DT:
             raise ValueError(f'dtype must be torch.bfloat16 or torch.float16, got {dtype}')
         if batch < 1 or max_len < 1:
             raise ValueError(f'batch {batch} and max_len {max_len} must be >= 1')
         self.H, self.batch, self.max_len, self.dtype, self.K = H, int(batch), int(max_len), dtype, K
+        self.far_field = bool(far_field)
+        if self.far_field and k.dim() == 2 and (k2 is None or k2.dim() == 2):    # other shapes: _filter says why
+            Lk2 = 0 if k2 is None else k2.shape[1]
+            self.far_window, self.far_fft_size, _ = far_layout(self.batch, H, k.shape[1], Lk2, dtype)
         self.k = _filter(k, H, self.max_len, 'k')
         self.k2 = None if k2 is None else _filter(k2, H, self.max_len, 'residual_filter')
         self.device = self.k.device
@@ -143,6 +175,8 @@ class _Decoder:
         # workspaces outgrown by a larger T: a graph captured earlier still writes to the address it was given
         self._ws_outgrown = []
         self._convs = {}
+        if self.far_field:
+            self._far_init()
         self.reset()
 
     # ---- views of the state (include/bffc.h: tail, z cache, s_u cache)
@@ -177,6 +211,10 @@ class _Decoder:
         if self.slots:
             raise RuntimeError('a slot decoder keeps one position per slot: read `positions`')
         pos, status = self._pos.tolist()
+        if status == 2:
+            raise RuntimeError(f'a decoding step would have run past the far field ({FAR_BLOCK} positions after the last '
+                               f'refresh) and did nothing; the position is still {pos}.  Replay refresh() at least every '
+                               f'{FAR_BLOCK} // T steps')
         if status:
             raise RuntimeError(f'a decoding step would have run past max_len = {self.max_len} and did nothing; '
                                f'the position is still {pos}')
@@ -191,6 +229,11 @@ class _Decoder:
         if not self.slots:
             raise RuntimeError('positions is for a decoder made with slots=True; read `pos`')
         pos, status = self._pos.tolist()
+        far = [b for b, s in enumerate(status) if s == 2]
+        if far:
+            raise RuntimeError(f'slots {far} would have run past their far field ({FAR_BLOCK} positions after their '
+                               f'last refresh) and kept their state; their positions are {[pos[b] for b in far]}.  '
+                               f'Replay refresh() at least every {FAR_BLOCK} // T steps and after every admission')
         bad = [b for b, s in enumerate(status) if s]
         if bad:
             raise RuntimeError(f'slots {bad} would have run past max_len = {self.max_len} and kept their state; their '
@@ -262,8 +305,104 @@ class _Decoder:
             self._pos[0].fill_(-1)
             self._pos[1].zero_()
             self._host_pos = [-1] * self.batch
+            if self.far_field:
+                self._far_pos.fill_(-1)
+                self._host_r = [-1] * self.batch
             return
         self._fill(None, None, None, 0)
+        if self.far_field:                 # no past: the refresh point is 0 and the far field zero, without an FFT
+            self._far_pos.zero_()
+            for o in self._far_out:
+                o[..., self.far_window:].zero_()
+            self._host_r = 0
+
+    # ---- far field (decode_far.cuh)
+    def _far_init(self):
+        """the persistent far inputs and outputs (one pair per filter, (B, H, W + FAR_BLOCK)), the refresh points and
+        one FlashFFTConv(n) per filter, whose eval-mode cache holds the filter's spectrum"""
+        shape = (self.batch, self.H, self.far_window + FAR_BLOCK)
+        nf = 1 if self.k2 is None else 2
+        self._far_in = [torch.empty(shape, dtype=self.dtype, device=self.device) for _ in range(nf)]
+        self._far_out = [torch.zeros(shape, dtype=self.dtype, device=self.device) for _ in range(nf)]
+        self._far_pos = torch.zeros(self.batch if self.slots else 1, dtype=torch.int64, device=self.device)
+        self._far_convs = [FlashFFTConv(self.far_fft_size, dtype=self.dtype).eval() for _ in range(nf)]
+        # spectra of k (and k2) of the latest eager transform: a captured refresh reads them, so that it does not wait
+        # on the eager-mode cache's event from outside the capture
+        self._far_kf = [None] * nf
+        self._host_r = None                # known refresh points (a list per slot with slots), or None
+
+    def _far_gather(self, slots, n, ins):
+        """bffc_conv_far_gather[_slots]: rows of the engine inputs from the caches, refresh points from the positions"""
+        l, B, H = _lib.lib(), self.batch, self.H
+        Lk2 = 0 if self.k2 is None else self.k2.shape[1]
+        common = (B, H, self.max_len, self.K, int(self.k2 is not None), self.k.shape[1], Lk2, _DT[self.dtype],
+                  _ptr(ins[0]), _ptr(ins[1] if len(ins) > 1 else None), _stream())
+        with _on_device(self.device):
+            if self.slots:
+                rc = l.bffc_conv_far_gather_slots(_ptr(self.state), self.state.numel(), _ptr(self._pos),
+                                                  _ptr(self._far_pos), _ptr(slots), n, *common)
+            else:
+                rc = l.bffc_conv_far_gather(_ptr(self.state), self.state.numel(), _ptr(self._pos),
+                                            _ptr(self._far_pos), *common)
+            _lib.check(rc)
+
+    def _far_transform(self, ins, outs):
+        capturing = torch.cuda.is_current_stream_capturing()
+        for i, (conv, k, x, y) in enumerate(zip(self._far_convs, (self.k, self.k2), ins, outs)):
+            _, kf = _fwd(conv, x, k, None, None, kf_engine=self._far_kf[i] if capturing else None, out=y)
+            if not capturing:
+                self._far_kf[i] = kf
+
+    @torch.no_grad()
+    def refresh(self):
+        """Recompute the far field of every active member at its current position (its refresh point becomes its
+        position), on the device: the positions are read there, so a refresh can be captured in a CUDA graph once one
+        eager refresh has made the FFT plan and the filter spectra.  Idle slots are gathered as zero rows."""
+        if not self.far_field:
+            raise RuntimeError('refresh is for a decoder made with far_field=True')
+        capturing = torch.cuda.is_current_stream_capturing()
+        if capturing and self._far_kf[0] is None:
+            raise RuntimeError('the far field\'s FFT plan and filter spectra are made on first use, which cannot happen '
+                               'during CUDA-graph capture: run one eager refresh() (or prefill) before capturing one')
+        self._far_gather(None, self.batch, self._far_in)
+        self._far_transform(self._far_in, self._far_out)
+        if capturing or self._host_pos is None:
+            self._host_r = None
+        elif self.slots:
+            self._host_r = list(self._host_pos)
+        else:
+            self._host_r = self._host_pos
+
+    def _far_admit(self, slots, lengths):
+        """refresh the admitted slots only: their rows gathered, transformed and copied into their slots' rows"""
+        idx = _device_ints(slots, torch.int64, self.device)
+        if not any(lengths):               # no past: refresh point 0 and a zero far field, without an FFT
+            self._far_pos.index_fill_(0, idx, 0)
+            for o in self._far_out:
+                o.index_fill_(0, idx, 0)
+        else:
+            n = len(slots)
+            ins = [x[:n] for x in self._far_in]            # scratch: a refresh gathers every row again
+            self._far_gather(_device_ints(slots, torch.int32, self.device), n, ins)
+            outs = [torch.empty_like(x) for x in ins]
+            self._far_transform(ins, outs)
+            for o, t in zip(self._far_out, outs):
+                o.index_copy_(0, idx, t)
+        if self._host_r is not None:
+            for b, l in zip(slots, lengths):
+                self._host_r[b] = l
+
+    def _far_sync(self):
+        """the host mirrors of the positions and refresh points, read back once when a capture made them unknown"""
+        if self._host_pos is None or self._host_r is None:
+            pos, r = self._pos.tolist(), self._far_pos.tolist()
+            self._host_pos, self._host_r = (list(pos[0]), list(r)) if self.slots else (pos[0], r[0])
+
+    def _far_before_step(self, T):
+        """an eager step's refresh: when some active member would pass its far field"""
+        pairs = zip(self._host_pos, self._host_r) if self.slots else [(self._host_pos, self._host_r)]
+        if any(p >= 0 and not 0 <= r <= p <= r + FAR_BLOCK - T for p, r in pairs):
+            self.refresh()
 
     def _conv(self, L):
         n = prefill_seqlen(L, max(self.k.shape[1], 0 if self.k2 is None else self.k2.shape[1]))
@@ -320,12 +459,16 @@ class _Decoder:
         if self._host_pos is not None:
             for b, l in zip(slots, lengths):
                 self._host_pos[b] = l
+        if self.far_field:
+            self._far_admit(slots, lengths)
 
     def _step(self, u, pregate, postgate):
         T = u.shape[-1]
         if not 1 <= T <= MAX_STEP_TOKENS:
             raise ValueError(f'a step takes 1 to {MAX_STEP_TOKENS} tokens, got {T} (a longer chunk is a prefill)')
         capturing = torch.cuda.is_current_stream_capturing()
+        if self.far_field and not capturing:
+            self._far_sync()                   # the checks below and the refresh need the host mirrors
         if self._host_pos is not None and not capturing:
             if self.slots:
                 over = [b for b, p in enumerate(self._host_pos) if p >= 0 and p + T > self.max_len]
@@ -338,6 +481,8 @@ class _Decoder:
         rows, wdt = self._tap_args()
         Lk = self.k.shape[1]
         Lk2 = 0 if self.k2 is None else self.k2.shape[1]
+        if self.far_field:
+            return self._step_far(roles, rows, wdt, T, Lk, Lk2, capturing)
         nws = (_lib.lib().bffc_conv_step_slots_workspace_bytes if self.slots else
                _lib.lib().bffc_conv_step_workspace_bytes)(self.batch, self.H, T, Lk, Lk2)
         if self._ws is None or self._ws.numel() < nws:
@@ -354,12 +499,30 @@ class _Decoder:
                           _DT[self.dtype], _ptr(self.state), self.state.numel(), _ptr(self._pos), _ptr(y),
                           self.H * T, self.batch, self.H, T, self.max_len, _ptr(self._ws), self._ws.numel(),
                           _stream()))
+        self._advance_host(T, capturing)
+        return y
+
+    def _advance_host(self, T, capturing):
         if capturing or self._host_pos is None:
             self._host_pos = None
         elif self.slots:
             self._host_pos = [p + T if p >= 0 else p for p in self._host_pos]
         else:
             self._host_pos += T
+
+    def _step_far(self, roles, rows, wdt, T, Lk, Lk2, capturing):
+        if not capturing:
+            self._far_before_step(T)
+        y = torch.empty((self.batch, self.H, T), dtype=self.dtype, device=self.device)
+        args = [a for t, s in roles for a in (_ptr(t), s)]
+        fo = self._far_out
+        fn = _lib.lib().bffc_conv_step_far_slots if self.slots else _lib.lib().bffc_conv_step_far
+        with _on_device(self.device):
+            _lib.check(fn(*args, _ptr(self.k), Lk, _ptr(self.k2), Lk2, *rows, wdt, self.K, self.K - 1,
+                          _DT[self.dtype], _ptr(self.state), self.state.numel(), _ptr(self._pos), _ptr(self._far_pos),
+                          _ptr(fo[0]), _ptr(fo[1] if len(fo) > 1 else None), _ptr(y), self.H * T, self.batch, self.H,
+                          T, self.max_len, _stream()))
+        self._advance_host(T, capturing)
         return y
 
 
@@ -376,10 +539,12 @@ class HyenaDecoder(_Decoder):
         y = x2 * causal_conv(x1 * v, k) [+ causal_conv(v, k2)]
 
     slots=True: one position per batch row (see the module docstring); every slot starts idle.
+    far_field=True: steps sum at most 2048 lags and a refresh every 2048 positions adds the rest by one FFT (see the
+    module docstring); filters that need an FFT past 4M points are refused.
     """
 
     def __init__(self, short_filter, k, d_model, batch, max_len, residual_filter=None, dtype=torch.bfloat16,
-                 slots=False):
+                 slots=False, far_field=False):
         if not isinstance(short_filter, _dw.FlashDepthWiseConv1d) or not short_filter.is_bhl:
             raise ValueError('short_filter must be a BHL FlashDepthWiseConv1d')
         if short_filter.d != 3 * d_model:
@@ -392,7 +557,7 @@ class HyenaDecoder(_Decoder):
             raise ValueError(f'short filter padding {P}: decoding needs the causal padding K - 1 = {K - 1} (padding '
                              f'{P} makes each output read {K - 1 - P} input(s) after its position)')
         self.short_filter, self.d_model = short_filter, d_model
-        super().__init__(k, residual_filter, d_model, batch, max_len, dtype, K, slots)
+        super().__init__(k, residual_filter, d_model, batch, max_len, dtype, K, slots, far_field)
         self._tap_args()
 
     def _tap_args(self):
@@ -440,6 +605,8 @@ class HyenaDecoder(_Decoder):
         k2 = None if self.k2 is None else self.k2[:, :min(self.k2.shape[1], L)]
         y = hyena_operator(self._conv(L), self.short_filter, x, k, self.d_model, residual_filter=k2)
         self._fill(v, x1, x2, L)
+        if self.far_field:
+            self.refresh()
         return y
 
     def _prefill_slots(self, x, lengths, slots):
@@ -477,11 +644,12 @@ class LongConvDecoder(_Decoder):
     decoded position by position.  k: (H, Lk), Lk <= max_len, taken at construction as contiguous fp32 (k itself when
     it already is, else a converted copy).  The gates given to prefill are the gates every step takes: z = u * pregate
     and z = u must not mix in one cache, so a step with another set of gates is refused.  With slots=True (one
-    position per batch row, see the module docstring) every slot shares the gate set of the first prefill or step."""
+    position per batch row, see the module docstring) every slot shares the gate set of the first prefill or step.
+    far_field=True: the far-field step (see the module docstring)."""
 
-    def __init__(self, k, batch, max_len, dtype=torch.bfloat16, slots=False):
+    def __init__(self, k, batch, max_len, dtype=torch.bfloat16, slots=False, far_field=False):
         self._gates = None                 # (pregate given, postgate given) of this sequence, once known
-        super().__init__(k, None, k.shape[0], batch, max_len, dtype, 1, slots)
+        super().__init__(k, None, k.shape[0], batch, max_len, dtype, 1, slots, far_field)
 
     def _same_gates(self, pregate, postgate):
         gates = (pregate is not None, postgate is not None)
@@ -527,6 +695,8 @@ class LongConvDecoder(_Decoder):
             ones = torch.ones_like(u)
             y = gated_long_conv(conv, u, k, ones if pregate is None else pregate, ones if postgate is None else postgate)
         self._fill(u, pregate, postgate, L)
+        if self.far_field:
+            self.refresh()
         return y
 
     def _prefill_slots(self, u, pregate, postgate, lengths, slots):

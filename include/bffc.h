@@ -475,6 +475,51 @@ int bffc_conv_step_slots(const void* u, int64_t u_bstride, const void* pregate, 
                          int max_len, void* workspace, size_t workspace_bytes, void* stream);
 
 /*
+ * Far field: a step whose cost does not grow with the context (INTEGRATION.md §9.4).  Each position column c has a
+ * refresh point r_c (far_pos: device int64 (P), 8-byte aligned; P = 1 for the shared position, B for slots).  With
+ * P_blk = 2048 outputs per refresh, an output t of member b in [r_b, r_b + P_blk) is
+ *     y[t] = round( s_postgate[t] * (F[t - r_b] + sum_{m=0}^{min(t - r_b, Lk-1)} k[m] z[t-m])
+ *                   + F2[t - r_b] + sum_{m=0}^{min(t - r_b, Lk2-1)} k2[m] s_u[t-m] )
+ * where F[i] = far_y[b, h, W + i] is the engine's FlashFFTConv(n) forward of what bffc_conv_far_gather wrote
+ * (F2: far_y2, with k2), read as fp32.  That is sum_{j < r_b} k[r_b + i - j] z[j] up to the engine's error.
+ * bffc_conv_far_layout: W (>= Lk - 1, with W + 2048 a multiple of the length multiple of n), the FFT size
+ *   n = max(256, next_pow2(roundup(max(Lk, Lk2) - 1, 64) + 2048)) and the bytes of one (B, H, W + 2048) 16-bit buffer
+ *   (the caller needs one input and one output per filter).  BFFC_ERR_INVALID when n would pass 4194304.
+ * bffc_conv_far_gather[_slots]: r_c = pos[0][c] (-1 for an idle slot) and the engine inputs far_u (from the z cache)
+ *   and far_v (from the s_u cache, with has_residual), (rows, H, W + 2048) 16-bit, 16-byte aligned:
+ *   far_u[i, h, j] = z[b, h, r_b - W + j] for j < W and r_b - W + j >= 0, else 0 (every element of an idle member's
+ *   row is 0).  Row i is member i (n = B; the _slots call with slots NULL) or member slots[i] (the _slots call, n rows,
+ *   a device int32[n] never read on the host; a slot outside [0, B) gives a zero row and sets nothing).  One launch.
+ * bffc_conv_step_far[_slots]: bffc_conv_step[_slots] with the far field; no workspace.  A member takes part when it
+ *   is active and r_b <= pos_b, pos_b + T - r_b <= 2048.  One that would run past its far field keeps its state and
+ *   position and sets its status word to 2 (slots: its y row is zeros; shared: nothing is written); past max_len it
+ *   sets 1 as before.  With r_b = 0 and F = F2 = 0 the outputs are bffc_conv_step's bits.  Two launches; the grid
+ *   depends on B and H only.
+ * Host arguments are checked before the device is looked at (BFFC_ERR_INVALID on any machine); far_pos and the slot
+ * list are never read on the host, so every call can be captured in a CUDA graph.
+ */
+int bffc_conv_far_layout(int B, int H, int Lk, int Lk2, int dtype, int* window, int* fft_size, size_t* buffer_bytes);
+int bffc_conv_far_gather(const void* state, size_t state_bytes, const int64_t* pos, int64_t* far_pos, int B, int H,
+                         int max_len, int K, int has_residual, int Lk, int Lk2, int dtype, void* far_u, void* far_v,
+                         void* stream);
+int bffc_conv_far_gather_slots(const void* state, size_t state_bytes, const int64_t* pos, int64_t* far_pos,
+                               const int32_t* slots, int n, int B, int H, int max_len, int K, int has_residual, int Lk,
+                               int Lk2, int dtype, void* far_u, void* far_v, void* stream);
+int bffc_conv_step_far(const void* u, int64_t u_bstride, const void* pregate, int64_t pregate_bstride,
+                       const void* postgate, int64_t postgate_bstride, const void* k, int Lk, const void* k2, int Lk2,
+                       const void* u_w, const void* u_bias, const void* pregate_w, const void* pregate_bias,
+                       const void* postgate_w, const void* postgate_bias, int w_dtype, int K, int padding, int dtype,
+                       void* state, size_t state_bytes, int64_t* pos, const int64_t* far_pos, const void* far_y,
+                       const void* far_y2, void* y, int64_t y_bstride, int B, int H, int T, int max_len, void* stream);
+int bffc_conv_step_far_slots(const void* u, int64_t u_bstride, const void* pregate, int64_t pregate_bstride,
+                             const void* postgate, int64_t postgate_bstride, const void* k, int Lk, const void* k2,
+                             int Lk2, const void* u_w, const void* u_bias, const void* pregate_w,
+                             const void* pregate_bias, const void* postgate_w, const void* postgate_bias, int w_dtype,
+                             int K, int padding, int dtype, void* state, size_t state_bytes, int64_t* pos,
+                             const int64_t* far_pos, const void* far_y, const void* far_y2, void* y, int64_t y_bstride,
+                             int B, int H, int T, int max_len, void* stream);
+
+/*
  * Packed documents regrouped by length class for the long convolution (no plan; INTEGRATION.md §11).  Rows (B, H, L)
  * hold several documents; a document of length l (1 <= l <= 2^21) belongs to the class c = max(128, next_pow2(l)) and is
  * convolved as one member of a (n_c, H, c) class batch by the plan of seqlen 2c with the filter k[:, :min(Lk, c)],
@@ -507,7 +552,8 @@ int bffc_docs_scatter(const void* items, int n_items, int64_t positions, int B, 
 
 /* Number of kernel launches the last bffc_fwd / bffc_bwd / bffc_fwd_host / filter-side transform /
  * bffc_dwconv1d_fwd (1) / bffc_dwconv1d_bwd (2) / bffc_conv_state_fill[_slots] (1) / bffc_conv_step[_slots] (2) /
- * bffc_docs_gather (1) / bffc_docs_scatter (1) on this thread enqueued (bench.py).  A bffc_bwd* on a deterministic plan
+ * bffc_conv_far_gather[_slots] (1) / bffc_conv_step_far[_slots] (2) / bffc_docs_gather (1) / bffc_docs_scatter (1)
+ * on this thread enqueued (bench.py).  A bffc_bwd* on a deterministic plan
  * counts the same launches as on a default plan, plus one slot sum per dk_f launch whose rows have S > 1 slabs. */
 int bffc_last_launch_count(void);
 
