@@ -381,14 +381,18 @@ int bffc_plan_create_ex(bffc_plan** out, int seqlen, int dtype, int flags, int m
     PLAN_TRY(cudaFuncSetAttribute(outer_tc_kernel<false, F>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemOuter));
     PLAN_TRY(cudaFuncSetAttribute(outer_tc_kernel<true, F>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemOuter));
     PLAN_TRY(cudaFuncSetAttribute(bffc::ffft::kf_from_filter_kernel<F>, cudaFuncAttributeMaxDynamicSharedMemorySize, bffc::ffft::kSmemBytes));
+    PLAN_TRY(cudaFuncSetAttribute(bffc::ffft::kf_from_filter_kernel<F, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, bffc::ffft::kSmemBytes));
   );
-  PLAN_TRY(cudaFuncSetAttribute(bffc::ffft::dk_from_dkf_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bffc::ffft::kSmemBytes));
+  PLAN_TRY(cudaFuncSetAttribute(bffc::ffft::dk_from_dkf_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, bffc::ffft::kSmemBytes));
+  PLAN_TRY(cudaFuncSetAttribute(bffc::ffft::dk_from_dkf_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, bffc::ffft::kSmemBytes));
   if (p->NE > kInner) {
     using namespace bffc::ffft;
     FMT_SWITCH(dtype, PLAN_TRY(cudaFuncSetAttribute(filter_rows_kernel<F>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes)););
     PLAN_TRY(cudaFuncSetAttribute(dk_rows_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes));
     COLS_SWITCH(p->R, PLAN_TRY(cudaFuncSetAttribute(filter_cols_kernel<RR>, cudaFuncAttributeMaxDynamicSharedMemorySize, ColRadix<RR>::kSmem));
-                      PLAN_TRY(cudaFuncSetAttribute(dk_cols_kernel<RR>, cudaFuncAttributeMaxDynamicSharedMemorySize, ColRadix<RR>::kSmem)););
+                      PLAN_TRY(cudaFuncSetAttribute(filter_cols_kernel<RR, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, ColRadix<RR>::kSmem));
+                      PLAN_TRY(cudaFuncSetAttribute(dk_cols_kernel<RR>, cudaFuncAttributeMaxDynamicSharedMemorySize, ColRadix<RR>::kSmem));
+                      PLAN_TRY(cudaFuncSetAttribute(dk_cols_kernel<RR, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, ColRadix<RR>::kSmem)););
   }
   // streams / events of bffc_fwd_host (copy-in, compute, copy-out; per-slot events)
   for (auto& st : p->hs) PLAN_TRY(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
@@ -455,19 +459,44 @@ static int filter_group(size_t pairs, int H) {
 // band that keeps every frequency of the plan's seqlen grid (min(f, N - f) <= N/2 < band)
 static int full_band(const bffc_plan* p) { return p->N / 2 + 1; }
 
-// bffc_kf_from_filter / bffc_kf_from_filter_band
+// two-sided lag map of bffc_kf_from_filter_lags / bffc_dk_from_dkf_lags: host checks, then the map the kernels take
+static int check_lags(const bffc_plan* p, int Lk, int period, int pos, int neg, const char* name) {
+  if (pos < 0 || neg < 0 || period < 0)
+    return fail(BFFC_ERR_INVALID, "%s: negative lag bound (period=%d pos=%d neg=%d)", name, period, pos, neg);
+  if (int64_t(pos) + neg > int64_t(p->N) - 1)
+    return fail(BFFC_ERR_INVALID, "%s: pos + neg = %lld exceeds seqlen - 1 = %d", name, (long long)pos + neg, p->N - 1);
+  if (neg > period) return fail(BFFC_ERR_INVALID, "%s: neg=%d exceeds period=%d", name, neg, period);
+  if (Lk > period) return fail(BFFC_ERR_INVALID, "%s: Lk=%d exceeds period=%d", name, Lk, period);
+  // composite sizes: a k index read both as lag m and as lag m - period must find both slots in one column of the
+  // column transform (dk_cols_kernel), i.e. seqlen - period a multiple of 8192
+  const int lo = std::max(period - neg, 0), hi = std::min(pos, Lk);
+  if (p->NE > kInner && lo < hi && (p->N - period) % kInner != 0)
+    return fail(BFFC_ERR_INVALID, "%s: k[%d, %d) is read at both ends, which needs seqlen - period (%d) to be a multiple "
+                "of %d", name, lo, hi, p->N - period, kInner);
+  return BFFC_OK;
+}
+
+// bffc_kf_from_filter / bffc_kf_from_filter_band / bffc_kf_from_filter_lags (lags: NULL for the plain map, slot d < Lk
+// from k[d])
 static int kf_from_filter(const bffc_plan* p, const void* k, int Lk, void* kf_engine, int H, int conj, int band,
-                          void* workspace, size_t workspace_bytes, void* stream, const char* name) {
+                          const bffc::ffft::Lags* lags, void* workspace, size_t workspace_bytes, void* stream,
+                          const char* name) {
   if (!p || !k || !kf_engine || H <= 0 || Lk <= 0) return fail(BFFC_ERR_INVALID, "%s: bad argument", name);
   if (band < 0) return fail(BFFC_ERR_INVALID, "%s: band=%d is negative", name, band);
-  if (Lk > p->N) return fail(BFFC_ERR_INVALID, "%s: Lk=%d exceeds seqlen %d", name, Lk, p->N);
+  if (!lags && Lk > p->N) return fail(BFFC_ERR_INVALID, "%s: Lk=%d exceeds seqlen %d", name, Lk, p->N);
   using namespace bffc::ffft;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const Lags lg = lags ? *lags : Lags{};
   g_launches = 0;
   if (p->NE == kInner) {
-    FMT_SWITCH(p->dtype, (kf_from_filter_kernel<F><<<(H + 1) / 2, kThreads, kSmemBytes, st>>>(
-        static_cast<const float*>(k), Lk, static_cast<uint4*>(kf_engine), H, p->kf_pack_scale, conj, p->tw8192, p->N,
-        band)););
+    if (lags)
+      FMT_SWITCH(p->dtype, (kf_from_filter_kernel<F, true><<<(H + 1) / 2, kThreads, kSmemBytes, st>>>(
+          static_cast<const float*>(k), Lk, static_cast<uint4*>(kf_engine), H, p->kf_pack_scale, conj, p->tw8192, p->N,
+          band, lg)););
+    else
+      FMT_SWITCH(p->dtype, (kf_from_filter_kernel<F><<<(H + 1) / 2, kThreads, kSmemBytes, st>>>(
+          static_cast<const float*>(k), Lk, static_cast<uint4*>(kf_engine), H, p->kf_pack_scale, conj, p->tw8192, p->N,
+          band, lg)););
     return launched();
   }
   const size_t per = filter_pair_bytes(p);
@@ -479,8 +508,12 @@ static int kf_from_filter(const bffc_plan* p, const void* k, int Lk, void* kf_en
     const int Hc = std::min(group, H - h0);
     const float* kc = static_cast<const float*>(k) + size_t(h0) * Lk;
     uint4* out = static_cast<uint4*>(kf_engine) + size_t(h0) * (p->NE / 4);
-    COLS_SWITCH(p->R, (filter_cols_kernel<RR><<<dim3(kInner / ColRadix<RR>::kTC, (Hc + 1) / 2), kColThreads, ColRadix<RR>::kSmem, st>>>(
-        kc, Lk, T, Hc, p->kf_pack_scale, p->tw512, p->tw_lo, p->tw_hi)););
+    if (lags)
+      COLS_SWITCH(p->R, (filter_cols_kernel<RR, true><<<dim3(kInner / ColRadix<RR>::kTC, (Hc + 1) / 2), kColThreads, ColRadix<RR>::kSmem, st>>>(
+          kc, Lk, T, Hc, p->kf_pack_scale, p->tw512, p->tw_lo, p->tw_hi, lg)););
+    else
+      COLS_SWITCH(p->R, (filter_cols_kernel<RR><<<dim3(kInner / ColRadix<RR>::kTC, (Hc + 1) / 2), kColThreads, ColRadix<RR>::kSmem, st>>>(
+          kc, Lk, T, Hc, p->kf_pack_scale, p->tw512, p->tw_lo, p->tw_hi, lg)););
     if (int rc = launched()) return rc;
     FMT_SWITCH(p->dtype, (filter_rows_kernel<F><<<dim3(p->R / 2 + 1, Hc), kThreads, kSmemBytes, st>>>(
         T, out, p->R, p->R0, p->R1, conj, p->tw8192, band)););
@@ -489,18 +522,26 @@ static int kf_from_filter(const bffc_plan* p, const void* k, int Lk, void* kf_en
   return BFFC_OK;
 }
 
-// bffc_dk_from_dkf / bffc_dk_from_dkf_band
-static int dk_from_dkf(const bffc_plan* p, const void* dkf_engine, void* dk, int Lk, int H, int band, void* workspace,
-                       size_t workspace_bytes, void* stream, const char* name) {
+// bffc_dk_from_dkf / bffc_dk_from_dkf_band / bffc_dk_from_dkf_lags (lags: NULL writes dk[m] = g[m], else dk accumulates
+// through the map)
+static int dk_from_dkf(const bffc_plan* p, const void* dkf_engine, void* dk, int Lk, int H, int band,
+                       const bffc::ffft::Lags* lags, void* workspace, size_t workspace_bytes, void* stream,
+                       const char* name) {
   if (!p || !dkf_engine || !dk || H <= 0 || Lk <= 0) return fail(BFFC_ERR_INVALID, "%s: bad argument", name);
   if (band < 0) return fail(BFFC_ERR_INVALID, "%s: band=%d is negative", name, band);
-  if (Lk > p->N) return fail(BFFC_ERR_INVALID, "%s: Lk=%d exceeds seqlen %d", name, Lk, p->N);
+  if (!lags && Lk > p->N) return fail(BFFC_ERR_INVALID, "%s: Lk=%d exceeds seqlen %d", name, Lk, p->N);
   using namespace bffc::ffft;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const Lags lg = lags ? *lags : Lags{};
   g_launches = 0;
   if (p->NE == kInner) {
-    dk_from_dkf_kernel<<<H, kThreads, kSmemBytes, st>>>(static_cast<const float2*>(dkf_engine), static_cast<float*>(dk), Lk,
-                                                         p->dk_scale, p->N, p->tw8192, band);
+    if (lags)
+      dk_from_dkf_kernel<true><<<H, kThreads, kSmemBytes, st>>>(static_cast<const float2*>(dkf_engine),
+                                                                static_cast<float*>(dk), Lk, p->dk_scale, p->N,
+                                                                p->tw8192, band, lg);
+    else
+      dk_from_dkf_kernel<false><<<H, kThreads, kSmemBytes, st>>>(static_cast<const float2*>(dkf_engine), static_cast<float*>(dk), Lk,
+                                                           p->dk_scale, p->N, p->tw8192, band, lg);
     return launched();
   }
   const size_t per = filter_pair_bytes(p);
@@ -515,8 +556,12 @@ static int dk_from_dkf(const bffc_plan* p, const void* dkf_engine, void* dk, int
     dk_rows_kernel<<<dim3(p->R / 2 + 1, Hc), kThreads, kSmemBytes, st>>>(in, T, p->R, p->R0, p->R1, p->tw8192, p->tw_lo,
                                                                           p->tw_hi, band);
     if (int rc = launched()) return rc;
-    COLS_SWITCH(p->R, (dk_cols_kernel<RR><<<dim3(kInner / ColRadix<RR>::kTC, (Hc + 1) / 2), kColThreads, ColRadix<RR>::kSmem, st>>>(
-        T, out, Lk, Hc, p->dk_scale / float(p->NE), p->tw512)););
+    if (lags)
+      COLS_SWITCH(p->R, (dk_cols_kernel<RR, true><<<dim3(kInner / ColRadix<RR>::kTC, (Hc + 1) / 2), kColThreads, ColRadix<RR>::kSmem, st>>>(
+          T, out, Lk, Hc, p->dk_scale / float(p->NE), p->tw512, lg)););
+    else
+      COLS_SWITCH(p->R, (dk_cols_kernel<RR><<<dim3(kInner / ColRadix<RR>::kTC, (Hc + 1) / 2), kColThreads, ColRadix<RR>::kSmem, st>>>(
+          T, out, Lk, Hc, p->dk_scale / float(p->NE), p->tw512, lg)););
     if (int rc = launched()) return rc;
   }
   return BFFC_OK;
@@ -524,23 +569,43 @@ static int dk_from_dkf(const bffc_plan* p, const void* dkf_engine, void* dk, int
 
 int bffc_kf_from_filter(const bffc_plan* p, const void* k, int Lk, void* kf_engine, int H, int conj, void* workspace,
                         size_t workspace_bytes, void* stream) {
-  return kf_from_filter(p, k, Lk, kf_engine, H, conj, p ? full_band(p) : 0, workspace, workspace_bytes, stream,
+  return kf_from_filter(p, k, Lk, kf_engine, H, conj, p ? full_band(p) : 0, nullptr, workspace, workspace_bytes, stream,
                         "bffc_kf_from_filter");
 }
 
 int bffc_kf_from_filter_band(const bffc_plan* p, const void* k, int Lk, void* kf_engine, int H, int conj, int band,
                              void* workspace, size_t workspace_bytes, void* stream) {
-  return kf_from_filter(p, k, Lk, kf_engine, H, conj, band, workspace, workspace_bytes, stream, "bffc_kf_from_filter_band");
+  return kf_from_filter(p, k, Lk, kf_engine, H, conj, band, nullptr, workspace, workspace_bytes, stream,
+                        "bffc_kf_from_filter_band");
+}
+
+int bffc_kf_from_filter_lags(const bffc_plan* p, const void* k, int Lk, int period, int pos, int neg, void* kf_engine,
+                             int H, int conj, void* workspace, size_t workspace_bytes, void* stream) {
+  const char* name = "bffc_kf_from_filter_lags";
+  if (!p) return fail(BFFC_ERR_INVALID, "%s: bad argument", name);
+  if (int rc = check_lags(p, Lk, period, pos, neg, name)) return rc;
+  const bffc::ffft::Lags lg{pos, neg, period, p->N};
+  return kf_from_filter(p, k, Lk, kf_engine, H, conj, full_band(p), &lg, workspace, workspace_bytes, stream, name);
 }
 
 int bffc_dk_from_dkf(const bffc_plan* p, const void* dkf_engine, void* dk, int Lk, int H, void* workspace,
                      size_t workspace_bytes, void* stream) {
-  return dk_from_dkf(p, dkf_engine, dk, Lk, H, p ? full_band(p) : 0, workspace, workspace_bytes, stream, "bffc_dk_from_dkf");
+  return dk_from_dkf(p, dkf_engine, dk, Lk, H, p ? full_band(p) : 0, nullptr, workspace, workspace_bytes, stream,
+                     "bffc_dk_from_dkf");
 }
 
 int bffc_dk_from_dkf_band(const bffc_plan* p, const void* dkf_engine, void* dk, int Lk, int H, int band, void* workspace,
                           size_t workspace_bytes, void* stream) {
-  return dk_from_dkf(p, dkf_engine, dk, Lk, H, band, workspace, workspace_bytes, stream, "bffc_dk_from_dkf_band");
+  return dk_from_dkf(p, dkf_engine, dk, Lk, H, band, nullptr, workspace, workspace_bytes, stream, "bffc_dk_from_dkf_band");
+}
+
+int bffc_dk_from_dkf_lags(const bffc_plan* p, const void* dkf_engine, void* dk, int Lk, int period, int pos, int neg,
+                          int H, void* workspace, size_t workspace_bytes, void* stream) {
+  const char* name = "bffc_dk_from_dkf_lags";
+  if (!p) return fail(BFFC_ERR_INVALID, "%s: bad argument", name);
+  if (int rc = check_lags(p, Lk, period, pos, neg, name)) return rc;
+  const bffc::ffft::Lags lg{pos, neg, period, p->N};
+  return dk_from_dkf(p, dkf_engine, dk, Lk, H, full_band(p), &lg, workspace, workspace_bytes, stream, name);
 }
 
 int bffc_dkf_unpack(const bffc_plan* p, const void* dkf_engine, void* dkf_natural, int H, void* stream) {

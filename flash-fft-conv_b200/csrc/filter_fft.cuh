@@ -137,12 +137,25 @@ DEVINL int pos_of_freq(int f) { return 512 * (f & 15) + 32 * ((f >> 4) & 15) + (
 // any band >= N/2 + 1 keeps every frequency.
 DEVINL bool in_band(int f, int N, int band) { return min(f, N - f) < band; }
 
+// Two-sided lag map of bffc_kf_from_filter_lags / bffc_dk_from_dkf_lags on an n-point plan (k rows of Lk): transform
+// slot d < pos holds k[d], slot n - j (1 <= j <= neg) holds k[period - j], a k index >= Lk reads as 0 and every other
+// slot is 0.  The plain calls read slot d < Lk from k[d]; they are the kernels' kLags = false instantiations, which do
+// not look at the map.
+struct Lags {
+  int pos, neg, period, n;
+  // the k index slot d reads, or -1
+  DEVINL int src(int d, int Lk) const {
+    const int s = d < pos ? d : (d < n && d >= n - neg ? d - (n - period) : -1);
+    return s < Lk ? s : -1;
+  }
+};
+
 // grid = ceil(H / 2): channels 2*blockIdx.x (real part) and 2*blockIdx.x + 1 (imaginary part)
 // N < 8192 (small sizes): the engine row holds the N-point spectrum K_N[f] = K_8192[f * 8192/N] (k has support < N).
-template <int kFmt>
+template <int kFmt, bool kLags = false>
 __global__ void __launch_bounds__(kThreads, 3) kf_from_filter_kernel(const float* __restrict__ k, int Lk, uint4* __restrict__ kf_eng,
                                                                      int H, float scale, int conj, const float2* __restrict__ tw,
-                                                                     int N, int band) {
+                                                                     int N, int band, Lags lg) {
   extern __shared__ float2 fbuf[];
   const int tid = threadIdx.x, ha = 2 * blockIdx.x, hb = ha + 1;
   const float* ka = k + size_t(ha) * Lk;
@@ -153,8 +166,14 @@ __global__ void __launch_bounds__(kThreads, 3) kf_from_filter_kernel(const float
 #pragma unroll
     for (int i = 0; i < 16; ++i) {
       const int n = tid + (16 * half + i) * kThreads;
-      a[i] = n < Lk ? __ldg(ka + n) : 0.f;
-      b[i] = n < Lk ? __ldg(kb + n) : 0.f;
+      if constexpr (kLags) {
+        const int s = lg.src(n, Lk);
+        a[i] = s >= 0 ? __ldg(ka + s) : 0.f;
+        b[i] = s >= 0 ? __ldg(kb + s) : 0.f;
+      } else {
+        a[i] = n < Lk ? __ldg(ka + n) : 0.f;
+        b[i] = n < Lk ? __ldg(kb + n) : 0.f;
+      }
     }
 #pragma unroll
     for (int i = 0; i < 16; ++i) fbuf[slot(tid + (16 * half + i) * kThreads)] = make_float2(a[i], hb < H ? b[i] : 0.f);
@@ -188,8 +207,12 @@ __global__ void __launch_bounds__(kThreads, 3) kf_from_filter_kernel(const float
 // N < 8192: the block sum D_N[f] (engine_order.cuh) goes to 8192-point frequency f * 8192/N (the rest is zero), whose
 // inverse transform is the N-periodic gradient.  The band limit masks D_N[f] as it is read (Re ifft of
 // the masked spectrum = ifft of the masked Hermitian part, the mask being symmetric).
+// kLags: dk[m] += g[m] (m < pos), then dk[m] += g[N - (period - m)] (period - m <= neg), g the N-periodic gradient;
+// one thread per element of dk, and each term rounded as torch's `dk += term` rounds it.
+template <bool kLags = false>
 __global__ void __launch_bounds__(kThreads, 3) dk_from_dkf_kernel(const float2* __restrict__ dkf_eng, float* __restrict__ dk, int Lk,
-                                                                  float scale, int N, const float2* __restrict__ tw, int band) {
+                                                                  float scale, int N, const float2* __restrict__ tw, int band,
+                                                                  Lags lg) {
   extern __shared__ float2 fbuf[];
   const int tid = threadIdx.x, h = blockIdx.x;
   const float2* src = dkf_eng + size_t(h) * kN;
@@ -216,7 +239,20 @@ __global__ void __launch_bounds__(kThreads, 3) dk_from_dkf_kernel(const float2* 
   __syncthreads();
   fft8192<1>(fbuf, tid, tw);
   const float s = scale / float(N);
-  for (int n = tid; n < Lk; n += kThreads) dk[size_t(h) * Lk + n] = fbuf[slot(pos_of_freq(n))].x * s;
+  if constexpr (kLags) {
+    float* d = dk + size_t(h) * Lk;
+    const int head = min(lg.pos, Lk), tail0 = max(lg.period - lg.neg, head), tail1 = min(lg.period, Lk);
+    for (int m = tid; m < head; m += kThreads) {         // head, and the tail term of an index read both ways
+      float acc = __fadd_rn(d[m], __fmul_rn(fbuf[slot(pos_of_freq(m))].x, s));
+      const int j = lg.period - m;
+      if (j <= lg.neg) acc = __fadd_rn(acc, __fmul_rn(fbuf[slot(pos_of_freq(N - j))].x, s));
+      d[m] = acc;
+    }
+    for (int m = tail0 + tid; m < tail1; m += kThreads)
+      d[m] = __fadd_rn(d[m], __fmul_rn(fbuf[slot(pos_of_freq(N - (lg.period - m)))].x, s));
+  } else {
+    for (int n = tid; n < Lk; n += kThreads) dk[size_t(h) * Lk + n] = fbuf[slot(pos_of_freq(n))].x * s;
+  }
 }
 
 // =====================================================================================================================
@@ -309,10 +345,13 @@ DEVINL float2 twiddle_n(int m, const float2* __restrict__ tw_lo, const float2* _
 }
 
 // grid (8192 / TC, ceil(Hc / 2)), kColThreads.  k: (Hc, Lk) fp32, zero beyond Lk.  T: (Hc, R/2 + 1, 8192) fp32 complex.
-template <int R>
+// kLags: the slots of the lag map lg; a run of four slots is one 16-byte load when it reads four consecutive, aligned k
+// values (the tail run starts at slot n - neg, usually off a multiple of four: its first group is read element-wise).
+template <int R, bool kLags = false>
 __global__ void __launch_bounds__(kColThreads) filter_cols_kernel(const float* __restrict__ k, int Lk, float2* __restrict__ T, int Hc,
                                                                   float scale, const float2* __restrict__ tw512,
-                                                                  const float2* __restrict__ tw_lo, const float2* __restrict__ tw_hi) {
+                                                                  const float2* __restrict__ tw_lo, const float2* __restrict__ tw_hi,
+                                                                  Lags lg) {
   using P = ColRadix<R>;
   constexpr int TC = P::kTC, TC4 = TC / 4, NV = R * TC4 / kColThreads;      // 4 x 16-byte loads per thread and channel
   extern __shared__ float2 cb[];
@@ -326,7 +365,21 @@ __global__ void __launch_bounds__(kColThreads) filter_cols_kernel(const float* _
   for (int i = 0; i < NV; ++i) {                       // all loads of the tile in flight before the first use
     const int e4 = tid + i * kColThreads, n1 = e4 / TC4, c4 = e4 % TC4;
     const int idx = n1 * kN + n20 + 4 * c4;
-    if (vec && idx + 3 < Lk) {
+    if constexpr (kLags) {
+      int s[4];
+#pragma unroll
+      for (int q = 0; q < 4; ++q) s[q] = lg.src(idx + q, Lk);
+      if (vec && s[0] >= 0 && (s[0] & 3) == 0 && s[1] == s[0] + 1 && s[2] == s[0] + 2 && s[3] == s[0] + 3) {
+        va[i] = __ldg(reinterpret_cast<const float4*>(ka + s[0]));
+        vb[i] = __ldg(reinterpret_cast<const float4*>(kb + s[0]));
+      } else {
+        float a[4], b[4];
+#pragma unroll
+        for (int q = 0; q < 4; ++q) { a[q] = s[q] >= 0 ? ka[s[q]] : 0.f; b[q] = s[q] >= 0 ? kb[s[q]] : 0.f; }
+        va[i] = make_float4(a[0], a[1], a[2], a[3]);
+        vb[i] = make_float4(b[0], b[1], b[2], b[3]);
+      }
+    } else if (vec && idx + 3 < Lk) {
       va[i] = __ldg(reinterpret_cast<const float4*>(ka + idx));
       vb[i] = __ldg(reinterpret_cast<const float4*>(kb + idx));
     } else {
@@ -447,9 +500,12 @@ __global__ void __launch_bounds__(kThreads, 3) dk_rows_kernel(const float2* __re
 }
 
 // grid (8192 / TC, ceil(Hc / 2)): inverse R-point DFTs down the columns, channels 2*blockIdx.y (real) / +1 (imaginary)
-template <int R>
+// kLags: dk accumulates through the lag map lg as in dk_from_dkf_kernel.  The slot of an index's head term owns it, else
+// the slot of its tail term; an index with both terms finds its tail slot in its own column, (N - period) / 8192 rows
+// further down (the host refuses a map where that is not so).
+template <int R, bool kLags = false>
 __global__ void __launch_bounds__(kColThreads) dk_cols_kernel(const float2* __restrict__ T, float* __restrict__ dk, int Lk, int Hc,
-                                                           float scale, const float2* __restrict__ tw512) {
+                                                           float scale, const float2* __restrict__ tw512, Lags lg) {
   using P = ColRadix<R>;
   constexpr int TC = P::kTC;
   extern __shared__ float2 cb[];
@@ -471,13 +527,43 @@ __global__ void __launch_bounds__(kColThreads) dk_cols_kernel(const float2* __re
   col_fft<R, 1>(cb, tid, tw512);
   float* da = dk + size_t(ha) * Lk;
   float* db = dk + size_t(hb) * Lk;
-  for (int e = tid; e < R * TC; e += kColThreads) {
-    const int n1 = e / TC, c = e % TC;
-    const int idx = n1 * kN + n20 + c;
-    if (idx >= Lk) continue;
-    const float2 x = cb[P::pos(n1) * TC + c];
-    da[idx] = x.x * scale;
-    if (two) db[idx] = x.y * scale;
+  if constexpr (kLags) {
+    const int shift = R * kN - lg.period;                 // tail slot of k index m: m + shift
+    for (int e = tid; e < R * TC; e += kColThreads) {
+      const int n1 = e / TC, c = e % TC;
+      const int idx = n1 * kN + n20 + c;
+      int m;
+      bool both = false;
+      if (idx < lg.pos) {
+        m = idx;
+        both = lg.period - m <= lg.neg;
+      } else if (idx >= R * kN - lg.neg) {
+        m = idx - shift;
+        if (m < lg.pos) continue;                         // owned by its head slot
+      } else {
+        continue;
+      }
+      if (m >= Lk) continue;
+      float2 x = cb[P::pos(n1) * TC + c];
+      float a = __fadd_rn(da[m], __fmul_rn(x.x, scale)), b = 0.f;
+      if (two) b = __fadd_rn(db[m], __fmul_rn(x.y, scale));
+      if (both) {
+        x = cb[P::pos(n1 + shift / kN) * TC + c];
+        a = __fadd_rn(a, __fmul_rn(x.x, scale));
+        b = __fadd_rn(b, __fmul_rn(x.y, scale));
+      }
+      da[m] = a;
+      if (two) db[m] = b;
+    }
+  } else {
+    for (int e = tid; e < R * TC; e += kColThreads) {
+      const int n1 = e / TC, c = e % TC;
+      const int idx = n1 * kN + n20 + c;
+      if (idx >= Lk) continue;
+      const float2 x = cb[P::pos(n1) * TC + c];
+      da[idx] = x.x * scale;
+      if (two) db[idx] = x.y * scale;
+    }
   }
 }
 

@@ -40,6 +40,9 @@ SYMBOLS = {
                                             _c.c_void_p, _c.c_size_t, _c.c_void_p]),
     'bffc_dk_from_dkf_band': (_c.c_int, [_c.c_void_p, _c.c_void_p, _c.c_void_p, _c.c_int, _c.c_int, _c.c_int, _c.c_void_p,
                                          _c.c_size_t, _c.c_void_p]),
+    'bffc_kf_from_filter_lags': (_c.c_int, [_c.c_void_p, _c.c_void_p] + [_c.c_int] * 4
+                                 + [_c.c_void_p, _c.c_int, _c.c_int, _c.c_void_p, _c.c_size_t, _c.c_void_p]),
+    'bffc_dk_from_dkf_lags': (_c.c_int, [_c.c_void_p] * 3 + [_c.c_int] * 5 + [_c.c_void_p, _c.c_size_t, _c.c_void_p]),
     'bffc_workspace_bytes': (_c.c_size_t, [_c.c_void_p, _c.c_int, _c.c_int, _c.c_int]),
     'bffc_workspace_bytes_ex': (_c.c_size_t, [_c.c_void_p, _c.c_int, _c.c_int, _c.c_int, _c.c_int, _c.c_int]),
     'bffc_workspace_bytes_blocked': (_c.c_size_t, [_c.c_void_p] + [_c.c_int] * 6),

@@ -130,7 +130,7 @@ class FlashFFTConv(torch.nn.Module):
         d = self.__dict__
         d['_plans'] = {}
         d['_host_ws'] = {}             # (device, bytes) -> (staging buffer, _StreamOrder of its latest call)
-        d['_kf_cache'] = None          # (weakref(k), k._version, device, kf_engine, band, _StreamOrder of its transform)
+        d['_kf_cache'] = None          # (weakref(k), k._version, device, kf_engine, band, lags, _StreamOrder of its transform)
         d['last_launches'] = 0         # kernels enqueued by the most recent operator call (bench.py); see _launched
         d['_class_mods'] = {}          # class length c -> FlashFFTConv(2c) of the packed-document path (docs.py)
 
@@ -188,17 +188,20 @@ class FlashFFTConv(torch.nn.Module):
         device = torch.device('cuda', torch.cuda.current_device()) if device is None else torch.device(device)
         return _forward_host(self, u, k, pregate, postgate, out, device)
 
-    def forward(self, u, k, pregate=None, postgate=None, docs=None):
+    def forward(self, u, k, pregate=None, postgate=None, docs=None, bidirectional=False):
         """y = postgate * conv(u * pregate, k), the gates both given or both None.  docs: a DocumentTable of packed
-        documents in the rows of u; each document is then convolved alone and causally (flashfftconv.docs,
-        INTEGRATION.md §11), with gradients to u, k and the gates."""
+        documents in the rows of u; each document is then convolved alone (flashfftconv.docs, INTEGRATION.md §11), with
+        gradients to u, k and the gates.  bidirectional: with docs, each document keeps the filter's negative lags too
+        (lag -j reads k[:, seqlen - j], as M2-BERT's two-sided filter of length seqlen = 2L has it), so it gets exactly
+        this module's circular convolution of the document alone; without it, only the causal lags.  Without docs the
+        flag changes nothing: the plain call is already the two-sided circular convolution."""
         if pregate is not None or postgate is not None:
             assert pregate is not None and postgate is not None       # conv.py:557-558
         if docs is not None:
             from . import docs as _docs
             _check_inputs(u, k, self, () if pregate is None else (pregate, postgate), views=True)
             _docs._check(docs, u)
-            return _docs.DocsConvFunc.apply(u, k, self, self.training, docs, pregate, postgate)
+            return _docs.DocsConvFunc.apply(u, k, self, self.training, docs, pregate, postgate, bool(bidirectional))
         if pregate is not None:
             return FlashFFTConvFunc.apply(u, k, self, self.training, pregate, postgate)
         return FlashFFTConvFunc.apply(u, k, self, self.training)
@@ -317,41 +320,49 @@ def _filter_workspace(plan, H, device):
     return (torch.empty(n, dtype=torch.uint8, device=device) if n else None), n
 
 
-def _pack_kf(mod, plan, k, conj=0, band=None):
+def _pack_kf(mod, plan, k, conj=0, band=None, lags=None):
     """k (H, Lk) fp32 device -> engine-order packed spectrum (H, N) int32 words by the library's own fp32 FFT
     (bffc_kf_from_filter_band): one launch for engine size 8192, column + row FFT launches per L2-sized channel group
     for the composite sizes (replaces conv.py:575 + :640).  band: None for the full spectrum (band seqlen / 2 + 1 keeps
-    every frequency), else the band limit (frequencies with min(f, seqlen - f) >= band are zeroed)."""
+    every frequency), else the band limit (frequencies with min(f, seqlen - f) >= band are zeroed).  lags: None, or
+    (period, pos, neg) of bffc_kf_from_filter_lags (the class filters of flashfftconv.docs; no band then)."""
     k32 = k.detach()
     if k32.dtype != torch.float32 or not k32.is_contiguous():
         k32 = k32.to(torch.float32).contiguous()
     H, Lk = k32.shape
     kf_engine = torch.empty((H, plan.fft_size), dtype=torch.int32, device=k.device)
     ws, ws_bytes = _filter_workspace(plan, H, k.device)
+    if lags is not None:
+        period, pos, neg = lags
+        _launched(mod, _lib.lib().bffc_kf_from_filter_lags(plan.handle, _ptr(k32), int(Lk), int(period), int(pos),
+                                                           int(neg), _ptr(kf_engine), int(H), int(conj), _ptr(ws),
+                                                           ws_bytes, _stream()))
+        return kf_engine
     band = mod.seqlen // 2 + 1 if band is None else band
     _launched(mod, _lib.lib().bffc_kf_from_filter_band(plan.handle, _ptr(k32), int(Lk), _ptr(kf_engine), int(H),
                                                        int(conj), int(band), _ptr(ws), ws_bytes, _stream()))
     return kf_engine
 
 
-def _kf_engine_for(mod, plan, k, cache_key=None, band=None, use_cache=None):
-    """Engine-order spectrum of `k` (band-limited unless band is None), cached in eval mode (use_cache=None: the
-    module's own mode) while the same tensor object is unmodified and the band is the same.  A hit on another stream
+def _kf_engine_for(mod, plan, k, cache_key=None, band=None, use_cache=None, lags=None):
+    """Engine-order spectrum of `k` (band-limited unless band is None; through the lag map `lags` of _pack_kf unless it
+    is None), cached in eval mode (use_cache=None: the module's own mode) while the same tensor object is unmodified
+    and the band and the lag map are the same.  A hit on another stream
     than the one that transformed the filter waits for the transform (_StreamOrder); a spectrum made while a CUDA graph
     is being captured exists only when the graph runs, and is not cached."""
     key = k if cache_key is None else cache_key
     if use_cache is None:
         use_cache = not mod.training
     if use_cache and mod._kf_cache is not None:
-        ref, ver, dev, kf, kf_band, order = mod._kf_cache
-        if ref() is key and ver == key._version and dev == k.device and kf_band == band:
+        ref, ver, dev, kf, kf_band, kf_lags, order = mod._kf_cache
+        if ref() is key and ver == key._version and dev == k.device and kf_band == band and kf_lags == lags:
             order.join(kf)
             return kf
-    kf = _pack_kf(mod, plan, k, band=band)
+    kf = _pack_kf(mod, plan, k, band=band, lags=lags)
     if use_cache and not torch.cuda.is_current_stream_capturing():
         order = _StreamOrder()
         order.mark()
-        mod.__dict__['_kf_cache'] = (weakref.ref(key), key._version, k.device, kf, band, order)
+        mod.__dict__['_kf_cache'] = (weakref.ref(key), key._version, k.device, kf, band, lags, order)
     else:
         mod.__dict__['_kf_cache'] = None
     return kf
@@ -391,14 +402,14 @@ class _on_device:
 
 
 def _fwd(mod, u, k, pregate, postgate, band=None, use_cache=None, kf_engine=None, taps=None, halo=None, out=None,
-         cache_key=None):
+         cache_key=None, lags=None):
     """y (contiguous) and the engine-order filter spectrum it used.  u and the gates: any (B, H, L) layout; those that
     qualify (batch_stride) are read in place, others copied.  band / use_cache: see _kf_engine_for; kf_engine: a
     spectrum of k already at hand.  taps: ((u_w, u_bias, pregate_w, pregate_bias, postgate_w, postgate_bias), w_dtype,
     K, padding), a short depthwise filter bffc_fwd_short_strided applies to u and the gates as it loads them; the rows
     are device addresses of (H, K) taps and (H) biases, None for a tensor that is not filtered.  halo: overlap-save
     blocks with this halo (bffc_fwd_blocked, blocked_long_conv), else None.  out: a contiguous (B, H, L) tensor to write y
-    into (L a multiple of bffc_length_multiple()).  cache_key: see _kf_engine_for."""
+    into (L a multiple of bffc_length_multiple()).  cache_key, lags: see _kf_engine_for."""
     B, H, L = u.shape
     dev = u.device
     plan = mod.plan(dev)
@@ -409,12 +420,12 @@ def _fwd(mod, u, k, pregate, postgate, band=None, use_cache=None, kf_engine=None
         if out is not None:
             raise RuntimeError(f'L={L} must be a multiple of bffc_length_multiple() to write into `out`')
         y, kf = _fwd(mod, _padded(u, Lp), k, _padded(pregate, Lp), _padded(postgate, Lp), band, use_cache, kf_engine,
-                     halo=halo)
+                     halo=halo, lags=lags)
         return y[..., :L].contiguous(), kf
     (u, u_bs), (pre, pre_bs), (post, post_bs) = [_engine_view(t, mod.dtype) for t in (u, pregate, postgate)]
     with _on_device(dev):
         if kf_engine is None:
-            kf_engine = _kf_engine_for(mod, plan, k, cache_key=cache_key, band=band, use_cache=use_cache)
+            kf_engine = _kf_engine_for(mod, plan, k, cache_key=cache_key, band=band, use_cache=use_cache, lags=lags)
         y = torch.empty((B, H, L), dtype=u.dtype, device=dev) if out is None else out
         ws, ws_bytes = _workspace(plan, B, H, L, pre is not None, False, dev, halo)
         if halo is not None:
@@ -432,7 +443,8 @@ def _fwd(mod, u, k, pregate, postgate, band=None, use_cache=None, kf_engine=None
     return y, kf_engine
 
 
-def _bwd(mod, dout, u, kf_engine, k_len, pregate, postgate, band=None, out=None, taps=None, halo=None):
+def _bwd(mod, dout, u, kf_engine, k_len, pregate, postgate, band=None, out=None, taps=None, halo=None, lags=None,
+         dk=None):
     """du, dk[, dpregate, dpostgate] — reference: FlashFFTConvFunc.backward, conv.py:1737-1822.  band: the forward's
     band limit (None: full spectrum); kf_engine is then the band-limited spectrum and dk gets the same mask.  Inputs:
     any (B, H, L) layout, as for _fwd.  out: optional (du, dpregate, dpostgate) tensors to write the gradients into
@@ -441,7 +453,8 @@ def _bwd(mod, dout, u, kf_engine, k_len, pregate, postgate, band=None, out=None,
     tensors, and du, dpregate, dpostgate the gradients with respect to their filtered versions.  halo: the forward's
     overlap-save blocks (bffc_bwd_blocked), else None.  Under torch.use_deterministic_algorithms(True) dk is summed in
     a fixed order (the module's deterministic plan): the same bits from run to run and on any GPU; du and the gate
-    gradients are the same in either mode."""
+    gradients are the same in either mode.  lags: the forward's lag map (_pack_kf); dk is then not made but added into
+    `dk`, an (H, k_len) fp32 tensor, through that map (bffc_dk_from_dkf_lags)."""
     B, H, L = u.shape
     plan = mod.plan(u.device, torch.are_deterministic_algorithms_enabled())
     Lp = _pad_len(plan, L)
@@ -449,7 +462,7 @@ def _bwd(mod, dout, u, kf_engine, k_len, pregate, postgate, band=None, out=None,
         if taps is not None:
             raise RuntimeError(f'L={L} must be a multiple of bffc_length_multiple() to fuse a short filter')
         r = _bwd(mod, _padded(dout, Lp), _padded(u, Lp), kf_engine, k_len, _padded(pregate, Lp), _padded(postgate, Lp),
-                 band, halo=halo)
+                 band, halo=halo, lags=lags, dk=dk)
         cut = lambda t: None if t is None else t[..., :L].contiguous()
         res = [cut(r[0]), r[1], cut(r[2]), cut(r[3])]
         for i, o in zip((0, 2, 3), out or ()):
@@ -497,11 +510,17 @@ def _bwd(mod, dout, u, kf_engine, k_len, pregate, postgate, band=None, out=None,
         # the kernels accumulate unnormalised pair-packed spectra in engine order; the reference takes
         # ifft(dk_f).real[..., :k_len] (conv.py:1817-1820): inverse fp32 FFT straight from engine order, 1/N, real part
         # (only the Hermitian part of dk_f contributes), sum over the batch-member blocks of the small sizes, [:k_len]
-        dk = torch.empty((H, k_len), dtype=torch.float32, device=u.device)
         fws, fws_bytes = _filter_workspace(plan, H, u.device)
-        band = mod.seqlen // 2 + 1 if band is None else band
-        _launched(mod, _lib.lib().bffc_dk_from_dkf_band(plan.handle, _ptr(dkf_engine), _ptr(dk), int(k_len), H,
-                                                        int(band), _ptr(fws), fws_bytes, _stream()))
+        if lags is not None:
+            period, pos, neg = lags
+            _launched(mod, _lib.lib().bffc_dk_from_dkf_lags(plan.handle, _ptr(dkf_engine), _ptr(dk), int(k_len),
+                                                            int(period), int(pos), int(neg), H, _ptr(fws), fws_bytes,
+                                                            _stream()))
+        else:
+            dk = torch.empty((H, k_len), dtype=torch.float32, device=u.device)
+            band = mod.seqlen // 2 + 1 if band is None else band
+            _launched(mod, _lib.lib().bffc_dk_from_dkf_band(plan.handle, _ptr(dkf_engine), _ptr(dk), int(k_len), H,
+                                                            int(band), _ptr(fws), fws_bytes, _stream()))
     du, dpre, dpost = (o if o is not None else t for t, _, o in dst)
     return du, dk, dpre, dpost
 

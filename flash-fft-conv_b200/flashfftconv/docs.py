@@ -12,6 +12,17 @@ needs the taps m <= t < c, and a term that wraps around the 2c-point circle land
 where the zero-filled input is zero.  No existing kernel changes: the new kernels only move data, one gather of every
 input into the class batches (bffc_docs_gather) and one scatter of every output back into the rows
 (bffc_docs_scatter), driven by a device item table that DocumentTable builds once per batch (INTEGRATION.md §11).
+
+bidirectional=True keeps the negative lags as well, read the way FlashFFTConv(N) (N = seqlen of the caller's module)
+reads them on its circle: with kk[h, d] = k[h, d] for d >= 0 and k[h, N + d] for d < 0 (0 past Lk),
+
+    y[b, h, t] = postgate[b, h, t] * sum_{s <= r < e} kk[h, t - r] * (u * pregate)[b, h, r]
+
+which is FlashFFTConv(N) of the document alone, zero-padded to L (M2-BERT's filter k_fwd | k_rev.flip of length
+N = 2L).  The class filter on the 2c-point circle is then k_c[d] = k[d] (d < min(Lk, c)), k_c[2c - j] = k[N - j]
+(1 <= j <= c - 1, N - j < Lk), zero elsewhere: every lag a document needs lies in (-c, c) and lands on its own slot.
+Both ways the class spectra come from bffc_kf_from_filter_lags(plan_2c, k, Lk, N, min(Lk, c), c - 1 or 0) and dk from
+bffc_dk_from_dkf_lags, which adds each class's terms into one zeroed dk in ascending c.
 """
 import ctypes
 
@@ -97,6 +108,8 @@ class DocumentTable:
         if device is None:
             device = cu_seqlens.device if cu_seqlens.is_cuda else torch.device('cuda', torch.cuda.current_device())
         device = torch.device(device)
+        if device.type == 'cuda' and device.index is None:      # 'cuda' names the current device, as tensors resolve it
+            device = torch.device('cuda', torch.cuda.current_device())
         items, self.classes, self.positions = document_items(cu_seqlens.cpu().numpy(), B, L)
         self.B, self.L = int(B), int(L)
         self.n_docs = cu_seqlens.numel() - 1
@@ -105,6 +118,33 @@ class DocumentTable:
         self.device = device
         self.items = torch.from_numpy(items).to(device)
         self.cu_seqlens = cu_seqlens.to(device).contiguous()
+
+    @classmethod
+    def from_lengths(cls, lengths, L, device=None):
+        """The table of a right-padded batch: row b holds one document of lengths[b] positions (0 <= lengths[b] <= L),
+        and its padding [lengths[b], L) is a document of its own, so no real token reads the padding.  lengths: a 1-D
+        integer tensor (an attention mask's `mask.sum(-1)`, GPU or CPU) or a sequence of ints; its size is B."""
+        if isinstance(lengths, torch.Tensor):
+            if lengths.dim() != 1 or lengths.dtype.is_floating_point or lengths.dtype.is_complex \
+                    or lengths.dtype == torch.bool:
+                raise RuntimeError('lengths must be a 1-D integer tensor')
+            if device is None and lengths.is_cuda:
+                device = lengths.device
+            lengths = lengths.cpu().tolist()
+        lens = np.asarray(list(lengths))
+        if lens.ndim != 1 or lens.size == 0 or lens.dtype.kind not in 'iu':
+            raise RuntimeError('lengths must be a non-empty 1-D sequence of integers')
+        L = int(L)
+        if L < 1:
+            raise RuntimeError(f'bad row length L={L}')
+        if (lens < 0).any() or (lens > L).any():
+            raise RuntimeError(f'every length must lie in [0, L={L}], got {lens.min()} .. {lens.max()}')
+        B = lens.size
+        starts = np.arange(B, dtype=np.int64) * L
+        cu = np.append(np.stack([starts, starts + lens]).T.reshape(-1), B * L)
+        if B * L > 0x7fffffff:
+            raise RuntimeError(f'B * L = {B * L} positions exceed the int32 offsets of cu_seqlens')
+        return cls(torch.from_numpy(cu.astype(np.int32)), B, L, device)
 
     def __repr__(self):
         return (f'DocumentTable(B={self.B}, L={self.L}, n_docs={self.n_docs}, classes={self.counts}, '
@@ -166,11 +206,16 @@ def _segments(docs, H, flat):
     return [flat[H * base:H * (base + n * c)].view(n, H, c) for c, n, base in docs.classes]
 
 
-def forward(mod, docs, u, k, pregate, postgate, k2=None, use_cache=None):
+def _lags(mod, k, c, bidirectional):
+    """(period, pos, neg) of class c's filter, read out of the caller's k (bffc_kf_from_filter_lags)."""
+    return mod.seqlen, min(k.shape[1], c), c - 1 if bidirectional else 0
+
+
+def forward(mod, docs, u, k, pregate, postgate, k2=None, use_cache=None, bidirectional=False):
     """(y, spectra): y = postgate * conv(u * pregate, k) [+ conv(u, k2)] per document, as a contiguous (B, H, L) tensor,
     and the per-class filter spectra [(kf, kf2)] the backward takes.  u and the gates: any (B, H, L) layout (rows
     contiguous: read in place).  Per class the calls are those of FlashFFTConv(2c) (and of hyena_mixer with k2) on the
-    class batch, so y is bit for bit theirs, scattered."""
+    class batch with the class filter (module docstring), so y is bit for bit theirs, scattered."""
     B, H, L = u.shape
     dev = u.device
     if use_cache is None:                 # the class modules follow the mode of `mod`, not their own
@@ -188,12 +233,12 @@ def forward(mod, docs, u, k, pregate, postgate, k2=None, use_cache=None):
             sub.__dict__['last_launches'] = 0
             u_c = segs[0][i]
             pre_c, post_c = (segs[1][i], segs[2][i]) if pregate is not None else (None, None)
-            _, kf = _conv._fwd(sub, u_c, k[:, :min(k.shape[1], c)], pre_c, post_c, use_cache=use_cache, out=y_c,
-                               cache_key=k)
+            _, kf = _conv._fwd(sub, u_c, k, pre_c, post_c, use_cache=use_cache, out=y_c,
+                               lags=_lags(mod, k, c, bidirectional))
             kf2 = None
             if k2 is not None:
-                y2, kf2 = _conv._fwd(sub, u_c, k2[:, :min(k2.shape[1], c)], None, None, use_cache=use_cache,
-                                     cache_key=k2)
+                y2, kf2 = _conv._fwd(sub, u_c, k2, None, None, use_cache=use_cache,
+                                     lags=_lags(mod, k2, c, bidirectional))
                 y_c.add_(y2)
             mod.__dict__['last_launches'] += sub.last_launches
             spectra.append((kf, kf2))
@@ -203,10 +248,10 @@ def forward(mod, docs, u, k, pregate, postgate, k2=None, use_cache=None):
     return y, spectra
 
 
-def backward(mod, docs, dout, u, pregate, postgate, spectra, k_len, k2_len=None, out=None):
+def backward(mod, docs, dout, u, pregate, postgate, spectra, k_len, k2_len=None, out=None, bidirectional=False):
     """(du, dk, dpregate, dpostgate, dk2) of `forward`.  out: optional (du, dpregate, dpostgate) (B, H, L) tensors with
-    contiguous rows (channel slices of one gradient) that the scatter writes in place.  dk is the sum of the classes'
-    dk_c, zero-extended to k_len and added in ascending c; likewise dk2."""
+    contiguous rows (channel slices of one gradient) that the scatter writes in place.  dk starts at zero and each class
+    adds its terms into it in ascending c, the head lags before the tail lags (bffc_dk_from_dkf_lags); likewise dk2."""
     B, H, L = u.shape
     dev = u.device
     gated = pregate is not None
@@ -229,14 +274,12 @@ def backward(mod, docs, dout, u, pregate, postgate, spectra, k_len, k2_len=None,
             dout_c, u_c = segs[0][i], segs[1][i]
             pre_c, post_c = (segs[2][i], segs[3][i]) if gated else (None, None)
             d_c = [s[i] for s in dsegs] + [None] * (3 - len(dsegs))
-            m = min(k_len, c)
-            du_c, dk_c, _, _ = _conv._bwd(sub, dout_c, u_c, kf, m, pre_c, post_c, out=d_c)
-            dk[:, :m] += dk_c
+            du_c, _, _, _ = _conv._bwd(sub, dout_c, u_c, kf, k_len, pre_c, post_c, out=d_c,
+                                       lags=_lags(mod, dk, c, bidirectional), dk=dk)
             if kf2 is not None:
-                m2 = min(k2_len, c)
-                du2, dk2_c, _, _ = _conv._bwd(sub, dout_c, u_c, kf2, m2, None, None)
+                du2, _, _, _ = _conv._bwd(sub, dout_c, u_c, kf2, k2_len, None, None,
+                                          lags=_lags(mod, dk2, c, bidirectional), dk=dk2)
                 du_c.add_(du2)
-                dk2[:, :m2] += dk2_c
             mod.__dict__['last_launches'] += sub.last_launches
         rows = [_rows(t) for t in dst]
         if docs.n_items:
@@ -250,13 +293,16 @@ def backward(mod, docs, dout, u, pregate, postgate, spectra, k_len, k2_len=None,
 
 
 class DocsConvFunc(torch.autograd.Function):
-    """FlashFFTConv(...)(u, k, pregate, postgate, docs=table): y = postgate * conv(u * pregate, k) per document."""
+    """FlashFFTConv(...)(u, k, pregate, postgate, docs=table, bidirectional=...): y = postgate * conv(u * pregate, k)
+    per document."""
 
     @staticmethod
-    def forward(ctx, u, k, mod, save, docs, pregate=None, postgate=None):
+    def forward(ctx, u, k, mod, save, docs, pregate=None, postgate=None, bidirectional=False):
         mod.__dict__['last_launches'] = 0
-        y, spectra = forward(mod, docs, u, k, pregate, postgate, use_cache=not mod.training)
+        y, spectra = forward(mod, docs, u, k, pregate, postgate, use_cache=not mod.training,
+                             bidirectional=bidirectional)
         ctx.mod, ctx.docs, ctx.k_len, ctx.spectra = mod, docs, k.shape[-1], spectra
+        ctx.bidirectional = bidirectional
         if save:
             ctx.save_for_backward(u, pregate, postgate)
         return y
@@ -265,8 +311,9 @@ class DocsConvFunc(torch.autograd.Function):
     def backward(ctx, dout):
         u, pregate, postgate = ctx.saved_tensors
         ctx.mod.__dict__['last_launches'] = 0
-        du, dk, dpre, dpost, _ = backward(ctx.mod, ctx.docs, dout, u, pregate, postgate, ctx.spectra, ctx.k_len)
-        return du, dk, None, None, None, dpre, dpost
+        du, dk, dpre, dpost, _ = backward(ctx.mod, ctx.docs, dout, u, pregate, postgate, ctx.spectra, ctx.k_len,
+                                          bidirectional=ctx.bidirectional)
+        return du, dk, None, None, None, dpre, dpost, None
 
 
 class MixerDocsFunc(torch.autograd.Function):
@@ -274,11 +321,12 @@ class MixerDocsFunc(torch.autograd.Function):
     (B, 3D, L) projection, read in place; the backward scatters d x1, d x2, d v into one (B, 3D, L) gradient."""
 
     @staticmethod
-    def forward(ctx, x1x2v, k, k2, mod, d_model, docs):
+    def forward(ctx, x1x2v, k, k2, mod, d_model, docs, bidirectional=False):
         x1, x2, v = x1x2v.split(d_model, dim=1)
         mod.__dict__['last_launches'] = 0
-        y, spectra = forward(mod, docs, v, k, x1, x2, k2)
+        y, spectra = forward(mod, docs, v, k, x1, x2, k2, bidirectional=bidirectional)
         ctx.mod, ctx.d_model, ctx.docs, ctx.spectra = mod, d_model, docs, spectra
+        ctx.bidirectional = bidirectional
         ctx.k_len = k.shape[-1]
         ctx.k2_len = None if k2 is None else k2.shape[-1]
         if any(ctx.needs_input_grad[:3]):
@@ -293,5 +341,5 @@ class MixerDocsFunc(torch.autograd.Function):
         grad = torch.empty_like(x1x2v, memory_format=torch.contiguous_format)
         dx1, dx2, dv = grad.split(ctx.d_model, dim=1)
         _, dk, _, _, dk2 = backward(ctx.mod, ctx.docs, dout, v, x1, x2, ctx.spectra, ctx.k_len, ctx.k2_len,
-                                    out=(dv, dx1, dx2))
-        return grad, dk, dk2, None, None, None
+                                    out=(dv, dx1, dx2), bidirectional=ctx.bidirectional)
+        return grad, dk, dk2, None, None, None, None

@@ -110,7 +110,7 @@ def _mixer_backward(mod, D, dout, x1x2v, kf, k_len, kf2, k2_len, short=None):
     return grad, dk, dk2
 
 
-def hyena_mixer(conv, x1x2v, k, d_model, residual_filter=None, docs=None):
+def hyena_mixer(conv, x1x2v, k, d_model, residual_filter=None, docs=None, bidirectional=False):
     """The long-convolution part of the reference's Hyena / M2 sequence mixers on the (B, 3*d_model, L) projection
     (monarch_mixer_sequence_mixer_flashfftconv.py:131-177): y = conv(x1 * v, k) * x2 [+ conv(v, k2)], where
     x1, x2, v = x1x2v.split(d_model, dim=1).
@@ -121,16 +121,18 @@ def hyena_mixer(conv, x1x2v, k, d_model, residual_filter=None, docs=None):
     its input gradient is added into the v slice of that gradient with one add.  Like gated_long_conv, this calls the
     engine directly rather than conv(...): forward hooks registered on the module do not run for it.
 
-    docs: a DocumentTable of packed documents in the rows of x1x2v; each document is then mixed alone and causally
-    (flashfftconv.docs): one gather of the three slices, read in place, into class batches, hyena_mixer's engine calls
-    per class, one scatter of y; the backward scatters d x1, d x2 and d v into the slices of one gradient."""
+    docs: a DocumentTable of packed documents in the rows of x1x2v; each document is then mixed alone (flashfftconv.docs):
+    one gather of the three slices, read in place, into class batches, hyena_mixer's engine calls per class, one scatter
+    of y; the backward scatters d x1, d x2 and d v into the slices of one gradient.  bidirectional: with docs, k and k2
+    keep their negative lags (lag -j reads k[:, conv.seqlen - j], M2-BERT's two-sided filters), else each document is
+    mixed causally.  Without docs the flag changes nothing: the plain call is already two-sided."""
     if docs is not None:
         x1, x2, v = x1x2v.split(d_model, dim=1)
         _conv._check_inputs(v, k, conv, (x1, x2), views=True)
         if residual_filter is not None:
             _conv._check_inputs(v, residual_filter, conv, views=True)
         _docs._check(docs, v)
-        return _docs.MixerDocsFunc.apply(x1x2v, k, residual_filter, conv, d_model, docs)
+        return _docs.MixerDocsFunc.apply(x1x2v, k, residual_filter, conv, d_model, docs, bool(bidirectional))
     return HyenaMixerFunc.apply(x1x2v, k, residual_filter, conv, d_model)
 
 
@@ -185,7 +187,7 @@ class ShortHyenaFunc(torch.autograd.Function):
         return dx, dw, dbias, dk, dk2, None, None, None
 
 
-def hyena_operator(conv, short_filter, x, k, d_model, residual_filter=None, docs=None):
+def hyena_operator(conv, short_filter, x, k, d_model, residual_filter=None, docs=None, bidirectional=False):
     """The whole Hyena / M2 sequence mixer from the raw (B, 3*d_model, L) projection x (the output of in_proj):
 
         s = short_filter(x)[..., :L];  x1, x2, v = s.split(d_model, dim=1)
@@ -202,7 +204,8 @@ def hyena_operator(conv, short_filter, x, k, d_model, residual_filter=None, docs
     `conv` and `short_filter` do not run for it.
 
     docs: a DocumentTable of packed documents in the rows of x.  The call is then short_filter(x, docs.cu_seqlens)
-    followed by hyena_mixer(..., docs=docs): both filters keep every document apart."""
+    followed by hyena_mixer(..., docs=docs, bidirectional=bidirectional): both filters keep every document apart.
+    Without docs, bidirectional changes nothing (see hyena_mixer)."""
     if not isinstance(short_filter, _dw.FlashDepthWiseConv1d) or not short_filter.is_bhl:
         raise RuntimeError('short_filter must be a BHL FlashDepthWiseConv1d')
     if short_filter.d != 3 * d_model:
@@ -214,7 +217,7 @@ def hyena_operator(conv, short_filter, x, k, d_model, residual_filter=None, docs
         raise RuntimeError(f'x must be (B, 3 * d_model = {3 * d_model}, L), got {tuple(x.shape)}')
     L = x.shape[-1]
     if docs is not None:
-        return hyena_mixer(conv, short_filter(x, docs.cu_seqlens), k, d_model, residual_filter, docs)
+        return hyena_mixer(conv, short_filter(x, docs.cu_seqlens), k, d_model, residual_filter, docs, bidirectional)
     if not _short_fused(conv, short_filter, x):
         return hyena_mixer(conv, short_filter(x)[..., :L], k, d_model, residual_filter)
     w, b = short_filter.weights, short_filter.bias

@@ -180,6 +180,30 @@ int bffc_kf_from_filter_band(const bffc_plan* plan, const void* k, int Lk, void*
 int bffc_dk_from_dkf_band(const bffc_plan* plan, const void* dkf_engine, void* dk, int Lk, int H, int band,
                           void* workspace, size_t workspace_bytes, void* stream);
 
+/*
+ * Two-sided filter-side transforms: the filter of a circular `period`-point convolution (lag -j read from k[period - j],
+ * as FlashFFTConv(period) reads it) placed on this plan's n-point circle (n = seqlen), with its lags cut to [-neg, pos).
+ * k is (H, Lk) fp32 with rows of Lk, Lk <= period (Lk may exceed n).
+ *   bffc_kf_from_filter_lags: kf_engine = pack(FFT_n(f)),  f[d] = k[h, d] for 0 <= d < pos,
+ *                             f[n - j] = k[h, period - j] for 1 <= j <= neg; a k index >= Lk reads as 0, other slots 0
+ *   bffc_dk_from_dkf_lags:    with g = ifft(unpack(dkf)).real the n-periodic gradient (what bffc_dk_from_dkf reads out),
+ *                             for every m < Lk in this order:
+ *                               dk[h, m] += g[m]                        if m < pos
+ *                               dk[h, m] += g[n - (period - m)]         if 1 <= period - m <= neg
+ *                             dk ACCUMULATES (zero it before the first call); each term is added as a separate fp32
+ *                             rounding, as `dk[:, idx] += term` in torch.  One thread per dk element: no atomics.
+ * pos = Lk, neg = 0 is bffc_kf_from_filter / bffc_dk_from_dkf of the same rows (the latter adding into dk).  Packed
+ * documents (flashfftconv.docs) run a class of length c on FlashFFTConv(2c) with period = seqlen of the caller's module,
+ * pos = min(Lk, c) and neg = c - 1 (bidirectional) or 0 (causal).  BFFC_ERR_INVALID, before the device is touched, for a
+ * negative period / pos / neg / Lk, pos + neg > n - 1, neg > period, Lk > period, and on composite plans (n > 8192) for a
+ * map that reads some k index both as a head and as a tail lag while n - period is not a multiple of 8192.  Workspace
+ * rule and launch count are those of the unbanded pair.
+ */
+int bffc_kf_from_filter_lags(const bffc_plan* plan, const void* k, int Lk, int period, int pos, int neg,
+                             void* kf_engine, int H, int conj, void* workspace, size_t workspace_bytes, void* stream);
+int bffc_dk_from_dkf_lags(const bffc_plan* plan, const void* dkf_engine, void* dk, int Lk, int period, int pos, int neg,
+                          int H, void* workspace, size_t workspace_bytes, void* stream);
+
 /* Scratch the caller must provide.  bffc_workspace_bytes_ex: exact need of bffc_fwd (backward = 0) or bffc_bwd
  * (backward = 1) for a gated / ungated call; bffc_workspace_bytes: enough for any call with these shapes.
  * seqlen <= 8192: 0, except the gated backward (two (B,H,L) tensors: the gated inputs handed to the dk_f kernel).

@@ -14,6 +14,16 @@ hyena_mixer (D = 768) on a (B, 3D, L) projection with and without the table.  Th
 each a CUDA-event window of at least --window seconds after warm-up; the median per arm is reported.
 
     python tools/docs_bench.py [--window 0.5] [--rounds 5]
+
+--bidirectional times the two-sided document call instead, at M2-BERT's shapes (FlashFFTConv(N) with a filter of
+length N = 2L): base at 2k (B=32, D=768, L=2048) and 8k (B=8, D=768, L=8192), fp16 and bf16, on seeded right-padded
+rows (DocumentTable.from_lengths) and on seeded packed rows.  Arms, forward + backward: the bidirectional document
+call, the causal document call on the same table (the same transform work), the plain call on the padded rows (what
+M2-BERT runs today), and hyena_mixer with the residual filter k2 (bidirectional, with the table).  One line per shape,
+dtype and layout, with the spread per arm and, from torch.profiler in a separate run, the filter-side kernels of one
+bidirectional forward + backward in launch order (one per class and call).
+
+    python tools/docs_bench.py --bidirectional [--window 0.5] [--rounds 5]
 """
 import argparse
 import json
@@ -43,11 +53,91 @@ def clocks():
         return f'unknown ({type(e).__name__})'
 
 
+M2_SHAPES = [('base_2k', 32, 768, 2048), ('base_8k', 8, 768, 8192)]
+
+
+def m2_tables(ffc, Bm, Lm, seed):
+    """{'padded': from_lengths of seeded lengths in [L/8, L], 'packed': seeded documents of 1 .. L/2 positions}."""
+    import numpy as np
+    rng = np.random.default_rng(seed)
+    lengths = rng.integers(Lm // 8, Lm + 1, size=Bm).tolist()
+    cu = [0]
+    for b in range(Bm):
+        t = 0
+        while t < Lm:
+            n = min(int(rng.integers(1, Lm // 2 + 1)), Lm - t)
+            t += n
+            cu.append(cu[-1] + n)
+    dev = torch.device('cuda')
+    return {'padded': ffc.DocumentTable.from_lengths(lengths, Lm, device=dev),
+            'packed': ffc.DocumentTable(torch.tensor(cu, dtype=torch.int32, device=dev), Bm, Lm)}
+
+
+def filter_kernels(fn):
+    """(name, microseconds) of the filter-side kernels (namespace bffc::ffft) of one fn() call, in launch order."""
+    from torch.profiler import ProfilerActivity, profile
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        fn()
+        torch.cuda.synchronize()
+    out = []
+    for e in sorted(prof.events(), key=lambda e: e.time_range.start):
+        if e.device_type.name == 'CUDA' and 'ffft' in e.name:
+            short = e.name.split('ffft::')[1].split('(')[0]
+            out.append((short, round(e.time_range.elapsed_us(), 2)))
+    return out
+
+
+def bidirectional(args):
+    import flashfftconv as ffc
+    dev = torch.device('cuda')
+    name, power = card()
+    for label, Bm, D, Lm in M2_SHAPES:
+        Nm = 2 * Lm
+        for dt, dts in ((torch.float16, 'fp16'), (torch.bfloat16, 'bf16')):
+            conv = ffc.FlashFFTConv(Nm, dtype=dt).to(dev)
+            torch.manual_seed(0)
+            proj = torch.randn(Bm, 3 * D, Lm, device=dev).to(dt).requires_grad_(True)
+            u = torch.randn(Bm, D, Lm, device=dev).to(dt).requires_grad_(True)
+            dout = torch.randn(Bm, D, Lm, device=dev).to(dt)
+            k = (torch.randn(D, Nm, device=dev) / Nm ** 0.5).requires_grad_(True)
+            k2 = (torch.randn(D, Nm, device=dev) / Nm ** 0.5).requires_grad_(True)
+            for layout, table in m2_tables(ffc, Bm, Lm, Lm).items():
+                res = {'bidirectional': True, 'shape': {'name': label, 'B': Bm, 'D': D, 'L': Lm, 'seqlen': Nm,
+                                                        'dtype': dts},
+                       'layout': layout, 'classes': {str(c): n for c, n in table.counts.items()},
+                       'card': name, 'power_limit': power, 'clocks_before': clocks()}
+
+                def fb(f):
+                    def run():
+                        f().backward(dout)
+                    return run
+                arms = {
+                    'bidi_docs_fwdbwd': fb(lambda: conv(u, k, docs=table, bidirectional=True)),
+                    'causal_docs_fwdbwd': fb(lambda: conv(u, k, docs=table)),
+                    'plain_padded_fwdbwd': fb(lambda: conv(u, k)),
+                    'mixer_k2_bidi_docs_fwdbwd': fb(lambda: ffc.hyena_mixer(conv, proj, k, D, k2, docs=table,
+                                                                            bidirectional=True)),
+                }
+                times = {a: [] for a in arms}
+                for _ in range(args.rounds):
+                    for a, fn in arms.items():
+                        times[a].append(timed(fn, args.window))
+                res.update({a + '_ms': statistics.median(v) for a, v in times.items()})
+                res['spread_pct'] = {a: 100 * (max(v) - min(v)) / statistics.median(v) for a, v in times.items()}
+                res['bidi_over_causal'] = res['bidi_docs_fwdbwd_ms'] / res['causal_docs_fwdbwd_ms']
+                res['filter_kernels_us'] = filter_kernels(arms['bidi_docs_fwdbwd'])
+                res['clocks_after'] = clocks()
+                print(json.dumps(res), flush=True)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument('--window', type=float, default=0.5)
     ap.add_argument('--rounds', type=int, default=5)
+    ap.add_argument('--bidirectional', action='store_true')
     args = ap.parse_args()
+    if args.bidirectional:
+        return bidirectional(args)
     import flashfftconv as ffc
     from flashfftconv import docs as docs_mod
     dev = torch.device('cuda')
