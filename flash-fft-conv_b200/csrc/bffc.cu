@@ -246,6 +246,17 @@ int bffc_abi_version(void) { return BFFC_ABI_VERSION; }
 const char* bffc_last_error(void) { return g_err; }
 int bffc_last_launch_count(void) { return g_launches; }
 
+#ifdef BFFC_PHASE_CLOCK
+// diagnostic build only (fwd3_r128.cuh, tools/fwd_phases.py): where the fused forward kernel adds its phase cycles
+// (a zeroed device buffer of 2 x (kPhases + 1) uint64), and whether pipeline 1 of each CTA stays idle
+int bffc_phase_clock(void* buf, int one_pipe) {
+  CUDA_TRY(cudaMemcpyToSymbol(bffc::r128::g_phase_buf, &buf, sizeof(buf)));
+  CUDA_TRY(cudaMemcpyToSymbol(bffc::r128::g_phase_one_pipe, &one_pipe, sizeof(one_pipe)));
+  return BFFC_OK;
+}
+int bffc_phase_count(void) { return bffc::r128::kPhases; }
+#endif
+
 static int levels_for(int N, bffc_level* lev) {
   switch (N) {
     case 256: case 512: case 1024: case 2048: case 4096: return 0;
@@ -845,6 +856,25 @@ struct PassOpts {
   bool corr = false;                // blocked: the pass is a correlation (du), its windows start at the block
 };
 
+// fwd3_kernel launch; dependent (the plain instantiation only, fwd3_r128.cuh kKfSlot): as a programmatic dependent of
+// the kernel before it on the stream, so that its prologue (plan-owned tables only) runs while that kernel finishes; it
+// waits for it before touching caller memory
+template <class K, class... A>
+static int launch_fwd3(K kern, bool dependent, int grid, cudaStream_t st, A&&... args) {
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr[0].val.programmaticStreamSerializationAllowed = 1;
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(grid);
+  cfg.blockDim = dim3(bffc::r128::kThreads3);
+  cfg.dynamicSmemBytes = bffc::r128::kSmemTotal3;
+  cfg.stream = st;
+  cfg.attrs = attr;
+  cfg.numAttrs = dependent ? 1 : 0;
+  CUDA_TRY(cudaLaunchKernelEx(&cfg, kern, std::forward<A>(args)...));
+  return launched();
+}
+
 // fused 8192-point kernel on (B, H, L) real sequences (seqlen <= 8192)
 static int launch_fused(const bffc_plan* p, Seq u, const void* kf, Seq pregate, Seq postgate, Seq y, int B, int H,
                         int L, cudaStream_t st, const PassOpts& po = PassOpts()) {
@@ -882,15 +912,16 @@ static int launch_fused(const bffc_plan* p, Seq u, const void* kf, Seq pregate, 
     static_cast<bffc::FwdParams&>(sprm) = prm;
     sprm.sf = *po.sf;
   }
+  int rc = 0;
   FMT_SWITCH(p->dtype,
     if (po.sf)             // the gated pipeline, also for a filtered u without gates
-      fwd3_kernel<false, true, F, true><<<g3, kThreads3, kSmemTotal3, st>>>(tm_u, tm_y, tm_g, gm, sprm);
+      rc = launch_fwd3(fwd3_kernel<false, true, F, true>, false, g3, st, tm_u, tm_y, tm_g, gm, sprm);
     else if (gated)
-      fwd3_kernel<false, true, F><<<g3, kThreads3, kSmemTotal3, st>>>(tm_u, tm_y, tm_g, gm, prm);
+      rc = launch_fwd3(fwd3_kernel<false, true, F>, false, g3, st, tm_u, tm_y, tm_g, gm, prm);
     else
-      fwd3_kernel<false, false, F><<<g3, kThreads3, kSmemTotal3, st>>>(tm_u, tm_y, tm_g, gm, prm);
+      rc = launch_fwd3(fwd3_kernel<false, false, F>, true, g3, st, tm_u, tm_y, tm_g, gm, prm);
   );
-  return launched();
+  return rc;
 }
 
 // fused kernel on complex rows held in two planes (in place); rows = pairs * kf_rows
@@ -904,9 +935,10 @@ static int launch_planes(const bffc_plan* p, void* pre, void* pim, const void* k
   prm.units = kf_rows * pairs;
   using namespace bffc::r128;
   const GateMaps gm{tm_r, tm_r, tm_r, tm_r, tm_r};      // unused in this mode
-  FMT_SWITCH(p->dtype, (fwd3_kernel<true, false, F><<<persistent_grid(p, prm.units, kPipes3), kThreads3, kSmemTotal3, st>>>(
-      tm_r, tm_r, tm_i, gm, prm)););
-  return launched();
+  int rc = 0;
+  FMT_SWITCH(p->dtype, rc = launch_fwd3(fwd3_kernel<true, false, F>, false, persistent_grid(p, prm.units, kPipes3), st, tm_r,
+                                        tm_r, tm_i, gm, prm););
+  return rc;
 }
 
 // dk_f kernel on real tiles (maps u, dout, u, dout) or on complex rows (planes: u re, dout re, u im, dout im).

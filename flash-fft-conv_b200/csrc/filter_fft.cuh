@@ -157,6 +157,7 @@ __global__ void __launch_bounds__(kThreads, 3) kf_from_filter_kernel(const float
                                                                      int H, float scale, int conj, const float2* __restrict__ tw,
                                                                      int N, int band, Lags lg) {
   extern __shared__ float2 fbuf[];
+  grid_dep_launch();      // the fused forward kernel after this one (launch_fwd3) may start its prologue
   const int tid = threadIdx.x, ha = 2 * blockIdx.x, hb = ha + 1;
   const float* ka = k + size_t(ha) * Lk;
   const float* kb = k + size_t(hb < H ? hb : ha) * Lk;

@@ -33,7 +33,46 @@ constexpr int kSmemBars3 = 128;
 constexpr int kSmemTwSt3 = 128 * 8;             // (stc, sts) of every row (RowTw::store); the (bc, bs) part of the
                                                 // table takes the fourth DFT-64 plane, which no stage reads
 constexpr int kSmemRows3 = kPipeThreads * 4;    // FragPos::packed() of every thread of a pipeline
-constexpr int kSmemTotal3 = kSmemData3 + kSmemF + kSmemG + kSmemBars3 + kSmemTwSt3 + kSmemRows3 + 1024;
+
+// Phase clock of the unit loop (diagnostic build only, -DBFFC_PHASE_CLOCK; tools/fwd_phases.py): each pipeline's
+// leader thread adds the clock64() cycles of every phase below to a shared-memory row, and at the end of the kernel
+// adds the rows and its unit count to g_phase_buf[pipe][kPhases + 1].  g_phase_one_pipe: pipeline 1 of every CTA stays
+// idle (pipeline 0 takes the CTA's units), which separates a phase's latency from contention with the other pipeline.
+// The normal build compiles none of it.
+enum Phase {
+  kPhTmaWait, kPhPass0, kPhStage1, kPhBarStage1, kPhPass1, kPhStage2, kPhKfWait, kPhPass3, kPhStage3, kPhPass5,
+  kPhBarPass5, kPhStoreY, kPhPublishY, kPhStage4, kPhBarStage4, kPhGateWait, kPhPass6, kPhPublishOut, kPhStoreOut,
+  kPhases
+};
+#ifdef BFFC_PHASE_CLOCK
+__device__ unsigned long long* g_phase_buf;
+__device__ int g_phase_one_pipe;
+constexpr int kSmemClock3 = kPipes3 * kPhases * 8;
+struct PhaseClock {
+  uint32_t row;
+  long long t;
+  DEVINL void init(uint32_t s) {
+    row = s;
+    for (int i = 0; i < kPhases; ++i) st_shared_u64(row + 8u * i, 0ull);
+    t = clock64();
+  }
+  DEVINL void mark(int ph) {
+    const long long now = clock64();
+    st_shared_u64(row + 8u * ph, ld_shared_u64(row + 8u * ph) + uint64_t(now - t));
+    t = clock64();
+  }
+  DEVINL void flush(int pipe, int units) {
+    if (g_phase_buf == nullptr) return;   // clock off (bffc_phase_clock(NULL, ...))
+    unsigned long long* g = g_phase_buf + pipe * (kPhases + 1);
+    for (int i = 0; i < kPhases; ++i) atomicAdd(g + i, ld_shared_u64(row + 8u * i));
+    atomicAdd(g + kPhases, (unsigned long long)units);
+  }
+};
+#else
+constexpr int kSmemClock3 = 0;
+#endif
+
+constexpr int kSmemTotal3 = kSmemData3 + kSmemF + kSmemG + kSmemBars3 + kSmemTwSt3 + kSmemRows3 + kSmemClock3 + 1024;
 static_assert(kSmemTotal3 <= 227 * 1024, "shared memory per block");
 
 struct GateMaps { CUtensorMap pre, post, post2, y2, xg; };
@@ -103,6 +142,12 @@ fwd3_kernel(const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CU
   static_assert(!(kPlanes && kGated), "composite sizes apply their gates in the outer stages");
   static_assert(!kShort || kGated, "the short filter runs in the gated pipeline");
   constexpr bool kBlocks = !kShort;     // overlap-save blocks (FwdParams::nblk) run in the plain and gated instantiations
+  // plain (ungated real sequences): k_f goes through the unit's slot (see pass 3), and the grid is launched as a
+  // programmatic dependent of the kernel before it, the filter transform (launch_fwd3).  The gated pipelines keep their
+  // global loads of k_f: at the 128-register cap the copy's bookkeeping costs them spill slots inside the unit loop.  So
+  // do the complex rows of the composite sizes: with one batch pair (1M, B = 2) every unit has a k_f row of its own, and
+  // the copy measured slower than the loads there.
+  constexpr bool kKfSlot = !kGated && !kPlanes;
   using NT = Num<kFmt>;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t sbase = (smem_u32(smem_raw) + 1023u) & ~1023u;
@@ -126,6 +171,7 @@ fwd3_kernel(const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CU
 
   const uint32_t bar_tma0 = s_bars + pipe * 16;
   const uint32_t bar_g = s_bars + 32;
+  const uint32_t bar_kf = s_bars + 40 + pipe * 8;  // kKfSlot: the unit's k_f block has landed in its slot
 
   if (tid == 0) {
     tma_prefetch_desc(&tm_u);
@@ -140,6 +186,7 @@ fwd3_kernel(const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CU
   if (leader) {
     mbar_init(bar_tma0, 1);
     mbar_init(bar_tma0 + 8, 1);
+    if (kKfSlot) mbar_init(bar_kf, 1);
   }
   fence_barrier_init();
   __syncthreads();
@@ -152,8 +199,15 @@ fwd3_kernel(const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CU
 
   const int gp = blockIdx.x * kPipes3 + pipe;
   const int GP = gridDim.x * kPipes3;
-  const int u_begin = int((long long)p.units * gp / GP);
-  const int u_end = int((long long)p.units * (gp + 1) / GP);
+#ifdef BFFC_PHASE_CLOCK
+  const bool one_pipe = g_phase_one_pipe != 0;
+#else
+  constexpr bool one_pipe = false;
+#endif
+  const int u_begin = one_pipe ? (pipe ? 0 : int((long long)p.units * blockIdx.x / gridDim.x))
+                               : int((long long)p.units * gp / GP);
+  const int u_end = one_pipe ? (pipe ? 0 : int((long long)p.units * (blockIdx.x + 1) / gridDim.x))
+                             : int((long long)p.units * (gp + 1) / GP);
   const uint32_t s_slot0 = sbase + pipe * 2 * kSlotBytes;
 
   auto seq_index = [&](int unit) {      // complex-rows mode: plane row of the unit
@@ -184,10 +238,13 @@ fwd3_kernel(const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CU
       load_tile<false, kBlocks>(dst + kTileBytes, &tm_u, bar, uh, ug, 1, p, p.win);
     }
   };
+  // k_f block of channel h: 16 x 128 x 2 words (re, im) of two 16-bit values = one slot
+  auto kf_row = [&](int h) { return reinterpret_cast<const uint8_t*>(p.kf) + size_t(h) * kSlotBytes; };
   // Everything the first stage needs from global memory is requested up front and lands while the tables below are
-  // built: the first unit's tiles (TMA), the three DFT-64 tiles the stages read (one bulk copy, needed before the first
-  // stage 2 only).
-  if (leader && u_begin < u_end) issue_load(u_begin, 0);
+  // built: the three DFT-64 tiles the stages read (one bulk copy, needed before the first stage 2 only) and, gated, the
+  // first unit's tiles (TMA).  Ungated, the prologue reads plan-owned tables only, so that it can run while the kernel
+  // before this one (the filter transform) finishes; caller memory is touched only after grid_dep_wait below.
+  if (!kKfSlot && leader && u_begin < u_end) issue_load(u_begin, 0);
   if (tid == 0) {
     mbar_expect_tx(bar_g, 3 * kGTileBytes);
     for (int c = 0; c < 3 * kGTileBytes; c += 8192)
@@ -212,6 +269,16 @@ fwd3_kernel(const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CU
     tw[0].load(s_twb, s_tws, fp.row[0], fp.q);
     tw[1].load(s_twb, s_tws, fp.row[1], fp.q);
   };
+  if constexpr (kKfSlot) {
+    grid_dep_wait();                    // u, k_f and every output: only from here on
+    grid_dep_launch();                  // a dependent's prologue may use the SMs this grid's CTAs leave
+    if (leader && u_begin < u_end) {    // k_f of the first two channels -> L2 (the loop prefetches the later ones)
+      issue_load(u_begin, 0);
+      const int h0 = u_begin / p.pairs;
+      bulk_prefetch_l2(kf_row(h0), kSlotBytes);
+      if ((h0 + 1) * p.pairs < u_end) bulk_prefetch_l2(kf_row(h0 + 1), kSlotBytes);
+    }
+  }
   fence_proxy_async_smem();             // DFT-128 image: generic stores -> wgmma operand reads
   __syncthreads();
   mbar_wait(bar_g, 0);
@@ -249,6 +316,13 @@ fwd3_kernel(const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CU
   Acc d;
   d.zero();
   uint32_t are[4][4], aim[4][4];
+#ifdef BFFC_PHASE_CLOCK
+  PhaseClock clk;
+  if (leader) clk.init(s_rows + kSmemRows3 + pipe * kPhases * 8);
+  auto mark = [&](int ph) { if (leader) clk.mark(ph); };
+#else
+  auto mark = [](int) {};
+#endif
 
   for (int unit = u_begin, n = 0; unit < u_end; ++unit, ++n) {
     const int slot = kGated ? 0 : (n & 1);
@@ -257,6 +331,7 @@ fwd3_kernel(const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CU
     const int h = unit / p.pairs;
 
     mbar_wait(bar_tma0 + 8 * slot, kGated ? (n & 1) : ((n >> 1) & 1));
+    mark(kPhTmaWait);
     if (kGated) {
       if constexpr (kShort) {
         // ---------------- pass 0: s(u) [* s(pregate)] in place
@@ -288,18 +363,31 @@ fwd3_kernel(const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CU
         }
       }
     }
+    mark(kPhPass0);
 
     // ---------------- stage 1: D1 = F128 * X
     f128_stage<kFmt>(d, s_f, hf, sX, p.kmask);
     f128_wait<false>(d, frag());
+    mark(kPhStage1);
+    // kKfSlot: X is no longer needed, so the slot takes this channel's k_f (pass 3 reads it from there; pass 5's barrier
+    // keeps Y from overwriting it early), and the next channel's block is brought into L2 when this one is started
+    if constexpr (kKfSlot) pipe_sync();   // both halves' stage 1 has read X
     if (leader) {
       if (kGated) {
         if (emit_xg) tma_store_wait_read0();   // pass 5 overwrites slot 0 after the barrier below
-      } else if (unit + 1 < u_end) {           // the other slot's last reader was the previous unit's output store
-        tma_store_wait_read0();
-        issue_load(unit + 1, slot ^ 1);
+      } else {
+        if constexpr (kKfSlot) {
+          mbar_expect_tx(bar_kf, kSlotBytes);
+          bulk_load(sX, kf_row(h), kSlotBytes, bar_kf);
+          if (unit == h * p.pairs && (h + 1) * p.pairs < u_end) bulk_prefetch_l2(kf_row(h + 1), kSlotBytes);
+        }
+        if (unit + 1 < u_end) {                // the other slot's last reader was the previous unit's output store
+          tma_store_wait_read0();
+          issue_load(unit + 1, slot ^ 1);
+        }
       }
     }
+    mark(kPhBarStage1);
 
     // ---------------- pass 1: * W^{k1 j} -> A operand of stage 2
     {
@@ -308,22 +396,32 @@ fwd3_kernel(const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CU
       twiddle_frag<false>(d, tw, p.tw_scale);
     }
     frag_to_a<kFmt>(d, are, aim);
+    mark(kPhPass1);
     // ---------------- stage 2: D_re = re * Gr + im * (-Gi),  D_im = re * Gi + im * Gr
     r64_stage<kFmt>(d, are, aim, s_g, s_g + 2 * kGTileBytes, s_g + kGTileBytes, s_g);
     wgmma_wait_regs(d);
+    mark(kPhStage2);
 
     // ---------------- pass 3: * k_f -> A operand of stage 3.  This thread's k2 = 8 i + 2 q + {0, 1}: one word pair
     // (re, im) of k_f per i, at eng::kf_pair(k1, 8 i + 2 q) — spelled out below: the helper changes this kernel's code.
+    // kKfSlot: the channel's k_f block is in the slot, at the same byte offsets (a warp's load: two 128-byte rows, no
+    // bank conflicts).
+    if constexpr (kKfSlot) mbar_wait(bar_kf, n & 1);
+    mark(kPhKfWait);
     {
       const FragPos fp = frag();
       const uint2* kfp = reinterpret_cast<const uint2*>(p.kf) + size_t(h) * 16 * 128 * 2 + (fp.q & 1);
+      const uint32_t kfs = sX + 8u * uint32_t(fp.q & 1);
       const f32x2 kfs2 = pk2(p.kf_scale, p.kf_scale);
 #pragma unroll
       for (int rr = 0; rr < 2; ++rr) {
         const int k1 = fp.row[rr];
         uint2 kv[8];
 #pragma unroll
-        for (int i = 0; i < 8; ++i) kv[i] = __ldg(kfp + ((2 * i + (fp.q >> 1)) * 128 + k1) * 2);
+        for (int i = 0; i < 8; ++i) {
+          if constexpr (kKfSlot) kv[i] = ld_shared_v2(kfs + uint32_t((2 * i + (fp.q >> 1)) * 128 + k1) * 16u);
+          else kv[i] = __ldg(kfp + ((2 * i + (fp.q >> 1)) * 128 + k1) * 2);
+        }
 #pragma unroll
         for (int i = 0; i < 8; ++i) {
           f32x2 kr2 = NT::unpack(kv[i].x), ki2 = NT::unpack(kv[i].y ^ p.kf_conj_mask);
@@ -337,9 +435,11 @@ fwd3_kernel(const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CU
       }
     }
     frag_to_a<kFmt>(d, are, aim);
+    mark(kPhPass3);
     // ---------------- stage 3: inverse radix-64, D_re = re * Gr + im * Gi,  D_im = re * (-Gi) + im * Gr
     r64_stage<kFmt>(d, are, aim, s_g, s_g + kGTileBytes, s_g + 2 * kGTileBytes, s_g);
     wgmma_wait_regs(d);
+    mark(kPhStage3);
 
     // ---------------- pass 5: * conj W -> Y tiles in the slot (MN-major B operand of stage 4)
     {
@@ -347,13 +447,20 @@ fwd3_kernel(const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CU
       row_tw(tw);
       twiddle_frag<true>(d, tw, p.tw_scale);
     }
-    pipe_sync();                          // both halves' stage 1 has read X (and the xg store has left the slot)
+    mark(kPhPass5);
+    pipe_sync();                          // both halves' stage 1 has read X (and the xg store has left the slot);
+                                          // kKfSlot: their pass 3 has read k_f.  Y overwrites the slot
+    mark(kPhBarPass5);
     frag_store_tile<kFmt>(sX, frag(), d);
+    mark(kPhStoreY);
     publish_smem();
+    mark(kPhPublishY);
     // ---------------- stage 4: conj F128 * Y (its pair butterfly runs in pass 6)
     f128_stage<kFmt>(d, s_f, hf, sX, 0xff);
     wgmma_wait_regs(d);
+    mark(kPhStage4);
     pipe_sync();                          // both halves' stage 4 has read Y: the slot takes the output
+    mark(kPhBarStage4);
 
     // ---------------- pass 6: pair butterfly, fp32 -> 16 bit output tiles (x output gate), TMA store.  The butterfly
     // works on copies of the accumulator on their way to 16 bit: rewriting the accumulator in place (f128_wait) costs
@@ -399,8 +506,11 @@ fwd3_kernel(const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CU
         pipe_sync();
       }
     }
+    mark(kPhGateWait);
     pass6(has_post);
+    mark(kPhPass6);
     publish_smem();
+    mark(kPhPublishOut);
     if (leader) {
       store_out(&tm_y);
       if (has_post2) {                    // slot 1 has been read by every thread (barrier above): second gate -> slot 1
@@ -429,9 +539,13 @@ fwd3_kernel(const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CU
       tma_store_wait_read0();
       issue_load(unit + 1, 0);
     }
+    mark(kPhStoreOut);
   }
 
   if (leader) tma_store_wait_all0();
+#ifdef BFFC_PHASE_CLOCK
+  if (leader) clk.flush(pipe, u_end - u_begin);
+#endif
 }
 
 }  // namespace r128

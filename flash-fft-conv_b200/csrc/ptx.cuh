@@ -64,6 +64,14 @@ DEVINL void bulk_load(uint32_t dst_smem, const void* src, uint32_t bytes, uint32
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
                ::"r"(dst_smem), "l"(reinterpret_cast<uint64_t>(src)), "r"(bytes), "r"(bar) : "memory");
 }
+// hint: bring [src, src + bytes) into L2; bytes % 16 == 0
+DEVINL void bulk_prefetch_l2(const void* src, uint32_t bytes) {
+  asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(reinterpret_cast<uint64_t>(src)), "r"(bytes) : "memory");
+}
+// Programmatic dependent launch: wait until the grids this one depends on have completed and their memory is visible
+// (returns at once when it was not launched as a dependent), and let dependents of this grid start launching
+DEVINL void grid_dep_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
+DEVINL void grid_dep_launch() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 DEVINL void tma_load_3d(uint32_t dst_smem, const void* map, uint32_t bar, int c0, int c1, int c2) {
   asm volatile(
       "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"

@@ -134,6 +134,12 @@ DEVINL uint2 ld_shared_v2(uint32_t addr) {
   return v;
 }
 DEVINL void st_shared_u32(uint32_t addr, uint32_t v) { asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(v) : "memory"); }
+DEVINL uint64_t ld_shared_u64(uint32_t addr) {
+  uint64_t v;
+  asm volatile("ld.shared.b64 %0, [%1];" : "=l"(v) : "r"(addr));
+  return v;
+}
+DEVINL void st_shared_u64(uint32_t addr, uint64_t v) { asm volatile("st.shared.b64 [%0], %1;" ::"r"(addr), "l"(v) : "memory"); }
 
 // DFT-128 image (row-major 128 x 128 in global memory) -> the K-major, 128B-swizzled operand image at `dst`
 DEVINL void load_dft128(uint8_t* dst, const __nv_bfloat16* dft, int tid, int nthreads) {
