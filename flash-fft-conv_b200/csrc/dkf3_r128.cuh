@@ -36,8 +36,10 @@ namespace bffc {
 struct DkfParams {
   const __nv_bfloat16* dft;  // see FwdParams
   const uint8_t* gtiles;
-  float2* dkf;               // [H][8192] complex fp32, engine order (engine_order.cuh)
-  int B, H, L, pairs, kmask;  // pairs = batch groups per channel; kmask as in FwdParams
+  float2* dkf;               // [rows][8192] complex fp32, engine order (engine_order.cuh); rows = H / cpg
+  int B, H, L, pairs, kmask;  // H: sequence rows per pair (channels * R); pairs = batch groups per channel; kmask as in
+                              // FwdParams
+  int cpg, R;                 // grouped filters: channels per dk_f row group, rows per channel (dkf_slabs.cuh unit map)
   int nseg, seg_bytes;        // segmented tiles (small sizes), see load_tile()
   float tw_scale;            // see FwdParams::tw_scale; dkf_unpack compensates
   int tw_n, tw_mask;         // see FwdParams
@@ -48,9 +50,9 @@ struct DkfParams {
 
 // dkf3_fixed_kernel: DkfParams and the slab partition of the launch (dkf_slabs.cuh)
 struct DkfDetParams : DkfParams {
-  int slabs;                 // S = slab::slabs(H, pairs)
+  int slabs;                 // S = slab::slabs(H / cpg, cpg * pairs)
   int accumulate;            // S = 1: add each row's sum into dk_f (a later batch chunk of the same rows); else store it
-  float2* part;              // S > 1: the launch's partial slots [H * S][8192], engine order; S = 1: null
+  float2* part;              // S > 1: the launch's partial slots [rows * S][8192], engine order; S = 1: null
 };
 
 namespace r128 {
@@ -65,7 +67,7 @@ static_assert(kSmemTotalDkf3 <= 227 * 1024, "shared memory per block");
 template <bool kDet, class P>
 __device__ __forceinline__ int first_unit(const P& p, long long total, unsigned i) {
   if constexpr (kDet)
-    return int(slab::slab_unit(p.pairs, p.slabs, slab::cta_slab((long long)p.H * p.slabs, i, gridDim.x)));
+    return int(slab::slab_unit(p.cpg * p.pairs, p.slabs, slab::cta_slab((long long)(p.H / p.cpg) * p.slabs, i, gridDim.x)));
   else
     return int(total * i / gridDim.x);
 }
@@ -97,15 +99,19 @@ __device__ __forceinline__ void dkf3_body(const CUtensorMap& tm_u, const CUtenso
   }
   __syncthreads();
 
-  // work split: the H * pairs units (channel-major: g = h * pairs + pr) are cut into gridDim.x contiguous ranges, so the
-  // grid is not limited by the channel count and no CTA carries a whole extra channel.  A channel that straddles two
-  // CTAs is completed by both through fp32 reductions into the zero-initialised gradient (red.global.add), as is every
-  // other flush.  kDet: the ranges end at slab boundaries, and every slab end flushes.
+  // work split: the H * pairs units (row-major over dk_f rows: g = row * M + member, dkf_slabs.cuh; ungrouped, M = pairs
+  // and g = h * pairs + pr) are cut into gridDim.x contiguous ranges, so the grid is not limited by the channel count and
+  // no CTA carries a whole extra row.  A row that straddles two CTAs is completed by both through fp32 reductions into
+  // the zero-initialised gradient (red.global.add), as is every other flush.  kDet: the ranges end at slab boundaries,
+  // and every slab end flushes.
   const long long total = (long long)p.H * p.pairs;
   const int g_begin = first_unit<kDet>(p, total, blockIdx.x), g_end = first_unit<kDet>(p, total, blockIdx.x + 1);
   const int n_units = g_end - g_begin;
-  auto unit_h = [&](int n) { return (g_begin + n) / p.pairs; };
+  const int M = p.cpg * p.pairs;                     // members of a dk_f row
+  auto unit_h = [&](int n) { return slab::unit_seq(p.R, p.cpg, p.pairs, g_begin + n); };  // its channel (* R + r)
   auto unit_pr = [&](int n) { return (g_begin + n) % p.pairs; };
+  auto unit_row = [&](int n) { return (g_begin + n) / M; };          // its dk_f row
+  auto unit_m = [&](int n) { return (g_begin + n) % M; };            // its member of that row
   auto issue_load = [&](int n, int which) {          // which: 0 = u pair, 1 = dout pair
     const int h = unit_h(n), pr = unit_pr(n);
     const uint32_t bar = which ? bar_tma_d : bar_tma_u;
@@ -194,14 +200,14 @@ __device__ __forceinline__ void dkf3_body(const CUtensorMap& tm_u, const CUtenso
         acc[32 + k] = fmaf(b, c[e], acc[32 + k]) - a * dd[e];
       }
     }
-    // ---- channel (or this CTA's share of it) finished: add it to the gradient spectrum
-    const bool flush = unit_pr(n) == p.pairs - 1 || n == n_units - 1;
+    // ---- dk_f row (or this CTA's share of it) finished: add it to the gradient spectrum
+    const bool flush = unit_m(n) == M - 1 || n == n_units - 1;
     if constexpr (kDet) {
       // a slab finished: its sum, stored into its partial slot, or as (or into, for a later batch chunk) the row of dk_f
-      if (!flush && slab::slab_of(p.pairs, p.slabs, unit_pr(n)) == slab::slab_of(p.pairs, p.slabs, unit_pr(n) + 1))
+      if (!flush && slab::slab_of(M, p.slabs, unit_m(n)) == slab::slab_of(M, p.slabs, unit_m(n) + 1))
         continue;
-      const int h = unit_h(n);
-      float2* row = p.part ? p.part + (size_t(h) * p.slabs + slab::slab_of(p.pairs, p.slabs, unit_pr(n))) * eng::kRowLen
+      const int h = unit_row(n);
+      float2* row = p.part ? p.part + (size_t(h) * p.slabs + slab::slab_of(M, p.slabs, unit_m(n))) * eng::kRowLen
                            : p.dkf + size_t(h) * eng::kRowLen;
       const bool add = p.accumulate && !p.part;
 #pragma unroll
@@ -221,7 +227,7 @@ __device__ __forceinline__ void dkf3_body(const CUtensorMap& tm_u, const CUtenso
 #pragma unroll
       for (int i = 0; i < 64; ++i) acc[i] = 0.f;
     } else if (flush) {
-      const int h = unit_h(n);
+      const int h = unit_row(n);
 #pragma unroll
       for (int rr = 0; rr < 2; ++rr) {
         const int k1 = fp.row[rr];

@@ -13,7 +13,14 @@
 // kSlabTarget sets how many slabs a launch with few rows is cut into: enough for every SM of an H100 to take several,
 // whole slabs, and no more, because each slab of an S > 1 launch costs one 64 KB slot written and read again.  S > 1
 // only when rows < kSlabTarget, so a launch has fewer than rows * (kSlabTarget / rows + 1) <= kSlabTarget + rows - 1
-// < 2 * kSlabTarget slots: less than 64 MB.
+// < 2 * kSlabTarget slots: less than 64 MB.  That holds for any (rows, pairs), so also for grouped filters below.
+//
+// Grouped filters (bffc_bwd_grouped): cpg consecutive channels of a launch share one filter row, so their units sum into
+// one dk_f row.  A launch holds whole groups of cpg channels, or part of one group (cpg = the launch's channels); each
+// channel has R rows (R = 1 for real sequences, the radix R = N / 8192 for the complex rows of the composite sizes).
+// The reduction is the one above with rows = (channels / cpg) * R and pairs = M = cpg * pairs: unit n belongs to
+// reduction row rho = n / M as member m = n % M = c * pairs + pr, channel c of the group, batch pair pr.  It reads the
+// sequence row (channel * R + r) of unit_seq.  cpg = 1 is the ungrouped map: rho = n / pairs, unit_seq(n) = rho.
 #pragma once
 
 namespace bffc {
@@ -41,6 +48,13 @@ SLAB_FN long long slab_unit(int pairs, int S, long long j) { return (j / S) * pa
 SLAB_FN long long partial_slots(int rows, int pairs) {
   const int S = slabs(rows, pairs);
   return S > 1 ? (long long)rows * S : 0;
+}
+// sequence row (channel * R + r of the launch) of unit n < 2^31: channel (rho / R) * cpg + c, row r = rho % R.  32-bit
+// arithmetic (the dk_f kernel's leader computes it where it issues the next loads); cpg = 1 is rho itself
+SLAB_FN int unit_seq(int R, int cpg, int pairs, int n) {
+  if (cpg == 1) return n / pairs;
+  const int M = cpg * pairs, rho = n / M;
+  return ((rho / R) * cpg + (n - rho * M) / pairs) * R + rho % R;
 }
 
 #undef SLAB_FN

@@ -72,7 +72,9 @@ struct PhaseClock {
 constexpr int kSmemClock3 = 0;
 #endif
 
-constexpr int kSmemTotal3 = kSmemData3 + kSmemF + kSmemG + kSmemBars3 + kSmemTwSt3 + kSmemRows3 + kSmemClock3 + 1024;
+constexpr int kSmemKb3 = kThreads3 * 4;         // gated: each thread's copy of its unit's k_f block (see pass 3)
+constexpr int kSmemTotal3 =
+    kSmemData3 + kSmemF + kSmemG + kSmemBars3 + kSmemTwSt3 + kSmemRows3 + kSmemClock3 + kSmemKb3 + 1024;
 static_assert(kSmemTotal3 <= 227 * 1024, "shared memory per block");
 
 struct GateMaps { CUtensorMap pre, post, post2, y2, xg; };
@@ -158,6 +160,7 @@ fwd3_kernel(const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CU
   const uint32_t s_twb = s_g + 3 * kGTileBytes;    // stage-1 twiddle table (RowTw::store)
   const uint32_t s_tws = s_bars + kSmemBars3;
   const uint32_t s_rows = s_tws + kSmemTwSt3;
+  auto s_kb = [&]() { return s_rows + kSmemRows3 + kSmemClock3 + 4u * threadIdx.x; };   // the thread's k_f block word
 
   const int tid = threadIdx.x;
   // warp-uniform by construction, so that the addresses and wgmma descriptors built from them live in uniform registers
@@ -238,8 +241,18 @@ fwd3_kernel(const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CU
       load_tile<false, kBlocks>(dst + kTileBytes, &tm_u, bar, uh, ug, 1, p, p.win);
     }
   };
-  // k_f block of channel h: 16 x 128 x 2 words (re, im) of two 16-bit values = one slot
+  // k_f block of filter row h: 16 x 128 x 2 words (re, im) of two 16-bit values = one slot
   auto kf_row = [&](int h) { return reinterpret_cast<const uint8_t*>(p.kf) + size_t(h) * kSlotBytes; };
+  // the k_f block of sequence row h: grouped filters share one filter row among kf_gs consecutive channels (FwdParams);
+  // the real sequences (kPlanes false) have one row per channel and no channel offset.  Complex rows with kf_gs == 1
+  // (every ungrouped call) take a uniform branch to block h, the index math of a kernel without groups; the real-sequence
+  // kernels need none (the plain one tracks the block from unit to unit, the gated ones compute it once per unit)
+  auto kf_block = [&](int h) {
+    if (kPlanes && p.kf_gs == 1) return h;
+    const uint32_t c = kPlanes ? uint32_t(p.kf_h0 + (h >> p.kf_rshift)) : uint32_t(h);     // the channel
+    const int g = int(__umulhi(c << 1, p.kf_gs_mul) >> p.kf_gs_shift);
+    return kPlanes ? (g << p.kf_rshift) | (h & ((1 << p.kf_rshift) - 1)) : g;
+  };
   // Everything the first stage needs from global memory is requested up front and lands while the tables below are
   // built: the three DFT-64 tiles the stages read (one bulk copy, needed before the first stage 2 only) and, gated, the
   // first unit's tiles (TMA).  Ungated, the prologue reads plan-owned tables only, so that it can run while the kernel
@@ -272,11 +285,11 @@ fwd3_kernel(const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CU
   if constexpr (kKfSlot) {
     grid_dep_wait();                    // u, k_f and every output: only from here on
     grid_dep_launch();                  // a dependent's prologue may use the SMs this grid's CTAs leave
-    if (leader && u_begin < u_end) {    // k_f of the first two channels -> L2 (the loop prefetches the later ones)
+    if (leader && u_begin < u_end) {    // k_f of the first two groups -> L2 (the loop prefetches the later ones)
       issue_load(u_begin, 0);
-      const int h0 = u_begin / p.pairs;
-      bulk_prefetch_l2(kf_row(h0), kSlotBytes);
-      if ((h0 + 1) * p.pairs < u_end) bulk_prefetch_l2(kf_row(h0 + 1), kSlotBytes);
+      const int g0 = kf_block(u_begin / p.pairs);
+      bulk_prefetch_l2(kf_row(g0), kSlotBytes);
+      if ((g0 + 1) * p.kf_gs * p.pairs < u_end) bulk_prefetch_l2(kf_row(g0 + 1), kSlotBytes);
     }
   }
   fence_proxy_async_smem();             // DFT-128 image: generic stores -> wgmma operand reads
@@ -324,11 +337,19 @@ fwd3_kernel(const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CU
   auto mark = [](int) {};
 #endif
 
+  // kKfSlot: the leader tracks the unit's k_f block (kf_g) and the first unit of the next group (kf_next) from unit to
+  // unit, so that no division sits between stage 1 and the copy it issues
+  const int kf_units = p.kf_gs * p.pairs;           // units of one group
+  int kf_g = kKfSlot ? kf_block(u_begin / p.pairs) : 0;
+  int kf_next = (kf_g + 1) * kf_units;
   for (int unit = u_begin, n = 0; unit < u_end; ++unit, ++n) {
     const int slot = kGated ? 0 : (n & 1);
     const uint32_t sX = s_slot0 + slot * kSlotBytes;
     const uint32_t sGate = s_slot0 + kSlotBytes;
     const int h = unit / p.pairs;
+    // gated: the unit's k_f block is computed here and parked in the thread's own shared-memory word until pass 3: at
+    // the 128-register cap the kShort instantiations spill when it is computed there or held in a register
+    if constexpr (kGated) st_shared_u32(s_kb(), uint32_t(kf_block(h)));
 
     mbar_wait(bar_tma0 + 8 * slot, kGated ? (n & 1) : ((n >> 1) & 1));
     mark(kPhTmaWait);
@@ -370,7 +391,7 @@ fwd3_kernel(const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CU
     f128_wait<false>(d, frag());
     mark(kPhStage1);
     // kKfSlot: X is no longer needed, so the slot takes this channel's k_f (pass 3 reads it from there; pass 5's barrier
-    // keeps Y from overwriting it early), and the next channel's block is brought into L2 when this one is started
+    // keeps Y from overwriting it early), and the next group's block is brought into L2 when this one is started
     if constexpr (kKfSlot) pipe_sync();   // both halves' stage 1 has read X
     if (leader) {
       if (kGated) {
@@ -378,8 +399,9 @@ fwd3_kernel(const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CU
       } else {
         if constexpr (kKfSlot) {
           mbar_expect_tx(bar_kf, kSlotBytes);
-          bulk_load(sX, kf_row(h), kSlotBytes, bar_kf);
-          if (unit == h * p.pairs && (h + 1) * p.pairs < u_end) bulk_prefetch_l2(kf_row(h + 1), kSlotBytes);
+          if (unit == kf_next) { ++kf_g; kf_next += kf_units; }
+          bulk_load(sX, kf_row(kf_g), kSlotBytes, bar_kf);
+          if (unit == kf_next - kf_units && kf_next < u_end) bulk_prefetch_l2(kf_row(kf_g + 1), kSlotBytes);
         }
         if (unit + 1 < u_end) {                // the other slot's last reader was the previous unit's output store
           tma_store_wait_read0();
@@ -410,7 +432,8 @@ fwd3_kernel(const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CU
     mark(kPhKfWait);
     {
       const FragPos fp = frag();
-      const uint2* kfp = reinterpret_cast<const uint2*>(p.kf) + size_t(h) * 16 * 128 * 2 + (fp.q & 1);
+      const uint2* kfp = reinterpret_cast<const uint2*>(p.kf) + size_t(kGated ? int(ld_shared_u32(s_kb())) : kf_block(h)) * 16 * 128 * 2 +
+                         (fp.q & 1);
       const uint32_t kfs = sX + 8u * uint32_t(fp.q & 1);
       const f32x2 kfs2 = pk2(p.kf_scale, p.kf_scale);
 #pragma unroll

@@ -49,6 +49,12 @@ struct FwdParams {
   int units;                 // H * pairs
   uint32_t kf_conj_mask;     // 0x80008000: multiply by conj(k_f) (du path of the backward: correlation), else 0
   int nblk, srows, win;      // overlap-save blocks, see load_tile (1, 0, 0 outside bffc_fwd_blocked / bffc_bwd_blocked)
+  int kf_gs, kf_h0, kf_rshift;  // grouped filters: sequence row h (channel * R + r, R = 2^kf_rshift) of the launch reads
+                                // the k_f block of row (kf_h0 + h / R) / kf_gs * R + r of kf (1, 0, 0: block h); R = 1
+                                // for real sequences.  Complex rows: kf starts at the group of the launch's first
+                                // channel, kf_h0 is that channel's place in its group
+  uint32_t kf_gs_mul;        // c / kf_gs = umulhi(2 c, kf_gs_mul) >> kf_gs_shift for 0 <= c < 2^31 (group_divisor in
+  int kf_gs_shift;           // bffc.cu): a few instructions and one register at the kernel's 128-register cap
 };
 // parameters of the fused kernel's kShort instantiations: the short filter taps of u, pregate, postgate (short_filter.cuh)
 struct FwdShortParams : FwdParams {

@@ -70,6 +70,15 @@ SYMBOLS = {
                                           _c.c_int64, _c.c_void_p, _c.c_void_p, _c.c_int64, _c.c_void_p, _c.c_int64]
                                + [_c.c_int] * 3 + [_c.c_void_p] * 6 + [_c.c_int] * 3
                                + [_c.c_void_p, _c.c_size_t, _c.c_void_p]),
+    'bffc_workspace_bytes_grouped': (_c.c_size_t, [_c.c_void_p] + [_c.c_int] * 7),
+    'bffc_fwd_grouped': (_c.c_int, [_c.c_void_p, _c.c_void_p, _c.c_int64, _c.c_void_p, _c.c_void_p, _c.c_int64,
+                                    _c.c_void_p, _c.c_int64, _c.c_void_p, _c.c_int64] + [_c.c_int] * 5
+                         + [_c.c_void_p] * 6 + [_c.c_int] * 3 + [_c.c_void_p, _c.c_size_t, _c.c_void_p]),
+    'bffc_bwd_grouped': (_c.c_int, [_c.c_void_p, _c.c_void_p, _c.c_int64, _c.c_void_p, _c.c_int64, _c.c_void_p,
+                                    _c.c_void_p, _c.c_void_p, _c.c_int64, _c.c_void_p, _c.c_int64, _c.c_void_p,
+                                    _c.c_int64, _c.c_void_p, _c.c_void_p, _c.c_int64, _c.c_void_p, _c.c_int64]
+                         + [_c.c_int] * 5 + [_c.c_void_p] * 6 + [_c.c_int] * 3
+                         + [_c.c_void_p, _c.c_size_t, _c.c_void_p]),
     'bffc_host_chunk_batch': (_c.c_int, [_c.c_void_p, _c.c_int, _c.c_int, _c.c_int]),
     'bffc_host_workspace_bytes': (_c.c_size_t, [_c.c_void_p, _c.c_int, _c.c_int, _c.c_int, _c.c_int]),
     'bffc_fwd_host': (_c.c_int, [_c.c_void_p] * 6 + [_c.c_int] * 3 + [_c.c_void_p, _c.c_size_t, _c.c_void_p]),

@@ -30,7 +30,8 @@ def blocked_long_conv(conv, u, k, pregate=None, postgate=None, docs=None):
     """y = postgate * causal_conv(u * pregate, k) of any length L, in overlap-save blocks of FlashFFTConv(8192).
 
     conv: a FlashFFTConv(8192, dtype) module; u, pregate, postgate: (B, H, L) tensors of conv.dtype (channel slices of a
-    projection are read in place), the gates both given or both None; k: (H, Lk) fp32 filter, Lk <= 4097.  Gradients
+    projection are read in place), the gates both given or both None; k: (H, Lk) fp32 filter, Lk <= 4097, or (G, Lk)
+    with G dividing H (the call on k.repeat_interleave(H // G, 0); dk is (G, Lk)).  Gradients
     flow to u, k and the gates.  A ragged L is zero-padded to a multiple of 64, which does not change a causal result.
     Packed documents (docs) are not kept apart by the blocks yet: a DocumentTable is refused."""
     _docs.refuse(docs, 'blocked_long_conv')

@@ -85,15 +85,13 @@ class _Plan:
         self._ws_bytes = {}
         self._filter_ws_bytes = {}
 
-    def workspace_bytes(self, B, H, L, gated, backward, halo=None):
-        """bffc_workspace_bytes_ex, or bffc_workspace_bytes_blocked for overlap-save blocks with this halo"""
-        key = (B, H, L, gated, backward, halo)
+    def workspace_bytes(self, B, H, L, gated, backward, halo=None, G=None):
+        """bffc_workspace_bytes_grouped of G filter rows (None: H), with overlap-save blocks of this halo (None: none)"""
+        key = (B, H, L, gated, backward, halo, G)
         n = self._ws_bytes.get(key)
         if n is None:
-            if halo is None:
-                n = _lib.lib().bffc_workspace_bytes_ex(self.handle, B, H, L, int(gated), int(backward))
-            else:
-                n = _lib.lib().bffc_workspace_bytes_blocked(self.handle, B, H, L, int(halo), int(gated), int(backward))
+            n = _lib.lib().bffc_workspace_bytes_grouped(self.handle, B, H, H if G is None else G, L,
+                                                         -1 if halo is None else int(halo), int(gated), int(backward))
             self._ws_bytes[key] = n
         return n
 
@@ -189,7 +187,9 @@ class FlashFFTConv(torch.nn.Module):
         return _forward_host(self, u, k, pregate, postgate, out, device)
 
     def forward(self, u, k, pregate=None, postgate=None, docs=None, bidirectional=False):
-        """y = postgate * conv(u * pregate, k), the gates both given or both None.  docs: a DocumentTable of packed
+        """y = postgate * conv(u * pregate, k), the gates both given or both None.  k: (H, Lk), or (G, Lk) with G
+        dividing H for a filter shared by groups of H // G consecutive channels: the call is then this call with
+        k.repeat_interleave(H // G, 0), and the gradient of k has shape (G, Lk), the sum over each group.  docs: a DocumentTable of packed
         documents in the rows of u; each document is then convolved alone (flashfftconv.docs, INTEGRATION.md §11), with
         gradients to u, k and the gates.  bidirectional: with docs, each document keeps the filter's negative lags too
         (lag -j reads k[:, seqlen - j], as M2-BERT's two-sided filter of length seqlen = 2L has it), so it gets exactly
@@ -280,7 +280,7 @@ def _engine_view(t, dtype):
 
 
 def _check_inputs(u, k, mod, gates=(), views=False, blocked=False):
-    """views: u and the gates may be any (B, H, L) layout (channel slices are used in place, others copied).  blocked:
+    """k: (G, Lk) with G dividing H (grouped filters, include/bffc.h bffc_fwd_grouped).  views: u and the gates may be any (B, H, L) layout (channel slices are used in place, others copied).  blocked:
     overlap-save blocks (blocked_long_conv), where L may exceed the seqlen."""
     if not u.is_cuda:
         raise RuntimeError('u must be a CUDA tensor (bffc has no CPU path)')          # monarch_fwd.h:7-13
@@ -289,8 +289,8 @@ def _check_inputs(u, k, mod, gates=(), views=False, blocked=False):
     if u.dim() != 3 or not (views or u.is_contiguous()):
         raise RuntimeError('u must be a contiguous (B, H, L) tensor')
     B, H, L = u.shape
-    if k.dim() != 2 or k.shape[0] != H or k.shape[1] > mod.seqlen:
-        raise RuntimeError(f'k must be (H={H}, Lk<={mod.seqlen}), got {tuple(k.shape)}')
+    if k.dim() != 2 or k.shape[0] < 1 or H % k.shape[0] or k.shape[1] > mod.seqlen:
+        raise RuntimeError(f'k must be (G, Lk<={mod.seqlen}) with G dividing H={H}, got {tuple(k.shape)}')
     if L > mod.seqlen and not blocked:
         raise RuntimeError(f'L={L} exceeds seqlen={mod.seqlen}')
     for g in gates:
@@ -381,8 +381,8 @@ def _padded(t, Lp):
     return torch.nn.functional.pad(t, (0, Lp - t.shape[-1]))          # one kernel: copy + zero tail
 
 
-def _workspace(plan, B, H, L, gated, backward, device, halo=None):
-    n = plan.workspace_bytes(B, H, L, gated, backward, halo)
+def _workspace(plan, B, H, L, gated, backward, device, halo=None, G=None):
+    n = plan.workspace_bytes(B, H, L, gated, backward, halo, G)
     return (torch.empty(n, dtype=torch.uint8, device=device) if n else None), n
 
 
@@ -401,6 +401,10 @@ class _on_device:
             self.ctx.__exit__(*a)
 
 
+# the taps argument of bffc_fwd_grouped / bffc_bwd_grouped without a short filter (K, padding and w_dtype are ignored)
+_NO_TAPS = ((None,) * 6, 0, 1, 0)
+
+
 def _fwd(mod, u, k, pregate, postgate, band=None, use_cache=None, kf_engine=None, taps=None, halo=None, out=None,
          cache_key=None, lags=None):
     """y (contiguous) and the engine-order filter spectrum it used.  u and the gates: any (B, H, L) layout; those that
@@ -409,7 +413,8 @@ def _fwd(mod, u, k, pregate, postgate, band=None, use_cache=None, kf_engine=None
     K, padding), a short depthwise filter bffc_fwd_short_strided applies to u and the gates as it loads them; the rows
     are device addresses of (H, K) taps and (H) biases, None for a tensor that is not filtered.  halo: overlap-save
     blocks with this halo (bffc_fwd_blocked, blocked_long_conv), else None.  out: a contiguous (B, H, L) tensor to write y
-    into (L a multiple of bffc_length_multiple()).  cache_key, lags: see _kf_engine_for."""
+    into (L a multiple of bffc_length_multiple()).  cache_key, lags: see _kf_engine_for.  k (and kf_engine) may have
+    G rows, G dividing H: channel h then uses row h // (H // G) (bffc_fwd_grouped)."""
     B, H, L = u.shape
     dev = u.device
     plan = mod.plan(dev)
@@ -426,19 +431,13 @@ def _fwd(mod, u, k, pregate, postgate, band=None, use_cache=None, kf_engine=None
     with _on_device(dev):
         if kf_engine is None:
             kf_engine = _kf_engine_for(mod, plan, k, cache_key=cache_key, band=band, use_cache=use_cache, lags=lags)
+        G = kf_engine.shape[0]
         y = torch.empty((B, H, L), dtype=u.dtype, device=dev) if out is None else out
-        ws, ws_bytes = _workspace(plan, B, H, L, pre is not None, False, dev, halo)
-        if halo is not None:
-            rc = _lib.lib().bffc_fwd_blocked(plan.handle, _ptr(u), u_bs, _ptr(kf_engine), _ptr(pre), pre_bs, _ptr(post),
-                                             post_bs, _ptr(y), H * L, B, H, L, int(halo), _ptr(ws), ws_bytes, _stream())
-        elif taps is None:
-            rc = _lib.lib().bffc_fwd_strided(plan.handle, _ptr(u), u_bs, _ptr(kf_engine), _ptr(pre), pre_bs, _ptr(post),
-                                             post_bs, _ptr(y), H * L, B, H, L, _ptr(ws), ws_bytes, _stream())
-        else:
-            rows, w_dtype, K, P = taps
-            rc = _lib.lib().bffc_fwd_short_strided(plan.handle, _ptr(u), u_bs, _ptr(kf_engine), _ptr(pre), pre_bs,
-                                                   _ptr(post), post_bs, _ptr(y), H * L, B, H, L, *rows, w_dtype, K, P,
-                                                   _ptr(ws), ws_bytes, _stream())
+        ws, ws_bytes = _workspace(plan, B, H, L, pre is not None, False, dev, halo, G)
+        rows, w_dtype, K, P = _NO_TAPS if taps is None else taps
+        rc = _lib.lib().bffc_fwd_grouped(plan.handle, _ptr(u), u_bs, _ptr(kf_engine), _ptr(pre), pre_bs, _ptr(post),
+                                         post_bs, _ptr(y), H * L, B, H, G, L, -1 if halo is None else int(halo), *rows,
+                                         w_dtype, K, P, _ptr(ws), ws_bytes, _stream())
         _launched(mod, rc)
     return y, kf_engine
 
@@ -454,7 +453,8 @@ def _bwd(mod, dout, u, kf_engine, k_len, pregate, postgate, band=None, out=None,
     overlap-save blocks (bffc_bwd_blocked), else None.  Under torch.use_deterministic_algorithms(True) dk is summed in
     a fixed order (the module's deterministic plan): the same bits from run to run and on any GPU; du and the gate
     gradients are the same in either mode.  lags: the forward's lag map (_pack_kf); dk is then not made but added into
-    `dk`, an (H, k_len) fp32 tensor, through that map (bffc_dk_from_dkf_lags)."""
+    `dk`, a (G, k_len) fp32 tensor, through that map (bffc_dk_from_dkf_lags).  kf_engine of G rows (grouped filters,
+    bffc_bwd_grouped): dk is (G, k_len), the sum of the gradients of each group's channels."""
     B, H, L = u.shape
     plan = mod.plan(u.device, torch.are_deterministic_algorithms_enabled())
     Lp = _pad_len(plan, L)
@@ -483,26 +483,17 @@ def _bwd(mod, dout, u, kf_engine, k_len, pregate, postgate, band=None, out=None,
         t = o if s is not None else torch.empty((B, H, L), dtype=u.dtype, device=u.device)
         dst.append((t, s if s is not None else H * L, o if s is None else None))
     (du, du_bs, _), (dpre, dpre_bs, _), (dpost, dpost_bs, _) = dst
+    G = kf_engine.shape[0]
     with _on_device(u.device):
-        dkf_engine = torch.empty((H, N, 2), dtype=torch.float32, device=u.device)
-        ws, ws_bytes = _workspace(plan, B, H, L, gated, True, u.device, halo)
+        dkf_engine = torch.empty((G, N, 2), dtype=torch.float32, device=u.device)
+        ws, ws_bytes = _workspace(plan, B, H, L, gated, True, u.device, halo, G)
+        rows, w_dtype, K, P = _NO_TAPS if taps is None else taps
         # kf_engine_conj = NULL: the kernels conjugate the forward's spectrum in their pointwise multiply
-        if halo is not None:
-            rc = _lib.lib().bffc_bwd_blocked(plan.handle, _ptr(dout), dout_bs, _ptr(u), u_bs, _ptr(kf_engine), None,
-                                             _ptr(pre), pre_bs, _ptr(post), post_bs, _ptr(du), du_bs, _ptr(dkf_engine),
-                                             _ptr(dpre), dpre_bs, _ptr(dpost), dpost_bs, B, H, L, int(halo), _ptr(ws),
-                                             ws_bytes, _stream())
-        elif taps is None:
-            rc = _lib.lib().bffc_bwd_strided(plan.handle, _ptr(dout), dout_bs, _ptr(u), u_bs, _ptr(kf_engine), None,
-                                             _ptr(pre), pre_bs, _ptr(post), post_bs, _ptr(du), du_bs, _ptr(dkf_engine),
-                                             _ptr(dpre), dpre_bs, _ptr(dpost), dpost_bs, B, H, L, _ptr(ws), ws_bytes,
-                                             _stream())
-        else:
-            rows, w_dtype, K, P = taps
-            rc = _lib.lib().bffc_bwd_short_strided(plan.handle, _ptr(dout), dout_bs, _ptr(u), u_bs, _ptr(kf_engine),
-                                                   None, _ptr(pre), pre_bs, _ptr(post), post_bs, _ptr(du), du_bs,
-                                                   _ptr(dkf_engine), _ptr(dpre), dpre_bs, _ptr(dpost), dpost_bs, B, H,
-                                                   L, *rows, w_dtype, K, P, _ptr(ws), ws_bytes, _stream())
+        rc = _lib.lib().bffc_bwd_grouped(plan.handle, _ptr(dout), dout_bs, _ptr(u), u_bs, _ptr(kf_engine), None,
+                                         _ptr(pre), pre_bs, _ptr(post), post_bs, _ptr(du), du_bs, _ptr(dkf_engine),
+                                         _ptr(dpre), dpre_bs, _ptr(dpost), dpost_bs, B, H, G, L,
+                                         -1 if halo is None else int(halo), *rows, w_dtype, K, P, _ptr(ws), ws_bytes,
+                                         _stream())
         _launched(mod, rc)
         for t, _, o in dst:
             if o is not None:
@@ -510,16 +501,16 @@ def _bwd(mod, dout, u, kf_engine, k_len, pregate, postgate, band=None, out=None,
         # the kernels accumulate unnormalised pair-packed spectra in engine order; the reference takes
         # ifft(dk_f).real[..., :k_len] (conv.py:1817-1820): inverse fp32 FFT straight from engine order, 1/N, real part
         # (only the Hermitian part of dk_f contributes), sum over the batch-member blocks of the small sizes, [:k_len]
-        fws, fws_bytes = _filter_workspace(plan, H, u.device)
+        fws, fws_bytes = _filter_workspace(plan, G, u.device)
         if lags is not None:
             period, pos, neg = lags
             _launched(mod, _lib.lib().bffc_dk_from_dkf_lags(plan.handle, _ptr(dkf_engine), _ptr(dk), int(k_len),
-                                                            int(period), int(pos), int(neg), H, _ptr(fws), fws_bytes,
+                                                            int(period), int(pos), int(neg), G, _ptr(fws), fws_bytes,
                                                             _stream()))
         else:
-            dk = torch.empty((H, k_len), dtype=torch.float32, device=u.device)
+            dk = torch.empty((G, k_len), dtype=torch.float32, device=u.device)
             band = mod.seqlen // 2 + 1 if band is None else band
-            _launched(mod, _lib.lib().bffc_dk_from_dkf_band(plan.handle, _ptr(dkf_engine), _ptr(dk), int(k_len), H,
+            _launched(mod, _lib.lib().bffc_dk_from_dkf_band(plan.handle, _ptr(dkf_engine), _ptr(dk), int(k_len), G,
                                                             int(band), _ptr(fws), fws_bytes, _stream()))
     du, dpre, dpost = (o if o is not None else t for t, _, o in dst)
     return du, dk, dpre, dpost

@@ -7,7 +7,8 @@ document [s, e) of row b, every channel h and s <= t < e:
     y[b, h, t] = postgate[b, h, t] * sum_{m=0}^{min(Lk-1, t-s)} k[h, m] * (u * pregate)[b, h, t - m]
 
 A document of length l belongs to the class c = max(128, next_pow2(l)) and is convolved as one member of a
-(n_c, H, c) class batch by FlashFFTConv(2c) with the filter k[:, :min(Lk, c)].  That is exact: an output t < l <= c
+(n_c, H, c) class batch by FlashFFTConv(2c) with the filter k[:, :min(Lk, c)] (a grouped k of G rows stays grouped:
+its class filters are G rows, and dk is (G, Lk)).  That is exact: an output t < l <= c
 needs the taps m <= t < c, and a term that wraps around the 2c-point circle lands at an index t - m + 2c >= c + 1 > l,
 where the zero-filled input is zero.  No existing kernel changes: the new kernels only move data, one gather of every
 input into the class batches (bffc_docs_gather) and one scatter of every output back into the rows
@@ -248,10 +249,12 @@ def forward(mod, docs, u, k, pregate, postgate, k2=None, use_cache=None, bidirec
     return y, spectra
 
 
-def backward(mod, docs, dout, u, pregate, postgate, spectra, k_len, k2_len=None, out=None, bidirectional=False):
+def backward(mod, docs, dout, u, pregate, postgate, spectra, k_len, k2_len=None, out=None, bidirectional=False,
+             k_rows=None, k2_rows=None):
     """(du, dk, dpregate, dpostgate, dk2) of `forward`.  out: optional (du, dpregate, dpostgate) (B, H, L) tensors with
     contiguous rows (channel slices of one gradient) that the scatter writes in place.  dk starts at zero and each class
-    adds its terms into it in ascending c, the head lags before the tail lags (bffc_dk_from_dkf_lags); likewise dk2."""
+    adds its terms into it in ascending c, the head lags before the tail lags (bffc_dk_from_dkf_lags); likewise dk2.
+    k_rows / k2_rows: the filters' row counts G (grouped filters, G dividing H; None: H), the rows of dk / dk2."""
     B, H, L = u.shape
     dev = u.device
     gated = pregate is not None
@@ -266,8 +269,8 @@ def backward(mod, docs, dout, u, pregate, postgate, spectra, k_len, k2_len=None,
             _move(mod, docs, H, ins, g, scatter=False)
         segs = [_segments(docs, H, t) for t in g]
         dsegs = [_segments(docs, H, t) for t in dg]
-        dk = torch.zeros((H, k_len), dtype=torch.float32, device=dev)
-        dk2 = None if k2_len is None else torch.zeros((H, k2_len), dtype=torch.float32, device=dev)
+        dk = torch.zeros((k_rows or H, k_len), dtype=torch.float32, device=dev)
+        dk2 = None if k2_len is None else torch.zeros((k2_rows or H, k2_len), dtype=torch.float32, device=dev)
         for i, ((c, _, _), (kf, kf2)) in enumerate(zip(docs.classes, spectra)):
             sub = _class_module(mod, c)
             sub.__dict__['last_launches'] = 0
@@ -301,7 +304,7 @@ class DocsConvFunc(torch.autograd.Function):
         mod.__dict__['last_launches'] = 0
         y, spectra = forward(mod, docs, u, k, pregate, postgate, use_cache=not mod.training,
                              bidirectional=bidirectional)
-        ctx.mod, ctx.docs, ctx.k_len, ctx.spectra = mod, docs, k.shape[-1], spectra
+        ctx.mod, ctx.docs, ctx.k_len, ctx.k_rows, ctx.spectra = mod, docs, k.shape[-1], k.shape[0], spectra
         ctx.bidirectional = bidirectional
         if save:
             ctx.save_for_backward(u, pregate, postgate)
@@ -312,7 +315,7 @@ class DocsConvFunc(torch.autograd.Function):
         u, pregate, postgate = ctx.saved_tensors
         ctx.mod.__dict__['last_launches'] = 0
         du, dk, dpre, dpost, _ = backward(ctx.mod, ctx.docs, dout, u, pregate, postgate, ctx.spectra, ctx.k_len,
-                                          bidirectional=ctx.bidirectional)
+                                          bidirectional=ctx.bidirectional, k_rows=ctx.k_rows)
         return du, dk, None, None, None, dpre, dpost, None
 
 
@@ -329,6 +332,7 @@ class MixerDocsFunc(torch.autograd.Function):
         ctx.bidirectional = bidirectional
         ctx.k_len = k.shape[-1]
         ctx.k2_len = None if k2 is None else k2.shape[-1]
+        ctx.k_rows, ctx.k2_rows = k.shape[0], None if k2 is None else k2.shape[0]
         if any(ctx.needs_input_grad[:3]):
             ctx.save_for_backward(x1x2v)
         return y
@@ -341,5 +345,6 @@ class MixerDocsFunc(torch.autograd.Function):
         grad = torch.empty_like(x1x2v, memory_format=torch.contiguous_format)
         dx1, dx2, dv = grad.split(ctx.d_model, dim=1)
         _, dk, _, _, dk2 = backward(ctx.mod, ctx.docs, dout, v, x1, x2, ctx.spectra, ctx.k_len, ctx.k2_len,
-                                    out=(dv, dx1, dx2), bidirectional=ctx.bidirectional)
+                                    out=(dv, dx1, dx2), bidirectional=ctx.bidirectional, k_rows=ctx.k_rows,
+                                    k2_rows=ctx.k2_rows)
         return grad, dk, dk2, None, None, None, None

@@ -34,7 +34,8 @@ def gated_long_conv(conv, v, k, x1, x2):
     """y = x2 * conv(v * x1, k) through FlashFFTConv's fused gates.
 
     conv: a FlashFFTConv module; v, x1, x2: (B, H, L) tensors of conv.dtype (channel slices are read in place); k: (H, Lk)
-    fp32 filter.  Gradients flow to v, k, x1 and x2 (FlashFFTConvFunc).  The call goes to the autograd function, not
+    fp32 filter, or (G, Lk) with G dividing H, shared by groups of H // G channels (exactly the call on
+    k.repeat_interleave(H // G, 0); its gradient is (G, Lk)).  Gradients flow to v, k, x1 and x2 (FlashFFTConvFunc).  The call goes to the autograd function, not
     through conv(...), so forward hooks registered on the module do not run for it."""
     return _conv.FlashFFTConvFunc.apply(v, k, conv, conv.training, x1, x2, None, None, True)
 
@@ -47,7 +48,7 @@ class HyenaMixerFunc(torch.autograd.Function):
         x1, x2, v = x1x2v.split(d_model, dim=1)
         _conv._check_inputs(v, k, mod, (x1, x2), views=True)
         if k2 is not None:
-            _conv._check_inputs(v, k2, mod, views=True)     # k2 must be (d_model, Lk <= seqlen), as k
+            _conv._check_inputs(v, k2, mod, views=True)     # k2 must be (G2, Lk <= seqlen), G2 dividing d_model, as k
         mod.__dict__['last_launches'] = 0
         y, kf, kf2 = _mixer_forward(mod, x1, x2, v, k, k2)
         ctx.mod, ctx.d_model = mod, d_model
@@ -118,7 +119,8 @@ def hyena_mixer(conv, x1x2v, k, d_model, residual_filter=None, docs=None, bidire
     One gated engine call on the three slices of the projection, read in place (a projection whose slices do not
     qualify, see conv.batch_stride, is copied first).  The backward writes d x1, d x2 and d v into one (B, 3*d_model, L)
     gradient, which is returned as the projection's gradient.  residual_filter k2: one more ungated call on the v slice;
-    its input gradient is added into the v slice of that gradient with one add.  Like gated_long_conv, this calls the
+    its input gradient is added into the v slice of that gradient with one add.  k and k2 may each be grouped, (G, Lk)
+    and (G2, Lk2) with G and G2 dividing d_model, as for gated_long_conv.  Like gated_long_conv, this calls the
     engine directly rather than conv(...): forward hooks registered on the module do not run for it.
 
     docs: a DocumentTable of packed documents in the rows of x1x2v; each document is then mixed alone (flashfftconv.docs):
@@ -195,7 +197,8 @@ def hyena_operator(conv, short_filter, x, k, d_model, residual_filter=None, docs
 
     short_filter: a BHL FlashDepthWiseConv1d(3 * d_model, K, padding) with 2 * padding >= K - 1 (so that it produces at
     least L outputs: padding = (K - 1) // 2 as in the flash examples, or K - 1 followed by [..., :L] as in the original
-    models); its `weights` and `bias` receive gradients, as do x, k and the residual filter k2.
+    models); its `weights` and `bias` receive gradients, as do x, k and the residual filter k2 (either may be grouped, as
+    for hyena_mixer).
 
     For K <= 4, seqlen < 1M and L a multiple of bffc_length_multiple, the forward is one engine call (two with k2) that
     applies the short filter where the kernels load x1, x2 and v, and so is the mixer part of the backward: s is neither

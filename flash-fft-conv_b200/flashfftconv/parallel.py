@@ -19,7 +19,11 @@ def channel_range(H, world, rank):
 
 
 def shard(u, k, world, rank, *gates):
-    """Slices of (B,H,L) tensors and the (H,Lk) filter owned by `rank` (contiguous copies)."""
+    """Slices of (B,H,L) tensors and the (H,Lk) filter owned by `rank` (contiguous copies).  A grouped filter (G < H
+    rows shared by groups of channels) is refused: a channel block can split a group."""
+    if k.dim() != 2 or k.shape[0] != u.shape[1]:
+        raise RuntimeError(f'shard: k must be (H={u.shape[1]}, Lk), got {tuple(k.shape)}; grouped filters are not '
+                           'sharded')
     h0, h1 = channel_range(u.shape[1], world, rank)
     out = [u[:, h0:h1].contiguous(), k[h0:h1].contiguous()]
     out += [g[:, h0:h1].contiguous() for g in gates]

@@ -335,6 +335,50 @@ int bffc_bwd_short_strided(const bffc_plan* plan, const void* dout, int64_t dout
                            void* workspace, size_t workspace_bytes, void* stream);
 
 /*
+ * Grouped filters: G filter rows shared by groups of gs = H / G consecutive channels (channel h uses row h / gs), as
+ * StripedHyena 2's grouped operators have them.  kf_engine is (G, N), from bffc_kf_from_filter* on the G rows;
+ * dkf_engine is (G, N) float2 and row g is the sum of the gradients of channels g * gs .. g * gs + gs - 1, so
+ * bffc_dk_from_dkf* on G rows gives dk (G, Lk).  Every result equals the ungrouped call on the filter expanded to H rows
+ * (k.repeat_interleave(gs, 0)), with dk summed over each group; G == H is the ungrouped call, with the same launches and
+ * the same bits.
+ *   - halo = -1: no overlap-save blocks (bffc_fwd_strided / bffc_bwd_strided); halo >= 0: the blocks and rules of
+ *     bffc_fwd_blocked / bffc_bwd_blocked.
+ *   - The six tap pointers all NULL: no short filter, and w_dtype, K and padding are ignored.  Otherwise the short filter
+ *     and rules of bffc_fwd_short_strided / bffc_bwd_short_strided.  Taps with halo >= 0, or on a 1M, 2M or 4M plan:
+ *     BFFC_ERR_UNSUPPORTED.
+ *   - G < 1, G > H or H % G != 0: BFFC_ERR_INVALID, before the device is looked at.
+ *   - Reduction order of dkf_engine: a dk_f launch sums the units of a group's channels (channel-major, then batch pair)
+ *     into its row.  Default plan: fp32 reductions into the zeroed rows, as bffc_bwd.  Deterministic plan: the fixed
+ *     partition of bffc_plan_create_ex with rows = the launch's groups (times seqlen / 8192 above seqlen 8192) and pairs
+ *     = gs x the batch pairs; so dkf_engine is a function of the inputs and the shape.  The backward of a composite size
+ *     cuts its channels into chunks of whole groups (a chunk's channel count rounded down to a multiple of gs), or, for
+ *     a group larger than a chunk, into chunks that end at the group's end; the first chunk stores the row, the later
+ *     ones (and later batch chunks) add into it, in chunk order.
+ *   - Workspace: bffc_workspace_bytes_grouped at the same arguments; 0 for arguments the calls refuse.  At G == H it is
+ *     bffc_workspace_bytes_ex (halo = -1) or bffc_workspace_bytes_blocked.
+ *   - Launches: G == H and every forward launch what the ungrouped call at the same shape launches.  A grouped backward
+ *     can launch more: (1) on a deterministic plan, fewer dk_f rows can be cut into slabs (S > 1, see
+ *     bffc_plan_create_ex), one more launch per such dk_f launch; (2) above seqlen 8192, once a backward is cut into
+ *     channel chunks (past the 4 GB plane budget), whole-group chunks can be more than the ungrouped call's: at most twice
+ *     as many while a group fits in a chunk, else ceil(gs / chunk) per group, each chunk with its 3-5 launches.
+ */
+size_t bffc_workspace_bytes_grouped(const bffc_plan* plan, int B, int H, int G, int L, int halo, int gated, int backward);
+int bffc_fwd_grouped(const bffc_plan* plan, const void* u, int64_t u_bstride, const void* kf_engine,
+                     const void* pregate, int64_t pregate_bstride, const void* postgate, int64_t postgate_bstride,
+                     void* y, int64_t y_bstride, int B, int H, int G, int L, int halo, const void* u_w,
+                     const void* u_bias, const void* pregate_w, const void* pregate_bias, const void* postgate_w,
+                     const void* postgate_bias, int w_dtype, int K, int padding, void* workspace, size_t workspace_bytes,
+                     void* stream);
+int bffc_bwd_grouped(const bffc_plan* plan, const void* dout, int64_t dout_bstride, const void* u, int64_t u_bstride,
+                     const void* kf_engine, const void* kf_engine_conj,
+                     const void* pregate, int64_t pregate_bstride, const void* postgate, int64_t postgate_bstride,
+                     void* du, int64_t du_bstride, void* dkf_engine, void* dpregate, int64_t dpregate_bstride,
+                     void* dpostgate, int64_t dpostgate_bstride, int B, int H, int G, int L, int halo,
+                     const void* u_w, const void* u_bias, const void* pregate_w, const void* pregate_bias,
+                     const void* postgate_w, const void* postgate_bias, int w_dtype, int K, int padding,
+                     void* workspace, size_t workspace_bytes, void* stream);
+
+/*
  * Forward on HOST buffers (the reference has no counterpart: its user writes u.cuda() -> conv -> y.cpu(),
  * README.md:108-149, three serial steps on one stream).  u_host, pregate_host, postgate_host, y_host: (B, H, L)
  * contiguous host memory of the plan dtype — page-locked for the copies to overlap; kf_engine: DEVICE, from
