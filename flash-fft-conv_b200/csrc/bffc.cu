@@ -19,6 +19,7 @@
 #include "dwconv1d.cuh"
 #include "decode_step.cuh"
 #include "decode_far.cuh"
+#include "decode_extend.cuh"
 #include "docs.cuh"
 
 #include <algorithm>
@@ -2407,6 +2408,228 @@ int bffc_conv_step_far_slots(const void* u, int64_t u_bstride, const void* prega
                        k, Lk, k2, Lk2, {u_w, pregate_w, postgate_w}, {u_bias, pregate_bias, postgate_bias}, w_dtype, K,
                        padding, dtype, state, state_bytes, pos, far_pos, far_y, far_y2, true, y, y_bstride, B, H, T,
                        max_len, stream);
+}
+
+}  // extern "C"
+
+// ------------------------------------------------------------------------------ extending a live sequence (no plan)
+namespace {
+
+namespace ext = bffc::decode_extend;
+
+// W, n and W + P of a chunk of T tokens with filters of Lk and Lk2 taps (decode_extend.cuh): W = roundup(L - 1, 64)
+// with L = max(Lk, Lk2), so W depends on the filters only; n = max(256, next_pow2(W + T (+ 2048 with the far field)));
+// W + P is that rounded up to max(64, the length multiple of n), which stays <= n because n is a multiple of it.
+// 0, or BFFC_ERR_INVALID when n would pass 4M.
+int extend_geometry(const char* fn, int Lk, int Lk2, int T, int far, int* W, int* n, long long* WP) {
+  const long long L = std::max(Lk, Lk2), w = (L - 1 + 63) / 64 * 64;
+  const long long need = w + T + (far ? ext::kFarOutputs : 0);
+  long long nn = 256;
+  while (nn < need) nn <<= 1;
+  if (nn > (1LL << 22))
+    return fail(BFFC_ERR_INVALID, "%s: a chunk of %d tokens with filters of %lld taps needs an FFT of %lld > 4194304 "
+                "points", fn, T, L, nn);
+  const long long q = std::max(64, length_multiple_for(int(nn)));
+  *W = int(w);
+  *n = int(nn);
+  *WP = (need + q - 1) / q * q;
+  return 0;
+}
+
+size_t extend_workspace_bytes(int n, int H, int T) {
+  return (size_t(ext::header_floats(n)) + size_t(n) * H * T) * sizeof(float);
+}
+
+// the filter lengths of an extend call: Lk2 >= 1 with a residual, else 0
+int extend_filters(const char* fn, int Lk, int Lk2, int residual, int max_len) {
+  if (Lk < 1 || Lk > max_len) return fail(BFFC_ERR_INVALID, "%s: Lk=%d outside [1, max_len=%d]", fn, Lk, max_len);
+  if (residual ? (Lk2 < 1 || Lk2 > max_len) : Lk2 != 0)
+    return fail(BFFC_ERR_INVALID, "%s: Lk2=%d (1..max_len=%d with a residual cache, else 0)", fn, Lk2, max_len);
+  return 0;
+}
+
+// one launch geometry for both kernels: columns over gridDim.x (4 per thread), (row, channel) pairs over gridDim.y
+dim3 extend_grid(long long cols, int n, int H) {
+  const long long per_block = 4LL * dec::kThreads;
+  return dim3(unsigned(std::max(1LL, (cols + per_block - 1) / per_block)),
+              unsigned(std::min<long long>(1LL * n * H, kMaxGridYZ)));
+}
+
+// bffc_conv_extend_gather (slot_map null: n = B rows, each of T tokens) and bffc_conv_extend_gather_slots
+int extend_gather(const char* fn, const void* const (&x)[3], const int64_t (&bs)[3], const void* const (&w)[3],
+                  const void* const (&bias)[3], int w_dtype, int K, int padding, int dtype, void* state,
+                  size_t state_bytes, int64_t* pos, const int32_t* slot_map, const int32_t* lengths, int n, bool slots,
+                  int B, int H, int T, int max_len, int has_residual, int Lk, int Lk2, int far, void* ext_u,
+                  void* ext_v, void* workspace, size_t workspace_bytes, void* stream) {
+  const int residual = has_residual != 0;
+  if (T < 1) return fail(BFFC_ERR_INVALID, "%s: T=%d below 1", fn, T);
+  if (int rc = decode_args(fn, dtype, B, H, T, max_len, K, padding, w_dtype, x, bs, w, bias, residual, state,
+                           state_bytes, pos))
+    return rc;
+  if (int rc = extend_filters(fn, Lk, Lk2, residual, max_len)) return rc;
+  if (slots) {
+    if (n < 1 || n > B) return fail(BFFC_ERR_INVALID, "%s: n=%d rows outside [1, B=%d]", fn, n, B);
+    if (!slot_map || reinterpret_cast<uintptr_t>(slot_map) % 4 || !lengths || reinterpret_cast<uintptr_t>(lengths) % 4)
+      return fail(BFFC_ERR_INVALID, "%s: slots / lengths null or not 4-byte aligned", fn);
+  }
+  if (!ext_u || reinterpret_cast<uintptr_t>(ext_u) % 16 || (residual && (!ext_v || reinterpret_cast<uintptr_t>(ext_v) % 16)))
+    return fail(BFFC_ERR_INVALID, "%s: ext_u (and ext_v with a residual cache) null or not 16-byte aligned", fn);
+  const size_t need = extend_workspace_bytes(n, H, T);
+  if (!workspace || reinterpret_cast<uintptr_t>(workspace) % 16 || workspace_bytes < need)
+    return fail(BFFC_ERR_INVALID, "%s: a 16-byte aligned workspace of %zu bytes required", fn, need);
+  int W = 0, nfft = 0;
+  long long WP = 0;
+  if (int rc = extend_geometry(fn, Lk, Lk2, T, far, &W, &nfft, &WP)) return rc;
+  if (int rc = check_device()) return rc;
+  ext::Params ep{};
+  ep.d = decode_params(B, H, max_len, K, residual, state, pos, x, bs, w, bias);
+  ep.d.slots = slots;
+  ep.d.w_dtype = w_dtype;                         // the gather reads the taps' dtype at run time
+  ep.d.T = T;
+  ep.rows = slot_map;
+  ep.lengths = lengths;
+  ep.n = n;
+  ep.W = W;
+  ep.WP = WP;
+  ep.eu = ext_u;
+  ep.ev = residual ? ext_v : nullptr;
+  ep.snap = static_cast<long long*>(workspace);
+  ep.post = static_cast<float*>(workspace) + ext::header_floats(n);
+  const dim3 grid = extend_grid(std::max<long long>(W, WP - W), n, H);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  g_launches = 0;
+  if (slots) {
+    if (dtype == BFFC_DTYPE_FP16) ext::gather<__half, true><<<grid, dec::kThreads, 0, st>>>(ep);
+    else ext::gather<__nv_bfloat16, true><<<grid, dec::kThreads, 0, st>>>(ep);
+  } else {
+    if (dtype == BFFC_DTYPE_FP16) ext::gather<__half, false><<<grid, dec::kThreads, 0, st>>>(ep);
+    else ext::gather<__nv_bfloat16, false><<<grid, dec::kThreads, 0, st>>>(ep);
+  }
+  return launched();
+}
+
+// bffc_conv_extend_finish (n = B, the shared position) and bffc_conv_extend_finish_slots
+int extend_finish(const char* fn, const void* ext_y, const void* ext_y2, int has_postgate, int dtype, int64_t* pos,
+                  int64_t* far_pos, void* far_y, void* far_y2, void* y, int64_t y_bstride, int n, bool slots, int B,
+                  int H, int T, int Lk, int Lk2, int far, const void* workspace, size_t workspace_bytes, void* stream) {
+  const int residual = ext_y2 != nullptr;
+  if (dtype != BFFC_DTYPE_BF16 && dtype != BFFC_DTYPE_FP16) return fail(BFFC_ERR_INVALID, "%s: dtype %d (BF16 0, FP16 1)", fn, dtype);
+  if (B < 1 || H < 1 || T < 1) return fail(BFFC_ERR_INVALID, "%s: bad shape B=%d H=%d T=%d", fn, B, H, T);
+  if (slots && (n < 1 || n > B)) return fail(BFFC_ERR_INVALID, "%s: n=%d rows outside [1, B=%d]", fn, n, B);
+  if (int rc = extend_filters(fn, Lk, Lk2, residual, INT_MAX)) return rc;
+  if (!ext_y || reinterpret_cast<uintptr_t>(ext_y) % 16 || reinterpret_cast<uintptr_t>(ext_y2) % 16)
+    return fail(BFFC_ERR_INVALID, "%s: ext_y null, or ext_y / ext_y2 not 16-byte aligned", fn);
+  if (!pos || reinterpret_cast<uintptr_t>(pos) % 8) return fail(BFFC_ERR_INVALID, "%s: pos null or not 8-byte aligned", fn);
+  if (far && (!far_pos || reinterpret_cast<uintptr_t>(far_pos) % 8 || !far_y || reinterpret_cast<uintptr_t>(far_y) % 2 ||
+              (residual && (!far_y2 || reinterpret_cast<uintptr_t>(far_y2) % 2))))
+    return fail(BFFC_ERR_INVALID, "%s: far_pos / far_y (and far_y2 with ext_y2) null or not aligned", fn);
+  if (!y || reinterpret_cast<uintptr_t>(y) % 2) return fail(BFFC_ERR_INVALID, "%s: y null or not aligned to its element", fn);
+  if (y_bstride < int64_t(H) * T)
+    return fail(BFFC_ERR_INVALID, "%s: batch stride %lld below H * length = %lld", fn, (long long)y_bstride, (long long)H * T);
+  const size_t need = extend_workspace_bytes(n, H, T);
+  if (!workspace || reinterpret_cast<uintptr_t>(workspace) % 16 || workspace_bytes < need)
+    return fail(BFFC_ERR_INVALID, "%s: a 16-byte aligned workspace of %zu bytes required", fn, need);
+  int W = 0, nfft = 0, Wf = 0, nf = 0;
+  long long WP = 0;
+  if (int rc = extend_geometry(fn, Lk, Lk2, T, far, &W, &nfft, &WP)) return rc;
+  if (far)
+    if (int rc = far_geometry(fn, Lk, Lk2, &Wf, &nf)) return rc;
+  if (int rc = check_device()) return rc;
+  ext::Params ep{};
+  ep.d.r[2].x = has_postgate ? ext_y : nullptr;    // only its presence is read
+  ep.d.pos = reinterpret_cast<long long*>(pos);
+  ep.d.y = y; ep.d.y_bs = y_bstride;
+  ep.d.B = B; ep.d.H = H; ep.d.T = T;
+  ep.d.slots = slots;
+  ep.n = n;
+  ep.W = W;
+  ep.WP = WP;
+  ep.eu = const_cast<void*>(ext_y);
+  ep.ev = const_cast<void*>(ext_y2);
+  ep.snap = static_cast<long long*>(const_cast<void*>(workspace));
+  ep.post = static_cast<float*>(const_cast<void*>(workspace)) + ext::header_floats(n);
+  ep.r = far ? reinterpret_cast<long long*>(far_pos) : nullptr;
+  ep.fy = far ? far_y : nullptr;
+  ep.fy2 = far && residual ? far_y2 : nullptr;
+  ep.Wf = Wf;
+  const dim3 grid = extend_grid(T + (far ? ext::kFarOutputs : 0), n, H);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  g_launches = 0;
+  if (slots) {
+    if (dtype == BFFC_DTYPE_FP16) ext::finish<__half, true><<<grid, dec::kThreads, 0, st>>>(ep);
+    else ext::finish<__nv_bfloat16, true><<<grid, dec::kThreads, 0, st>>>(ep);
+  } else {
+    if (dtype == BFFC_DTYPE_FP16) ext::finish<__half, false><<<grid, dec::kThreads, 0, st>>>(ep);
+    else ext::finish<__nv_bfloat16, false><<<grid, dec::kThreads, 0, st>>>(ep);
+  }
+  return launched();
+}
+
+}  // namespace
+
+extern "C" {
+
+int bffc_conv_extend_layout(int B, int H, int Lk, int Lk2, int T, int far, int dtype, int* window, int* fft_size,
+                            size_t* row_bytes) {
+  const char* fn = "bffc_conv_extend_layout";
+  if (dtype != BFFC_DTYPE_BF16 && dtype != BFFC_DTYPE_FP16) return fail(BFFC_ERR_INVALID, "%s: dtype %d (BF16 0, FP16 1)", fn, dtype);
+  if (B < 1 || H < 1 || Lk < 1 || Lk2 < 0 || T < 1)
+    return fail(BFFC_ERR_INVALID, "%s: bad shape B=%d H=%d Lk=%d Lk2=%d T=%d", fn, B, H, Lk, Lk2, T);
+  int W = 0, n = 0;
+  long long WP = 0;
+  if (int rc = extend_geometry(fn, Lk, Lk2, T, far, &W, &n, &WP)) return rc;
+  if (window) *window = W;
+  if (fft_size) *fft_size = n;
+  if (row_bytes) *row_bytes = size_t(WP) * 2;
+  return 0;
+}
+
+size_t bffc_conv_extend_workspace_bytes(int n, int H, int T) {
+  if (n < 1 || H < 1 || T < 1) return 0;
+  return extend_workspace_bytes(n, H, T);
+}
+
+int bffc_conv_extend_gather(const void* u, int64_t u_bstride, const void* pregate, int64_t pregate_bstride,
+                            const void* postgate, int64_t postgate_bstride, const void* u_w, const void* u_bias,
+                            const void* pregate_w, const void* pregate_bias, const void* postgate_w,
+                            const void* postgate_bias, int w_dtype, int K, int padding, int dtype, void* state,
+                            size_t state_bytes, int64_t* pos, int B, int H, int T, int max_len, int has_residual,
+                            int Lk, int Lk2, int far, void* ext_u, void* ext_v, void* workspace,
+                            size_t workspace_bytes, void* stream) {
+  return extend_gather("bffc_conv_extend_gather", {u, pregate, postgate}, {u_bstride, pregate_bstride, postgate_bstride},
+                       {u_w, pregate_w, postgate_w}, {u_bias, pregate_bias, postgate_bias}, w_dtype, K, padding, dtype,
+                       state, state_bytes, pos, nullptr, nullptr, B, false, B, H, T, max_len, has_residual, Lk, Lk2,
+                       far, ext_u, ext_v, workspace, workspace_bytes, stream);
+}
+
+int bffc_conv_extend_gather_slots(const void* u, int64_t u_bstride, const void* pregate, int64_t pregate_bstride,
+                                  const void* postgate, int64_t postgate_bstride, const void* u_w, const void* u_bias,
+                                  const void* pregate_w, const void* pregate_bias, const void* postgate_w,
+                                  const void* postgate_bias, int w_dtype, int K, int padding, int dtype, void* state,
+                                  size_t state_bytes, int64_t* pos, const int32_t* slots, const int32_t* lengths, int n,
+                                  int B, int H, int T, int max_len, int has_residual, int Lk, int Lk2, int far,
+                                  void* ext_u, void* ext_v, void* workspace, size_t workspace_bytes, void* stream) {
+  return extend_gather("bffc_conv_extend_gather_slots", {u, pregate, postgate},
+                       {u_bstride, pregate_bstride, postgate_bstride}, {u_w, pregate_w, postgate_w},
+                       {u_bias, pregate_bias, postgate_bias}, w_dtype, K, padding, dtype, state, state_bytes, pos,
+                       slots, lengths, n, true, B, H, T, max_len, has_residual, Lk, Lk2, far, ext_u, ext_v, workspace,
+                       workspace_bytes, stream);
+}
+
+int bffc_conv_extend_finish(const void* ext_y, const void* ext_y2, int has_postgate, int dtype, int64_t* pos,
+                            int64_t* far_pos, void* far_y, void* far_y2, void* y, int64_t y_bstride, int B, int H,
+                            int T, int Lk, int Lk2, int far, const void* workspace, size_t workspace_bytes,
+                            void* stream) {
+  return extend_finish("bffc_conv_extend_finish", ext_y, ext_y2, has_postgate, dtype, pos, far_pos, far_y, far_y2, y,
+                       y_bstride, B, false, B, H, T, Lk, Lk2, far, workspace, workspace_bytes, stream);
+}
+
+int bffc_conv_extend_finish_slots(const void* ext_y, const void* ext_y2, int has_postgate, int dtype, int64_t* pos,
+                                  int64_t* far_pos, void* far_y, void* far_y2, void* y, int64_t y_bstride, int n,
+                                  int B, int H, int T, int Lk, int Lk2, int far, const void* workspace,
+                                  size_t workspace_bytes, void* stream) {
+  return extend_finish("bffc_conv_extend_finish_slots", ext_y, ext_y2, has_postgate, dtype, pos, far_pos, far_y,
+                       far_y2, y, y_bstride, n, true, B, H, T, Lk, Lk2, far, workspace, workspace_bytes, stream);
 }
 
 }  // extern "C"

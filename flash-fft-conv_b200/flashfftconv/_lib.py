@@ -119,6 +119,19 @@ SYMBOLS = {
     'bffc_conv_step_far_slots': (_c.c_int, [_c.c_void_p, _c.c_int64] * 3 + [_c.c_void_p, _c.c_int] * 2
                                  + [_c.c_void_p] * 6 + [_c.c_int] * 4 + [_c.c_void_p, _c.c_size_t]
                                  + [_c.c_void_p] * 5 + [_c.c_int64] + [_c.c_int] * 4 + [_c.c_void_p]),
+    'bffc_conv_extend_layout': (_c.c_int, [_c.c_int] * 7 + [_c.POINTER(_c.c_int), _c.POINTER(_c.c_int),
+                                                            _c.POINTER(_c.c_size_t)]),
+    'bffc_conv_extend_workspace_bytes': (_c.c_size_t, [_c.c_int] * 3),
+    'bffc_conv_extend_gather': (_c.c_int, [_c.c_void_p, _c.c_int64] * 3 + [_c.c_void_p] * 6 + [_c.c_int] * 4
+                                + [_c.c_void_p, _c.c_size_t, _c.c_void_p] + [_c.c_int] * 8
+                                + [_c.c_void_p] * 3 + [_c.c_size_t, _c.c_void_p]),
+    'bffc_conv_extend_gather_slots': (_c.c_int, [_c.c_void_p, _c.c_int64] * 3 + [_c.c_void_p] * 6 + [_c.c_int] * 4
+                                      + [_c.c_void_p, _c.c_size_t, _c.c_void_p] + [_c.c_void_p] * 2 + [_c.c_int] * 9
+                                      + [_c.c_void_p] * 3 + [_c.c_size_t, _c.c_void_p]),
+    'bffc_conv_extend_finish': (_c.c_int, [_c.c_void_p] * 2 + [_c.c_int] * 2 + [_c.c_void_p] * 5 + [_c.c_int64]
+                                + [_c.c_int] * 6 + [_c.c_void_p, _c.c_size_t, _c.c_void_p]),
+    'bffc_conv_extend_finish_slots': (_c.c_int, [_c.c_void_p] * 2 + [_c.c_int] * 2 + [_c.c_void_p] * 5 + [_c.c_int64]
+                                      + [_c.c_int] * 7 + [_c.c_void_p, _c.c_size_t, _c.c_void_p]),
     'bffc_docs_gather':(_c.c_int, [_c.c_void_p, _c.c_int, _c.c_int64] + [_c.c_int] * 3
                          + [_c.POINTER(_c.c_void_p), _c.POINTER(_c.c_int64), _c.POINTER(_c.c_void_p), _c.c_int,
                             _c.c_void_p]),

@@ -8,9 +8,11 @@ bffc_conv_step, include/bffc.h):
     dec = HyenaDecoder(short_filter, k, d_model, batch, max_len, residual_filter=None, dtype=torch.bfloat16)
     y_prompt = dec.prefill(x_prompt)     # (B, 3D, L) -> (B, D, L); L may be 0
     y_new = dec.step(x_new)              # (B, 3D, T) -> (B, D, T), 1 <= T <= 64
+    y_turn = dec.extend(x_turn)          # (B, 3D, T) -> (B, D, T), any T >= 1: the next user turn, a prompt piece
 
     lc = LongConvDecoder(k, batch, max_len, dtype)
     y = lc.prefill(u, pregate, postgate); y_t = lc.step(u_t, pregate_t, postgate_t)     # gates optional
+    y_c = lc.extend(u_c, pregate_c, postgate_c)                                          # the same gates
 
 HyenaDecoder is hyena_operator(conv, short_filter, x, k, d_model, residual_filter) position by position, for a causal
 short filter (padding = K - 1, the original Hyena / HyenaDNA models); LongConvDecoder is FlashFFTConv's gated
@@ -18,7 +20,17 @@ convolution.  prefill computes y of the prompt with the FFT engine and fills the
 A step's outputs do not depend on how the tokens are grouped into steps or on the other batch members, bit for bit.
 
 Limits: inference only (the decoders run under torch.no_grad(); nothing is differentiated); causal short filters only;
-T <= 64 tokens per step (a longer chunk is a prefill); caches in (B, H, max_len) layout.
+T <= 64 tokens per step (a longer chunk is an extend); an extend's FFT of n = max(256, next_pow2(W + T (+ 2048 with
+the far field))) points, W = roundup(max(Lk, Lk2) - 1, 64), at most 4M; caches in (B, H, max_len) layout.
+
+Extend (bffc_conv_extend_gather / bffc_conv_extend_finish, include/bffc.h, INTEGRATION.md §9.5) appends a chunk of any
+length to a live sequence: a multi-turn chat's next message, a long prompt admitted in pieces, tool output.  One
+FlashFFTConv(n) forward per filter over the last W cached z values and the chunk's own gives every output of the chunk;
+its z, s_u and tail are bit for bit those a prefill of the whole sequence leaves, so later steps are unchanged.  On a
+far-field decoder the same transform, 2048 outputs longer, refreshes every extended member at its new position.  With
+slots, extend(x, lengths=[...], slots=[...]) appends right-padded rows to the listed slots only.  A captured extend
+replays with the T, lengths and slots it was captured with; run one eager extend with that T first (it makes the FFT
+plan and the filter spectra).
 
 `step` is capturable in a CUDA graph: the position lives on the device and the step neither allocates in the library
 nor synchronises.  Run one eager step with the same T first (it sizes the workspace), then:
@@ -105,6 +117,18 @@ def far_layout(batch, H, Lk, Lk2, dtype):
     return W.value, n.value, nbytes.value
 
 
+def extend_layout(batch, H, Lk, Lk2, T, far, dtype):
+    """(W, n, W + P) of an extend by T tokens with filters of Lk and Lk2 taps (Lk2 = 0 without a residual filter), from
+    bffc_conv_extend_layout: engine rows of W + P elements, FFT size n.  ValueError when the chunk needs an FFT past 4M
+    points."""
+    W, n, nbytes = ctypes.c_int(), ctypes.c_int(), ctypes.c_size_t()
+    rc = _lib.lib().bffc_conv_extend_layout(int(batch), int(H), int(Lk), int(Lk2), int(T), int(bool(far)), _DT[dtype],
+                                            ctypes.byref(W), ctypes.byref(n), ctypes.byref(nbytes))
+    if rc:
+        raise ValueError(f'extend: {_lib.lib().bffc_last_error().decode()}')
+    return W.value, n.value, nbytes.value // 2
+
+
 def _host_ints(v, name):
     """a host sequence or CPU tensor of ints as a list"""
     if isinstance(v, torch.Tensor):
@@ -175,6 +199,11 @@ class _Decoder:
         # workspaces outgrown by a larger T: a graph captured earlier still writes to the address it was given
         self._ws_outgrown = []
         self._convs = {}
+        # extend: one FlashFFTConv(n) per filter and FFT size, and the spectra of the latest eager transform at that
+        # size (a captured extend reads them, as a captured refresh reads _far_kf)
+        self._ext_convs, self._ext_kf = {}, {}
+        # pinned slot lists and lengths a captured extend copies from at every replay
+        self._ext_held = []
         if self.far_field:
             self._far_init()
         self.reset()
@@ -525,6 +554,113 @@ class _Decoder:
         self._advance_host(T, capturing)
         return y
 
+    # ---- extend (decode_extend.cuh)
+    def _extend(self, u, pregate, postgate, lengths, slots):
+        """bffc_conv_extend_gather[_slots], the engine forward of k (and k2) on the rows it wrote, and
+        bffc_conv_extend_finish[_slots]: y of the chunk, the caches appended, the positions advanced (far field: every
+        extended member refreshed at its new position)"""
+        T = u.shape[-1]
+        if T < 1:
+            raise ValueError('extend takes at least one token')
+        capturing = torch.cuda.is_current_stream_capturing()
+        if self.slots:
+            n = u.shape[0]
+            if not 1 <= n <= self.batch:
+                raise ValueError(f'{n} rows for {self.batch} slots')
+            idx = self._slot_list(slots, n)
+            lens = [T] * n if lengths is None else _host_ints(lengths, 'lengths')
+            if len(lens) != n:
+                raise ValueError(f'{len(lens)} lengths for {n} rows')
+            bad = [l for l in lens if not 0 <= l <= T]
+            if bad:
+                raise ValueError(f'lengths {bad} outside [0, T = {T}]')
+        else:
+            if lengths is not None or slots is not None:
+                raise ValueError('lengths and slots are for a decoder made with slots=True')
+            n, idx, lens = self.batch, list(range(self.batch)), [T] * self.batch
+        roles = self._roles(u, pregate, postgate, T, n)
+        Lk = self.k.shape[1]
+        Lk2 = 0 if self.k2 is None else self.k2.shape[1]
+        W, nfft, WP = extend_layout(self.batch, self.H, Lk, Lk2, T, self.far_field, self.dtype)
+        if capturing and nfft not in self._ext_kf:
+            raise RuntimeError(f'run one eager extend with T = {T} before capturing it (it makes the FFT plan and the '
+                               'filter spectra)')
+        if self.far_field and not capturing:
+            self._far_sync()
+        if self._host_pos is not None and not capturing:
+            if self.slots:
+                idle = [b for b in idx if self._host_pos[b] < 0]
+                if idle:
+                    raise ValueError(f'slots {idle} are idle: admit a prompt into them with prefill first')
+                over = [b for b, l in zip(idx, lens) if self._host_pos[b] + l > self.max_len]
+                if over:
+                    raise ValueError(f'slots {over} at positions {[self._host_pos[b] for b in over]} + '
+                                     f'{[lens[idx.index(b)] for b in over]} tokens exceed max_len = {self.max_len}')
+            elif self._host_pos + T > self.max_len:
+                raise ValueError(f'position {self._host_pos} + {T} tokens exceeds max_len = {self.max_len}')
+        rows, wdt = self._tap_args()
+        l, dt, dev = _lib.lib(), _DT[self.dtype], self.device
+        nf = 1 if self.k2 is None else 2
+        ins = [torch.empty((n, self.H, WP), dtype=self.dtype, device=dev) for _ in range(nf)]
+        ws = torch.empty(l.bffc_conv_extend_workspace_bytes(n, self.H, T), dtype=torch.uint8, device=dev)
+        args = [a for t, s in roles for a in (_ptr(t), s)]
+        common = (self.batch, self.H, T, self.max_len, int(self.k2 is not None), Lk, Lk2, int(self.far_field),
+                  _ptr(ins[0]), _ptr(ins[1] if nf > 1 else None), _ptr(ws), ws.numel(), _stream())
+        with _on_device(dev):
+            if self.slots:
+                host = torch.tensor(idx + lens, dtype=torch.int32).pin_memory()
+                if capturing:              # every replay copies from this buffer
+                    self._ext_held.append(host)
+                meta = host.to(dev, non_blocking=True)
+                rc = l.bffc_conv_extend_gather_slots(*args, *rows, wdt, self.K, self.K - 1, dt, _ptr(self.state),
+                                                     self.state.numel(), _ptr(self._pos), _ptr(meta), _ptr(meta[n:]),
+                                                     n, *common)
+            else:
+                rc = l.bffc_conv_extend_gather(*args, *rows, wdt, self.K, self.K - 1, dt, _ptr(self.state),
+                                               self.state.numel(), _ptr(self._pos), *common)
+            _lib.check(rc)
+        convs = self._ext_convs.get(nfft)
+        if convs is None:
+            convs = self._ext_convs[nfft] = [FlashFFTConv(nfft, dtype=self.dtype).eval() for _ in range(nf)]
+        kfs = self._ext_kf.get(nfft, [None] * nf)
+        outs = []
+        for i, (conv, k, x) in enumerate(zip(convs, (self.k, self.k2), ins)):
+            out, kf = _fwd(conv, x, k, None, None, kf_engine=kfs[i] if capturing else None)
+            outs.append(out)
+            kfs[i] = kf
+        if not capturing:
+            self._ext_kf[nfft] = kfs
+        y = torch.empty((n, self.H, T), dtype=self.dtype, device=dev)
+        fo = self._far_out if self.far_field else [None, None]
+        far = (_ptr(self._far_pos), _ptr(fo[0]), _ptr(fo[1] if len(fo) > 1 else None)) if self.far_field else \
+            (None, None, None)
+        tail = (self.H, T, Lk, Lk2, int(self.far_field), _ptr(ws), ws.numel(), _stream())
+        with _on_device(dev):
+            head = (_ptr(outs[0]), _ptr(outs[1] if nf > 1 else None), int(roles[2][0] is not None), dt, _ptr(self._pos),
+                    *far, _ptr(y), self.H * T)
+            if self.slots:
+                rc = l.bffc_conv_extend_finish_slots(*head, n, self.batch, *tail)
+            else:
+                rc = l.bffc_conv_extend_finish(*head, self.batch, *tail)
+            _lib.check(rc)
+        if capturing or self._host_pos is None:
+            self._host_pos = None
+            if self.far_field:
+                self._host_r = None
+        else:
+            if self.slots:
+                for b, ln in zip(idx, lens):
+                    self._host_pos[b] += ln
+            else:
+                self._host_pos += T
+            if self.far_field and self._host_r is not None:
+                if self.slots:
+                    for b in idx:
+                        self._host_r[b] = self._host_pos[b]
+                else:
+                    self._host_r = self._host_pos
+        return y
+
 
 class HyenaDecoder(_Decoder):
     """hyena_operator(conv, short_filter, x, k, d_model, residual_filter) decoded position by position.
@@ -638,6 +774,18 @@ class HyenaDecoder(_Decoder):
         v, x1, x2 = self._split(x)
         return self._step(v, x1, x2)
 
+    @torch.no_grad()
+    def extend(self, x, *, lengths=None, slots=None):
+        """y (B, d_model, T) of the next T >= 1 positions of the projection x (B, 3 * d_model, T), by one FFT over the
+        cached window and the chunk (see the module docstring).  The state afterwards is bit for bit the one a prefill
+        of the whole sequence leaves.  With slots: x (n, 3 * d_model, T) right-padded, row i the next lengths[i] <= T
+        positions of slot slots[i] (slots=None: n = batch, every slot; lengths=None: T each); other slots are untouched.
+        Returns (n, d_model, T), zero at t >= lengths[i]."""
+        if x.dim() != 3:
+            raise ValueError(f'x must be (B, 3 * d_model = {3 * self.d_model}, T), got {tuple(x.shape)}')
+        v, x1, x2 = self._split(x)
+        return self._extend(v, x1, x2, lengths, slots)
+
 
 class LongConvDecoder(_Decoder):
     """y = postgate * causal_conv(u * pregate, k) (FlashFFTConv's gated convolution; either gate may be absent)
@@ -728,3 +876,12 @@ class LongConvDecoder(_Decoder):
         refuse(docs, 'LongConvDecoder')
         self._same_gates(pregate, postgate)
         return self._step(u, pregate, postgate)
+
+    @torch.no_grad()
+    def extend(self, u, pregate=None, postgate=None, *, lengths=None, slots=None):
+        """y (B, H, T) of the next T >= 1 positions by one FFT over the cached window and the chunk, with the gates the
+        sequence was started with; lengths and slots as HyenaDecoder.extend."""
+        if u.dim() != 3:
+            raise ValueError(f'u must be (B, {self.H}, T), got {tuple(u.shape)}')
+        self._same_gates(pregate, postgate)
+        return self._extend(u, pregate, postgate, lengths, slots)

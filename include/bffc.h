@@ -588,6 +588,61 @@ int bffc_conv_step_far_slots(const void* u, int64_t u_bstride, const void* prega
                              int B, int H, int T, int max_len, void* stream);
 
 /*
+ * Extending a live sequence by a chunk of T >= 1 tokens (INTEGRATION.md §9.5): one FFT over the cached window and the
+ * chunk, per row, gives every output of the chunk and (with far) the far field at the new position.  Member b at
+ * position p_b takes l_b tokens (T, or with the _slots calls lengths[i] clamped to [0, T]); its outputs t < l_b are
+ *     y[p_b + t] = round( s_postgate[t] * F[W + t] + F2[W + t] )            (no postgate: factor 1; no k2: no F2)
+ * where F / F2 are the engine's FlashFFTConv(n) forward with k / k2 of what bffc_conv_extend_gather wrote to ext_u /
+ * ext_v, read as fp32.  The chunk's z, s_u and tail are bit for bit those bffc_conv_state_fill writes for the whole
+ * sequence, so prefill(x[:a]) then an extend by x[a:b] leaves the state of prefill(x[:b]).
+ * bffc_conv_extend_layout: W = roundup(max(Lk, Lk2) - 1, 64) (the filters only, so a given T keeps one geometry), the
+ *   FFT size n = max(256, next_pow2(W + T + (far ? 2048 : 0))) and row_bytes = 2 (W + P) of one 16-bit engine row, W + P
+ *   being W + T (+ 2048) rounded up to the length multiple of n; engine buffers are (rows, H, W + P).
+ *   BFFC_ERR_INVALID when n would pass 4194304.
+ * bffc_conv_extend_workspace_bytes(n, H, T): the workspace both calls share (a snapshot of the rows' members,
+ *   positions and lengths, then s_postgate of the chunk), 16-byte aligned; 0 for a bad shape.
+ * bffc_conv_extend_gather[_slots]: row i is member i (B rows, every one of T tokens) or member slots[i] with lengths[i]
+ *   (the _slots call, n rows; slots and lengths are device int32[n], never read on the host).  Inputs (rows, H, T) as
+ *   bffc_conv_step's; the right padding of a short row is never read.  Writes
+ *     ext_u[i, h, j] = z[b, h, p_b - W + j] for j < W (0 below position 0), the chunk's z for W <= j < W + l_b, else 0
+ *   and ext_v likewise from the s_u cache (with has_residual); appends the chunk's z (and s_u) to the caches at
+ *   [p_b, p_b + l_b) and rewrites the tail.  A member that is idle (-1) or would pass max_len reads and writes nothing
+ *   of its state and gets a zero row; one that would pass max_len sets its status word to 1.  One launch.
+ * bffc_conv_extend_finish[_slots]: y (rows, H, T) (element (i, h, t) at y + i * y_bstride + h * T + t), zero at t >= l_b
+ *   and for skipped members; positions advanced by l_b.  With far: far_y[b, h, W_far + i] = F[W + l_b + i] for
+ *   i < 2048 (F2 into far_y2), W_far from bffc_conv_far_layout, and far_pos[c] = p_b + l_b: every extended member is
+ *   refreshed at its new position.  has_postgate: the gather had a postgate.  One launch.
+ * Host arguments are checked before the device is looked at (BFFC_ERR_INVALID on any machine).  Offsets are 64-bit,
+ * (row, channel) pairs go over gridDim.y in groups of at most 65535, and nothing is read on the host, so a gather, the
+ * engine forwards and a finish can be captured in a CUDA graph together.
+ */
+int bffc_conv_extend_layout(int B, int H, int Lk, int Lk2, int T, int far, int dtype, int* window, int* fft_size,
+                            size_t* row_bytes);
+size_t bffc_conv_extend_workspace_bytes(int n, int H, int T);
+int bffc_conv_extend_gather(const void* u, int64_t u_bstride, const void* pregate, int64_t pregate_bstride,
+                            const void* postgate, int64_t postgate_bstride, const void* u_w, const void* u_bias,
+                            const void* pregate_w, const void* pregate_bias, const void* postgate_w,
+                            const void* postgate_bias, int w_dtype, int K, int padding, int dtype, void* state,
+                            size_t state_bytes, int64_t* pos, int B, int H, int T, int max_len, int has_residual,
+                            int Lk, int Lk2, int far, void* ext_u, void* ext_v, void* workspace,
+                            size_t workspace_bytes, void* stream);
+int bffc_conv_extend_gather_slots(const void* u, int64_t u_bstride, const void* pregate, int64_t pregate_bstride,
+                                  const void* postgate, int64_t postgate_bstride, const void* u_w, const void* u_bias,
+                                  const void* pregate_w, const void* pregate_bias, const void* postgate_w,
+                                  const void* postgate_bias, int w_dtype, int K, int padding, int dtype, void* state,
+                                  size_t state_bytes, int64_t* pos, const int32_t* slots, const int32_t* lengths, int n,
+                                  int B, int H, int T, int max_len, int has_residual, int Lk, int Lk2, int far,
+                                  void* ext_u, void* ext_v, void* workspace, size_t workspace_bytes, void* stream);
+int bffc_conv_extend_finish(const void* ext_y, const void* ext_y2, int has_postgate, int dtype, int64_t* pos,
+                            int64_t* far_pos, void* far_y, void* far_y2, void* y, int64_t y_bstride, int B, int H,
+                            int T, int Lk, int Lk2, int far, const void* workspace, size_t workspace_bytes,
+                            void* stream);
+int bffc_conv_extend_finish_slots(const void* ext_y, const void* ext_y2, int has_postgate, int dtype, int64_t* pos,
+                                  int64_t* far_pos, void* far_y, void* far_y2, void* y, int64_t y_bstride, int n,
+                                  int B, int H, int T, int Lk, int Lk2, int far, const void* workspace,
+                                  size_t workspace_bytes, void* stream);
+
+/*
  * Packed documents regrouped by length class for the long convolution (no plan; INTEGRATION.md §11).  Rows (B, H, L)
  * hold several documents; a document of length l (1 <= l <= 2^21) belongs to the class c = max(128, next_pow2(l)) and is
  * convolved as one member of a (n_c, H, c) class batch by the plan of seqlen 2c with the filter k[:, :min(Lk, c)],
@@ -620,7 +675,8 @@ int bffc_docs_scatter(const void* items, int n_items, int64_t positions, int B, 
 
 /* Number of kernel launches the last bffc_fwd / bffc_bwd / bffc_fwd_host / filter-side transform /
  * bffc_dwconv1d_fwd (1) / bffc_dwconv1d_bwd (2) / bffc_conv_state_fill[_slots] (1) / bffc_conv_step[_slots] (2) /
- * bffc_conv_far_gather[_slots] (1) / bffc_conv_step_far[_slots] (2) / bffc_docs_gather (1) / bffc_docs_scatter (1)
+ * bffc_conv_far_gather[_slots] (1) / bffc_conv_step_far[_slots] (2) / bffc_conv_extend_gather[_slots] (1) /
+ * bffc_conv_extend_finish[_slots] (1) / bffc_docs_gather (1) / bffc_docs_scatter (1)
  * on this thread enqueued (bench.py).  A bffc_bwd* on a deterministic plan
  * counts the same launches as on a default plan, plus one slot sum per dk_f launch whose rows have S > 1 slabs. */
 int bffc_last_launch_count(void);
