@@ -20,6 +20,8 @@
 #include "decode_step.cuh"
 #include "decode_far.cuh"
 #include "decode_extend.cuh"
+#include "modal.cuh"
+#include "decode_modal.cuh"
 #include "docs.cuh"
 
 #include <algorithm>
@@ -2707,6 +2709,286 @@ int bffc_docs_scatter(const void* items, int n_items, int64_t positions, int B, 
                          dst_bstride, gathered, n_tensors, &prm))
     return rc;
   return docs_launch(prm, true, stream);
+}
+
+}  // extern "C"
+
+// ------------------------------------------------------------------------- modal filters and their decoding (no plan)
+namespace {
+
+namespace mdl = bffc::modal;
+namespace dmd = bffc::decode_modal;
+
+bool misaligned(const void* q, uintptr_t a) { return reinterpret_cast<uintptr_t>(q) % a != 0; }
+
+int modal_args(const char* fn, const void* v, const void* x, int G, int N) {
+  if (N < 1 || N > mdl::kMaxN) return fail(BFFC_ERR_INVALID, "%s: N=%d outside [1, %d]", fn, N, mdl::kMaxN);
+  if (G < 1) return fail(BFFC_ERR_INVALID, "%s: G=%d < 1", fn, G);
+  if (!v || !x || misaligned(v, 8) || misaligned(x, 8))
+    return fail(BFFC_ERR_INVALID, "%s: v / x null or not 8-byte aligned (complex64)", fn);
+  return 0;
+}
+
+int groups_args(const char* fn, int H, int G) {
+  if (H < 1 || G < 1 || H % G) return fail(BFFC_ERR_INVALID, "%s: G=%d does not divide H=%d", fn, G, H);
+  return 0;
+}
+
+size_t partial_bytes(long long rows, int N, long long L, bool grad) {
+  const long long nch = mdl::chunks_of(L, mdl::tiles_per_chunk(L));
+  return size_t(rows) * size_t(nch) * size_t(N) * sizeof(float2) * (grad ? 2 : 1);
+}
+
+unsigned grid_rows(long long rows) { return unsigned(std::min<long long>(std::max<long long>(rows, 1), kMaxGridYZ)); }
+
+unsigned grid_flat(long long items, int threads) {
+  return unsigned(std::min<long long>(std::max<long long>((items + threads - 1) / threads, 1), 1 << 20));
+}
+
+// the reduction both the backward and the transpose run: partials per chunk, then the chunks in order
+template <class In, bool kGrad>
+int modal_reduce(mdl::RedParams& prm, void* workspace, cudaStream_t st) {
+  const long long rows = static_cast<long long>(prm.B) * prm.H;
+  prm.tpc = mdl::tiles_per_chunk(prm.len);
+  prm.nch = mdl::chunks_of(prm.len, prm.tpc);
+  prm.part0 = static_cast<float2*>(workspace);
+  prm.part1 = kGrad ? prm.part0 + rows * prm.nch * prm.N : nullptr;
+  g_launches = 0;
+  if (prm.nch > 0) {
+    mdl::reduce_tiles<In, kGrad><<<dim3(unsigned(prm.nch), grid_rows(rows)), mdl::kThreads, 0, st>>>(prm);
+    if (int rc = launched()) return rc;
+  }
+  mdl::reduce_finish<kGrad><<<grid_flat(rows * prm.N, mdl::kThreads), mdl::kThreads, 0, st>>>(prm);
+  return launched();
+}
+
+int modal_roles(const char* fn, int dtype, int w_dtype, int K, int padding, int H, int len,
+                const void* const (&x)[3], const int64_t (&bs)[3], const void* const (&w)[3],
+                const void* const (&bias)[3], const void* tail, const int64_t* pos) {
+  if (dtype != BFFC_DTYPE_BF16 && dtype != BFFC_DTYPE_FP16) return fail(BFFC_ERR_INVALID, "%s: dtype %d (BF16 0, FP16 1)", fn, dtype);
+  if (K < 1 || K > dec::kMaxK) return fail(BFFC_ERR_INVALID, "%s: K=%d outside [1, %d]", fn, K, dec::kMaxK);
+  if (padding != K - 1) return fail(BFFC_ERR_INVALID, "%s: padding %d is not the causal padding K - 1 = %d", fn, padding, K - 1);
+  if (w_dtype != BFFC_DTYPE_BF16 && w_dtype != BFFC_DTYPE_FP16 && w_dtype != BFFC_DTYPE_FP32)
+    return fail(BFFC_ERR_INVALID, "%s: w_dtype %d (BF16 0, FP16 1, FP32 2)", fn, w_dtype);
+  const size_t ew = w_dtype == BFFC_DTYPE_FP32 ? 4 : 2;
+  for (int r = 0; r < 3; ++r) {
+    if (bias[r] && !w[r]) return fail(BFFC_ERR_INVALID, "%s: a bias needs the taps of its tensor", fn);
+    if (w[r] && !x[r] && len > 0) return fail(BFFC_ERR_INVALID, "%s: taps for an absent input", fn);
+    if (misaligned(w[r], ew) || misaligned(bias[r], ew)) return fail(BFFC_ERR_INVALID, "%s: taps not aligned to their element", fn);
+    if (!x[r]) continue;
+    if (misaligned(x[r], 2)) return fail(BFFC_ERR_INVALID, "%s: input not aligned to its element", fn);
+    if (bs[r] < int64_t(H) * len)
+      return fail(BFFC_ERR_INVALID, "%s: batch stride %lld below H * length = %lld", fn, (long long)bs[r], (long long)H * len);
+  }
+  if (!x[0] && len > 0) return fail(BFFC_ERR_INVALID, "%s: null u", fn);
+  if ((K > 1 && !tail) || misaligned(tail, 2)) return fail(BFFC_ERR_INVALID, "%s: tail null or not aligned", fn);
+  if (!pos || misaligned(pos, 8)) return fail(BFFC_ERR_INVALID, "%s: pos null or not 8-byte aligned", fn);
+  return 0;
+}
+
+dmd::Params modal_dec_params(const void* const (&x)[3], const int64_t (&bs)[3], const void* const (&w)[3],
+                             const void* const (&bias)[3], int w_dtype, int K, void* tail, int64_t* pos, bool slots,
+                             int Bs, int H, int T) {
+  dmd::Params p{};
+  for (int r = 0; r < 3; ++r) p.r[r] = dec::Role{x[r], bs[r], w[r], bias[r]};
+  p.w_dtype = w_dtype;
+  p.K = K;
+  p.tail = tail;
+  p.pos = reinterpret_cast<long long*>(pos);
+  p.slots = slots;
+  p.Bs = Bs; p.H = H; p.T = T;
+  return p;
+}
+
+int slot_lists(const char* fn, const int32_t* slot_map, const int32_t* lengths) {
+  if (misaligned(slot_map, 4) || misaligned(lengths, 4))
+    return fail(BFFC_ERR_INVALID, "%s: slots / lengths not 4-byte aligned", fn);
+  return 0;
+}
+
+}  // namespace
+
+extern "C" {
+
+int bffc_modal_fwd(const void* v, const void* x, int rows, int N, int64_t L, float* k, void* stream) {
+  const char* fn = "bffc_modal_fwd";
+  if (int rc = modal_args(fn, v, x, 1, N)) return rc;
+  if (rows < 1 || L < 1) return fail(BFFC_ERR_INVALID, "%s: rows=%d L=%lld must be >= 1", fn, rows, (long long)L);
+  if (!k || misaligned(k, 4)) return fail(BFFC_ERR_INVALID, "%s: k null or not 4-byte aligned", fn);
+  if (int rc = check_device()) return rc;
+  mdl::FwdParams prm{static_cast<const float2*>(v), static_cast<const float2*>(x), k, L, rows, N};
+  const long long tiles = mdl::tiles_of(L);
+  if (tiles > INT32_MAX) return fail(BFFC_ERR_INVALID, "%s: L=%lld too long", fn, (long long)L);
+  g_launches = 0;
+  mdl::fwd<<<dim3(unsigned(tiles), grid_rows(rows)), mdl::kThreads, 0, static_cast<cudaStream_t>(stream)>>>(prm);
+  return launched();
+}
+
+size_t bffc_modal_workspace_bytes(int B, int H, int N, int64_t L, int grad) {
+  if (B < 1 || H < 1 || N < 1 || N > mdl::kMaxN || L < 0) return 0;
+  return std::max<size_t>(partial_bytes(static_cast<long long>(B) * H, N, L, grad != 0), 16);
+}
+
+int bffc_modal_bwd(const void* v, const void* x, int rows, int N, int64_t L, const float* dk, void* dv, void* dx,
+                   void* workspace, size_t workspace_bytes, void* stream) {
+  const char* fn = "bffc_modal_bwd";
+  if (int rc = modal_args(fn, v, x, 1, N)) return rc;
+  if (rows < 1 || L < 1) return fail(BFFC_ERR_INVALID, "%s: rows=%d L=%lld must be >= 1", fn, rows, (long long)L);
+  if (!dk || misaligned(dk, 4)) return fail(BFFC_ERR_INVALID, "%s: dk null or not 4-byte aligned", fn);
+  if (!dv || !dx || misaligned(dv, 8) || misaligned(dx, 8))
+    return fail(BFFC_ERR_INVALID, "%s: dv / dx null or not 8-byte aligned", fn);
+  const size_t need = bffc_modal_workspace_bytes(1, rows, N, L, 1);
+  if (!workspace || misaligned(workspace, 16) || workspace_bytes < need)
+    return fail(BFFC_ERR_INVALID, "%s: a 16-byte aligned workspace of %zu bytes required", fn, need);
+  if (int rc = check_device()) return rc;
+  mdl::RedParams prm{};
+  prm.w = dk; prm.w_bs = int64_t(rows) * L; prm.len = L;
+  prm.B = 1; prm.H = rows; prm.gs = 1;
+  prm.v = static_cast<const float2*>(v); prm.x = static_cast<const float2*>(x); prm.N = N;
+  prm.dv = static_cast<float2*>(dv); prm.dx = static_cast<float2*>(dx);
+  return modal_reduce<float, true>(prm, workspace, static_cast<cudaStream_t>(stream));
+}
+
+int bffc_modal_transpose(const void* w, int64_t w_bstride, int w_dtype, int B, int H, int64_t len,
+                         const int32_t* lengths, int reversed, const void* v, const void* x, int G, int N,
+                         const void* init, void* out, const int32_t* slots, int Bs, void* workspace,
+                         size_t workspace_bytes, void* stream) {
+  const char* fn = "bffc_modal_transpose";
+  if (int rc = modal_args(fn, v, x, G, N)) return rc;
+  if (int rc = groups_args(fn, H, G)) return rc;
+  if (B < 1 || len < 0) return fail(BFFC_ERR_INVALID, "%s: B=%d len=%lld", fn, B, (long long)len);
+  if (w_dtype != BFFC_DTYPE_BF16 && w_dtype != BFFC_DTYPE_FP16 && w_dtype != BFFC_DTYPE_FP32)
+    return fail(BFFC_ERR_INVALID, "%s: w_dtype %d (BF16 0, FP16 1, FP32 2)", fn, w_dtype);
+  if ((len > 0 && !w) || misaligned(w, w_dtype == BFFC_DTYPE_FP32 ? 4 : 2))
+    return fail(BFFC_ERR_INVALID, "%s: w null or not aligned to its element", fn);
+  if (w_bstride < int64_t(H) * len)
+    return fail(BFFC_ERR_INVALID, "%s: batch stride %lld below H * len = %lld", fn, (long long)w_bstride, (long long)H * len);
+  if (!out || misaligned(out, 8) || misaligned(init, 8))
+    return fail(BFFC_ERR_INVALID, "%s: out null, or out / init not 8-byte aligned", fn);
+  if (int rc = slot_lists(fn, slots, lengths)) return rc;
+  if (slots ? Bs < 1 : Bs != B) return fail(BFFC_ERR_INVALID, "%s: Bs=%d (B=%d without slots)", fn, Bs, B);
+  const size_t need = bffc_modal_workspace_bytes(B, H, N, len, 0);
+  if (!workspace || misaligned(workspace, 16) || workspace_bytes < need)
+    return fail(BFFC_ERR_INVALID, "%s: a 16-byte aligned workspace of %zu bytes required", fn, need);
+  if (int rc = check_device()) return rc;
+  mdl::RedParams prm{};
+  prm.w = w; prm.w_bs = w_bstride; prm.len = len; prm.lengths = lengths; prm.reversed = reversed != 0;
+  prm.B = B; prm.H = H; prm.gs = H / G;
+  prm.v = static_cast<const float2*>(v); prm.x = static_cast<const float2*>(x); prm.N = N;
+  prm.init = static_cast<const float2*>(init); prm.out = static_cast<float2*>(out);
+  prm.slot_map = slots; prm.Bs = Bs;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (w_dtype == BFFC_DTYPE_FP32) return modal_reduce<float, false>(prm, workspace, st);
+  if (w_dtype == BFFC_DTYPE_FP16) return modal_reduce<__half, false>(prm, workspace, st);
+  return modal_reduce<__nv_bfloat16, false>(prm, workspace, st);
+}
+
+int bffc_modal_chunk(const void* u, int64_t u_bstride, const void* pregate, int64_t pregate_bstride,
+                     const void* postgate, int64_t postgate_bstride, const void* u_w, const void* u_bias,
+                     const void* pregate_w, const void* pregate_bias, const void* postgate_w,
+                     const void* postgate_bias, int w_dtype, int K, int padding, int dtype, void* tail, int64_t* pos,
+                     int slots, const int32_t* slot_map, const int32_t* lengths, int n, int B, int H, int T,
+                     int fresh, void* z, float* post, void* stream) {
+  const char* fn = "bffc_modal_chunk";
+  const void* const x[3] = {u, pregate, postgate};
+  const int64_t bs[3] = {u_bstride, pregate_bstride, postgate_bstride};
+  const void* const w[3] = {u_w, pregate_w, postgate_w};
+  const void* const bias[3] = {u_bias, pregate_bias, postgate_bias};
+  if (B < 1 || H < 1 || T < 0 || n < 1 || n > B)
+    return fail(BFFC_ERR_INVALID, "%s: bad shape B=%d H=%d T=%d n=%d", fn, B, H, T, n);
+  if (int rc = modal_roles(fn, dtype, w_dtype, K, padding, H, T, x, bs, w, bias, tail, pos)) return rc;
+  if (int rc = slot_lists(fn, slot_map, lengths)) return rc;
+  if (!slots && (slot_map || lengths || n != B))
+    return fail(BFFC_ERR_INVALID, "%s: slots and lengths need the slot mode (n = B rows without)", fn);
+  if ((T > 0 && !z) || misaligned(z, 2) || misaligned(post, 4))
+    return fail(BFFC_ERR_INVALID, "%s: z null, or z / post not aligned", fn);
+  if (int rc = check_device()) return rc;
+  dmd::Params p = modal_dec_params(x, bs, w, bias, w_dtype, K, tail, pos, slots != 0, B, H, T);
+  p.n = n; p.slot_map = slot_map; p.lengths = lengths; p.fresh = fresh != 0; p.z = z; p.post = post;
+  const dim3 grid(unsigned(H), grid_rows(n));
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  g_launches = 0;
+  if (dtype == BFFC_DTYPE_FP16) dmd::chunk<__half><<<grid, dmd::kChunkThreads, 0, st>>>(p);
+  else dmd::chunk<__nv_bfloat16><<<grid, dmd::kChunkThreads, 0, st>>>(p);
+  return launched();
+}
+
+int bffc_modal_step(const void* u, int64_t u_bstride, const void* pregate, int64_t pregate_bstride,
+                    const void* postgate, int64_t postgate_bstride, const void* u_w, const void* u_bias,
+                    const void* pregate_w, const void* pregate_bias, const void* postgate_w, const void* postgate_bias,
+                    int w_dtype, int K, int padding, int dtype, void* tail, void* h, const void* v, const void* x_,
+                    int G, int N, int64_t* pos, int slots, void* y, int64_t y_bstride, int B, int H, int T,
+                    void* stream) {
+  const char* fn = "bffc_modal_step";
+  const void* const x[3] = {u, pregate, postgate};
+  const int64_t bs[3] = {u_bstride, pregate_bstride, postgate_bstride};
+  const void* const w[3] = {u_w, pregate_w, postgate_w};
+  const void* const bias[3] = {u_bias, pregate_bias, postgate_bias};
+  if (T < 1 || T > dec::kMaxT) return fail(BFFC_ERR_INVALID, "%s: T=%d outside [1, %d]", fn, T, dec::kMaxT);
+  if (B < 1) return fail(BFFC_ERR_INVALID, "%s: B=%d < 1", fn, B);
+  if (int rc = modal_args(fn, v, x_, G, N)) return rc;
+  if (int rc = groups_args(fn, H, G)) return rc;
+  if (int rc = modal_roles(fn, dtype, w_dtype, K, padding, H, T, x, bs, w, bias, tail, pos)) return rc;
+  if (!h || misaligned(h, 8)) return fail(BFFC_ERR_INVALID, "%s: h null or not 8-byte aligned", fn);
+  if (!y || misaligned(y, 2)) return fail(BFFC_ERR_INVALID, "%s: y null or not aligned to its element", fn);
+  if (y_bstride < int64_t(H) * T)
+    return fail(BFFC_ERR_INVALID, "%s: batch stride %lld below H * T = %lld", fn, (long long)y_bstride, (long long)H * T);
+  if (int rc = check_device()) return rc;
+  dmd::Params p = modal_dec_params(x, bs, w, bias, w_dtype, K, tail, pos, slots != 0, B, H, T);
+  p.h = static_cast<float2*>(h); p.v = static_cast<const float2*>(v); p.x = static_cast<const float2*>(x_);
+  p.N = N; p.gs = H / G; p.y = y; p.y_bs = y_bstride;
+  const dim3 grid(unsigned(H), grid_rows((B + dmd::kStepWarps - 1) / dmd::kStepWarps));
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  g_launches = 0;
+  auto launch = [&](auto tt, auto mpl, auto mode) {
+    using T_ = typename decltype(tt)::type;
+    dmd::step<T_, decltype(mpl)::value, decltype(mode)::value><<<grid, dmd::kStepThreads, 0, st>>>(p);
+  };
+  auto with_mpl = [&](auto tt, auto mode) {
+    if (N <= 32) launch(tt, std::integral_constant<int, 1>(), mode);
+    else if (N <= 64) launch(tt, std::integral_constant<int, 2>(), mode);
+    else if (N <= 256) launch(tt, std::integral_constant<int, 8>(), mode);
+    else launch(tt, std::integral_constant<int, 32>(), mode);
+  };
+  auto with_mode = [&](auto tt) {
+    if (slots) with_mpl(tt, std::true_type());
+    else with_mpl(tt, std::false_type());
+  };
+  if (dtype == BFFC_DTYPE_FP16) with_mode(Tag<__half>());
+  else with_mode(Tag<__nv_bfloat16>());
+  return launched();
+}
+
+int bffc_modal_extend_finish(const void* yconv, const float* post, const void* h, const void* v, const void* x, int G,
+                             int N, int dtype, int64_t* pos, int slots, const int32_t* slot_map,
+                             const int32_t* lengths, int n, int B, int H, int T, void* y, int64_t y_bstride,
+                             void* stream) {
+  const char* fn = "bffc_modal_extend_finish";
+  if (dtype != BFFC_DTYPE_BF16 && dtype != BFFC_DTYPE_FP16) return fail(BFFC_ERR_INVALID, "%s: dtype %d (BF16 0, FP16 1)", fn, dtype);
+  if (B < 1 || T < 1 || n < 1 || n > B) return fail(BFFC_ERR_INVALID, "%s: bad shape B=%d T=%d n=%d", fn, B, T, n);
+  if (int rc = modal_args(fn, v, x, G, N)) return rc;
+  if (int rc = groups_args(fn, H, G)) return rc;
+  if (int rc = slot_lists(fn, slot_map, lengths)) return rc;
+  if (!slots && (slot_map || lengths || n != B))
+    return fail(BFFC_ERR_INVALID, "%s: slots and lengths need the slot mode (n = B rows without)", fn);
+  if (!yconv || misaligned(yconv, 2) || misaligned(post, 4) || !h || misaligned(h, 8) || !pos || misaligned(pos, 8))
+    return fail(BFFC_ERR_INVALID, "%s: yconv, h or pos null or not aligned", fn);
+  if (!y || misaligned(y, 2)) return fail(BFFC_ERR_INVALID, "%s: y null or not aligned to its element", fn);
+  if (y_bstride < int64_t(H) * T)
+    return fail(BFFC_ERR_INVALID, "%s: batch stride %lld below H * T = %lld", fn, (long long)y_bstride, (long long)H * T);
+  if (int rc = check_device()) return rc;
+  dmd::Params p{};
+  p.h = const_cast<float2*>(static_cast<const float2*>(h));
+  p.v = static_cast<const float2*>(v); p.x = static_cast<const float2*>(x); p.N = N; p.gs = H / G;
+  p.pos = reinterpret_cast<long long*>(pos); p.slots = slots != 0;
+  p.Bs = B; p.H = H; p.T = T; p.y = y; p.y_bs = y_bstride;
+  p.n = n; p.slot_map = slot_map; p.lengths = lengths; p.post = const_cast<float*>(post); p.yconv = yconv;
+  const dim3 grid(unsigned(mdl::tiles_of(T)), grid_rows(static_cast<long long>(n) * H));
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  g_launches = 0;
+  if (dtype == BFFC_DTYPE_FP16) dmd::extend_finish<__half><<<grid, mdl::kThreads, 0, st>>>(p);
+  else dmd::extend_finish<__nv_bfloat16><<<grid, mdl::kThreads, 0, st>>>(p);
+  return launched();
 }
 
 }  // extern "C"

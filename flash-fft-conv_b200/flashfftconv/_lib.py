@@ -132,6 +132,20 @@ SYMBOLS = {
                                 + [_c.c_int] * 6 + [_c.c_void_p, _c.c_size_t, _c.c_void_p]),
     'bffc_conv_extend_finish_slots': (_c.c_int, [_c.c_void_p] * 2 + [_c.c_int] * 2 + [_c.c_void_p] * 5 + [_c.c_int64]
                                       + [_c.c_int] * 7 + [_c.c_void_p, _c.c_size_t, _c.c_void_p]),
+    'bffc_modal_fwd': (_c.c_int, [_c.c_void_p, _c.c_void_p, _c.c_int, _c.c_int, _c.c_int64, _c.c_void_p, _c.c_void_p]),
+    'bffc_modal_workspace_bytes': (_c.c_size_t, [_c.c_int] * 3 + [_c.c_int64, _c.c_int]),
+    'bffc_modal_bwd': (_c.c_int, [_c.c_void_p, _c.c_void_p, _c.c_int, _c.c_int, _c.c_int64] + [_c.c_void_p] * 4
+                       + [_c.c_size_t, _c.c_void_p]),
+    'bffc_modal_transpose': (_c.c_int, [_c.c_void_p, _c.c_int64] + [_c.c_int] * 3 + [_c.c_int64, _c.c_void_p, _c.c_int]
+                             + [_c.c_void_p] * 2 + [_c.c_int] * 2 + [_c.c_void_p] * 3 + [_c.c_int, _c.c_void_p,
+                                                                                           _c.c_size_t, _c.c_void_p]),
+    'bffc_modal_chunk': (_c.c_int, [_c.c_void_p, _c.c_int64] * 3 + [_c.c_void_p] * 6 + [_c.c_int] * 4
+                         + [_c.c_void_p] * 2 + [_c.c_int] + [_c.c_void_p] * 2 + [_c.c_int] * 5 + [_c.c_void_p] * 3),
+    'bffc_modal_step': (_c.c_int, [_c.c_void_p, _c.c_int64] * 3 + [_c.c_void_p] * 6 + [_c.c_int] * 4
+                        + [_c.c_void_p] * 4 + [_c.c_int] * 2 + [_c.c_void_p, _c.c_int, _c.c_void_p, _c.c_int64]
+                        + [_c.c_int] * 3 + [_c.c_void_p]),
+    'bffc_modal_extend_finish': (_c.c_int, [_c.c_void_p] * 5 + [_c.c_int] * 3 + [_c.c_void_p, _c.c_int]
+                                 + [_c.c_void_p] * 2 + [_c.c_int] * 4 + [_c.c_void_p, _c.c_int64, _c.c_void_p]),
     'bffc_docs_gather':(_c.c_int, [_c.c_void_p, _c.c_int, _c.c_int64] + [_c.c_int] * 3
                          + [_c.POINTER(_c.c_void_p), _c.POINTER(_c.c_int64), _c.POINTER(_c.c_void_p), _c.c_int,
                             _c.c_void_p]),

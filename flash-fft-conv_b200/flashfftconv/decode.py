@@ -74,6 +74,14 @@ run (before it, the far field is zero and the outputs are the direct step's bits
 grouping tokens into steps changes no bit.  For graphs, capture a step and a refresh (after one eager refresh) and
 replay the refresh at least every floor(2048 / T) steps and after every admission; a replayed step past the far field
 does nothing for that member and sets a status that `pos` / `positions` report.
+
+Modal filters (k = ModalFilter(v, x), modal.py; INTEGRATION.md §13): the long filter k[m] = 2 Re sum_n v_n exp(x_n m),
+untruncated, of H3 / S4D.  The decoder keeps h (B, H, N) complex64 and the tail, no cache and no max_len
+(bffc_modal_chunk / bffc_modal_step / bffc_modal_extend_finish / bffc_modal_transpose, include/bffc.h).  A step of
+T <= 64 tokens is one launch: h <- exp(x) h + z, y = s_postgate * 2 Re(v . h) per token; a prefill's y comes from the FFT
+engine with k = log_vandermonde(v, x, L) and its state from one transpose of the prompt's z; an extend convolves the
+chunk by the FFT engine and adds the state's contribution.  Slots, lengths, graphs and `positions` work as above;
+far_field and a residual filter are refused.
 """
 import ctypes
 
@@ -84,6 +92,7 @@ from . import depthwise_1d as _dw
 from .conv import FlashFFTConv, _DT, _fwd, _on_device, _ptr, _stream
 from .docs import refuse
 from .gated import gated_long_conv, hyena_mixer, hyena_operator
+from .modal import ModalFilter, _params as _modal_params, log_vandermonde, transpose_into as _modal_transpose
 
 MAX_STEP_TOKENS = 64
 MAX_KERNEL_SIZE = 32
@@ -177,6 +186,12 @@ class _Decoder:
     def __init__(self, k, k2, H, batch, max_len, dtype, K, slots=False, far_field=False):
         if dtype not in _DT:
             raise ValueError(f'dtype must be torch.bfloat16 or torch.float16, got {dtype}')
+        self.modal = isinstance(k, ModalFilter)
+        if self.modal:
+            self._modal_init(k, k2, H, batch, dtype, K, slots, far_field)
+            return
+        if max_len is None:
+            raise ValueError('max_len is required (only a ModalFilter decodes without a cache)')
         if batch < 1 or max_len < 1:
             raise ValueError(f'batch {batch} and max_len {max_len} must be >= 1')
         self.H, self.batch, self.max_len, self.dtype, self.K = H, int(batch), int(max_len), dtype, K
@@ -208,6 +223,114 @@ class _Decoder:
             self._far_init()
         self.reset()
 
+    # ---- modal filter (decode_modal.cuh): a state of N complex numbers per (member, channel), no cache
+    def _modal_init(self, f, k2, H, batch, dtype, K, slots, far_field):
+        if far_field:
+            raise ValueError('far_field=True: a ModalFilter decoder keeps a state of fixed size and has no far field')
+        if k2 is not None:
+            raise ValueError('a residual filter next to a ModalFilter is not supported')
+        if batch < 1:
+            raise ValueError(f'batch {batch} must be >= 1')
+        v, x = _modal_params(f.v, f.x, 'ModalFilter')
+        if H % v.shape[0]:
+            raise ValueError(f'ModalFilter has G = {v.shape[0]} rows, which do not divide H = {H}')
+        self.H, self.batch, self.max_len, self.dtype, self.K = H, int(batch), None, dtype, K
+        self.far_field, self.slots = False, bool(slots)
+        self.v, self.x = v.detach(), x.detach()
+        self._ones = torch.ones_like(self.v)      # the state's transpose has coefficients 1 (h, not v * h)
+        self.k = self.k2 = None
+        self.device = v.device
+        self._modal_tail = torch.zeros((3, self.batch, H, K - 1), dtype=dtype, device=self.device)
+        self.modal_state = torch.zeros((self.batch, H, v.shape[1]), dtype=torch.complex64, device=self.device)
+        self._pos = position_array(self.batch, self.slots, self.device)
+        self._host_pos = [-1] * self.batch if self.slots else 0
+        # extend: per chunk length T, the FlashFFTConv, k[:T] and the spectrum of the latest eager transform (a captured
+        # extend reads it); pinned slot lists a captured extend copies from
+        self._modal_ext, self._ext_held, self._convs = {}, [], {}
+        self.reset()
+
+    def _prompt_filters(self, L):
+        """k (and k2) of a prompt of L positions: the first min(Lk, L) taps, or the modal filter's first L"""
+        if self.modal:
+            return log_vandermonde(self.v, self.x, L), None
+        k = self.k[:, :min(self.k.shape[1], L)]
+        return k, None if self.k2 is None else self.k2[:, :min(self.k2.shape[1], L)]
+
+    def _modal_chunk(self, u, pregate, postgate, T, n, meta, fresh, post):
+        """bffc_modal_chunk: z (n, H, T) of the rows, s_postgate into post (or None), the tails rewritten"""
+        roles = self._roles(u, pregate, postgate, T, n) if T else [(None, 0)] * 3
+        rows, wdt = self._tap_args() if T else ([None] * 6, _lib.BFFC_DTYPE_FP32)
+        args = [a for t, s in roles for a in (_ptr(t), s)]
+        z = torch.empty((n, self.H, T), dtype=self.dtype, device=self.device)
+        with _on_device(self.device):
+            _lib.check(_lib.lib().bffc_modal_chunk(*args, *rows, wdt, self.K, self.K - 1, _DT[self.dtype],
+                                                   _ptr(self._modal_tail), _ptr(self._pos), int(self.slots),
+                                                   _ptr(None if meta is None else meta[:n]),
+                                                   _ptr(None if meta is None else meta[n:]), n, self.batch, self.H, T,
+                                                   int(fresh), _ptr(z), _ptr(post), _stream()))
+        return z
+
+    def _modal_fill(self, u, pregate, postgate, L, slots=None, lengths=None):
+        """a prefill's state: the tails, the positions, and h from one reversed transpose of the prompt's z"""
+        n = self.batch if slots is None else len(slots)
+        meta = None if slots is None else _device_ints(slots + lengths, torch.int32, self.device)
+        z = self._modal_chunk(u, pregate, postgate, L, n, meta, True, None)
+        _modal_transpose(z, L, self._ones, self.x, self.modal_state, lengths=None if meta is None else meta[n:],
+                         slots=None if meta is None else meta[:n], reversed=True)
+        if slots is None:
+            self._host_pos = L
+        elif self._host_pos is not None:
+            for b, l in zip(slots, lengths):
+                self._host_pos[b] = l
+
+    def _modal_step(self, u, pregate, postgate, T):
+        capturing = torch.cuda.is_current_stream_capturing()
+        roles = self._roles(u, pregate, postgate, T)
+        rows, wdt = self._tap_args()
+        args = [a for t, s in roles for a in (_ptr(t), s)]
+        y = torch.empty((self.batch, self.H, T), dtype=self.dtype, device=self.device)
+        G, N = self.v.shape
+        with _on_device(self.device):
+            _lib.check(_lib.lib().bffc_modal_step(*args, *rows, wdt, self.K, self.K - 1, _DT[self.dtype],
+                                                  _ptr(self._modal_tail), _ptr(self.modal_state), _ptr(self.v),
+                                                  _ptr(self.x), G, N, _ptr(self._pos), int(self.slots), _ptr(y),
+                                                  self.H * T, self.batch, self.H, T, _stream()))
+        self._advance_host(T, capturing)
+        return y
+
+    def _modal_extend(self, u, pregate, postgate, T, n, idx, lens, capturing):
+        """chunk -> the engine's convolution of z with k[:T] -> finish (y, positions) -> transpose (the state)"""
+        meta = None
+        if self.slots:
+            host = torch.tensor(idx + lens, dtype=torch.int32).pin_memory()
+            if capturing:                  # every replay copies from this buffer
+                self._ext_held.append(host)
+            meta = host.to(self.device, non_blocking=True)
+        ent = self._modal_ext.get(T)
+        if ent is None:
+            if capturing:
+                raise RuntimeError(f'run one eager extend with T = {T} before capturing it (it makes the FFT plan and '
+                                   'the filter spectrum)')
+            ent = self._modal_ext[T] = [FlashFFTConv(prefill_seqlen(T, T), dtype=self.dtype).eval(),
+                                        log_vandermonde(self.v, self.x, T), None]
+        post = None if postgate is None else torch.empty((n, self.H, T), dtype=torch.float32, device=self.device)
+        z = self._modal_chunk(u, pregate, postgate, T, n, meta, False, post)
+        conv, kT, kf = ent
+        yconv, kf = _fwd(conv, z, kT, None, None, kf_engine=kf if capturing else None)
+        if not capturing:
+            ent[2] = kf
+        y = torch.empty((n, self.H, T), dtype=self.dtype, device=self.device)
+        G, N = self.v.shape
+        sl, ln = (None, None) if meta is None else (meta[:n], meta[n:])
+        with _on_device(self.device):
+            _lib.check(_lib.lib().bffc_modal_extend_finish(_ptr(yconv), _ptr(post), _ptr(self.modal_state),
+                                                           _ptr(self.v), _ptr(self.x), G, N, _DT[self.dtype],
+                                                           _ptr(self._pos), int(self.slots), _ptr(sl), _ptr(ln), n,
+                                                           self.batch, self.H, T, _ptr(y), self.H * T, _stream()))
+        _modal_transpose(z, T, self._ones, self.x, self.modal_state, init=self.modal_state, lengths=ln, slots=sl,
+                         reversed=True)
+        return y
+
     # ---- views of the state (include/bffc.h: tail, z cache, s_u cache)
     def _caches(self):
         B, H, n, K = self.batch, self.H, self.max_len, self.K
@@ -231,7 +354,7 @@ class _Decoder:
     @property
     def tail(self):
         """(3, B, H, K - 1) raw inputs of the last K - 1 positions of u, pregate and postgate."""
-        return self._caches()[0]
+        return self._modal_tail if self.modal else self._caches()[0]
 
     @property
     def pos(self):
@@ -306,7 +429,7 @@ class _Decoder:
 
     def _admission(self, n, L, lengths, slots):
         """(slots, lengths) of a slot prefill of n right-padded prompts of L positions, validated on the host"""
-        if L > self.max_len:
+        if self.max_len is not None and L > self.max_len:
             raise ValueError(f'prompt of {L} positions exceeds max_len = {self.max_len}')
         if lengths is None:
             raise ValueError('a slot decoder\'s prefill takes lengths=[...] (one per prompt row)')
@@ -434,7 +557,7 @@ class _Decoder:
             self.refresh()
 
     def _conv(self, L):
-        n = prefill_seqlen(L, max(self.k.shape[1], 0 if self.k2 is None else self.k2.shape[1]))
+        n = prefill_seqlen(L, L if self.modal else max(self.k.shape[1], 0 if self.k2 is None else self.k2.shape[1]))
         conv = self._convs.get(n)
         if conv is None:
             conv = self._convs[n] = FlashFFTConv(n, dtype=self.dtype).eval()
@@ -462,6 +585,8 @@ class _Decoder:
         return [None] * 6, _lib.BFFC_DTYPE_FP32
 
     def _fill(self, u, pregate, postgate, L):
+        if self.modal:
+            return self._modal_fill(u, pregate, postgate, L)
         roles = self._roles(u, pregate, postgate, L) if L else [(None, 0)] * 3
         rows, wdt = self._tap_args() if L else ([None] * 6, _lib.BFFC_DTYPE_FP32)
         args = [a for t, s in roles for a in (_ptr(t), s)]
@@ -474,6 +599,8 @@ class _Decoder:
 
     def _fill_slots(self, u, pregate, postgate, L, slots, lengths):
         """one bffc_conv_state_fill_slots call: prompt row i (already zero past lengths[i]) into slot slots[i]"""
+        if self.modal:
+            return self._modal_fill(u, pregate, postgate, L, slots, lengths)
         n = len(slots)
         roles = self._roles(u, pregate, postgate, L, n) if L else [(None, 0)] * 3
         rows, wdt = self._tap_args() if L else ([None] * 6, _lib.BFFC_DTYPE_FP32)
@@ -495,6 +622,8 @@ class _Decoder:
         T = u.shape[-1]
         if not 1 <= T <= MAX_STEP_TOKENS:
             raise ValueError(f'a step takes 1 to {MAX_STEP_TOKENS} tokens, got {T} (a longer chunk is a prefill)')
+        if self.modal:
+            return self._modal_step(u, pregate, postgate, T)
         capturing = torch.cuda.is_current_stream_capturing()
         if self.far_field and not capturing:
             self._far_sync()                   # the checks below and the refresh need the host mirrors
@@ -578,6 +707,14 @@ class _Decoder:
             if lengths is not None or slots is not None:
                 raise ValueError('lengths and slots are for a decoder made with slots=True')
             n, idx, lens = self.batch, list(range(self.batch)), [T] * self.batch
+        if self.modal:
+            if self._host_pos is not None and not capturing and self.slots:
+                idle = [b for b in idx if self._host_pos[b] < 0]
+                if idle:
+                    raise ValueError(f'slots {idle} are idle: admit a prompt into them with prefill first')
+            y = self._modal_extend(u, pregate, postgate, T, n, idx, lens, capturing)
+            self._advance_extend(idx, lens, T, capturing)
+            return y
         roles = self._roles(u, pregate, postgate, T, n)
         Lk = self.k.shape[1]
         Lk2 = 0 if self.k2 is None else self.k2.shape[1]
@@ -643,16 +780,11 @@ class _Decoder:
             else:
                 rc = l.bffc_conv_extend_finish(*head, self.batch, *tail)
             _lib.check(rc)
+        self._advance_extend(idx, lens, T, capturing)
         if capturing or self._host_pos is None:
-            self._host_pos = None
             if self.far_field:
                 self._host_r = None
         else:
-            if self.slots:
-                for b, ln in zip(idx, lens):
-                    self._host_pos[b] += ln
-            else:
-                self._host_pos += T
             if self.far_field and self._host_r is not None:
                 if self.slots:
                     for b in idx:
@@ -660,6 +792,15 @@ class _Decoder:
                 else:
                     self._host_r = self._host_pos
         return y
+
+    def _advance_extend(self, idx, lens, T, capturing):
+        if capturing or self._host_pos is None:
+            self._host_pos = None
+        elif self.slots:
+            for b, ln in zip(idx, lens):
+                self._host_pos[b] += ln
+        else:
+            self._host_pos += T
 
 
 class HyenaDecoder(_Decoder):
@@ -677,9 +818,12 @@ class HyenaDecoder(_Decoder):
     slots=True: one position per batch row (see the module docstring); every slot starts idle.
     far_field=True: steps sum at most 2048 lags and a refresh every 2048 positions adds the rest by one FFT (see the
     module docstring); filters that need an FFT past 4M points are refused.
+    k = ModalFilter(v, x) (modal.py): the untruncated modal filter, (G, N) parameters with G dividing d_model; the
+    decoder keeps a state of N complex numbers per (member, channel) and no cache, so max_len is not needed.  far_field
+    and residual_filter are refused with it.
     """
 
-    def __init__(self, short_filter, k, d_model, batch, max_len, residual_filter=None, dtype=torch.bfloat16,
+    def __init__(self, short_filter, k, d_model, batch, max_len=None, residual_filter=None, dtype=torch.bfloat16,
                  slots=False, far_field=False):
         if not isinstance(short_filter, _dw.FlashDepthWiseConv1d) or not short_filter.is_bhl:
             raise ValueError('short_filter must be a BHL FlashDepthWiseConv1d')
@@ -730,15 +874,14 @@ class HyenaDecoder(_Decoder):
         if lengths is not None or slots is not None:
             raise ValueError('lengths and slots are for a decoder made with slots=True')
         L = x.shape[-1]
-        if L > self.max_len:
+        if self.max_len is not None and L > self.max_len:
             raise ValueError(f'prompt of {L} positions exceeds max_len = {self.max_len}')
         x = x.contiguous()                 # the short filter takes a contiguous projection
         v, x1, x2 = self._split(x)
         if L == 0:
             self.reset()
             return x.new_empty((x.shape[0], self.d_model, 0))
-        k = self.k[:, :min(self.k.shape[1], L)]
-        k2 = None if self.k2 is None else self.k2[:, :min(self.k2.shape[1], L)]
+        k, k2 = self._prompt_filters(L)
         y = hyena_operator(self._conv(L), self.short_filter, x, k, self.d_model, residual_filter=k2)
         self._fill(v, x1, x2, L)
         if self.far_field:
@@ -757,8 +900,7 @@ class HyenaDecoder(_Decoder):
         if L == 0:
             y = x.new_empty((n, self.d_model, 0))
         else:
-            k = self.k[:, :min(self.k.shape[1], L)]
-            k2 = None if self.k2 is None else self.k2[:, :min(self.k2.shape[1], L)]
+            k, k2 = self._prompt_filters(L)
             # the short filter's bias makes s non-zero past a prompt's end; zeroed there, the transform's rounding
             # scales with each prompt alone rather than with its padded row
             s = self._mask(self.short_filter(x)[..., :L], lens)
@@ -793,11 +935,15 @@ class LongConvDecoder(_Decoder):
     it already is, else a converted copy).  The gates given to prefill are the gates every step takes: z = u * pregate
     and z = u must not mix in one cache, so a step with another set of gates is refused.  With slots=True (one
     position per batch row, see the module docstring) every slot shares the gate set of the first prefill or step.
-    far_field=True: the far-field step (see the module docstring)."""
+    far_field=True: the far-field step (see the module docstring).  k = ModalFilter(v, x) (modal.py): the untruncated
+    modal filter with a fixed-size state and no max_len; H = channels, or v.shape[0] when channels is None (G = H)."""
 
-    def __init__(self, k, batch, max_len, dtype=torch.bfloat16, slots=False, far_field=False):
+    def __init__(self, k, batch, max_len=None, dtype=torch.bfloat16, slots=False, far_field=False, channels=None):
         self._gates = None                 # (pregate given, postgate given) of this sequence, once known
-        super().__init__(k, None, k.shape[0], batch, max_len, dtype, 1, slots, far_field)
+        if channels is not None and not isinstance(k, ModalFilter):
+            raise ValueError('channels is for a ModalFilter (an (H, Lk) k has H rows)')
+        H = (k.v.shape[0] if channels is None else int(channels)) if isinstance(k, ModalFilter) else k.shape[0]
+        super().__init__(k, None, H, batch, max_len, dtype, 1, slots, far_field)
 
     def _same_gates(self, pregate, postgate):
         gates = (pregate is not None, postgate is not None)
@@ -827,7 +973,7 @@ class LongConvDecoder(_Decoder):
         if lengths is not None or slots is not None:
             raise ValueError('lengths and slots are for a decoder made with slots=True')
         L = u.shape[-1]
-        if L > self.max_len:
+        if self.max_len is not None and L > self.max_len:
             raise ValueError(f'prompt of {L} positions exceeds max_len = {self.max_len}')
         self._roles(u, pregate, postgate, L)
         if L == 0:
@@ -836,7 +982,7 @@ class LongConvDecoder(_Decoder):
         self._gates = None
         self._same_gates(pregate, postgate)
         conv = self._conv(L)
-        k = self.k[:, :min(self.k.shape[1], L)]
+        k = self._prompt_filters(L)[0]
         if pregate is None and postgate is None:
             y = conv(u.contiguous(), k)
         else:                              # a missing gate is 1: the products with it are exact
@@ -859,7 +1005,7 @@ class LongConvDecoder(_Decoder):
             y = torch.empty_like(u)
         else:
             conv = self._conv(L)
-            k = self.k[:, :min(self.k.shape[1], L)]
+            k = self._prompt_filters(L)[0]
             if pregate is None and postgate is None:
                 y = conv(u, k)
             else:

@@ -673,6 +673,60 @@ int bffc_docs_scatter(const void* items, int n_items, int64_t positions, int B, 
                       const void* const* gathered, void* const* dst, const int64_t* dst_bstride, int n_tensors,
                       void* stream);
 
+/*
+ * Modal (diagonal state-space, S4D / H3) filters and their decoding (no plan; INTEGRATION.md §13).  v and x are
+ * complex64 (rows, N), interleaved float2, 8-byte aligned, 1 <= N <= 1024; E = exp(x).
+ * bffc_modal_fwd: k[r, l] = 2 Re sum_n v[r, n] E_n^l, fp32 (rows, L), L >= 1.  One launch.
+ * bffc_modal_bwd: dv[r, n] = 2 sum_l dk[r, l] conj(E_n^l) and dx[r, n] = 2 conj(v[r, n]) sum_l dk[r, l] l conj(E_n^l)
+ *   (torch's complex-gradient convention), complex64 (rows, N).  Two launches; the sum over l runs in a fixed order that
+ *   depends on the shape only (no atomics), so dv and dx are bit-reproducible on any device.
+ * bffc_modal_workspace_bytes(B, H, N, L, grad): the workspace of bffc_modal_bwd (B = 1, H = rows, grad = 1) or of
+ *   bffc_modal_transpose (grad = 0); 0 for a bad shape.
+ * bffc_modal_transpose: out[s_b, h, n] = v[g, n] sum_{l < len_b} w[b, h, l'] E_{g,n}^l (+ init[s_b, h, n] E_{g,n}^len_b)
+ *   with g = h / (H / G), w (B, H, len) of w_dtype (bf16, fp16 or fp32) with contiguous rows at batch stride w_bstride,
+ *   len_b = lengths[b] clamped to [0, len] (len without lengths), l' = l or len_b - 1 - l (reversed), s_b = slots[b]
+ *   (rows outside [0, Bs) skipped) or b (Bs = B).  out and init are (Bs, H, N) complex64 and may be the same buffer.
+ *   lengths and slots are device int32[B], never read on the host.  Two launches (one when len = 0), fixed order.
+ * The decoding calls keep a tail (3, B, H, K - 1) of raw inputs (dtype), a state h (B, H, N) complex64 and the (2, P)
+ * int64 position array of bffc_conv_step (P = 1, or P = B with slots; -1 an idle slot).  Inputs, taps and strides as
+ * bffc_conv_step's; parameters (G, N) with H % G == 0, channel h reading row h / (H / G).
+ * bffc_modal_chunk: row i (member slot_map[i] with slots, else i; n = B rows without slots) of lengths[i] (or T) tokens:
+ *   z (n, H, T) (the direct step's z, zero past the length) and, when post is not null, s_postgate (n, H, T) fp32; the
+ *   member's tail rewritten.  fresh: the tail before the chunk is zero and the member's position becomes its length
+ *   (a prefill); otherwise an idle member is skipped (zero rows).  One launch.
+ * bffc_modal_step: T in [1, 64] tokens per member: h <- E h + z, y = round(s_postgate * 2 Re sum_n v_n h_n) per token,
+ *   positions advanced by T; an idle member gets a zero y row and its state is not touched.  One launch.
+ * bffc_modal_extend_finish: y[i, h, t] = round(s_postgate[t] * (yconv[t] + 2 Re sum_n v_n E_n^(t+1) h_n)) for t below
+ *   the row's length (zero past it and for idle members), positions advanced by the length.  Two-step extend: chunk,
+ *   the engine's convolution of z with k[:T] into yconv, this call, then bffc_modal_transpose with init = out = h.
+ * Host arguments are checked before the device is looked at (BFFC_ERR_INVALID on any machine); positions, slots and
+ * lengths are read on the device only, so every call can be captured in a CUDA graph.
+ */
+int bffc_modal_fwd(const void* v, const void* x, int rows, int N, int64_t L, float* k, void* stream);
+size_t bffc_modal_workspace_bytes(int B, int H, int N, int64_t L, int grad);
+int bffc_modal_bwd(const void* v, const void* x, int rows, int N, int64_t L, const float* dk, void* dv, void* dx,
+                   void* workspace, size_t workspace_bytes, void* stream);
+int bffc_modal_transpose(const void* w, int64_t w_bstride, int w_dtype, int B, int H, int64_t len,
+                         const int32_t* lengths, int reversed, const void* v, const void* x, int G, int N,
+                         const void* init, void* out, const int32_t* slots, int Bs, void* workspace,
+                         size_t workspace_bytes, void* stream);
+int bffc_modal_chunk(const void* u, int64_t u_bstride, const void* pregate, int64_t pregate_bstride,
+                     const void* postgate, int64_t postgate_bstride, const void* u_w, const void* u_bias,
+                     const void* pregate_w, const void* pregate_bias, const void* postgate_w,
+                     const void* postgate_bias, int w_dtype, int K, int padding, int dtype, void* tail, int64_t* pos,
+                     int slots, const int32_t* slot_map, const int32_t* lengths, int n, int B, int H, int T,
+                     int fresh, void* z, float* post, void* stream);
+int bffc_modal_step(const void* u, int64_t u_bstride, const void* pregate, int64_t pregate_bstride,
+                    const void* postgate, int64_t postgate_bstride, const void* u_w, const void* u_bias,
+                    const void* pregate_w, const void* pregate_bias, const void* postgate_w, const void* postgate_bias,
+                    int w_dtype, int K, int padding, int dtype, void* tail, void* h, const void* v, const void* x,
+                    int G, int N, int64_t* pos, int slots, void* y, int64_t y_bstride, int B, int H, int T,
+                    void* stream);
+int bffc_modal_extend_finish(const void* yconv, const float* post, const void* h, const void* v, const void* x, int G,
+                             int N, int dtype, int64_t* pos, int slots, const int32_t* slot_map,
+                             const int32_t* lengths, int n, int B, int H, int T, void* y, int64_t y_bstride,
+                             void* stream);
+
 /* Number of kernel launches the last bffc_fwd / bffc_bwd / bffc_fwd_host / filter-side transform /
  * bffc_dwconv1d_fwd (1) / bffc_dwconv1d_bwd (2) / bffc_conv_state_fill[_slots] (1) / bffc_conv_step[_slots] (2) /
  * bffc_conv_far_gather[_slots] (1) / bffc_conv_step_far[_slots] (2) / bffc_conv_extend_gather[_slots] (1) /
