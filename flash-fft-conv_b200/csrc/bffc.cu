@@ -22,6 +22,7 @@
 #include "decode_extend.cuh"
 #include "modal.cuh"
 #include "decode_modal.cuh"
+#include "fir_conv.cuh"
 #include "docs.cuh"
 
 #include <algorithm>
@@ -2988,6 +2989,131 @@ int bffc_modal_extend_finish(const void* yconv, const float* post, const void* h
   g_launches = 0;
   if (dtype == BFFC_DTYPE_FP16) dmd::extend_finish<__half><<<grid, mdl::kThreads, 0, st>>>(p);
   else dmd::extend_finish<__nv_bfloat16><<<grid, mdl::kThreads, 0, st>>>(p);
+  return launched();
+}
+
+}  // extern "C"
+
+// ------------------------------------------------------------------ direct convolution with short filters (no plan)
+namespace {
+
+namespace fir = bffc::fir;
+
+// The checks bffc_fir_fwd and bffc_fir_bwd share: shape, dtype, filter, the gates and every tensor's pointer and stride.
+int fir_args(const char* fn, int G, int Lk, int B, int H, int64_t L, int dtype, const float* k, const void* pregate,
+             const void* postgate, std::initializer_list<std::pair<const void*, int64_t>> tensors) {
+  if (dtype != BFFC_DTYPE_BF16 && dtype != BFFC_DTYPE_FP16) return fail(BFFC_ERR_INVALID, "%s: dtype %d (BF16 0, FP16 1)", fn, dtype);
+  if (B < 1 || H < 1 || L < 1 || L % 8)
+    return fail(BFFC_ERR_INVALID, "%s: B=%d H=%d L=%lld (L >= 1, a multiple of 8)", fn, B, H, (long long)L);
+  if (Lk < 1 || Lk > fir::kMaxLk) return fail(BFFC_ERR_INVALID, "%s: Lk=%d outside [1, %d]", fn, Lk, fir::kMaxLk);
+  if (int rc = groups_args(fn, H, G)) return rc;
+  if (!k || misaligned(k, 4)) return fail(BFFC_ERR_INVALID, "%s: k null or not 4-byte aligned", fn);
+  if (!pregate != !postgate) return fail(BFFC_ERR_INVALID, "%s: pregate and postgate must both be given or both be null", fn);
+  for (const auto& t : tensors) {
+    if (!t.first || misaligned(t.first, 16)) return fail(BFFC_ERR_INVALID, "%s: a tensor is null or not 16-byte aligned", fn);
+    if (t.second < int64_t(H) * L || t.second % 8)
+      return fail(BFFC_ERR_INVALID, "%s: batch stride %lld below H * L = %lld or not a multiple of 8", fn,
+                  (long long)t.second, (long long)H * L);
+  }
+  return 0;
+}
+
+dim3 fir_grid(long long slabs, long long rows) { return dim3(unsigned(slabs), grid_rows(rows)); }
+
+#define FIR_P_SWITCH(P_, ...)                                \
+  do {                                                       \
+    if ((P_) == 0) { constexpr int PP = 0; __VA_ARGS__ }     \
+    else if ((P_) == 1) { constexpr int PP = 1; __VA_ARGS__ } \
+    else { constexpr int PP = 2; __VA_ARGS__ }               \
+  } while (0)
+
+template <class T>
+void fir_fwd_launch(const fir::Params& p, int P, bool gated, dim3 grid, cudaStream_t st) {
+  FIR_P_SWITCH(P, {
+    if (gated) fir::fwd<T, PP, true><<<grid, fir::kThreads, 0, st>>>(p);
+    else fir::fwd<T, PP, false><<<grid, fir::kThreads, 0, st>>>(p);
+  });
+}
+
+template <class T>
+void fir_bwd_launch(const fir::Params& p, int P, bool gated, dim3 grid, cudaStream_t st) {
+  FIR_P_SWITCH(P, {
+    if (gated) fir::bwd<T, PP, true><<<grid, fir::kThreads, 0, st>>>(p);
+    else fir::bwd<T, PP, false><<<grid, fir::kThreads, 0, st>>>(p);
+  });
+}
+
+}  // namespace
+
+extern "C" {
+
+int bffc_fir_fwd(const void* u, int64_t u_bstride, const void* pregate, int64_t pregate_bstride, const void* postgate,
+                 int64_t postgate_bstride, const float* k, int G, int Lk, int B, int H, int64_t L, int dtype, void* y,
+                 int64_t y_bstride, void* stream) {
+  const char* fn = "bffc_fir_fwd";
+  const bool gated = pregate != nullptr;
+  if (int rc = gated ? fir_args(fn, G, Lk, B, H, L, dtype, k, pregate, postgate,
+                                {{u, u_bstride}, {pregate, pregate_bstride}, {postgate, postgate_bstride}, {y, y_bstride}})
+                     : fir_args(fn, G, Lk, B, H, L, dtype, k, pregate, postgate, {{u, u_bstride}, {y, y_bstride}}))
+    return rc;
+  if (int rc = check_device()) return rc;
+  fir::Params p{};
+  p.u = static_cast<const uint16_t*>(u); p.u_bs = u_bstride;
+  p.pre = static_cast<const uint16_t*>(pregate); p.pre_bs = pregate_bstride;
+  p.post = static_cast<const uint16_t*>(postgate); p.post_bs = postgate_bstride;
+  p.y = static_cast<uint16_t*>(y); p.y_bs = y_bstride;
+  p.k = k; p.L = L; p.slabs = fir::slabs_of(L); p.B = B; p.H = H; p.gs = H / G; p.Lk = Lk;
+  const dim3 grid = fir_grid(p.slabs, static_cast<long long>(B) * H);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  g_launches = 0;
+  if (dtype == BFFC_DTYPE_FP16) fir_fwd_launch<__half>(p, fir::p_of(Lk), gated, grid, st);
+  else fir_fwd_launch<__nv_bfloat16>(p, fir::p_of(Lk), gated, grid, st);
+  return launched();
+}
+
+size_t bffc_fir_workspace_bytes(int B, int H, int64_t L, int Lk) {
+  if (B < 1 || H < 1 || L < 1 || Lk < 1 || Lk > fir::kMaxLk) return 0;
+  return std::max<size_t>(size_t(B) * size_t(H) * size_t(fir::slabs_of(L)) * size_t(Lk) * sizeof(float), 16);
+}
+
+int bffc_fir_bwd(const void* dout, int64_t dout_bstride, const void* u, int64_t u_bstride, const void* pregate,
+                 int64_t pregate_bstride, const void* postgate, int64_t postgate_bstride, const float* k, int G, int Lk,
+                 int B, int H, int64_t L, int dtype, void* du, int64_t du_bstride, void* dpregate,
+                 int64_t dpregate_bstride, void* dpostgate, int64_t dpostgate_bstride, float* dk, void* workspace,
+                 size_t workspace_bytes, void* stream) {
+  const char* fn = "bffc_fir_bwd";
+  const bool gated = pregate != nullptr;
+  if (int rc = gated ? fir_args(fn, G, Lk, B, H, L, dtype, k, pregate, postgate,
+                                {{dout, dout_bstride}, {u, u_bstride}, {pregate, pregate_bstride},
+                                 {postgate, postgate_bstride}, {du, du_bstride}, {dpregate, dpregate_bstride},
+                                 {dpostgate, dpostgate_bstride}})
+                     : fir_args(fn, G, Lk, B, H, L, dtype, k, pregate, postgate,
+                                {{dout, dout_bstride}, {u, u_bstride}, {du, du_bstride}}))
+    return rc;
+  if (!gated && (dpregate || dpostgate))
+    return fail(BFFC_ERR_INVALID, "%s: gate gradients requested from an ungated call", fn);
+  if (!dk || misaligned(dk, 4)) return fail(BFFC_ERR_INVALID, "%s: dk null or not 4-byte aligned", fn);
+  const size_t need = bffc_fir_workspace_bytes(B, H, L, Lk);
+  if (!workspace || misaligned(workspace, 16) || workspace_bytes < need)
+    return fail(BFFC_ERR_INVALID, "%s: a 16-byte aligned workspace of %zu bytes required", fn, need);
+  if (int rc = check_device()) return rc;
+  fir::Params p{};
+  p.dout = static_cast<const uint16_t*>(dout); p.dout_bs = dout_bstride;
+  p.u = static_cast<const uint16_t*>(u); p.u_bs = u_bstride;
+  p.pre = static_cast<const uint16_t*>(pregate); p.pre_bs = pregate_bstride;
+  p.post = static_cast<const uint16_t*>(postgate); p.post_bs = postgate_bstride;
+  p.y = static_cast<uint16_t*>(du); p.y_bs = du_bstride;
+  p.dpre = static_cast<uint16_t*>(dpregate); p.dpre_bs = dpregate_bstride;
+  p.dpost = static_cast<uint16_t*>(dpostgate); p.dpost_bs = dpostgate_bstride;
+  p.k = k; p.dk = dk; p.part = static_cast<float*>(workspace);
+  p.L = L; p.slabs = fir::slabs_of(L); p.B = B; p.H = H; p.gs = H / G; p.Lk = Lk;
+  const dim3 grid = fir_grid(p.slabs, static_cast<long long>(B) * H);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  g_launches = 0;
+  if (dtype == BFFC_DTYPE_FP16) fir_bwd_launch<__half>(p, fir::p_of(Lk), gated, grid, st);
+  else fir_bwd_launch<__nv_bfloat16>(p, fir::p_of(Lk), gated, grid, st);
+  if (int rc = launched()) return rc;
+  fir::dk_reduce<<<unsigned(G), fir::kReduceThreads, 0, st>>>(p);
   return launched();
 }
 

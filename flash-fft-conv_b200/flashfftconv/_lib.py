@@ -146,6 +146,11 @@ SYMBOLS = {
                         + [_c.c_int] * 3 + [_c.c_void_p]),
     'bffc_modal_extend_finish': (_c.c_int, [_c.c_void_p] * 5 + [_c.c_int] * 3 + [_c.c_void_p, _c.c_int]
                                  + [_c.c_void_p] * 2 + [_c.c_int] * 4 + [_c.c_void_p, _c.c_int64, _c.c_void_p]),
+    'bffc_fir_fwd': (_c.c_int, [_c.c_void_p, _c.c_int64] * 3 + [_c.c_void_p] + [_c.c_int] * 4 + [_c.c_int64, _c.c_int]
+                     + [_c.c_void_p, _c.c_int64, _c.c_void_p]),
+    'bffc_fir_workspace_bytes': (_c.c_size_t, [_c.c_int, _c.c_int, _c.c_int64, _c.c_int]),
+    'bffc_fir_bwd': (_c.c_int, [_c.c_void_p, _c.c_int64] * 4 + [_c.c_void_p] + [_c.c_int] * 4 + [_c.c_int64, _c.c_int]
+                     + [_c.c_void_p, _c.c_int64] * 3 + [_c.c_void_p] * 2 + [_c.c_size_t, _c.c_void_p]),
     'bffc_docs_gather':(_c.c_int, [_c.c_void_p, _c.c_int, _c.c_int64] + [_c.c_int] * 3
                          + [_c.POINTER(_c.c_void_p), _c.POINTER(_c.c_int64), _c.POINTER(_c.c_void_p), _c.c_int,
                             _c.c_void_p]),

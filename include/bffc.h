@@ -727,10 +727,36 @@ int bffc_modal_extend_finish(const void* yconv, const float* post, const void* h
                              const int32_t* lengths, int n, int B, int H, int T, void* y, int64_t y_bstride,
                              void* stream);
 
+/*
+ * Direct causal convolution with filters of 1 to 128 taps on the tensor cores (no plan; INTEGRATION.md §14):
+ *   y[b, h, t] = postgate[b, h, t] * sum_{m < min(t + 1, Lk)} k[h / (H / G), m] z[b, h, t - m],  z = u * pregate
+ * u, pregate, postgate, dout and every output are (B, H, L) of dtype (BF16 or FP16) with contiguous rows at their own
+ * batch stride (a multiple of 8 and >= H * L), 16-byte aligned; L >= 1 is a multiple of 8 (a caller zero-pads a ragged
+ * L).  k is fp32 (G, Lk) with G dividing H.  The gates are both given or both null (then z = u and y = the sum).
+ * Rounding points (csrc/fir_conv.cuh): each group's taps scaled by a power of two to max |k| in [1, 2) and rounded once
+ * to dtype; z and w = dout * postgate rounded once to dtype; fp32 accumulation, unscaled in fp32, gated, rounded once.
+ * bffc_fir_fwd: y.  One launch.
+ * bffc_fir_bwd: du, dpregate and dpostgate (gated calls only; null otherwise) and dk (G, Lk) fp32, the sum over each
+ *   group.  Two launches: one pass over dout and the inputs writes the input gradients and one dk partial per (member,
+ *   channel, slab of up to 65536 samples), then the group sums of the partials in a fixed order (no atomics): dk is
+ *   bit-reproducible on any device, stream or graph replay.
+ * bffc_fir_workspace_bytes(B, H, L, Lk): the workspace of bffc_fir_bwd (16-byte aligned); 0 for a bad shape.
+ * Every host argument is checked before the device is looked at (BFFC_ERR_INVALID on any machine).
+ */
+int bffc_fir_fwd(const void* u, int64_t u_bstride, const void* pregate, int64_t pregate_bstride, const void* postgate,
+                 int64_t postgate_bstride, const float* k, int G, int Lk, int B, int H, int64_t L, int dtype, void* y,
+                 int64_t y_bstride, void* stream);
+size_t bffc_fir_workspace_bytes(int B, int H, int64_t L, int Lk);
+int bffc_fir_bwd(const void* dout, int64_t dout_bstride, const void* u, int64_t u_bstride, const void* pregate,
+                 int64_t pregate_bstride, const void* postgate, int64_t postgate_bstride, const float* k, int G, int Lk,
+                 int B, int H, int64_t L, int dtype, void* du, int64_t du_bstride, void* dpregate,
+                 int64_t dpregate_bstride, void* dpostgate, int64_t dpostgate_bstride, float* dk, void* workspace,
+                 size_t workspace_bytes, void* stream);
+
 /* Number of kernel launches the last bffc_fwd / bffc_bwd / bffc_fwd_host / filter-side transform /
  * bffc_dwconv1d_fwd (1) / bffc_dwconv1d_bwd (2) / bffc_conv_state_fill[_slots] (1) / bffc_conv_step[_slots] (2) /
  * bffc_conv_far_gather[_slots] (1) / bffc_conv_step_far[_slots] (2) / bffc_conv_extend_gather[_slots] (1) /
- * bffc_conv_extend_finish[_slots] (1) / bffc_docs_gather (1) / bffc_docs_scatter (1)
+ * bffc_conv_extend_finish[_slots] (1) / bffc_docs_gather (1) / bffc_docs_scatter (1) / bffc_fir_fwd (1) / bffc_fir_bwd (2)
  * on this thread enqueued (bench.py).  A bffc_bwd* on a deterministic plan
  * counts the same launches as on a default plan, plus one slot sum per dk_f launch whose rows have S > 1 slabs. */
 int bffc_last_launch_count(void);
