@@ -11,10 +11,13 @@
 // array (P = 1 shared, P = B slots; -1 an idle slot).  There is no cache and no max_len.
 //
 // step: one launch, grid (H, member groups), one warp per (member, channel).  Lane j holds modes j + 32 i, i < kMpl
-// (kMpl = 1, 2, 8 or 32 from N), in registers; the sum over n is lane-wise in ascending i, then a butterfly over the
-// warp, so every output's tree depends on N only: T tokens in one step and T single steps, or a member alone and inside
-// a batch, give the same bits.  An idle member is neither read nor written and gets a zero y row.  The block of channel
-// 0 advances the member's position; other blocks read only its sign, which an advance does not change.
+// (kMpl = 1, 2, 8 or 32 from N), in registers.  E stays in fp64 (exp(x) of the fp32 x, rounded to fp64 only), and each
+// token's E h + z is formed in fp64 from the fp32 h and rounded to fp32 once.  The state's error is then one fp32
+// rounding per token, carried by |E| <= 1; with E rounded to fp32 it was the error of E^p, which grows with the position
+// p, so an undamped mode's state drifted without bound.  The sum over n is lane-wise in ascending i, then a butterfly
+// over the warp, so every output's tree depends on N only: T tokens in one step and T single steps, or a member alone
+// and inside a batch, give the same bits.  An idle member is neither read nor written and gets a zero y row.  The block
+// of channel 0 advances the member's position; other blocks read only its sign, which an advance does not change.
 // chunk: z (and s_postgate) of a chunk of T tokens per row from the raw inputs and the tail, the tail rewritten; for a
 //   prefill (fresh) the tail before the chunk is zero and the position becomes the row's length.  One launch.
 // extend_finish: y[t] = round(s_post[t] * (F[t] + 2 Re sum_n v_n E_n^(t+1) h_n)) for t < len, with F the engine's
@@ -71,13 +74,14 @@ __device__ __forceinline__ float short_s(const Params& p, const decode::Role& r,
 
 template <class T, int kMpl, bool kSlots>
 __global__ void __launch_bounds__(kStepThreads) step(const Params p) {
-  __shared__ float2 se[32 * kMpl], sv[32 * kMpl];
+  __shared__ double2 se[32 * kMpl];
+  __shared__ float2 sv[32 * kMpl];
   __shared__ float ext[kStepWarps][decode::kMaxK - 1 + decode::kMaxT];
   __shared__ float sz[kStepWarps][decode::kMaxT], sp[kStepWarps][decode::kMaxT], sy[kStepWarps][decode::kMaxT];
   const int h = blockIdx.x, lane = threadIdx.x & 31, warp = threadIdx.x >> 5, T_ = p.T, K = p.K;
   const long long pr = h / p.gs;
   for (int n = threadIdx.x; n < 32 * kMpl; n += kStepThreads) {
-    se[n] = n < p.N ? modal::cexp1(p.x[pr * p.N + n]) : make_float2(0.f, 0.f);
+    se[n] = n < p.N ? modal::cexp1_d(p.x[pr * p.N + n]) : make_double2(0.0, 0.0);
     sv[n] = n < p.N ? p.v[pr * p.N + n] : make_float2(0.f, 0.f);
   }
   __syncthreads();
@@ -126,8 +130,10 @@ __global__ void __launch_bounds__(kStepThreads) step(const Params p) {
       for (int i = 0; i < kMpl; ++i) {
         const int n = lane + 32 * i;
         if (n < p.N) {
-          const float2 e = se[n], v = sv[n];
-          st[i] = make_float2(fmaf(e.x, st[i].x, fmaf(-e.y, st[i].y, z)), fmaf(e.x, st[i].y, e.y * st[i].x));
+          const double2 e = se[n];
+          const float2 v = sv[n];
+          const double hx = st[i].x, hy = st[i].y;
+          st[i] = make_float2(float(fma(e.x, hx, fma(-e.y, hy, double(z)))), float(fma(e.x, hy, e.y * hx)));
           acc += fmaf(v.x, st[i].x, -v.y * st[i].y);
         }
       }
