@@ -23,6 +23,7 @@
 #include "modal.cuh"
 #include "decode_modal.cuh"
 #include "fir_conv.cuh"
+#include "decode_fir.cuh"
 #include "docs.cuh"
 
 #include <algorithm>
@@ -3114,6 +3115,156 @@ int bffc_fir_bwd(const void* dout, int64_t dout_bstride, const void* u, int64_t 
   else fir_bwd_launch<__nv_bfloat16>(p, fir::p_of(Lk), gated, grid, st);
   if (int rc = launched()) return rc;
   fir::dk_reduce<<<unsigned(G), fir::kReduceThreads, 0, st>>>(p);
+  return launched();
+}
+
+}  // extern "C"
+
+// ------------------------------------------------------------------ decoding with a short explicit filter (no plan)
+namespace {
+
+namespace dfr = bffc::decode_fir;
+
+// the checks bffc_fir_decode_step and bffc_fir_decode_gather make on the filter length, the state and the slot lists
+int fir_dec_args(const char* fn, int Lk, int B, int H, int K, int dtype, const void* state, size_t state_bytes,
+                 const int32_t* slot_map, const int32_t* lengths) {
+  if (Lk < 1 || Lk > fir::kMaxLk)
+    return fail(BFFC_ERR_INVALID, "%s: Lk=%d outside [1, %d] (longer filters: the direct or far-field decoders)", fn,
+                Lk, fir::kMaxLk);
+  const size_t need = bffc_fir_decode_state_bytes(B, H, K, Lk, dtype);
+  if (need == 0) return fail(BFFC_ERR_INVALID, "%s: bad shape B=%d H=%d K=%d Lk=%d dtype=%d", fn, B, H, K, Lk, dtype);
+  if (!state || misaligned(state, 16) || state_bytes < need)
+    return fail(BFFC_ERR_INVALID, "%s: a 16-byte aligned state of %zu bytes required", fn, need);
+  return slot_lists(fn, slot_map, lengths);
+}
+
+dfr::Params fir_dec_params(const void* const (&x)[3], const int64_t (&bs)[3], const void* const (&w)[3],
+                           const void* const (&bias)[3], int w_dtype, int K, const float* k, int G, int Lk,
+                           void* state, int64_t* pos, bool slots, int B, int H, int T) {
+  dfr::Params p{};
+  for (int r = 0; r < 3; ++r) p.r[r] = dec::Role{x[r], bs[r], w[r], bias[r]};
+  p.w_dtype = w_dtype;
+  p.K = K;
+  p.tail = state;
+  p.ring = static_cast<unsigned char*>(state) + dfr::ring_offset(B, H, K);
+  p.k = k; p.Lk = Lk; p.gs = H / G;
+  p.pos = reinterpret_cast<long long*>(pos);
+  p.slots = slots;
+  p.Bs = B; p.H = H; p.T = T;
+  return p;
+}
+
+}  // namespace
+
+extern "C" {
+
+size_t bffc_fir_decode_state_bytes(int B, int H, int K, int Lk, int dtype) {
+  if (B < 1 || H < 1 || K < 1 || K > dec::kMaxK || Lk < 1 || Lk > fir::kMaxLk) return 0;
+  if (dtype != BFFC_DTYPE_BF16 && dtype != BFFC_DTYPE_FP16) return 0;
+  const size_t bytes = size_t(dfr::ring_offset(B, H, K)) + size_t(2) * size_t(B) * size_t(H) * size_t(Lk - 1);
+  return std::max<size_t>(bytes, 16);
+}
+
+int64_t bffc_fir_decode_row_len(int Lk, int T) {
+  if (Lk < 1 || Lk > fir::kMaxLk || T < 1) return 0;
+  return dfr::row_len_of(Lk, T);
+}
+
+int bffc_fir_decode_step(const void* u, int64_t u_bstride, const void* pregate, int64_t pregate_bstride,
+                         const void* postgate, int64_t postgate_bstride, const void* u_w, const void* u_bias,
+                         const void* pregate_w, const void* pregate_bias, const void* postgate_w,
+                         const void* postgate_bias, int w_dtype, int K, int padding, int dtype, const float* k, int G,
+                         int Lk, void* state, size_t state_bytes, int64_t* pos, int slots, void* y, int64_t y_bstride,
+                         int B, int H, int T, void* stream) {
+  const char* fn = "bffc_fir_decode_step";
+  const void* const x[3] = {u, pregate, postgate};
+  const int64_t bs[3] = {u_bstride, pregate_bstride, postgate_bstride};
+  const void* const w[3] = {u_w, pregate_w, postgate_w};
+  const void* const bias[3] = {u_bias, pregate_bias, postgate_bias};
+  if (T < 1 || T > dec::kMaxT) return fail(BFFC_ERR_INVALID, "%s: T=%d outside [1, %d]", fn, T, dec::kMaxT);
+  if (B < 1 || H < 1) return fail(BFFC_ERR_INVALID, "%s: B=%d H=%d must be >= 1", fn, B, H);
+  if (int rc = modal_roles(fn, dtype, w_dtype, K, padding, H, T, x, bs, w, bias, state, pos)) return rc;
+  if (int rc = fir_dec_args(fn, Lk, B, H, K, dtype, state, state_bytes, nullptr, nullptr)) return rc;
+  if (int rc = groups_args(fn, H, G)) return rc;
+  if (!k || misaligned(k, 4)) return fail(BFFC_ERR_INVALID, "%s: k null or not 4-byte aligned", fn);
+  if (!y || misaligned(y, 2)) return fail(BFFC_ERR_INVALID, "%s: y null or not aligned to its element", fn);
+  if (y_bstride < int64_t(H) * T)
+    return fail(BFFC_ERR_INVALID, "%s: batch stride %lld below H * T = %lld", fn, (long long)y_bstride, (long long)H * T);
+  if (int rc = check_device()) return rc;
+  dfr::Params p = fir_dec_params(x, bs, w, bias, w_dtype, K, k, G, Lk, state, pos, slots != 0, B, H, T);
+  p.y = y; p.y_bs = y_bstride;
+  const dim3 grid(unsigned((H + dfr::kStepWarps - 1) / dfr::kStepWarps), grid_rows(B));
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  g_launches = 0;
+  if (dtype == BFFC_DTYPE_FP16) {
+    if (slots) dfr::step<__half, true><<<grid, dfr::kStepThreads, 0, st>>>(p);
+    else dfr::step<__half, false><<<grid, dfr::kStepThreads, 0, st>>>(p);
+  } else {
+    if (slots) dfr::step<__nv_bfloat16, true><<<grid, dfr::kStepThreads, 0, st>>>(p);
+    else dfr::step<__nv_bfloat16, false><<<grid, dfr::kStepThreads, 0, st>>>(p);
+  }
+  return launched();
+}
+
+int bffc_fir_decode_gather(const void* u, int64_t u_bstride, const void* pregate, int64_t pregate_bstride,
+                           const void* postgate, int64_t postgate_bstride, const void* u_w, const void* u_bias,
+                           const void* pregate_w, const void* pregate_bias, const void* postgate_w,
+                           const void* postgate_bias, int w_dtype, int K, int padding, int dtype, int Lk, void* state,
+                           size_t state_bytes, int64_t* pos, int slots, const int32_t* slot_map,
+                           const int32_t* lengths, int n, int B, int H, int T, int fresh, void* ext_u,
+                           void* ext_pregate, void* ext_postgate, void* stream) {
+  const char* fn = "bffc_fir_decode_gather";
+  const void* const x[3] = {u, pregate, postgate};
+  const int64_t bs[3] = {u_bstride, pregate_bstride, postgate_bstride};
+  const void* const w[3] = {u_w, pregate_w, postgate_w};
+  const void* const bias[3] = {u_bias, pregate_bias, postgate_bias};
+  if (B < 1 || H < 1 || T < 1 || n < 1 || n > B)
+    return fail(BFFC_ERR_INVALID, "%s: bad shape B=%d H=%d T=%d n=%d", fn, B, H, T, n);
+  if (int rc = modal_roles(fn, dtype, w_dtype, K, padding, H, T, x, bs, w, bias, state, pos)) return rc;
+  if (int rc = fir_dec_args(fn, Lk, B, H, K, dtype, state, state_bytes, slot_map, lengths)) return rc;
+  if (!slots && (slot_map || lengths || n != B))
+    return fail(BFFC_ERR_INVALID, "%s: slots and lengths need the slot mode (n = B rows without)", fn);
+  if (!ext_u || !ext_pregate || !ext_postgate || misaligned(ext_u, 16) || misaligned(ext_pregate, 16) ||
+      misaligned(ext_postgate, 16))
+    return fail(BFFC_ERR_INVALID, "%s: engine rows null or not 16-byte aligned", fn);
+  if (int rc = check_device()) return rc;
+  dfr::Params p = fir_dec_params(x, bs, w, bias, w_dtype, K, nullptr, H, Lk, state, pos, slots != 0, B, H, T);   // no taps read
+  p.n = n; p.slot_map = slot_map; p.lengths = lengths; p.fresh = fresh != 0;
+  p.eu = ext_u; p.epre = ext_pregate; p.epost = ext_postgate;
+  const dim3 grid(unsigned(H), grid_rows(n));
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  g_launches = 0;
+  if (dtype == BFFC_DTYPE_FP16) dfr::gather<__half><<<grid, dfr::kGatherThreads, 0, st>>>(p);
+  else dfr::gather<__nv_bfloat16><<<grid, dfr::kGatherThreads, 0, st>>>(p);
+  return launched();
+}
+
+int bffc_fir_decode_finish(const void* ext_y, int dtype, int Lk, int64_t* pos, int slots, const int32_t* slot_map,
+                           const int32_t* lengths, int n, int B, int H, int T, int fresh, void* y, int64_t y_bstride,
+                           void* stream) {
+  const char* fn = "bffc_fir_decode_finish";
+  if (dtype != BFFC_DTYPE_BF16 && dtype != BFFC_DTYPE_FP16) return fail(BFFC_ERR_INVALID, "%s: dtype %d (BF16 0, FP16 1)", fn, dtype);
+  if (B < 1 || H < 1 || T < 1 || n < 1 || n > B)
+    return fail(BFFC_ERR_INVALID, "%s: bad shape B=%d H=%d T=%d n=%d", fn, B, H, T, n);
+  if (Lk < 1 || Lk > fir::kMaxLk) return fail(BFFC_ERR_INVALID, "%s: Lk=%d outside [1, %d]", fn, Lk, fir::kMaxLk);
+  if (int rc = slot_lists(fn, slot_map, lengths)) return rc;
+  if (!slots && (slot_map || lengths || n != B))
+    return fail(BFFC_ERR_INVALID, "%s: slots and lengths need the slot mode (n = B rows without)", fn);
+  if (!ext_y || misaligned(ext_y, 16) || !pos || misaligned(pos, 8))
+    return fail(BFFC_ERR_INVALID, "%s: ext_y or pos null or not aligned", fn);
+  if (!y || misaligned(y, 2)) return fail(BFFC_ERR_INVALID, "%s: y null or not aligned to its element", fn);
+  if (y_bstride < int64_t(H) * T)
+    return fail(BFFC_ERR_INVALID, "%s: batch stride %lld below H * T = %lld", fn, (long long)y_bstride, (long long)H * T);
+  if (int rc = check_device()) return rc;
+  dfr::Params p{};
+  p.Lk = Lk; p.pos = reinterpret_cast<long long*>(pos); p.slots = slots != 0;
+  p.Bs = B; p.H = H; p.T = T; p.y = y; p.y_bs = y_bstride;
+  p.n = n; p.slot_map = slot_map; p.lengths = lengths; p.fresh = fresh != 0; p.ey = ext_y;
+  const dim3 grid(unsigned((T + dfr::kFinishThreads - 1) / dfr::kFinishThreads), grid_rows(static_cast<long long>(n) * H));
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  g_launches = 0;
+  if (dtype == BFFC_DTYPE_FP16) dfr::finish<__half><<<grid, dfr::kFinishThreads, 0, st>>>(p);
+  else dfr::finish<__nv_bfloat16><<<grid, dfr::kFinishThreads, 0, st>>>(p);
   return launched();
 }
 

@@ -6,4 +6,4 @@ from .block_conv import blocked_long_conv  # noqa: F401
 from .decode import HyenaDecoder, LongConvDecoder  # noqa: F401
 from .docs import DocumentTable  # noqa: F401
 from .modal import ModalFilter, log_vandermonde, log_vandermonde_transpose  # noqa: F401
-from .fir_conv import fir_conv, fir_mixer  # noqa: F401
+from .fir_conv import FirFilter, fir_conv, fir_mixer  # noqa: F401

@@ -82,6 +82,14 @@ T <= 64 tokens is one launch: h <- exp(x) h + z, y = s_postgate * 2 Re(v . h) pe
 engine with k = log_vandermonde(v, x, L) and its state from one transpose of the prompt's z; an extend convolves the
 chunk by the FFT engine and adds the state's contribution.  Slots, lengths, graphs and `positions` work as above;
 far_field and a residual filter are refused.
+
+Short explicit filters (k = FirFilter(k), fir_conv.py; INTEGRATION.md §14.1): the Hyena-SE / Hyena-MR filters of 1 to
+128 taps, (G, Lk) grouped.  The decoder keeps the tail and a ring of the last Lk - 1 z values per (member, channel), no
+cache and no max_len (bffc_fir_decode_step / bffc_fir_decode_gather / bffc_fir_decode_finish, include/bffc.h), and
+decodes the operator fir_conv / fir_mixer compute, with their rounded taps.  A step of T <= 64 tokens is one launch; a
+prefill or an extend is one gather, one bffc_fir_fwd on the tensor cores over [ring | chunk] and one finish, and a
+fresh prefill's y is fir_mixer's (fir_conv's) bit for bit.  Slots, lengths, graphs and `positions` work as above;
+far_field and a residual filter are refused.
 """
 import ctypes
 
@@ -91,6 +99,7 @@ from . import _lib
 from . import depthwise_1d as _dw
 from .conv import FlashFFTConv, _DT, _fwd, _on_device, _ptr, _stream
 from .docs import refuse
+from .fir_conv import FirFilter
 from .gated import gated_long_conv, hyena_mixer, hyena_operator
 from .modal import ModalFilter, _params as _modal_params, log_vandermonde, transpose_into as _modal_transpose
 
@@ -186,9 +195,12 @@ class _Decoder:
     def __init__(self, k, k2, H, batch, max_len, dtype, K, slots=False, far_field=False):
         if dtype not in _DT:
             raise ValueError(f'dtype must be torch.bfloat16 or torch.float16, got {dtype}')
-        self.modal = isinstance(k, ModalFilter)
+        self.modal, self.fir = isinstance(k, ModalFilter), isinstance(k, FirFilter)
         if self.modal:
             self._modal_init(k, k2, H, batch, dtype, K, slots, far_field)
+            return
+        if self.fir:
+            self._fir_init(k, k2, H, batch, dtype, K, slots, far_field)
             return
         if max_len is None:
             raise ValueError('max_len is required (only a ModalFilter decodes without a cache)')
@@ -248,6 +260,111 @@ class _Decoder:
         # extend reads it); pinned slot lists a captured extend copies from
         self._modal_ext, self._ext_held, self._convs = {}, [], {}
         self.reset()
+
+    # ---- short explicit filter (decode_fir.cuh): the tail and a ring of the last Lk - 1 z values, no cache
+    def _fir_init(self, f, k2, H, batch, dtype, K, slots, far_field):
+        if far_field:
+            raise ValueError('far_field=True: a FirFilter decoder keeps a state of fixed size and has no far field')
+        if k2 is not None:
+            raise ValueError('a residual filter next to a FirFilter is not supported')
+        if batch < 1:
+            raise ValueError(f'batch {batch} must be >= 1')
+        G, Lk = f.k.shape
+        if H % G:
+            raise ValueError(f'FirFilter has G = {G} rows, which do not divide H = {H}')
+        self.H, self.batch, self.max_len, self.dtype, self.K = H, int(batch), None, dtype, K
+        self.far_field, self.slots = False, bool(slots)
+        self.fir_k = f.k
+        self.k = self.k2 = None
+        self.device = f.k.device
+        nbytes = _lib.lib().bffc_fir_decode_state_bytes(self.batch, H, K, Lk, _DT[dtype])
+        self.state = torch.zeros(nbytes, dtype=torch.uint8, device=self.device)
+        self._pos = position_array(self.batch, self.slots, self.device)
+        self._host_pos = [-1] * self.batch if self.slots else 0
+        self._ext_held = []                # pinned slot lists a captured extend copies from
+        self.reset()
+
+    def _fir_views(self):
+        """(tail (3, B, H, K - 1), ring (B, H, Lk - 1)) views of the state (include/bffc.h)"""
+        B, H, K, R = self.batch, self.H, self.K, self.fir_k.shape[1] - 1
+        off = (6 * B * H * (K - 1) + 255) // 256 * 256
+        tail = self.state[:6 * B * H * (K - 1)].view(self.dtype).view(3, B, H, K - 1)
+        ring = self.state[off:off + 2 * B * H * R].view(self.dtype).view(B, H, R)
+        return tail, ring
+
+    @property
+    def fir_ring(self):
+        """(B, H, Lk - 1) of a FirFilter decoder: the last Lk - 1 z values of each row, oldest first (zero before the
+        sequence start)."""
+        return self._fir_views()[1]
+
+    def _fir_run(self, u, pregate, postgate, T, n, idx, lens, fresh, capturing):
+        """gather -> bffc_fir_fwd of k on [ring | chunk] -> finish: y (n, H, T) of a prefill (fresh) or an extend"""
+        roles = self._roles(u, pregate, postgate, T, n)
+        rows, wdt = self._tap_args()
+        args = [a for t, s in roles for a in (_ptr(t), s)]
+        l, dt, dev, H = _lib.lib(), _DT[self.dtype], self.device, self.H
+        G, Lk = self.fir_k.shape
+        Lr = l.bffc_fir_decode_row_len(Lk, T)
+        ext = torch.empty((4, n, H, Lr), dtype=self.dtype, device=dev)    # u, pregate, postgate, y rows
+        meta = sl = ln = None
+        if self.slots:
+            host = torch.tensor(idx + lens, dtype=torch.int32).pin_memory()
+            if capturing:                  # every replay copies from this buffer
+                self._ext_held.append(host)
+            meta = host.to(dev, non_blocking=True)
+            sl, ln = meta[:n], meta[n:]
+        y = torch.empty((n, H, T), dtype=self.dtype, device=dev)
+        with _on_device(dev):
+            _lib.check(l.bffc_fir_decode_gather(*args, *rows, wdt, self.K, self.K - 1, dt, Lk, _ptr(self.state),
+                                                self.state.numel(), _ptr(self._pos), int(self.slots), _ptr(sl),
+                                                _ptr(ln), n, self.batch, H, T, int(fresh), _ptr(ext[0]), _ptr(ext[1]),
+                                                _ptr(ext[2]), _stream()))
+            _lib.check(l.bffc_fir_fwd(_ptr(ext[0]), H * Lr, _ptr(ext[1]), H * Lr, _ptr(ext[2]), H * Lr,
+                                      _ptr(self.fir_k), G, Lk, n, H, Lr, dt, _ptr(ext[3]), H * Lr, _stream()))
+            _lib.check(l.bffc_fir_decode_finish(_ptr(ext[3]), dt, Lk, _ptr(self._pos), int(self.slots), _ptr(sl),
+                                                _ptr(ln), n, self.batch, H, T, int(fresh), _ptr(y), H * T, _stream()))
+        return y
+
+    def _fir_prefill(self, u, pregate, postgate, L, slots=None, lengths=None):
+        """a prefill: an extend from the zero state (the state of the rows is overwritten, not read)"""
+        if slots is None:
+            if L == 0:
+                self.reset()
+                return torch.empty((self.batch, self.H, 0), dtype=self.dtype, device=self.device)
+            y = self._fir_run(u, pregate, postgate, L, self.batch, None, None, True, False)
+            self._host_pos = L
+            return y
+        n = len(slots)
+        if L == 0:                         # an empty prompt: the admitted slots restart at position 0
+            idx = _device_ints(slots, torch.int64, self.device)
+            tail, ring = self._fir_views()
+            tail.index_fill_(1, idx, 0)
+            ring.index_fill_(0, idx, 0)
+            self._pos[0].index_fill_(0, idx, 0)
+            self._pos[1].index_fill_(0, idx, 0)
+            y = torch.empty((n, self.H, 0), dtype=self.dtype, device=self.device)
+        else:
+            y = self._fir_run(u, pregate, postgate, L, n, slots, lengths, True, False)
+        if self._host_pos is not None:
+            for b, l in zip(slots, lengths):
+                self._host_pos[b] = l
+        return y
+
+    def _fir_step(self, u, pregate, postgate, T):
+        capturing = torch.cuda.is_current_stream_capturing()
+        roles = self._roles(u, pregate, postgate, T)
+        rows, wdt = self._tap_args()
+        args = [a for t, s in roles for a in (_ptr(t), s)]
+        y = torch.empty((self.batch, self.H, T), dtype=self.dtype, device=self.device)
+        G, Lk = self.fir_k.shape
+        with _on_device(self.device):
+            _lib.check(_lib.lib().bffc_fir_decode_step(*args, *rows, wdt, self.K, self.K - 1, _DT[self.dtype],
+                                                       _ptr(self.fir_k), G, Lk, _ptr(self.state), self.state.numel(),
+                                                       _ptr(self._pos), int(self.slots), _ptr(y), self.H * T,
+                                                       self.batch, self.H, T, _stream()))
+        self._advance_host(T, capturing)
+        return y
 
     def _prompt_filters(self, L):
         """k (and k2) of a prompt of L positions: the first min(Lk, L) taps, or the modal filter's first L"""
@@ -354,6 +471,8 @@ class _Decoder:
     @property
     def tail(self):
         """(3, B, H, K - 1) raw inputs of the last K - 1 positions of u, pregate and postgate."""
+        if self.fir:
+            return self._fir_views()[0]
         return self._modal_tail if self.modal else self._caches()[0]
 
     @property
@@ -585,6 +704,11 @@ class _Decoder:
         return [None] * 6, _lib.BFFC_DTYPE_FP32
 
     def _fill(self, u, pregate, postgate, L):
+        if self.fir:                       # only reset() comes here: the zero state at position 0
+            self.state.zero_()
+            self._pos.zero_()
+            self._host_pos = 0
+            return
         if self.modal:
             return self._modal_fill(u, pregate, postgate, L)
         roles = self._roles(u, pregate, postgate, L) if L else [(None, 0)] * 3
@@ -624,6 +748,8 @@ class _Decoder:
             raise ValueError(f'a step takes 1 to {MAX_STEP_TOKENS} tokens, got {T} (a longer chunk is a prefill)')
         if self.modal:
             return self._modal_step(u, pregate, postgate, T)
+        if self.fir:
+            return self._fir_step(u, pregate, postgate, T)
         capturing = torch.cuda.is_current_stream_capturing()
         if self.far_field and not capturing:
             self._far_sync()                   # the checks below and the refresh need the host mirrors
@@ -713,6 +839,15 @@ class _Decoder:
                 if idle:
                     raise ValueError(f'slots {idle} are idle: admit a prompt into them with prefill first')
             y = self._modal_extend(u, pregate, postgate, T, n, idx, lens, capturing)
+            self._advance_extend(idx, lens, T, capturing)
+            return y
+        if self.fir:
+            if self._host_pos is not None and not capturing and self.slots:
+                idle = [b for b in idx if self._host_pos[b] < 0]
+                if idle:
+                    raise ValueError(f'slots {idle} are idle: admit a prompt into them with prefill first')
+            y = self._fir_run(u, pregate, postgate, T, n, idx if self.slots else None, lens if self.slots else None,
+                              False, capturing)
             self._advance_extend(idx, lens, T, capturing)
             return y
         roles = self._roles(u, pregate, postgate, T, n)
@@ -878,6 +1013,8 @@ class HyenaDecoder(_Decoder):
             raise ValueError(f'prompt of {L} positions exceeds max_len = {self.max_len}')
         x = x.contiguous()                 # the short filter takes a contiguous projection
         v, x1, x2 = self._split(x)
+        if self.fir:
+            return self._fir_prefill(v, x1, x2, L)
         if L == 0:
             self.reset()
             return x.new_empty((x.shape[0], self.d_model, 0))
@@ -895,6 +1032,8 @@ class HyenaDecoder(_Decoder):
         slots, lens = self._admission(n, L, lengths, slots)
         for name, t in zip(('v', 'x1', 'x2'), self._split(x)):   # shape, dtype and device before any work
             self._check(t, name, L, n)
+        if self.fir:                       # the gather reads no input past a row's length
+            return self._fir_prefill(*self._split(x), L, slots, lens)
         x = self._mask(x, lens)            # contiguous, zero past each length
         v, x1, x2 = self._split(x)
         if L == 0:
@@ -940,9 +1079,12 @@ class LongConvDecoder(_Decoder):
 
     def __init__(self, k, batch, max_len=None, dtype=torch.bfloat16, slots=False, far_field=False, channels=None):
         self._gates = None                 # (pregate given, postgate given) of this sequence, once known
-        if channels is not None and not isinstance(k, ModalFilter):
-            raise ValueError('channels is for a ModalFilter (an (H, Lk) k has H rows)')
-        H = (k.v.shape[0] if channels is None else int(channels)) if isinstance(k, ModalFilter) else k.shape[0]
+        if channels is not None and not isinstance(k, (ModalFilter, FirFilter)):
+            raise ValueError('channels is for a ModalFilter or a FirFilter (an (H, Lk) k has H rows)')
+        if isinstance(k, FirFilter):
+            H = k.k.shape[0] if channels is None else int(channels)
+        else:
+            H = (k.v.shape[0] if channels is None else int(channels)) if isinstance(k, ModalFilter) else k.shape[0]
         super().__init__(k, None, H, batch, max_len, dtype, 1, slots, far_field)
 
     def _same_gates(self, pregate, postgate):
@@ -981,6 +1123,8 @@ class LongConvDecoder(_Decoder):
             return torch.empty_like(u)
         self._gates = None
         self._same_gates(pregate, postgate)
+        if self.fir:
+            return self._fir_prefill(u, pregate, postgate, L)
         conv = self._conv(L)
         k = self._prompt_filters(L)[0]
         if pregate is None and postgate is None:
@@ -1000,6 +1144,8 @@ class LongConvDecoder(_Decoder):
         slots, lens = self._admission(n, L, lengths, slots)
         self._roles(u, pregate, postgate, L, n)
         self._same_gates(pregate, postgate)
+        if self.fir:                       # the gather reads no input past a row's length
+            return self._fir_prefill(u, pregate, postgate, L, slots, lens)
         u, pregate, postgate = (self._mask(t, lens) for t in (u, pregate, postgate))
         if L == 0:
             y = torch.empty_like(u)

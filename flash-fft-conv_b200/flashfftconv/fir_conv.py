@@ -9,6 +9,10 @@ short explicit filters of StripedHyena 2's Hyena-SE and Hyena-MR operators: no F
 L >= 1; channel slices of a projection are read in place (conv.batch_stride).  k is fp32 (H, Lk) or (G, Lk) with G
 dividing H and 1 <= Lk <= 128; channel h uses row h // (H // G) and dk is (G, Lk), summed over each group.  A ragged L
 is zero-padded to a multiple of 8, which does not change a causal result.
+
+FirFilter(k) hands such a filter to the decoders (decode.py): LongConvDecoder(FirFilter(k), batch) and
+HyenaDecoder(short_filter, FirFilter(k), d_model, batch) decode fir_conv / fir_mixer with its rounded taps, in a state
+of the tail and the last Lk - 1 z values per (member, channel), whatever the context length.
 """
 import torch
 
@@ -17,6 +21,27 @@ from . import docs as _docs
 from .conv import _DT, _on_device, _ptr, _stream, batch_stride
 
 MAX_TAPS = 128
+
+
+class FirFilter:
+    """A short explicit filter for the decoders: k fp32 (G, Lk) on CUDA, contiguous, 1 <= Lk <= 128, channel h using row
+    h // (H // G).  The decoders read k at every call, so in-place updates to it are seen; they decode the operator
+    fir_conv and fir_mixer compute, with the same rounded taps.  A plain (H, Lk) tensor instead goes to the direct
+    decoder, which keeps a cache of the whole context and multiplies by the fp32 taps."""
+
+    def __init__(self, k):
+        if not isinstance(k, torch.Tensor) or k.dtype != torch.float32 or not k.is_cuda or k.dim() != 2:
+            raise ValueError(f'FirFilter: k must be an fp32 (G, Lk) CUDA tensor, got '
+                             f'{tuple(getattr(k, "shape", ()))} {getattr(k, "dtype", type(k).__name__)}')
+        if not 1 <= k.shape[1] <= MAX_TAPS:
+            raise ValueError(f'FirFilter: Lk = {k.shape[1]} outside [1, {MAX_TAPS}]; decode a longer filter as a plain '
+                             f'(H, Lk) k with the direct decoder (max_len) or far_field=True')
+        if k.shape[0] < 1 or not k.is_contiguous():
+            raise ValueError('FirFilter: k must be contiguous with at least one row (its storage is read at every call)')
+        self.k = k
+
+    def __repr__(self):
+        return f'FirFilter(G={self.k.shape[0]}, Lk={self.k.shape[1]})'
 
 
 def _check(u, k, gates, name):

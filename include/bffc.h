@@ -753,11 +753,55 @@ int bffc_fir_bwd(const void* dout, int64_t dout_bstride, const void* u, int64_t 
                  int64_t dpregate_bstride, void* dpostgate, int64_t dpostgate_bstride, float* dk, void* workspace,
                  size_t workspace_bytes, void* stream);
 
+/*
+ * Decoding with a short explicit filter of 1 to 128 taps (no plan; INTEGRATION.md §14.1): the operator bffc_fir_fwd
+ * computes, y = round(s_postgate * 2^-s sum_{m < min(t + 1, Lk)} k^[g, m] z[t - m]) with fir_conv's rounded taps k^
+ * (each group's row scaled by 2^s to max |k| in [1, 2) and rounded once to dtype) and z = round(s_u * s_pregate) of the
+ * short filter's outputs, as bffc_conv_step forms them.  k is fp32 (G, Lk), G dividing H, read at every call.
+ * Inputs, short-filter taps and strides as bffc_conv_step's; positions the (2, P) int64 array of bffc_conv_step (P = 1,
+ * or P = B with slots; -1 an idle slot).
+ * bffc_fir_decode_state_bytes(B, H, K, Lk, dtype): one state buffer (16-byte aligned): the tail (3, B, H, K - 1) at
+ *   offset 0, then at roundup(6 B H (K - 1), 256) the ring (B, H, Lk - 1) of the last Lk - 1 z values, oldest first
+ *   (zero for positions before 0).  Nothing depends on the context length.  0 for a bad shape.
+ * bffc_fir_decode_row_len(Lk, T): W + roundup(T, 8) with W = roundup(Lk - 1, 64), the length of the engine rows of an
+ *   extend of T tokens; 0 for a bad argument.
+ * bffc_fir_decode_step: T in [1, 64] tokens per member; the ring shifted by T, the positions advanced by T; an idle
+ *   member gets a zero y row and its state is not touched.  The sum over lags has a fixed order that depends on Lk
+ *   only.  One launch.
+ * bffc_fir_decode_gather: row i (member slot_map[i] with slots, else i; n = B rows without slots) of lengths[i] (or T)
+ *   tokens into ext_u, ext_pregate and ext_postgate, each (n, H, bffc_fir_decode_row_len(Lk, T)): [ring | z | 0],
+ *   ones, and [0 | s_postgate (1 without a postgate) | 0], for one gated bffc_fir_fwd of k into ext_y; the tail and
+ *   the ring rewritten.  fresh: the state before the chunk is zero (a prefill); otherwise an idle member is skipped.
+ *   One launch.
+ * bffc_fir_decode_finish: y[i, h, t] = ext_y[i, h, W + t] for t below the row's length (zero past it and for idle
+ *   members); positions advanced by the length (fresh: set to it, status cleared).  One launch.
+ * Host arguments are checked before the device is looked at (BFFC_ERR_INVALID on any machine); positions, slots and
+ * lengths are read on the device only, so every call can be captured in a CUDA graph.
+ */
+size_t bffc_fir_decode_state_bytes(int B, int H, int K, int Lk, int dtype);
+int64_t bffc_fir_decode_row_len(int Lk, int T);
+int bffc_fir_decode_step(const void* u, int64_t u_bstride, const void* pregate, int64_t pregate_bstride,
+                         const void* postgate, int64_t postgate_bstride, const void* u_w, const void* u_bias,
+                         const void* pregate_w, const void* pregate_bias, const void* postgate_w,
+                         const void* postgate_bias, int w_dtype, int K, int padding, int dtype, const float* k, int G,
+                         int Lk, void* state, size_t state_bytes, int64_t* pos, int slots, void* y, int64_t y_bstride,
+                         int B, int H, int T, void* stream);
+int bffc_fir_decode_gather(const void* u, int64_t u_bstride, const void* pregate, int64_t pregate_bstride,
+                           const void* postgate, int64_t postgate_bstride, const void* u_w, const void* u_bias,
+                           const void* pregate_w, const void* pregate_bias, const void* postgate_w,
+                           const void* postgate_bias, int w_dtype, int K, int padding, int dtype, int Lk, void* state,
+                           size_t state_bytes, int64_t* pos, int slots, const int32_t* slot_map,
+                           const int32_t* lengths, int n, int B, int H, int T, int fresh, void* ext_u,
+                           void* ext_pregate, void* ext_postgate, void* stream);
+int bffc_fir_decode_finish(const void* ext_y, int dtype, int Lk, int64_t* pos, int slots, const int32_t* slot_map,
+                           const int32_t* lengths, int n, int B, int H, int T, int fresh, void* y, int64_t y_bstride,
+                           void* stream);
+
 /* Number of kernel launches the last bffc_fwd / bffc_bwd / bffc_fwd_host / filter-side transform /
  * bffc_dwconv1d_fwd (1) / bffc_dwconv1d_bwd (2) / bffc_conv_state_fill[_slots] (1) / bffc_conv_step[_slots] (2) /
  * bffc_conv_far_gather[_slots] (1) / bffc_conv_step_far[_slots] (2) / bffc_conv_extend_gather[_slots] (1) /
  * bffc_conv_extend_finish[_slots] (1) / bffc_docs_gather (1) / bffc_docs_scatter (1) / bffc_fir_fwd (1) / bffc_fir_bwd (2)
- * on this thread enqueued (bench.py).  A bffc_bwd* on a deterministic plan
+ * / bffc_fir_decode_step (1) / bffc_fir_decode_gather (1) / bffc_fir_decode_finish (1) on this thread enqueued (bench.py).  A bffc_bwd* on a deterministic plan
  * counts the same launches as on a default plan, plus one slot sum per dk_f launch whose rows have S > 1 slabs. */
 int bffc_last_launch_count(void);
 
