@@ -92,537 +92,91 @@ fresh prefill's y is fir_mixer's (fir_conv's) bit for bit.  Slots, lengths, grap
 far_field and a residual filter are refused.
 """
 import ctypes
+import functools
+import weakref
 
 import torch
 
 from . import _lib
 from . import depthwise_1d as _dw
-from .conv import FlashFFTConv, _DT, _fwd, _on_device, _ptr, _stream
+from .conv import _DT
+# FAR_BLOCK and the layout functions are part of this module's interface
+from .decode_state import (FAR_BLOCK, CacheState, FirState, ModalState, PositionBook, _mask, extend_layout,  # noqa: F401
+                           far_layout, position_array, prefill_seqlen, state_layout)
 from .docs import refuse
 from .fir_conv import FirFilter
 from .gated import gated_long_conv, hyena_mixer, hyena_operator
-from .modal import ModalFilter, _params as _modal_params, log_vandermonde, transpose_into as _modal_transpose
+from .modal import ModalFilter
 
 MAX_STEP_TOKENS = 64
 MAX_KERNEL_SIZE = 32
-FAR_BLOCK = 2048            # outputs per far-field refresh (decode_far.cuh kBlockOutputs)
 
 
-def prefill_seqlen(L, Lk):
-    """FFT size of a prefill of L positions with an Lk-tap filter: the next power of two >= max(256, L + min(Lk, L) - 1),
-    so the circular convolution of the first min(Lk, L) taps does not wrap."""
-    need = max(256, L + min(Lk, L) - 1)
-    return 1 << (need - 1).bit_length()
+def _no_taps(device):
+    """(rows of the u, pregate, postgate taps and biases, w_dtype) of the short filter; none here"""
+    return [None] * 6, _lib.BFFC_DTYPE_FP32
 
 
-def state_layout(B, H, max_len, K, residual):
-    """(z cache offset, s_u cache offset, total bytes) of a decoding state, the layout include/bffc.h documents and
-    state_layout in bffc.cu computes (tests/test_decode.py checks the total against bffc_conv_state_bytes)."""
-    a256 = lambda n: (n + 255) // 256 * 256
-    zc = a256(6 * B * H * (K - 1))
-    vc = zc + a256(2 * B * H * max_len)
-    return zc, vc, vc + (vc - zc if residual else 0)
+def _short_filter_taps(short_filter, D, K, device):
+    """the taps of the short filter's parameters as they are now (a .to(), .half() or load_state_dict(assign=True)
+    replaces their storage)"""
+    w, b = short_filter.weights, short_filter.bias
+    if w.dtype != b.dtype or w.dtype not in _dw._DT or not (w.is_contiguous() and b.is_contiguous()):
+        raise ValueError('short filter weights and bias must be contiguous and of one dtype')
+    if w.device != device or b.device != device:
+        raise ValueError(f'short filter on {w.device}, k on {device}')
+    es = w.element_size()
+    # rows of x1, x2, v in the (3D, K) weight and (3D) bias; roles u = v, pregate = x1, postgate = x2
+    w1, w2, wv = (w.data_ptr() + i * D * K * es for i in range(3))
+    b1, b2, bv = (b.data_ptr() + i * D * es for i in range(3))
+    return [ctypes.c_void_p(a) for a in (wv, bv, w1, b1, w2, b2)], _dw._DT[w.dtype]
 
 
-def far_layout(batch, H, Lk, Lk2, dtype):
-    """(W, n, bytes of one (batch, H, W + FAR_BLOCK) buffer) of the far field of filters of Lk and Lk2 taps (Lk2 = 0
-    without a residual filter), from bffc_conv_far_layout.  ValueError when the filters need an FFT past 4M points."""
-    W, n, nbytes = ctypes.c_int(), ctypes.c_int(), ctypes.c_size_t()
-    rc = _lib.lib().bffc_conv_far_layout(int(batch), int(H), int(Lk), int(Lk2), _DT[dtype], ctypes.byref(W),
-                                         ctypes.byref(n), ctypes.byref(nbytes))
-    if rc:
-        raise ValueError(f'far_field=True: {_lib.lib().bffc_last_error().decode()}')
-    return W.value, n.value, nbytes.value
+class _Decoder(PositionBook):
+    """One decoding state, whose class the type of k picks (decode_state.py), behind the public calls; the decoder is the
+    position book of its sequences.  The subclasses name the roles and compute a prompt's y."""
 
-
-def extend_layout(batch, H, Lk, Lk2, T, far, dtype):
-    """(W, n, W + P) of an extend by T tokens with filters of Lk and Lk2 taps (Lk2 = 0 without a residual filter), from
-    bffc_conv_extend_layout: engine rows of W + P elements, FFT size n.  ValueError when the chunk needs an FFT past 4M
-    points."""
-    W, n, nbytes = ctypes.c_int(), ctypes.c_int(), ctypes.c_size_t()
-    rc = _lib.lib().bffc_conv_extend_layout(int(batch), int(H), int(Lk), int(Lk2), int(T), int(bool(far)), _DT[dtype],
-                                            ctypes.byref(W), ctypes.byref(n), ctypes.byref(nbytes))
-    if rc:
-        raise ValueError(f'extend: {_lib.lib().bffc_last_error().decode()}')
-    return W.value, n.value, nbytes.value // 2
-
-
-def _host_ints(v, name):
-    """a host sequence or CPU tensor of ints as a list"""
-    if isinstance(v, torch.Tensor):
-        if v.is_cuda or v.dim() != 1 or v.dtype.is_floating_point or v.dtype == torch.bool:
-            raise ValueError(f'{name} must be a host sequence or a 1-D CPU integer tensor')
-        return [int(i) for i in v.tolist()]
-    return [int(i) for i in v]
-
-
-def position_array(batch, slots, device):
-    """The device position array of a decoder (include/bffc.h): int64 (2, P), row 0 the positions, row 1 the status
-    words.  P = batch with slots, every slot idle (-1); P = 1 without, kept as the int64[2] {0, 0} of the shared calls."""
-    if not slots:
-        return torch.zeros(2, dtype=torch.int64, device=device)
-    pos = torch.zeros(2, batch, dtype=torch.int64, device=device)
-    pos[0].fill_(-1)
-    return pos
-
-
-def _device_ints(values, dtype, device):
-    """a host list as a device tensor, copied from pinned memory without waiting for the stream's work"""
-    return torch.tensor(values, dtype=dtype).pin_memory().to(device, non_blocking=True)
-
-
-def _rows(t, H, T):
-    """(tensor, batch stride) of a (B, H, T) view with contiguous rows (element (b, h, t) at b * stride + h * T + t),
-    copying `t` when its layout does not qualify."""
-    _, sh, st = t.stride()
-    if (H > 1 and sh != T) or (T > 1 and st != 1):
-        t = t.contiguous()
-    return t, t.stride(0)
-
-
-def _filter(k, H, max_len, name):
-    """k as the step reads it: contiguous fp32 (the tensor itself when it already is, else a converted copy)"""
-    if k.dim() != 2 or k.shape[0] != H or not 1 <= k.shape[1] <= max_len:
-        raise ValueError(f'{name} must be ({H}, Lk) with 1 <= Lk <= max_len = {max_len}, got {tuple(k.shape)}')
-    if not k.is_cuda:
-        raise ValueError(f'{name} must be a CUDA tensor')
-    return k.detach().to(torch.float32).contiguous()
-
-
-class _Decoder:
-    """The state of one batch of sequences and the two library calls; the subclasses name the roles."""
-
-    def __init__(self, k, k2, H, batch, max_len, dtype, K, slots=False, far_field=False):
+    def __init__(self, k, k2, H, batch, max_len, dtype, K, slots=False, far_field=False, taps=_no_taps):
         if dtype not in _DT:
             raise ValueError(f'dtype must be torch.bfloat16 or torch.float16, got {dtype}')
-        self.modal, self.fir = isinstance(k, ModalFilter), isinstance(k, FirFilter)
-        if self.modal:
-            self._modal_init(k, k2, H, batch, dtype, K, slots, far_field)
-            return
-        if self.fir:
-            self._fir_init(k, k2, H, batch, dtype, K, slots, far_field)
-            return
-        if max_len is None:
-            raise ValueError('max_len is required (only a ModalFilter decodes without a cache)')
-        if batch < 1 or max_len < 1:
-            raise ValueError(f'batch {batch} and max_len {max_len} must be >= 1')
-        self.H, self.batch, self.max_len, self.dtype, self.K = H, int(batch), int(max_len), dtype, K
-        self.far_field = bool(far_field)
-        if self.far_field and k.dim() == 2 and (k2 is None or k2.dim() == 2):    # other shapes: _filter says why
-            Lk2 = 0 if k2 is None else k2.shape[1]
-            self.far_window, self.far_fft_size, _ = far_layout(self.batch, H, k.shape[1], Lk2, dtype)
-        self.k = _filter(k, H, self.max_len, 'k')
-        self.k2 = None if k2 is None else _filter(k2, H, self.max_len, 'residual_filter')
-        self.device = self.k.device
-        dt = _DT[dtype]
-        nbytes = _lib.lib().bffc_conv_state_bytes(self.batch, H, self.max_len, K, int(self.k2 is not None), dt)
-        self.state = torch.zeros(nbytes, dtype=torch.uint8, device=self.device)
-        self.slots = bool(slots)
-        # (2, P) positions and status words (include/bffc.h): P = 1 shared, kept as int64[2]; P = batch with slots
-        self._pos = position_array(self.batch, self.slots, self.device)
-        # known position (a list per slot with slots), or None after a graph capture
-        self._host_pos = [-1] * self.batch if self.slots else 0
-        self._ws = None
-        # workspaces outgrown by a larger T: a graph captured earlier still writes to the address it was given
-        self._ws_outgrown = []
-        self._convs = {}
-        # extend: one FlashFFTConv(n) per filter and FFT size, and the spectra of the latest eager transform at that
-        # size (a captured extend reads them, as a captured refresh reads _far_kf)
-        self._ext_convs, self._ext_kf = {}, {}
-        # pinned slot lists and lengths a captured extend copies from at every replay
-        self._ext_held = []
+        kind = ModalState if isinstance(k, ModalFilter) else FirState if isinstance(k, FirFilter) else CacheState
+        self._state = s = kind(k, k2, H, batch, max_len, dtype, K, slots, far_field, taps)
+        super().__init__(s.batch, s.slots, s.device, s.max_len)
+        s.book = weakref.proxy(self)       # a strong one would keep a dropped decoder and its caches until a collection
+        self.H, self.K, self.dtype, self.device, self.far_field = s.H, s.K, s.dtype, s.device, bool(far_field)
         if self.far_field:
-            self._far_init()
+            self.far_window, self.far_fft_size = s.far_window, s.far_fft_size
         self.reset()
 
-    # ---- modal filter (decode_modal.cuh): a state of N complex numbers per (member, channel), no cache
-    def _modal_init(self, f, k2, H, batch, dtype, K, slots, far_field):
-        if far_field:
-            raise ValueError('far_field=True: a ModalFilter decoder keeps a state of fixed size and has no far field')
-        if k2 is not None:
-            raise ValueError('a residual filter next to a ModalFilter is not supported')
-        if batch < 1:
-            raise ValueError(f'batch {batch} must be >= 1')
-        v, x = _modal_params(f.v, f.x, 'ModalFilter')
-        if H % v.shape[0]:
-            raise ValueError(f'ModalFilter has G = {v.shape[0]} rows, which do not divide H = {H}')
-        self.H, self.batch, self.max_len, self.dtype, self.K = H, int(batch), None, dtype, K
-        self.far_field, self.slots = False, bool(slots)
-        self.v, self.x = v.detach(), x.detach()
-        self._ones = torch.ones_like(self.v)      # the state's transpose has coefficients 1 (h, not v * h)
-        self.k = self.k2 = None
-        self.device = v.device
-        self._modal_tail = torch.zeros((3, self.batch, H, K - 1), dtype=dtype, device=self.device)
-        self.modal_state = torch.zeros((self.batch, H, v.shape[1]), dtype=torch.complex64, device=self.device)
-        self._pos = position_array(self.batch, self.slots, self.device)
-        self._host_pos = [-1] * self.batch if self.slots else 0
-        # extend: per chunk length T, the FlashFFTConv, k[:T] and the spectrum of the latest eager transform (a captured
-        # extend reads it); pinned slot lists a captured extend copies from
-        self._modal_ext, self._ext_held, self._convs = {}, [], {}
-        self.reset()
+    @property
+    def tail(self):
+        """(3, B, H, K - 1) raw inputs of the last K - 1 positions of u, pregate and postgate."""
+        return self._state.tail
 
-    # ---- short explicit filter (decode_fir.cuh): the tail and a ring of the last Lk - 1 z values, no cache
-    def _fir_init(self, f, k2, H, batch, dtype, K, slots, far_field):
-        if far_field:
-            raise ValueError('far_field=True: a FirFilter decoder keeps a state of fixed size and has no far field')
-        if k2 is not None:
-            raise ValueError('a residual filter next to a FirFilter is not supported')
-        if batch < 1:
-            raise ValueError(f'batch {batch} must be >= 1')
-        G, Lk = f.k.shape
-        if H % G:
-            raise ValueError(f'FirFilter has G = {G} rows, which do not divide H = {H}')
-        self.H, self.batch, self.max_len, self.dtype, self.K = H, int(batch), None, dtype, K
-        self.far_field, self.slots = False, bool(slots)
-        self.fir_k = f.k
-        self.k = self.k2 = None
-        self.device = f.k.device
-        nbytes = _lib.lib().bffc_fir_decode_state_bytes(self.batch, H, K, Lk, _DT[dtype])
-        self.state = torch.zeros(nbytes, dtype=torch.uint8, device=self.device)
-        self._pos = position_array(self.batch, self.slots, self.device)
-        self._host_pos = [-1] * self.batch if self.slots else 0
-        self._ext_held = []                # pinned slot lists a captured extend copies from
-        self.reset()
+    @property
+    def z_cache(self):
+        """(B, H, max_len) cache of z = s_u * s_pregate; slots [0, pos) are valid."""
+        return self._state.z_cache
 
-    def _fir_views(self):
-        """(tail (3, B, H, K - 1), ring (B, H, Lk - 1)) views of the state (include/bffc.h)"""
-        B, H, K, R = self.batch, self.H, self.K, self.fir_k.shape[1] - 1
-        off = (6 * B * H * (K - 1) + 255) // 256 * 256
-        tail = self.state[:6 * B * H * (K - 1)].view(self.dtype).view(3, B, H, K - 1)
-        ring = self.state[off:off + 2 * B * H * R].view(self.dtype).view(B, H, R)
-        return tail, ring
+    @property
+    def v_cache(self):
+        """(B, H, max_len) cache of s_u (kept when there is a residual filter), else None."""
+        return self._state.v_cache
+
+    @property
+    def modal_state(self):
+        """(B, H, N) complex64 h of a ModalFilter decoder."""
+        return self._state.modal_state
 
     @property
     def fir_ring(self):
         """(B, H, Lk - 1) of a FirFilter decoder: the last Lk - 1 z values of each row, oldest first (zero before the
         sequence start)."""
-        return self._fir_views()[1]
-
-    def _fir_run(self, u, pregate, postgate, T, n, idx, lens, fresh, capturing):
-        """gather -> bffc_fir_fwd of k on [ring | chunk] -> finish: y (n, H, T) of a prefill (fresh) or an extend"""
-        roles = self._roles(u, pregate, postgate, T, n)
-        rows, wdt = self._tap_args()
-        args = [a for t, s in roles for a in (_ptr(t), s)]
-        l, dt, dev, H = _lib.lib(), _DT[self.dtype], self.device, self.H
-        G, Lk = self.fir_k.shape
-        Lr = l.bffc_fir_decode_row_len(Lk, T)
-        ext = torch.empty((4, n, H, Lr), dtype=self.dtype, device=dev)    # u, pregate, postgate, y rows
-        meta = sl = ln = None
-        if self.slots:
-            host = torch.tensor(idx + lens, dtype=torch.int32).pin_memory()
-            if capturing:                  # every replay copies from this buffer
-                self._ext_held.append(host)
-            meta = host.to(dev, non_blocking=True)
-            sl, ln = meta[:n], meta[n:]
-        y = torch.empty((n, H, T), dtype=self.dtype, device=dev)
-        with _on_device(dev):
-            _lib.check(l.bffc_fir_decode_gather(*args, *rows, wdt, self.K, self.K - 1, dt, Lk, _ptr(self.state),
-                                                self.state.numel(), _ptr(self._pos), int(self.slots), _ptr(sl),
-                                                _ptr(ln), n, self.batch, H, T, int(fresh), _ptr(ext[0]), _ptr(ext[1]),
-                                                _ptr(ext[2]), _stream()))
-            _lib.check(l.bffc_fir_fwd(_ptr(ext[0]), H * Lr, _ptr(ext[1]), H * Lr, _ptr(ext[2]), H * Lr,
-                                      _ptr(self.fir_k), G, Lk, n, H, Lr, dt, _ptr(ext[3]), H * Lr, _stream()))
-            _lib.check(l.bffc_fir_decode_finish(_ptr(ext[3]), dt, Lk, _ptr(self._pos), int(self.slots), _ptr(sl),
-                                                _ptr(ln), n, self.batch, H, T, int(fresh), _ptr(y), H * T, _stream()))
-        return y
-
-    def _fir_prefill(self, u, pregate, postgate, L, slots=None, lengths=None):
-        """a prefill: an extend from the zero state (the state of the rows is overwritten, not read)"""
-        if slots is None:
-            if L == 0:
-                self.reset()
-                return torch.empty((self.batch, self.H, 0), dtype=self.dtype, device=self.device)
-            y = self._fir_run(u, pregate, postgate, L, self.batch, None, None, True, False)
-            self._host_pos = L
-            return y
-        n = len(slots)
-        if L == 0:                         # an empty prompt: the admitted slots restart at position 0
-            idx = _device_ints(slots, torch.int64, self.device)
-            tail, ring = self._fir_views()
-            tail.index_fill_(1, idx, 0)
-            ring.index_fill_(0, idx, 0)
-            self._pos[0].index_fill_(0, idx, 0)
-            self._pos[1].index_fill_(0, idx, 0)
-            y = torch.empty((n, self.H, 0), dtype=self.dtype, device=self.device)
-        else:
-            y = self._fir_run(u, pregate, postgate, L, n, slots, lengths, True, False)
-        if self._host_pos is not None:
-            for b, l in zip(slots, lengths):
-                self._host_pos[b] = l
-        return y
-
-    def _fir_step(self, u, pregate, postgate, T):
-        capturing = torch.cuda.is_current_stream_capturing()
-        roles = self._roles(u, pregate, postgate, T)
-        rows, wdt = self._tap_args()
-        args = [a for t, s in roles for a in (_ptr(t), s)]
-        y = torch.empty((self.batch, self.H, T), dtype=self.dtype, device=self.device)
-        G, Lk = self.fir_k.shape
-        with _on_device(self.device):
-            _lib.check(_lib.lib().bffc_fir_decode_step(*args, *rows, wdt, self.K, self.K - 1, _DT[self.dtype],
-                                                       _ptr(self.fir_k), G, Lk, _ptr(self.state), self.state.numel(),
-                                                       _ptr(self._pos), int(self.slots), _ptr(y), self.H * T,
-                                                       self.batch, self.H, T, _stream()))
-        self._advance_host(T, capturing)
-        return y
-
-    def _prompt_filters(self, L):
-        """k (and k2) of a prompt of L positions: the first min(Lk, L) taps, or the modal filter's first L"""
-        if self.modal:
-            return log_vandermonde(self.v, self.x, L), None
-        k = self.k[:, :min(self.k.shape[1], L)]
-        return k, None if self.k2 is None else self.k2[:, :min(self.k2.shape[1], L)]
-
-    def _modal_chunk(self, u, pregate, postgate, T, n, meta, fresh, post):
-        """bffc_modal_chunk: z (n, H, T) of the rows, s_postgate into post (or None), the tails rewritten"""
-        roles = self._roles(u, pregate, postgate, T, n) if T else [(None, 0)] * 3
-        rows, wdt = self._tap_args() if T else ([None] * 6, _lib.BFFC_DTYPE_FP32)
-        args = [a for t, s in roles for a in (_ptr(t), s)]
-        z = torch.empty((n, self.H, T), dtype=self.dtype, device=self.device)
-        with _on_device(self.device):
-            _lib.check(_lib.lib().bffc_modal_chunk(*args, *rows, wdt, self.K, self.K - 1, _DT[self.dtype],
-                                                   _ptr(self._modal_tail), _ptr(self._pos), int(self.slots),
-                                                   _ptr(None if meta is None else meta[:n]),
-                                                   _ptr(None if meta is None else meta[n:]), n, self.batch, self.H, T,
-                                                   int(fresh), _ptr(z), _ptr(post), _stream()))
-        return z
-
-    def _modal_fill(self, u, pregate, postgate, L, slots=None, lengths=None):
-        """a prefill's state: the tails, the positions, and h from one reversed transpose of the prompt's z"""
-        n = self.batch if slots is None else len(slots)
-        meta = None if slots is None else _device_ints(slots + lengths, torch.int32, self.device)
-        z = self._modal_chunk(u, pregate, postgate, L, n, meta, True, None)
-        _modal_transpose(z, L, self._ones, self.x, self.modal_state, lengths=None if meta is None else meta[n:],
-                         slots=None if meta is None else meta[:n], reversed=True)
-        if slots is None:
-            self._host_pos = L
-        elif self._host_pos is not None:
-            for b, l in zip(slots, lengths):
-                self._host_pos[b] = l
-
-    def _modal_step(self, u, pregate, postgate, T):
-        capturing = torch.cuda.is_current_stream_capturing()
-        roles = self._roles(u, pregate, postgate, T)
-        rows, wdt = self._tap_args()
-        args = [a for t, s in roles for a in (_ptr(t), s)]
-        y = torch.empty((self.batch, self.H, T), dtype=self.dtype, device=self.device)
-        G, N = self.v.shape
-        with _on_device(self.device):
-            _lib.check(_lib.lib().bffc_modal_step(*args, *rows, wdt, self.K, self.K - 1, _DT[self.dtype],
-                                                  _ptr(self._modal_tail), _ptr(self.modal_state), _ptr(self.v),
-                                                  _ptr(self.x), G, N, _ptr(self._pos), int(self.slots), _ptr(y),
-                                                  self.H * T, self.batch, self.H, T, _stream()))
-        self._advance_host(T, capturing)
-        return y
-
-    def _modal_extend(self, u, pregate, postgate, T, n, idx, lens, capturing):
-        """chunk -> the engine's convolution of z with k[:T] -> finish (y, positions) -> transpose (the state)"""
-        meta = None
-        if self.slots:
-            host = torch.tensor(idx + lens, dtype=torch.int32).pin_memory()
-            if capturing:                  # every replay copies from this buffer
-                self._ext_held.append(host)
-            meta = host.to(self.device, non_blocking=True)
-        ent = self._modal_ext.get(T)
-        if ent is None:
-            if capturing:
-                raise RuntimeError(f'run one eager extend with T = {T} before capturing it (it makes the FFT plan and '
-                                   'the filter spectrum)')
-            ent = self._modal_ext[T] = [FlashFFTConv(prefill_seqlen(T, T), dtype=self.dtype).eval(),
-                                        log_vandermonde(self.v, self.x, T), None]
-        post = None if postgate is None else torch.empty((n, self.H, T), dtype=torch.float32, device=self.device)
-        z = self._modal_chunk(u, pregate, postgate, T, n, meta, False, post)
-        conv, kT, kf = ent
-        yconv, kf = _fwd(conv, z, kT, None, None, kf_engine=kf if capturing else None)
-        if not capturing:
-            ent[2] = kf
-        y = torch.empty((n, self.H, T), dtype=self.dtype, device=self.device)
-        G, N = self.v.shape
-        sl, ln = (None, None) if meta is None else (meta[:n], meta[n:])
-        with _on_device(self.device):
-            _lib.check(_lib.lib().bffc_modal_extend_finish(_ptr(yconv), _ptr(post), _ptr(self.modal_state),
-                                                           _ptr(self.v), _ptr(self.x), G, N, _DT[self.dtype],
-                                                           _ptr(self._pos), int(self.slots), _ptr(sl), _ptr(ln), n,
-                                                           self.batch, self.H, T, _ptr(y), self.H * T, _stream()))
-        _modal_transpose(z, T, self._ones, self.x, self.modal_state, init=self.modal_state, lengths=ln, slots=sl,
-                         reversed=True)
-        return y
-
-    # ---- views of the state (include/bffc.h: tail, z cache, s_u cache)
-    def _caches(self):
-        B, H, n, K = self.batch, self.H, self.max_len, self.K
-        zc, vc, _ = state_layout(B, H, n, K, self.k2 is not None)
-        as_dt = lambda off, count: self.state[off:off + 2 * count].view(self.dtype)
-        tail = as_dt(0, 3 * B * H * (K - 1)).view(3, B, H, K - 1)
-        z = as_dt(zc, B * H * n).view(B, H, n)
-        v = as_dt(vc, B * H * n).view(B, H, n) if self.k2 is not None else None
-        return tail, z, v
-
-    @property
-    def z_cache(self):
-        """(B, H, max_len) cache of z = s_u * s_pregate; slots [0, pos) are valid."""
-        return self._caches()[1]
-
-    @property
-    def v_cache(self):
-        """(B, H, max_len) cache of s_u (kept when there is a residual filter), else None."""
-        return self._caches()[2]
-
-    @property
-    def tail(self):
-        """(3, B, H, K - 1) raw inputs of the last K - 1 positions of u, pregate and postgate."""
-        if self.fir:
-            return self._fir_views()[0]
-        return self._modal_tail if self.modal else self._caches()[0]
-
-    @property
-    def pos(self):
-        """Number of positions decoded so far, read from the device (a synchronisation).  Raises when a step ran past
-        max_len (it then wrote nothing)."""
-        if self.slots:
-            raise RuntimeError('a slot decoder keeps one position per slot: read `positions`')
-        pos, status = self._pos.tolist()
-        if status == 2:
-            raise RuntimeError(f'a decoding step would have run past the far field ({FAR_BLOCK} positions after the last '
-                               f'refresh) and did nothing; the position is still {pos}.  Replay refresh() at least every '
-                               f'{FAR_BLOCK} // T steps')
-        if status:
-            raise RuntimeError(f'a decoding step would have run past max_len = {self.max_len} and did nothing; '
-                               f'the position is still {pos}')
-        self._host_pos = pos
-        return pos
-
-    @property
-    def positions(self):
-        """Per-slot positions read from the device (a synchronisation), -1 for an idle slot.  Raises naming every slot
-        whose status is set (a step would have taken it past max_len; it kept its state and position).  Admitting the
-        slot again clears its status."""
-        if not self.slots:
-            raise RuntimeError('positions is for a decoder made with slots=True; read `pos`')
-        pos, status = self._pos.tolist()
-        far = [b for b, s in enumerate(status) if s == 2]
-        if far:
-            raise RuntimeError(f'slots {far} would have run past their far field ({FAR_BLOCK} positions after their '
-                               f'last refresh) and kept their state; their positions are {[pos[b] for b in far]}.  '
-                               f'Replay refresh() at least every {FAR_BLOCK} // T steps and after every admission')
-        bad = [b for b, s in enumerate(status) if s]
-        if bad:
-            raise RuntimeError(f'slots {bad} would have run past max_len = {self.max_len} and kept their state; their '
-                               f'positions are {[pos[b] for b in bad]}')
-        self._host_pos = list(pos)
-        return pos
-
-    def release(self, slots):
-        """Idle the given slots on the device, with no synchronisation (the slot indices go to the device from pinned
-        memory, ordered on the current stream): their state is kept but no longer read, their rows of y are zero, and
-        a later prefill may admit a new prompt into them."""
-        self._need_slots('release')
-        if slots is None:
-            raise ValueError('release takes the slots to idle (reset() idles every slot)')
-        idx = self._slot_list(slots, None)
-        if not idx:
-            return
-        i = _device_ints(idx, torch.int64, self.device)
-        self._pos[0].index_fill_(0, i, -1)
-        self._pos[1].index_fill_(0, i, 0)
-        if self._host_pos is not None:
-            for b in idx:
-                self._host_pos[b] = -1
-
-    def _need_slots(self, what):
-        if not self.slots:
-            raise RuntimeError(f'{what} is for a decoder made with slots=True')
-
-    def _slot_list(self, slots, n):
-        """slots as a validated list: distinct, in [0, batch), n of them (n = batch and every slot for None)"""
-        idx = list(range(self.batch)) if slots is None else _host_ints(slots, 'slots')
-        if n is not None and len(idx) != n:
-            raise ValueError(f'{len(idx)} slots for {n} prompts' if slots is not None else
-                             f'slots=None admits every one of the {self.batch} slots, got {n} prompts')
-        bad = [b for b in idx if not 0 <= b < self.batch]
-        if bad:
-            raise ValueError(f'slots {bad} outside [0, {self.batch})')
-        if len(set(idx)) != len(idx):
-            raise ValueError(f'slots {idx} are not distinct')
-        return idx
-
-    def _admission(self, n, L, lengths, slots):
-        """(slots, lengths) of a slot prefill of n right-padded prompts of L positions, validated on the host"""
-        if self.max_len is not None and L > self.max_len:
-            raise ValueError(f'prompt of {L} positions exceeds max_len = {self.max_len}')
-        if lengths is None:
-            raise ValueError('a slot decoder\'s prefill takes lengths=[...] (one per prompt row)')
-        if not 1 <= n <= self.batch:
-            raise ValueError(f'{n} prompts for {self.batch} slots')
-        lens = _host_ints(lengths, 'lengths')
-        if len(lens) != n:
-            raise ValueError(f'{len(lens)} lengths for {n} prompts')
-        bad = [l for l in lens if not 0 <= l <= L]
-        if bad:
-            raise ValueError(f'lengths {bad} outside [0, L = {L}]')
-        return self._slot_list(slots, n), lens
-
-    @staticmethod
-    def _mask(t, lens):
-        """t (n, C, L) zero at positions t >= lens[i] of row i (NaN and large values in the padding included)"""
-        if t is None:
-            return None
-        keep = torch.arange(t.shape[-1], device=t.device)[None] < _device_ints(lens, torch.int64, t.device)[:, None]
-        return torch.where(keep[:, None, :], t, torch.zeros((), dtype=t.dtype, device=t.device))
+        return self._state.fir_ring
 
     def reset(self):
         """Start over with an empty prompt (with slots: every slot idle)."""
-        if self.slots:
-            self._pos[0].fill_(-1)
-            self._pos[1].zero_()
-            self._host_pos = [-1] * self.batch
-            if self.far_field:
-                self._far_pos.fill_(-1)
-                self._host_r = [-1] * self.batch
-            return
-        self._fill(None, None, None, 0)
-        if self.far_field:                 # no past: the refresh point is 0 and the far field zero, without an FFT
-            self._far_pos.zero_()
-            for o in self._far_out:
-                o[..., self.far_window:].zero_()
-            self._host_r = 0
-
-    # ---- far field (decode_far.cuh)
-    def _far_init(self):
-        """the persistent far inputs and outputs (one pair per filter, (B, H, W + FAR_BLOCK)), the refresh points and
-        one FlashFFTConv(n) per filter, whose eval-mode cache holds the filter's spectrum"""
-        shape = (self.batch, self.H, self.far_window + FAR_BLOCK)
-        nf = 1 if self.k2 is None else 2
-        self._far_in = [torch.empty(shape, dtype=self.dtype, device=self.device) for _ in range(nf)]
-        self._far_out = [torch.zeros(shape, dtype=self.dtype, device=self.device) for _ in range(nf)]
-        self._far_pos = torch.zeros(self.batch if self.slots else 1, dtype=torch.int64, device=self.device)
-        self._far_convs = [FlashFFTConv(self.far_fft_size, dtype=self.dtype).eval() for _ in range(nf)]
-        # spectra of k (and k2) of the latest eager transform: a captured refresh reads them, so that it does not wait
-        # on the eager-mode cache's event from outside the capture
-        self._far_kf = [None] * nf
-        self._host_r = None                # known refresh points (a list per slot with slots), or None
-
-    def _far_gather(self, slots, n, ins):
-        """bffc_conv_far_gather[_slots]: rows of the engine inputs from the caches, refresh points from the positions"""
-        l, B, H = _lib.lib(), self.batch, self.H
-        Lk2 = 0 if self.k2 is None else self.k2.shape[1]
-        common = (B, H, self.max_len, self.K, int(self.k2 is not None), self.k.shape[1], Lk2, _DT[self.dtype],
-                  _ptr(ins[0]), _ptr(ins[1] if len(ins) > 1 else None), _stream())
-        with _on_device(self.device):
-            if self.slots:
-                rc = l.bffc_conv_far_gather_slots(_ptr(self.state), self.state.numel(), _ptr(self._pos),
-                                                  _ptr(self._far_pos), _ptr(slots), n, *common)
-            else:
-                rc = l.bffc_conv_far_gather(_ptr(self.state), self.state.numel(), _ptr(self._pos),
-                                            _ptr(self._far_pos), *common)
-            _lib.check(rc)
-
-    def _far_transform(self, ins, outs):
-        capturing = torch.cuda.is_current_stream_capturing()
-        for i, (conv, k, x, y) in enumerate(zip(self._far_convs, (self.k, self.k2), ins, outs)):
-            _, kf = _fwd(conv, x, k, None, None, kf_engine=self._far_kf[i] if capturing else None, out=y)
-            if not capturing:
-                self._far_kf[i] = kf
+        self._state.reset()
 
     @torch.no_grad()
     def refresh(self):
@@ -631,311 +185,50 @@ class _Decoder:
         eager refresh has made the FFT plan and the filter spectra.  Idle slots are gathered as zero rows."""
         if not self.far_field:
             raise RuntimeError('refresh is for a decoder made with far_field=True')
-        capturing = torch.cuda.is_current_stream_capturing()
-        if capturing and self._far_kf[0] is None:
-            raise RuntimeError('the far field\'s FFT plan and filter spectra are made on first use, which cannot happen '
-                               'during CUDA-graph capture: run one eager refresh() (or prefill) before capturing one')
-        self._far_gather(None, self.batch, self._far_in)
-        self._far_transform(self._far_in, self._far_out)
-        if capturing or self._host_pos is None:
-            self._host_r = None
-        elif self.slots:
-            self._host_r = list(self._host_pos)
-        else:
-            self._host_r = self._host_pos
+        self._state.refresh()
 
-    def _far_admit(self, slots, lengths):
-        """refresh the admitted slots only: their rows gathered, transformed and copied into their slots' rows"""
-        idx = _device_ints(slots, torch.int64, self.device)
-        if not any(lengths):               # no past: refresh point 0 and a zero far field, without an FFT
-            self._far_pos.index_fill_(0, idx, 0)
-            for o in self._far_out:
-                o.index_fill_(0, idx, 0)
-        else:
-            n = len(slots)
-            ins = [x[:n] for x in self._far_in]            # scratch: a refresh gathers every row again
-            self._far_gather(_device_ints(slots, torch.int32, self.device), n, ins)
-            outs = [torch.empty_like(x) for x in ins]
-            self._far_transform(ins, outs)
-            for o, t in zip(self._far_out, outs):
-                o.index_copy_(0, idx, t)
-        if self._host_r is not None:
-            for b, l in zip(slots, lengths):
-                self._host_r[b] = l
-
-    def _far_sync(self):
-        """the host mirrors of the positions and refresh points, read back once when a capture made them unknown"""
-        if self._host_pos is None or self._host_r is None:
-            pos, r = self._pos.tolist(), self._far_pos.tolist()
-            self._host_pos, self._host_r = (list(pos[0]), list(r)) if self.slots else (pos[0], r[0])
-
-    def _far_before_step(self, T):
-        """an eager step's refresh: when some active member would pass its far field"""
-        pairs = zip(self._host_pos, self._host_r) if self.slots else [(self._host_pos, self._host_r)]
-        if any(p >= 0 and not 0 <= r <= p <= r + FAR_BLOCK - T for p, r in pairs):
-            self.refresh()
-
-    def _conv(self, L):
-        n = prefill_seqlen(L, L if self.modal else max(self.k.shape[1], 0 if self.k2 is None else self.k2.shape[1]))
-        conv = self._convs.get(n)
-        if conv is None:
-            conv = self._convs[n] = FlashFFTConv(n, dtype=self.dtype).eval()
-        return conv
-
-    def _check(self, t, name, T, n=None):
-        n = self.batch if n is None else n
-        if t.dim() != 3 or t.shape[0] != n or t.shape[1] != self.H or t.shape[2] != T:
-            raise ValueError(f'{name} must be ({n}, {self.H}, {T}), got {tuple(t.shape)}')
-        if t.dtype != self.dtype or t.device != self.device:
-            raise ValueError(f'{name} must be {self.dtype} on {self.device}, got {t.dtype} on {t.device}')
-
-    def _roles(self, u, pregate, postgate, T, n=None):
-        out = []
-        for name, t in (('u', u), ('pregate', pregate), ('postgate', postgate)):
-            if t is None:
-                out.append((None, 0))
-            else:
-                self._check(t, name, T, n)
-                out.append(_rows(t, self.H, T))
-        return out
-
-    def _tap_args(self):
-        """(rows of the u, pregate, postgate taps and biases, w_dtype) of the short filter; none here"""
-        return [None] * 6, _lib.BFFC_DTYPE_FP32
-
+    # ---- the state's internals that tests and tools read, under the decoder's names
     def _fill(self, u, pregate, postgate, L):
-        if self.fir:                       # only reset() comes here: the zero state at position 0
-            self.state.zero_()
-            self._pos.zero_()
-            self._host_pos = 0
-            return
-        if self.modal:
-            return self._modal_fill(u, pregate, postgate, L)
-        roles = self._roles(u, pregate, postgate, L) if L else [(None, 0)] * 3
-        rows, wdt = self._tap_args() if L else ([None] * 6, _lib.BFFC_DTYPE_FP32)
-        args = [a for t, s in roles for a in (_ptr(t), s)]
-        with _on_device(self.device):
-            _lib.check(_lib.lib().bffc_conv_state_fill(*args, *rows, wdt, self.K, self.K - 1, _DT[self.dtype],
-                                                       self.batch, self.H, L, self.max_len, int(self.k2 is not None),
-                                                       _ptr(self.state), self.state.numel(), _ptr(self._pos),
-                                                       _stream()))
-        self._host_pos = L
+        return self._state.fill(u, pregate, postgate, L)
 
     def _fill_slots(self, u, pregate, postgate, L, slots, lengths):
-        """one bffc_conv_state_fill_slots call: prompt row i (already zero past lengths[i]) into slot slots[i]"""
-        if self.modal:
-            return self._modal_fill(u, pregate, postgate, L, slots, lengths)
-        n = len(slots)
-        roles = self._roles(u, pregate, postgate, L, n) if L else [(None, 0)] * 3
-        rows, wdt = self._tap_args() if L else ([None] * 6, _lib.BFFC_DTYPE_FP32)
-        args = [a for t, s in roles for a in (_ptr(t), s)]
-        meta = _device_ints(slots + lengths, torch.int32, self.device)
-        with _on_device(self.device):
-            _lib.check(_lib.lib().bffc_conv_state_fill_slots(*args, *rows, wdt, self.K, self.K - 1, _DT[self.dtype],
-                                                             self.batch, self.H, n, L, _ptr(meta),
-                                                             _ptr(meta[n:]), self.max_len, int(self.k2 is not None),
-                                                             _ptr(self.state), self.state.numel(), _ptr(self._pos),
-                                                             _stream()))
-        if self._host_pos is not None:
-            for b, l in zip(slots, lengths):
-                self._host_pos[b] = l
-        if self.far_field:
-            self._far_admit(slots, lengths)
+        return self._state.fill(u, pregate, postgate, L, slots, lengths)
+
+    def _fir_views(self):
+        return self._state.tail, self._state.fir_ring
+
+    _ws = property(lambda self: self._state._ws)
+    _far_out = property(lambda self: self._state.far_out)
+    _far_pos = property(lambda self: self._state.far_book._row)
+
+    @property
+    def _host_r(self):
+        return self._state.far_book._host_pos
+
+    @_host_r.setter
+    def _host_r(self, r):
+        self._state.far_book._host_pos = r
+
+    def _prefill(self, inputs, L, slots, lengths):
+        """y of a prompt (inputs: what the subclass's _split makes the roles) and the state filled from it"""
+        if slots is None and L == 0:
+            self.reset()
+            u = self._split(*inputs)[0]
+            return u.new_empty((u.shape[0], self.H, 0))
+        return self._state.prefill(self, inputs, L, slots, lengths)
 
     def _step(self, u, pregate, postgate):
         T = u.shape[-1]
         if not 1 <= T <= MAX_STEP_TOKENS:
             raise ValueError(f'a step takes 1 to {MAX_STEP_TOKENS} tokens, got {T} (a longer chunk is a prefill)')
-        if self.modal:
-            return self._modal_step(u, pregate, postgate, T)
-        if self.fir:
-            return self._fir_step(u, pregate, postgate, T)
-        capturing = torch.cuda.is_current_stream_capturing()
-        if self.far_field and not capturing:
-            self._far_sync()                   # the checks below and the refresh need the host mirrors
-        if self._host_pos is not None and not capturing:
-            if self.slots:
-                over = [b for b, p in enumerate(self._host_pos) if p >= 0 and p + T > self.max_len]
-                if over:
-                    raise ValueError(f'slots {over} at positions {[self._host_pos[b] for b in over]} + {T} tokens '
-                                     f'exceed max_len = {self.max_len}')
-            elif self._host_pos + T > self.max_len:
-                raise ValueError(f'position {self._host_pos} + {T} tokens exceeds max_len = {self.max_len}')
-        roles = self._roles(u, pregate, postgate, T)
-        rows, wdt = self._tap_args()
-        Lk = self.k.shape[1]
-        Lk2 = 0 if self.k2 is None else self.k2.shape[1]
-        if self.far_field:
-            return self._step_far(roles, rows, wdt, T, Lk, Lk2, capturing)
-        nws = (_lib.lib().bffc_conv_step_slots_workspace_bytes if self.slots else
-               _lib.lib().bffc_conv_step_workspace_bytes)(self.batch, self.H, T, Lk, Lk2)
-        if self._ws is None or self._ws.numel() < nws:
-            if capturing:
-                raise RuntimeError(f'run one eager step with T = {T} before capturing it (it sizes the workspace)')
-            if self._ws is not None:
-                self._ws_outgrown.append(self._ws)
-            self._ws = torch.empty(nws, dtype=torch.uint8, device=self.device)
-        y = torch.empty((self.batch, self.H, T), dtype=self.dtype, device=self.device)
-        args = [a for t, s in roles for a in (_ptr(t), s)]
-        fn = _lib.lib().bffc_conv_step_slots if self.slots else _lib.lib().bffc_conv_step
-        with _on_device(self.device):
-            _lib.check(fn(*args, _ptr(self.k), Lk, _ptr(self.k2), Lk2, *rows, wdt, self.K, self.K - 1,
-                          _DT[self.dtype], _ptr(self.state), self.state.numel(), _ptr(self._pos), _ptr(y),
-                          self.H * T, self.batch, self.H, T, self.max_len, _ptr(self._ws), self._ws.numel(),
-                          _stream()))
-        self._advance_host(T, capturing)
-        return y
+        return self._state.step(u, pregate, postgate, T)
 
-    def _advance_host(self, T, capturing):
-        if capturing or self._host_pos is None:
-            self._host_pos = None
-        elif self.slots:
-            self._host_pos = [p + T if p >= 0 else p for p in self._host_pos]
-        else:
-            self._host_pos += T
-
-    def _step_far(self, roles, rows, wdt, T, Lk, Lk2, capturing):
-        if not capturing:
-            self._far_before_step(T)
-        y = torch.empty((self.batch, self.H, T), dtype=self.dtype, device=self.device)
-        args = [a for t, s in roles for a in (_ptr(t), s)]
-        fo = self._far_out
-        fn = _lib.lib().bffc_conv_step_far_slots if self.slots else _lib.lib().bffc_conv_step_far
-        with _on_device(self.device):
-            _lib.check(fn(*args, _ptr(self.k), Lk, _ptr(self.k2), Lk2, *rows, wdt, self.K, self.K - 1,
-                          _DT[self.dtype], _ptr(self.state), self.state.numel(), _ptr(self._pos), _ptr(self._far_pos),
-                          _ptr(fo[0]), _ptr(fo[1] if len(fo) > 1 else None), _ptr(y), self.H * T, self.batch, self.H,
-                          T, self.max_len, _stream()))
-        self._advance_host(T, capturing)
-        return y
-
-    # ---- extend (decode_extend.cuh)
     def _extend(self, u, pregate, postgate, lengths, slots):
-        """bffc_conv_extend_gather[_slots], the engine forward of k (and k2) on the rows it wrote, and
-        bffc_conv_extend_finish[_slots]: y of the chunk, the caches appended, the positions advanced (far field: every
-        extended member refreshed at its new position)"""
         T = u.shape[-1]
         if T < 1:
             raise ValueError('extend takes at least one token')
-        capturing = torch.cuda.is_current_stream_capturing()
-        if self.slots:
-            n = u.shape[0]
-            if not 1 <= n <= self.batch:
-                raise ValueError(f'{n} rows for {self.batch} slots')
-            idx = self._slot_list(slots, n)
-            lens = [T] * n if lengths is None else _host_ints(lengths, 'lengths')
-            if len(lens) != n:
-                raise ValueError(f'{len(lens)} lengths for {n} rows')
-            bad = [l for l in lens if not 0 <= l <= T]
-            if bad:
-                raise ValueError(f'lengths {bad} outside [0, T = {T}]')
-        else:
-            if lengths is not None or slots is not None:
-                raise ValueError('lengths and slots are for a decoder made with slots=True')
-            n, idx, lens = self.batch, list(range(self.batch)), [T] * self.batch
-        if self.modal:
-            if self._host_pos is not None and not capturing and self.slots:
-                idle = [b for b in idx if self._host_pos[b] < 0]
-                if idle:
-                    raise ValueError(f'slots {idle} are idle: admit a prompt into them with prefill first')
-            y = self._modal_extend(u, pregate, postgate, T, n, idx, lens, capturing)
-            self._advance_extend(idx, lens, T, capturing)
-            return y
-        if self.fir:
-            if self._host_pos is not None and not capturing and self.slots:
-                idle = [b for b in idx if self._host_pos[b] < 0]
-                if idle:
-                    raise ValueError(f'slots {idle} are idle: admit a prompt into them with prefill first')
-            y = self._fir_run(u, pregate, postgate, T, n, idx if self.slots else None, lens if self.slots else None,
-                              False, capturing)
-            self._advance_extend(idx, lens, T, capturing)
-            return y
-        roles = self._roles(u, pregate, postgate, T, n)
-        Lk = self.k.shape[1]
-        Lk2 = 0 if self.k2 is None else self.k2.shape[1]
-        W, nfft, WP = extend_layout(self.batch, self.H, Lk, Lk2, T, self.far_field, self.dtype)
-        if capturing and nfft not in self._ext_kf:
-            raise RuntimeError(f'run one eager extend with T = {T} before capturing it (it makes the FFT plan and the '
-                               'filter spectra)')
-        if self.far_field and not capturing:
-            self._far_sync()
-        if self._host_pos is not None and not capturing:
-            if self.slots:
-                idle = [b for b in idx if self._host_pos[b] < 0]
-                if idle:
-                    raise ValueError(f'slots {idle} are idle: admit a prompt into them with prefill first')
-                over = [b for b, l in zip(idx, lens) if self._host_pos[b] + l > self.max_len]
-                if over:
-                    raise ValueError(f'slots {over} at positions {[self._host_pos[b] for b in over]} + '
-                                     f'{[lens[idx.index(b)] for b in over]} tokens exceed max_len = {self.max_len}')
-            elif self._host_pos + T > self.max_len:
-                raise ValueError(f'position {self._host_pos} + {T} tokens exceeds max_len = {self.max_len}')
-        rows, wdt = self._tap_args()
-        l, dt, dev = _lib.lib(), _DT[self.dtype], self.device
-        nf = 1 if self.k2 is None else 2
-        ins = [torch.empty((n, self.H, WP), dtype=self.dtype, device=dev) for _ in range(nf)]
-        ws = torch.empty(l.bffc_conv_extend_workspace_bytes(n, self.H, T), dtype=torch.uint8, device=dev)
-        args = [a for t, s in roles for a in (_ptr(t), s)]
-        common = (self.batch, self.H, T, self.max_len, int(self.k2 is not None), Lk, Lk2, int(self.far_field),
-                  _ptr(ins[0]), _ptr(ins[1] if nf > 1 else None), _ptr(ws), ws.numel(), _stream())
-        with _on_device(dev):
-            if self.slots:
-                host = torch.tensor(idx + lens, dtype=torch.int32).pin_memory()
-                if capturing:              # every replay copies from this buffer
-                    self._ext_held.append(host)
-                meta = host.to(dev, non_blocking=True)
-                rc = l.bffc_conv_extend_gather_slots(*args, *rows, wdt, self.K, self.K - 1, dt, _ptr(self.state),
-                                                     self.state.numel(), _ptr(self._pos), _ptr(meta), _ptr(meta[n:]),
-                                                     n, *common)
-            else:
-                rc = l.bffc_conv_extend_gather(*args, *rows, wdt, self.K, self.K - 1, dt, _ptr(self.state),
-                                               self.state.numel(), _ptr(self._pos), *common)
-            _lib.check(rc)
-        convs = self._ext_convs.get(nfft)
-        if convs is None:
-            convs = self._ext_convs[nfft] = [FlashFFTConv(nfft, dtype=self.dtype).eval() for _ in range(nf)]
-        kfs = self._ext_kf.get(nfft, [None] * nf)
-        outs = []
-        for i, (conv, k, x) in enumerate(zip(convs, (self.k, self.k2), ins)):
-            out, kf = _fwd(conv, x, k, None, None, kf_engine=kfs[i] if capturing else None)
-            outs.append(out)
-            kfs[i] = kf
-        if not capturing:
-            self._ext_kf[nfft] = kfs
-        y = torch.empty((n, self.H, T), dtype=self.dtype, device=dev)
-        fo = self._far_out if self.far_field else [None, None]
-        far = (_ptr(self._far_pos), _ptr(fo[0]), _ptr(fo[1] if len(fo) > 1 else None)) if self.far_field else \
-            (None, None, None)
-        tail = (self.H, T, Lk, Lk2, int(self.far_field), _ptr(ws), ws.numel(), _stream())
-        with _on_device(dev):
-            head = (_ptr(outs[0]), _ptr(outs[1] if nf > 1 else None), int(roles[2][0] is not None), dt, _ptr(self._pos),
-                    *far, _ptr(y), self.H * T)
-            if self.slots:
-                rc = l.bffc_conv_extend_finish_slots(*head, n, self.batch, *tail)
-            else:
-                rc = l.bffc_conv_extend_finish(*head, self.batch, *tail)
-            _lib.check(rc)
-        self._advance_extend(idx, lens, T, capturing)
-        if capturing or self._host_pos is None:
-            if self.far_field:
-                self._host_r = None
-        else:
-            if self.far_field and self._host_r is not None:
-                if self.slots:
-                    for b in idx:
-                        self._host_r[b] = self._host_pos[b]
-                else:
-                    self._host_r = self._host_pos
-        return y
-
-    def _advance_extend(self, idx, lens, T, capturing):
-        if capturing or self._host_pos is None:
-            self._host_pos = None
-        elif self.slots:
-            for b, ln in zip(idx, lens):
-                self._host_pos[b] += ln
-        else:
-            self._host_pos += T
+        slots, lens = self._admission(u.shape[0], T, lengths, slots, extend=True)
+        return self._state.extend(u, pregate, postgate, T, self.batch if slots is None else len(slots), slots, lens)
 
 
 class HyenaDecoder(_Decoder):
@@ -972,28 +265,26 @@ class HyenaDecoder(_Decoder):
             raise ValueError(f'short filter padding {P}: decoding needs the causal padding K - 1 = {K - 1} (padding '
                              f'{P} makes each output read {K - 1 - P} input(s) after its position)')
         self.short_filter, self.d_model = short_filter, d_model
-        super().__init__(k, residual_filter, d_model, batch, max_len, dtype, K, slots, far_field)
-        self._tap_args()
-
-    def _tap_args(self):
-        """the taps of the short filter's parameters as they are now (a .to(), .half() or load_state_dict(assign=True)
-        replaces their storage)"""
-        w, b, D, K = self.short_filter.weights, self.short_filter.bias, self.d_model, self.K
-        if w.dtype != b.dtype or w.dtype not in _dw._DT or not (w.is_contiguous() and b.is_contiguous()):
-            raise ValueError('short filter weights and bias must be contiguous and of one dtype')
-        if w.device != self.device or b.device != self.device:
-            raise ValueError(f'short filter on {w.device}, k on {self.device}')
-        es = w.element_size()
-        # rows of x1, x2, v in the (3D, K) weight and (3D) bias; roles u = v, pregate = x1, postgate = x2
-        w1, w2, wv = (w.data_ptr() + i * D * K * es for i in range(3))
-        b1, b2, bv = (b.data_ptr() + i * D * es for i in range(3))
-        return [ctypes.c_void_p(a) for a in (wv, bv, w1, b1, w2, b2)], _dw._DT[w.dtype]
+        super().__init__(k, residual_filter, d_model, batch, max_len, dtype, K, slots, far_field,
+                         functools.partial(_short_filter_taps, short_filter, d_model, K))
+        _short_filter_taps(short_filter, d_model, K, self.device)
 
     def _split(self, x):
         if x.dim() != 3 or x.shape[1] != 3 * self.d_model:
             raise ValueError(f'x must be (B, 3 * d_model = {3 * self.d_model}, T), got {tuple(x.shape)}')
         x1, x2, v = x.split(self.d_model, dim=1)
         return v, x1, x2
+
+    def _operator(self, conv, inputs, k, k2, lengths):
+        """y of a prompt x on the FFT engine: hyena_operator; with slots (x zero past each length) the short filter and
+        hyena_mixer"""
+        x, = inputs
+        if lengths is None:
+            return hyena_operator(conv, self.short_filter, x, k, self.d_model, residual_filter=k2)
+        # the short filter's bias makes s non-zero past a prompt's end; zeroed there, the transform's rounding scales
+        # with each prompt alone rather than with its padded row
+        s = _mask(self.short_filter(x)[..., :x.shape[-1]], lengths)
+        return hyena_mixer(conv, s, k, self.d_model, residual_filter=k2)
 
     @torch.no_grad()
     def prefill(self, x, docs=None, *, lengths=None, slots=None):
@@ -1004,48 +295,16 @@ class HyenaDecoder(_Decoder):
         slots[i] (slots=None: n = batch, every slot restarts); other slots are untouched.  Returns (n, d_model, L), zero
         at t >= lengths[i]."""
         refuse(docs, 'HyenaDecoder')
-        if self.slots:
-            return self._prefill_slots(x, lengths, slots)
-        if lengths is not None or slots is not None:
-            raise ValueError('lengths and slots are for a decoder made with slots=True')
-        L = x.shape[-1]
-        if self.max_len is not None and L > self.max_len:
-            raise ValueError(f'prompt of {L} positions exceeds max_len = {self.max_len}')
-        x = x.contiguous()                 # the short filter takes a contiguous projection
-        v, x1, x2 = self._split(x)
-        if self.fir:
-            return self._fir_prefill(v, x1, x2, L)
-        if L == 0:
-            self.reset()
-            return x.new_empty((x.shape[0], self.d_model, 0))
-        k, k2 = self._prompt_filters(L)
-        y = hyena_operator(self._conv(L), self.short_filter, x, k, self.d_model, residual_filter=k2)
-        self._fill(v, x1, x2, L)
-        if self.far_field:
-            self.refresh()
-        return y
-
-    def _prefill_slots(self, x, lengths, slots):
-        if x.dim() != 3:
+        if self.slots and x.dim() != 3:
             raise ValueError(f'x must be (n, 3 * d_model = {3 * self.d_model}, L), got {tuple(x.shape)}')
         n, L = x.shape[0], x.shape[-1]
         slots, lens = self._admission(n, L, lengths, slots)
-        for name, t in zip(('v', 'x1', 'x2'), self._split(x)):   # shape, dtype and device before any work
-            self._check(t, name, L, n)
-        if self.fir:                       # the gather reads no input past a row's length
-            return self._fir_prefill(*self._split(x), L, slots, lens)
-        x = self._mask(x, lens)            # contiguous, zero past each length
-        v, x1, x2 = self._split(x)
-        if L == 0:
-            y = x.new_empty((n, self.d_model, 0))
+        if slots is None:
+            x = x.contiguous()             # the short filter takes a contiguous projection
         else:
-            k, k2 = self._prompt_filters(L)
-            # the short filter's bias makes s non-zero past a prompt's end; zeroed there, the transform's rounding
-            # scales with each prompt alone rather than with its padded row
-            s = self._mask(self.short_filter(x)[..., :L], lens)
-            y = self._mask(hyena_mixer(self._conv(L), s, k, self.d_model, residual_filter=k2), lens)
-        self._fill_slots(v, x1, x2, L, slots, lens)
-        return y
+            v, x1, x2 = self._split(x)     # shape, dtype and device before any work
+            self._state.check(L, n, v=v, x1=x1, x2=x2)
+        return self._prefill((x,), L, slots, lens)
 
     @torch.no_grad()
     def step(self, x, docs=None):
@@ -1101,6 +360,17 @@ class LongConvDecoder(_Decoder):
         self._gates = None
         super().reset()
 
+    def _split(self, u, pregate, postgate):
+        return u, pregate, postgate
+
+    def _operator(self, conv, inputs, k, k2, lengths):
+        """y of a prompt on the FFT engine: the gated convolution"""
+        u, pregate, postgate = inputs
+        if pregate is None and postgate is None:
+            return conv(u.contiguous(), k)
+        ones = torch.ones_like(u)          # a missing gate is 1: the products with it are exact
+        return gated_long_conv(conv, u, k, ones if pregate is None else pregate, ones if postgate is None else postgate)
+
     @torch.no_grad()
     def prefill(self, u, pregate=None, postgate=None, docs=None, *, lengths=None, slots=None):
         """y (B, H, L) of the prompt by the FFT engine, and the cache filled from it; starts a new sequence.  Packed
@@ -1110,57 +380,15 @@ class LongConvDecoder(_Decoder):
         slot slots[i] (slots=None: n = batch, every slot restarts); other slots are untouched.  Returns (n, H, L), zero
         at t >= lengths[i]."""
         refuse(docs, 'LongConvDecoder')
-        if self.slots:
-            return self._prefill_slots(u, pregate, postgate, lengths, slots)
-        if lengths is not None or slots is not None:
-            raise ValueError('lengths and slots are for a decoder made with slots=True')
-        L = u.shape[-1]
-        if self.max_len is not None and L > self.max_len:
-            raise ValueError(f'prompt of {L} positions exceeds max_len = {self.max_len}')
-        self._roles(u, pregate, postgate, L)
-        if L == 0:
-            self.reset()
-            return torch.empty_like(u)
-        self._gates = None
-        self._same_gates(pregate, postgate)
-        if self.fir:
-            return self._fir_prefill(u, pregate, postgate, L)
-        conv = self._conv(L)
-        k = self._prompt_filters(L)[0]
-        if pregate is None and postgate is None:
-            y = conv(u.contiguous(), k)
-        else:                              # a missing gate is 1: the products with it are exact
-            ones = torch.ones_like(u)
-            y = gated_long_conv(conv, u, k, ones if pregate is None else pregate, ones if postgate is None else postgate)
-        self._fill(u, pregate, postgate, L)
-        if self.far_field:
-            self.refresh()
-        return y
-
-    def _prefill_slots(self, u, pregate, postgate, lengths, slots):
-        if u.dim() != 3:
+        if self.slots and u.dim() != 3:
             raise ValueError(f'u must be (n, {self.H}, L), got {tuple(u.shape)}')
         n, L = u.shape[0], u.shape[-1]
         slots, lens = self._admission(n, L, lengths, slots)
-        self._roles(u, pregate, postgate, L, n)
+        self._state.check(L, None if slots is None else n, u=u, pregate=pregate, postgate=postgate)
+        if slots is None:                  # a new sequence: the gates of its prompt (an empty one resets them)
+            self._gates = None
         self._same_gates(pregate, postgate)
-        if self.fir:                       # the gather reads no input past a row's length
-            return self._fir_prefill(u, pregate, postgate, L, slots, lens)
-        u, pregate, postgate = (self._mask(t, lens) for t in (u, pregate, postgate))
-        if L == 0:
-            y = torch.empty_like(u)
-        else:
-            conv = self._conv(L)
-            k = self._prompt_filters(L)[0]
-            if pregate is None and postgate is None:
-                y = conv(u, k)
-            else:
-                ones = torch.ones_like(u)
-                y = gated_long_conv(conv, u, k, ones if pregate is None else pregate,
-                                    ones if postgate is None else postgate)
-            y = self._mask(y, lens)
-        self._fill_slots(u, pregate, postgate, L, slots, lens)
-        return y
+        return self._prefill((u, pregate, postgate), L, slots, lens)
 
     @torch.no_grad()
     def step(self, u, pregate=None, postgate=None, docs=None):

@@ -222,6 +222,48 @@ def test_slot_release_validates_slots():
             d.release(bad)
 
 
+def test_position_book_mirror():
+    """the host mirror follows admissions, steps (active slots only) and ragged extends, refuses what would pass max_len
+    or extend an idle slot, and is forgotten under capture (the device then decides)"""
+    from flashfftconv.decode_state import PositionBook
+    b = PositionBook(3, True, 'cpu', 100)
+    b._put([0, 2], [10, 5])
+    assert b._host_pos == [10, -1, 5]
+    b._advance(4, False)
+    assert b._host_pos == [14, -1, 9]
+    b._advance(8, False, ([2, 0], [3, 8]))
+    assert b._host_pos == [22, -1, 12]
+    with pytest.raises(ValueError, match=r'slots \[1\] are idle'):
+        b._check_room(4, False, ([1], [4]))
+    with pytest.raises(ValueError, match=r'slots \[0\] at positions \[22\] \+ \[79\] tokens exceed'):
+        b._check_room(79, False, ([0, 2], [79, 1]))
+    with pytest.raises(ValueError, match=r'slots \[0\] at positions \[22\] \+ 79 tokens exceed'):
+        b._check_room(79, False)
+    b._check_room(78, False)
+    far = PositionBook(3, True, 'cpu')
+    far._follow(b, None, False)
+    assert far._host_pos == [22, -1, 12]
+    b._advance(1, False, ([2], [1]))
+    far._follow(b, [2], False)
+    assert far._host_pos == [22, -1, 13]
+    b._advance(1, True)
+    assert b._host_pos is None
+    b._check_room(1000, False)
+    far._follow(b, None, False)
+    assert far._host_pos is None
+    b._restart()
+    assert b._host_pos == [-1] * 3 and b._pos.tolist() == [[-1] * 3, [0] * 3]
+    s = PositionBook(1, False, 'cpu', 10)
+    s._put(None, 6)
+    s._advance(3, False, None)
+    assert s._host_pos == 9
+    with pytest.raises(ValueError, match='exceeds max_len'):
+        s._check_room(2, False)
+    assert s._admission(1, 10, None, None) == (None, None)
+    with pytest.raises(ValueError, match='exceeds max_len'):
+        s._admission(1, 11, None, None)
+
+
 def test_shared_decoder_refuses_slot_calls():
     d = _host_decoder(slots=False)
     with pytest.raises(RuntimeError, match='slots=True'):
