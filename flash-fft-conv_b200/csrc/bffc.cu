@@ -3029,34 +3029,49 @@ dim3 fir_grid(long long slabs, long long rows) { return dim3(unsigned(slabs), gr
   } while (0)
 
 template <class T>
-void fir_fwd_launch(const fir::Params& p, int P, bool gated, dim3 grid, cudaStream_t st) {
+void fir_fwd_launch(const fir::Params& p, int P, bool gated, bool docs, dim3 grid, cudaStream_t st) {
   FIR_P_SWITCH(P, {
-    if (gated) fir::fwd<T, PP, true><<<grid, fir::kThreads, 0, st>>>(p);
-    else fir::fwd<T, PP, false><<<grid, fir::kThreads, 0, st>>>(p);
+    auto kernel = docs ? (gated ? bffc::fir_docs::fwd<T, PP, true> : bffc::fir_docs::fwd<T, PP, false>)
+                       : (gated ? fir::fwd<T, PP, true> : fir::fwd<T, PP, false>);
+    kernel<<<grid, fir::kThreads, 0, st>>>(p);
   });
 }
 
 template <class T>
-void fir_bwd_launch(const fir::Params& p, int P, bool gated, dim3 grid, cudaStream_t st) {
+void fir_bwd_launch(const fir::Params& p, int P, bool gated, bool docs, dim3 grid, cudaStream_t st) {
   FIR_P_SWITCH(P, {
-    if (gated) fir::bwd<T, PP, true><<<grid, fir::kThreads, 0, st>>>(p);
-    else fir::bwd<T, PP, false><<<grid, fir::kThreads, 0, st>>>(p);
+    auto kernel = docs ? (gated ? bffc::fir_docs::bwd<T, PP, true> : bffc::fir_docs::bwd<T, PP, false>)
+                       : (gated ? fir::bwd<T, PP, true> : fir::bwd<T, PP, false>);
+    kernel<<<grid, fir::kThreads, 0, st>>>(p);
   });
 }
 
-}  // namespace
+// the document arguments of bffc_fir_fwd_varlen / bffc_fir_bwd_varlen (host side only: the offsets live on the device)
+int fir_docs_args(const char* fn, const int32_t* cu_seqlens, int n_docs, int B, int64_t L, int64_t L_docs) {
+  if (!cu_seqlens || misaligned(cu_seqlens, 4))
+    return fail(BFFC_ERR_INVALID, "%s: cu_seqlens is null or not 4-byte aligned", fn);
+  if (n_docs < B) return fail(BFFC_ERR_INVALID, "%s: n_docs=%d < B=%d (every row start is a document offset)", fn, n_docs, B);
+  if (L_docs <= L - 8 || L_docs > L)
+    return fail(BFFC_ERR_INVALID, "%s: L_docs=%lld outside (L - 8, L] = (%lld, %lld]", fn, (long long)L_docs,
+                (long long)L - 8, (long long)L);
+  if (int64_t(B) * L_docs > 0x7fffffffLL)
+    return fail(BFFC_ERR_INVALID, "%s: B * L_docs = %lld positions exceed the int32 offsets of cu_seqlens", fn,
+                (long long)(int64_t(B) * L_docs));
+  return 0;
+}
 
-extern "C" {
-
-int bffc_fir_fwd(const void* u, int64_t u_bstride, const void* pregate, int64_t pregate_bstride, const void* postgate,
-                 int64_t postgate_bstride, const float* k, int G, int Lk, int B, int H, int64_t L, int dtype, void* y,
-                 int64_t y_bstride, void* stream) {
-  const char* fn = "bffc_fir_fwd";
+// bffc_fir_fwd / bffc_fir_fwd_varlen (cu_seqlens non-null: the fir_docs kernel, its arguments checked by the caller)
+int fir_fwd(const char* fn, const void* u, int64_t u_bstride, const void* pregate, int64_t pregate_bstride,
+            const void* postgate, int64_t postgate_bstride, const float* k, int G, int Lk, int B, int H, int64_t L,
+            int dtype, void* y, int64_t y_bstride, const int32_t* cu_seqlens, int n_docs, int64_t L_docs,
+            void* stream) {
   const bool gated = pregate != nullptr;
   if (int rc = gated ? fir_args(fn, G, Lk, B, H, L, dtype, k, pregate, postgate,
                                 {{u, u_bstride}, {pregate, pregate_bstride}, {postgate, postgate_bstride}, {y, y_bstride}})
                      : fir_args(fn, G, Lk, B, H, L, dtype, k, pregate, postgate, {{u, u_bstride}, {y, y_bstride}}))
     return rc;
+  if (cu_seqlens)
+    if (int rc = fir_docs_args(fn, cu_seqlens, n_docs, B, L, L_docs)) return rc;
   if (int rc = check_device()) return rc;
   fir::Params p{};
   p.u = static_cast<const uint16_t*>(u); p.u_bs = u_bstride;
@@ -3064,25 +3079,21 @@ int bffc_fir_fwd(const void* u, int64_t u_bstride, const void* pregate, int64_t 
   p.post = static_cast<const uint16_t*>(postgate); p.post_bs = postgate_bstride;
   p.y = static_cast<uint16_t*>(y); p.y_bs = y_bstride;
   p.k = k; p.L = L; p.slabs = fir::slabs_of(L); p.B = B; p.H = H; p.gs = H / G; p.Lk = Lk;
+  p.cu = cu_seqlens; p.ndocs = n_docs; p.Ld = int(L_docs);
   const dim3 grid = fir_grid(p.slabs, static_cast<long long>(B) * H);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   g_launches = 0;
-  if (dtype == BFFC_DTYPE_FP16) fir_fwd_launch<__half>(p, fir::p_of(Lk), gated, grid, st);
-  else fir_fwd_launch<__nv_bfloat16>(p, fir::p_of(Lk), gated, grid, st);
+  if (dtype == BFFC_DTYPE_FP16) fir_fwd_launch<__half>(p, fir::p_of(Lk), gated, cu_seqlens != nullptr, grid, st);
+  else fir_fwd_launch<__nv_bfloat16>(p, fir::p_of(Lk), gated, cu_seqlens != nullptr, grid, st);
   return launched();
 }
 
-size_t bffc_fir_workspace_bytes(int B, int H, int64_t L, int Lk) {
-  if (B < 1 || H < 1 || L < 1 || Lk < 1 || Lk > fir::kMaxLk) return 0;
-  return std::max<size_t>(size_t(B) * size_t(H) * size_t(fir::slabs_of(L)) * size_t(Lk) * sizeof(float), 16);
-}
-
-int bffc_fir_bwd(const void* dout, int64_t dout_bstride, const void* u, int64_t u_bstride, const void* pregate,
-                 int64_t pregate_bstride, const void* postgate, int64_t postgate_bstride, const float* k, int G, int Lk,
-                 int B, int H, int64_t L, int dtype, void* du, int64_t du_bstride, void* dpregate,
-                 int64_t dpregate_bstride, void* dpostgate, int64_t dpostgate_bstride, float* dk, void* workspace,
-                 size_t workspace_bytes, void* stream) {
-  const char* fn = "bffc_fir_bwd";
+// bffc_fir_bwd / bffc_fir_bwd_varlen
+int fir_bwd(const char* fn, const void* dout, int64_t dout_bstride, const void* u, int64_t u_bstride,
+            const void* pregate, int64_t pregate_bstride, const void* postgate, int64_t postgate_bstride, const float* k,
+            int G, int Lk, int B, int H, int64_t L, int dtype, void* du, int64_t du_bstride, void* dpregate,
+            int64_t dpregate_bstride, void* dpostgate, int64_t dpostgate_bstride, float* dk, void* workspace,
+            size_t workspace_bytes, const int32_t* cu_seqlens, int n_docs, int64_t L_docs, void* stream) {
   const bool gated = pregate != nullptr;
   if (int rc = gated ? fir_args(fn, G, Lk, B, H, L, dtype, k, pregate, postgate,
                                 {{dout, dout_bstride}, {u, u_bstride}, {pregate, pregate_bstride},
@@ -3097,6 +3108,8 @@ int bffc_fir_bwd(const void* dout, int64_t dout_bstride, const void* u, int64_t 
   const size_t need = bffc_fir_workspace_bytes(B, H, L, Lk);
   if (!workspace || misaligned(workspace, 16) || workspace_bytes < need)
     return fail(BFFC_ERR_INVALID, "%s: a 16-byte aligned workspace of %zu bytes required", fn, need);
+  if (cu_seqlens)
+    if (int rc = fir_docs_args(fn, cu_seqlens, n_docs, B, L, L_docs)) return rc;
   if (int rc = check_device()) return rc;
   fir::Params p{};
   p.dout = static_cast<const uint16_t*>(dout); p.dout_bs = dout_bstride;
@@ -3108,14 +3121,64 @@ int bffc_fir_bwd(const void* dout, int64_t dout_bstride, const void* u, int64_t 
   p.dpost = static_cast<uint16_t*>(dpostgate); p.dpost_bs = dpostgate_bstride;
   p.k = k; p.dk = dk; p.part = static_cast<float*>(workspace);
   p.L = L; p.slabs = fir::slabs_of(L); p.B = B; p.H = H; p.gs = H / G; p.Lk = Lk;
+  p.cu = cu_seqlens; p.ndocs = n_docs; p.Ld = int(L_docs);
   const dim3 grid = fir_grid(p.slabs, static_cast<long long>(B) * H);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   g_launches = 0;
-  if (dtype == BFFC_DTYPE_FP16) fir_bwd_launch<__half>(p, fir::p_of(Lk), gated, grid, st);
-  else fir_bwd_launch<__nv_bfloat16>(p, fir::p_of(Lk), gated, grid, st);
+  if (dtype == BFFC_DTYPE_FP16) fir_bwd_launch<__half>(p, fir::p_of(Lk), gated, cu_seqlens != nullptr, grid, st);
+  else fir_bwd_launch<__nv_bfloat16>(p, fir::p_of(Lk), gated, cu_seqlens != nullptr, grid, st);
   if (int rc = launched()) return rc;
   fir::dk_reduce<<<unsigned(G), fir::kReduceThreads, 0, st>>>(p);
   return launched();
+}
+
+}  // namespace
+
+extern "C" {
+
+int bffc_fir_fwd(const void* u, int64_t u_bstride, const void* pregate, int64_t pregate_bstride, const void* postgate,
+                 int64_t postgate_bstride, const float* k, int G, int Lk, int B, int H, int64_t L, int dtype, void* y,
+                 int64_t y_bstride, void* stream) {
+  return fir_fwd("bffc_fir_fwd", u, u_bstride, pregate, pregate_bstride, postgate, postgate_bstride, k, G, Lk, B, H, L,
+                 dtype, y, y_bstride, nullptr, 0, L, stream);
+}
+
+int bffc_fir_fwd_varlen(const void* u, int64_t u_bstride, const void* pregate, int64_t pregate_bstride,
+                        const void* postgate, int64_t postgate_bstride, const float* k, int G, int Lk, int B, int H,
+                        int64_t L, int dtype, void* y, int64_t y_bstride, const int32_t* cu_seqlens, int n_docs,
+                        int64_t L_docs, void* stream) {
+  const char* fn = "bffc_fir_fwd_varlen";
+  if (!cu_seqlens) return fail(BFFC_ERR_INVALID, "%s: cu_seqlens is null", fn);
+  return fir_fwd(fn, u, u_bstride, pregate, pregate_bstride, postgate, postgate_bstride, k, G, Lk, B, H, L, dtype, y,
+                 y_bstride, cu_seqlens, n_docs, L_docs, stream);
+}
+
+size_t bffc_fir_workspace_bytes(int B, int H, int64_t L, int Lk) {
+  if (B < 1 || H < 1 || L < 1 || Lk < 1 || Lk > fir::kMaxLk) return 0;
+  return std::max<size_t>(size_t(B) * size_t(H) * size_t(fir::slabs_of(L)) * size_t(Lk) * sizeof(float), 16);
+}
+
+int bffc_fir_bwd(const void* dout, int64_t dout_bstride, const void* u, int64_t u_bstride, const void* pregate,
+                 int64_t pregate_bstride, const void* postgate, int64_t postgate_bstride, const float* k, int G, int Lk,
+                 int B, int H, int64_t L, int dtype, void* du, int64_t du_bstride, void* dpregate,
+                 int64_t dpregate_bstride, void* dpostgate, int64_t dpostgate_bstride, float* dk, void* workspace,
+                 size_t workspace_bytes, void* stream) {
+  return fir_bwd("bffc_fir_bwd", dout, dout_bstride, u, u_bstride, pregate, pregate_bstride, postgate,
+                 postgate_bstride, k, G, Lk, B, H, L, dtype, du, du_bstride, dpregate, dpregate_bstride, dpostgate,
+                 dpostgate_bstride, dk, workspace, workspace_bytes, nullptr, 0, L, stream);
+}
+
+int bffc_fir_bwd_varlen(const void* dout, int64_t dout_bstride, const void* u, int64_t u_bstride, const void* pregate,
+                        int64_t pregate_bstride, const void* postgate, int64_t postgate_bstride, const float* k, int G,
+                        int Lk, int B, int H, int64_t L, int dtype, void* du, int64_t du_bstride, void* dpregate,
+                        int64_t dpregate_bstride, void* dpostgate, int64_t dpostgate_bstride, float* dk,
+                        void* workspace, size_t workspace_bytes, const int32_t* cu_seqlens, int n_docs,
+                        int64_t L_docs, void* stream) {
+  const char* fn = "bffc_fir_bwd_varlen";
+  if (!cu_seqlens) return fail(BFFC_ERR_INVALID, "%s: cu_seqlens is null", fn);
+  return fir_bwd(fn, dout, dout_bstride, u, u_bstride, pregate, pregate_bstride, postgate, postgate_bstride, k, G, Lk,
+                 B, H, L, dtype, du, du_bstride, dpregate, dpregate_bstride, dpostgate, dpostgate_bstride, dk,
+                 workspace, workspace_bytes, cu_seqlens, n_docs, L_docs, stream);
 }
 
 }  // extern "C"

@@ -25,6 +25,8 @@
 #include <cstdint>
 #include <type_traits>
 
+#include "doc_search.cuh"
+
 namespace bffc {
 namespace dw {
 
@@ -201,55 +203,7 @@ struct Shape {
 // validated; the searches stay inside cu[0 .. ndocs] whatever they hold.
 //
 // A thread keeps its taps as bit masks (bit k: tap k kept), one word per position: the forward's, or in the backward
-// the partials' in bits [0, KMAX) and du's in bits [KMAX, 2 KMAX).
-//
-// index d in [lo, hi) with cu[d] <= f < cu[d + 1], given cu[lo] <= f < cu[hi]
-__device__ __forceinline__ int find_doc(const int* __restrict__ cu, int lo, int hi, int f) {
-  while (hi - lo > 1) {
-    const int mid = (lo + hi) >> 1;
-    if (__ldg(cu + mid) <= f) lo = mid;
-    else hi = mid;
-  }
-  return lo;
-}
-
-// bits [a, b) of a 32-bit word (a, b clamped to [0, 32])
-__device__ __forceinline__ uint32_t bit_range(int a, int b) {
-  a = min(max(a, 0), 32);
-  b = min(max(b, a), 32);
-  const uint32_t below_b = b == 32 ? 0xffffffffu : (1u << b) - 1u, below_a = a == 32 ? 0xffffffffu : (1u << a) - 1u;
-  return below_b & ~below_a;
-}
-
-// The document of a thread's positions in row b, for positions visited in non-decreasing order: a position inside the
-// current document costs a compare; crossing a boundary searches from the current document on.
-struct DocCursor {
-  const int* cu;
-  int base, L, P, ndocs, d, o, e;     // [o, e): the current document, row coordinates (empty before the first search)
-  __device__ __forceinline__ DocCursor(const Shape& sh, int b)
-      : cu(sh.cu), base(b * sh.L), L(sh.L), P(sh.P), ndocs(sh.ndocs), d(0), o(0), e(0) {}
-  // (klo, khi) of position p; no taps past the row
-  __device__ __forceinline__ int2 taps(int p) {
-    if (p >= L) return make_int2(0, 0);
-    if (p >= e) {
-      d = find_doc(cu, d, ndocs, base + p);
-      o = __ldg(cu + d) - base;
-      e = __ldg(cu + d + 1) - base;
-    }
-    return make_int2(P - (p - o), P + (e - p));
-  }
-  __device__ __forceinline__ uint32_t fwd_mask(int p) {
-    const int2 t = taps(p);
-    return bit_range(t.x, t.y);
-  }
-  template <int KMAX>
-  __device__ __forceinline__ auto bwd_mask(int p) {
-    using M = std::conditional_t<(2 * KMAX <= 32), uint32_t, uint64_t>;
-    const int2 t = taps(p);
-    // both ranges cut at KMAX: the partials' bits must not reach the du half
-    return M(bit_range(t.x, min(t.y, KMAX))) | (M(bit_range(2 * P - t.y + 1, min(2 * P - t.x + 1, KMAX))) << KMAX);
-  }
-};
+// the partials' in bits [0, KMAX) and du's in bits [KMAX, 2 KMAX).  find_doc and DocCursor are in doc_search.cuh.
 template <class M>
 __device__ __forceinline__ float tap_in(float x, M mask, int bit) { return ((mask >> bit) & 1) ? x : 0.f; }
 

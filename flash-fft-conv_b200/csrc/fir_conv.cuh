@@ -1,4 +1,5 @@
-// fir_conv.cuh — causal convolution with filters of up to 128 taps on the tensor cores (bffc_fir_fwd, bffc_fir_bwd).
+// fir_conv.cuh — causal convolution with filters of up to 128 taps on the tensor cores (bffc_fir_fwd, bffc_fir_bwd;
+// with packed documents bffc_fir_fwd_varlen, bffc_fir_bwd_varlen: the kDoc path below the helpers).
 //
 //   y[t] = postgate[t] * sum_{m < min(t + 1, Lk)} k[g, m] z[t - m],   z = u * pregate,   g = h / (H / G)
 //
@@ -33,6 +34,8 @@
 
 #include <type_traits>
 
+#include "doc_search.cuh"
+
 namespace bffc {
 namespace fir {
 
@@ -61,6 +64,8 @@ struct Params {
   float* dk;
   long long L, slabs;
   int B, H, gs, Lk;
+  const int* cu;                                   // packed documents (the fir_docs kernels): offsets cu[0 .. ndocs]
+  int ndocs, Ld;                                   // into the flattened (B, Ld) positions, Ld in (L - 8, L]
 };
 
 template <class T> __device__ __forceinline__ float to_f(uint16_t x);
@@ -218,17 +223,184 @@ __device__ __forceinline__ void toeplitz_mma(float (&acc)[8][4], const uint16_t*
   }
 }
 
-template <class T, int P, bool kGated>
-__global__ void __launch_bounds__(kThreads, 4) fwd(const Params p) {
+// ------------------------------------------------------------------------------------------------ packed documents
+// Row b holds documents [cu[d] - b Ld, cu[d + 1] - b Ld) of its first Ld positions; the padding [Ld, L) belongs to no
+// document.  The segments of a row are its documents and, from Ld on, the padding.  A boundary c (a segment start) is
+// interior when 0 < c < L.  For a tile of outputs t0 .. t0 + 4095:
+//   forward row R (outputs t0 + 64 R ..) is dirty when an interior boundary lies in (t0 + 64 (R - P), t0 + 64 R + 64),
+//     the positions its GEMM reads (Z rows R - P .. R);
+//   backward row R is dirty when one lies in (t0 + 64 R, t0 + 64 (R + P + 1)), the positions du's GEMM reads.
+// A clean row's GEMM touches one document only (and zeros outside the row), so it is exact, and its outputs are the plain
+// kernel's bits.  Dirty rows are recomputed on the CUDA cores with each lag of another segment left out by selection: a
+// NaN or inf in one document reaches no other one.  dk: the cut outputs of forward-dirty rows (lags reaching past their
+// segment's start, or in the padding) leave W before the diagonal-sum GEMM, and their same-document pairs are added in
+// a fixed order (dk_pairs).
+//
+// The window of a tile is the positions t0 - 64 P .. t0 + kHi (kHi = 4096 forward, 4096 + 64 P backward); reach[i] is
+// min(Lk - 1, t - s) for its position t = t0 - 64 P + i in the segment [s, e): t - m lies in t's segment iff
+// m <= reach[i], and t + m iff m <= reach[i + m].  One search per tile finds the first segment; tiles without an
+// interior boundary in the window skip the rest.
+struct DocTile {
+  uint8_t reach[kTile + 4 * kBlock];
+  uint8_t fdirty[kRows], bdirty[kRows];            // forward / backward dirty rows
+  int d0, dirty;                                   // the first segment's document, whether the window has a boundary
+};
+constexpr int kDocWords = int(sizeof(DocTile) + 3) / 4;
+
+// thread 0: the first segment reaching into the window, and whether an interior boundary follows inside it
+template <int P, int kHi>
+__device__ __forceinline__ void doc_find(const Params& p, long long b, long long t0, DocTile& dt) {
+  if (threadIdx.x != 0) return;
+  const int base = int(b) * p.Ld;
+  const int d = find_doc(p.cu, 0, p.ndocs, base + int(max(t0 - P * kBlock, 0LL)));
+  const long long c = min(__ldg(p.cu + d + 1) - base, p.Ld);
+  dt.d0 = d;
+  dt.dirty = c < min(t0 + kHi, p.L);
+}
+
+// every thread, on a tile with a boundary: reach[] and the dirty rows, one thread per segment.  Ends with a barrier.
+template <int P, int kHi>
+__device__ void doc_tables(const Params& p, long long b, long long t0, DocTile& dt) {
+  const int Lk1 = p.Lk - 1;
+  for (int i = threadIdx.x; i < int(sizeof(dt.reach)) / 4; i += kThreads)
+    reinterpret_cast<uint32_t*>(dt.reach)[i] = 0x01010101u * uint32_t(Lk1);
+  if (threadIdx.x < 2 * kRows / 4) reinterpret_cast<uint32_t*>(dt.fdirty)[threadIdx.x] = 0u;
+  __syncthreads();
+  const long long base = b * p.Ld, lo = t0 - P * kBlock, hi = t0 + kHi;
+  for (int j = dt.d0 + threadIdx.x; j <= p.ndocs; j += kThreads) {
+    const long long s = min(max(__ldg(p.cu + j) - base, 0LL), (long long)p.Ld);
+    if (s >= hi) break;
+    const bool pad = s == p.Ld;                                // the padding, and the positions past the row
+    const long long e = pad ? hi : j < p.ndocs ? min(max(__ldg(p.cu + j + 1) - base, s), (long long)p.Ld) : s;
+    for (long long t = max(s, lo); t < min(min(e, s + Lk1), hi); ++t) dt.reach[t - lo] = uint8_t(t - s);
+    if (s > 0 && s < p.L) {
+      const int q = int(s - t0);
+      for (int R = max(q >> 6, 0); R <= min((q + kBlock * P - 1) >> 6, kRows - 1); ++R) dt.fdirty[R] = 1;
+      for (int R = max((q >> 6) - P, 0); R <= min((q - 1) >> 6, kRows - 1); ++R) dt.bdirty[R] = 1;
+    }
+    if (pad) break;
+  }
+  __syncthreads();
+}
+
+// The CUDA-core sums below give each thread 4 consecutive outputs (uchar4 of reach) and slide their operands along the
+// lags, so a tap and one new operand are read per lag for 4 products.  Each output still sums its lags in ascending
+// order with one fmaf each.
+
+// sf rows of the forward-dirty outputs: unscale * sum_{m <= reach} k^[m] z[t - m], m ascending
+template <class T, int P>
+__device__ __forceinline__ void fwd_dirty(float* sf, const uint16_t* zs, const uint16_t* taps, const DocTile& dt,
+                                          float unscale) {
+  auto z = [&](int x) { return to_f<T>(zs[(x >> 6) * kS + (x & 63)]); };
+  for (int i = 4 * threadIdx.x; i < kTile; i += 4 * kThreads) {
+    if (!dt.fdirty[i >> 6]) continue;
+    const int q = i + P * kBlock;                          // window position of output i; z[t_j - m] = z(q + j - m)
+    const uchar4 n = *reinterpret_cast<const uchar4*>(dt.reach + q);
+    const int nmax = max(max(n.x, n.y), max(n.z, n.w));
+    float a0 = 0.f, a1 = 0.f, a2 = 0.f, a3 = 0.f;
+    float z0 = z(q), z1 = z(q + 1), z2 = z(q + 2), z3 = z(q + 3);
+    for (int m = 0; m <= nmax; ++m) {
+      const float kk = to_f<T>(taps[m]);
+      if (m <= n.x) a0 = fmaf(kk, z0, a0);
+      if (m <= n.y) a1 = fmaf(kk, z1, a1);
+      if (m <= n.z) a2 = fmaf(kk, z2, a2);
+      if (m <= n.w) a3 = fmaf(kk, z3, a3);
+      z3 = z2;
+      z2 = z1;
+      z1 = z0;
+      z0 = z(max(q - m - 1, 0));
+    }
+    *reinterpret_cast<float4*>(sf + (i >> 6) * kSF + (i & 63)) =
+        make_float4(a0 * unscale, a1 * unscale, a2 * unscale, a3 * unscale);
+  }
+}
+
+// sf rows of the backward-dirty outputs: unscale * sum_m k^[m] w[t + m] over t's segment, m ascending
+template <class T, int P>
+__device__ __forceinline__ void du_dirty(float* sf, const uint16_t* ws, const uint16_t* taps, const DocTile& dt,
+                                         float unscale, int Lk) {
+  constexpr int kLast = (kRows + P) * kBlock - 1;           // the W tile's last sample
+  auto w = [&](int x) { x = min(x, kLast); return to_f<T>(ws[(x >> 6) * kS + (x & 63)]); };
+  for (int i = 4 * threadIdx.x; i < kTile; i += 4 * kThreads) {
+    if (!dt.bdirty[i >> 6]) continue;
+    const int q = i + P * kBlock;                          // w[t_j + m] = w(i + j + m), its reach reach[q + j + m]
+    float a0 = 0.f, a1 = 0.f, a2 = 0.f, a3 = 0.f;
+    float w0 = w(i), w1 = w(i + 1), w2 = w(i + 2), w3 = w(i + 3);
+    int r0 = dt.reach[q], r1 = dt.reach[q + 1], r2 = dt.reach[q + 2], r3 = dt.reach[q + 3];
+    bool l0 = true, l1 = true, l2 = true, l3 = true;      // t_j + m still in t_j's segment
+    for (int m = 0; m < Lk; ++m) {
+      l0 = l0 && r0 >= m;
+      l1 = l1 && r1 >= m;
+      l2 = l2 && r2 >= m;
+      l3 = l3 && r3 >= m;
+      if (!(l0 || l1 || l2 || l3)) break;
+      const float kk = to_f<T>(taps[m]);
+      if (l0) a0 = fmaf(kk, w0, a0);
+      if (l1) a1 = fmaf(kk, w1, a1);
+      if (l2) a2 = fmaf(kk, w2, a2);
+      if (l3) a3 = fmaf(kk, w3, a3);
+      w0 = w1;
+      w1 = w2;
+      w2 = w3;
+      w3 = w(i + m + 4);
+      r0 = r1;
+      r1 = r2;
+      r2 = r3;
+      r3 = dt.reach[min(q + m + 4, int(sizeof(dt.reach)) - 1)];
+    }
+    *reinterpret_cast<float4*>(sf + (i >> 6) * kSF + (i & 63)) =
+        make_float4(a0 * unscale, a1 * unscale, a2 * unscale, a3 * unscale);
+  }
+}
+
+// dk of the dirty tile's cut outputs: the outputs t of forward-dirty rows whose lags reach past their segment's start
+// (reach < Lk - 1) or that lie in the padding (t >= Ld).  Every other W entry's GEMM pairs lie in its own document.
+__device__ __forceinline__ bool dk_cut(const DocTile& dt, int i, int q, long long t0, long long Ld, int Lk) {
+  return dt.fdirty[i >> 6] && (dt.reach[q] < Lk - 1 || t0 + i >= Ld);
+}
+
+// The cut outputs' same-document pairs w[t] z[t - m]: thread (m, c) = (tid % NL, tid / NL), NL = the lag slots (a power
+// of two >= Lk), sums chunk c of the tile's rows (64 NL / kThreads rows) in ascending t into part[c * NL + m].
+template <class T, int P>
+__device__ __forceinline__ void dk_pairs(float* part, const uint16_t* ws, const uint16_t* zs, const DocTile& dt,
+                                         long long t0, long long Ld, int Lk, int NL) {
+  const int m = threadIdx.x & (NL - 1), c = threadIdx.x / NL, rows = kRows * NL / kThreads;
+  auto z = [&](int x) { return to_f<T>(zs[(x >> 6) * kS + (x & 63)]); };
+  float sum = 0.f;
+  for (int R = c * rows; R < (c + 1) * rows && m < Lk; ++R) {
+    if (!dt.fdirty[R]) continue;
+    for (int i = R * kBlock; i < R * kBlock + kBlock; i += 4) {
+      const int q = i + P * kBlock;
+      const uchar4 r = *reinterpret_cast<const uchar4*>(dt.reach + q);
+      if (min(min(r.x, r.y), min(r.z, r.w)) == Lk - 1) continue;     // none of the four is cut inside a document
+      const int rr[4] = {r.x, r.y, r.z, r.w};
+#pragma unroll
+      for (int j = 0; j < 4; ++j)
+        if (rr[j] < Lk - 1 && rr[j] >= m && t0 + i + j < Ld)
+          sum = fmaf(to_f<T>(ws[R * kS + (i & 63) + j]), z(q + j - m), sum);
+    }
+  }
+  part[c * NL + m] = sum;
+}
+
+// ------------------------------------------------------------------------------------------------------ kernels
+// The bodies serve the plain kernels (fir::fwd, fir::bwd) and, with kDoc, the packed-document ones (fir_docs::).  The
+// forward body takes Params by value and the backward's by reference: so the plain kernels compile to the same code
+// as when they were written as kernels.
+template <class T, int P, bool kGated, bool kDoc>
+__device__ __forceinline__ void fwd_body(const Params p) {
   constexpr int kNF = 8 * P + 2;
   constexpr int kZ = kRows + P;
-  constexpr int kBytes = kZ * kS * 2 > kRows * kSF * 4 ? kZ * kS * 2 : kRows * kSF * 4;
-  __shared__ alignas(16) unsigned char smem[kBytes];          // the Z tile, then (aliased) the fp32 staging tile
-  __shared__ uint32_t frag_s[kNF * 64];
+  constexpr int kZB = kZ * kS * 2, kSB = kRows * kSF * 4;
+  constexpr int kBytes = kDoc ? kZB + kSB : kZB > kSB ? kZB : kSB;
+  constexpr int kFrag = kDoc && kDocWords > kNF * 64 ? kDocWords : kNF * 64;
+  __shared__ alignas(16) unsigned char smem[kBytes];          // the Z tile, then (aliased; kDoc: after it) the staging
+  __shared__ uint32_t frag_s[kFrag];                           // kDoc: the tile's DocTile once bf holds the fragments
   __shared__ uint16_t taps[kMaxLk];
   __shared__ float red[kWarps];
   uint16_t* zs = reinterpret_cast<uint16_t*>(smem);
-  float* sf = reinterpret_cast<float*>(smem);
+  float* sf = reinterpret_cast<float*>(smem + (kDoc ? kZB : 0));
+  DocTile* dt = reinterpret_cast<DocTile*>(frag_s);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const long long rows = (long long)p.B * p.H;
   const long long tile0 = (long long)blockIdx.x * kSlabTiles;
@@ -259,12 +431,22 @@ __global__ void __launch_bounds__(kThreads, 4) fwd(const Params p) {
       const long long t0 = tile * kTile;
       __syncthreads();                                         // the previous tile's staging reads are done
       load_tile<T, kGated, kZ>(zs, u, pre, t0 - P * kBlock, p.L);
+      if constexpr (kDoc) doc_find<P, kTile>(p, b, t0, *dt);
       __syncthreads();
+      bool dirty = false;
+      if constexpr (kDoc) {
+        dirty = dt->dirty;
+        if (dirty) doc_tables<P, kTile>(p, b, t0, *dt);
+      }
       float acc[8][4];
       toeplitz_mma<T, P, false>(acc, zs, [&](int f, int r) { return bf[f][r]; }, warp, lane);
       __syncthreads();                                         // Z reads are done before the staging tile aliases it
       stage(sf, acc, unscale, warp, lane);
       __syncthreads();
+      if (dirty) {
+        fwd_dirty<T, P>(sf, zs, taps, *dt, unscale);
+        __syncthreads();
+      }
 #pragma unroll
       for (int i = 0; i < kTile / 8 / kThreads; ++i) {
         const int v = threadIdx.x + i * kThreads;
@@ -295,14 +477,21 @@ __global__ void __launch_bounds__(kThreads, 4) fwd(const Params p) {
 // The backward: per tile of one row, (gated) dpostgate from the recomputed forward sum, then du (and dpregate) from
 // dZ, then the dk partial of every lag from C_r's diagonals, accumulated over the slab's tiles in order.
 template <class T, int P, bool kGated>
-__global__ void __launch_bounds__(kThreads, 3) bwd(const Params p) {
+__global__ void __launch_bounds__(kThreads, 4) fwd(const Params p) {
+  fwd_body<T, P, kGated, false>(p);
+}
+
+template <class T, int P, bool kGated, bool kDoc>
+__device__ __forceinline__ void bwd_body(const Params& p) {
   constexpr int kNF = 8 * P + 2;
   constexpr int kZ = kRows + P;
+  constexpr int kFrag = kDoc && kDocWords > kNF * 64 ? kDocWords : kNF * 64;
   __shared__ alignas(16) uint16_t zs[kZ * kS];
   __shared__ alignas(16) uint16_t ws[kZ * kS];
   __shared__ alignas(16) float sf[kRows * kSF];
   __shared__ uint32_t frag_f[kGated ? kNF * 64 : 1];          // forward fragments (gated: the recomputed y)
-  __shared__ uint32_t frag_t[kNF * 64];
+  __shared__ uint32_t frag_t[kFrag];                           // kDoc: the tile's DocTile once bt holds the fragments
+  DocTile* dt = reinterpret_cast<DocTile*>(frag_t);
   __shared__ uint16_t taps[kMaxLk];
   __shared__ float dkacc[kMaxLk];
   __shared__ float red[kWarps];
@@ -343,7 +532,13 @@ __global__ void __launch_bounds__(kThreads, 3) bwd(const Params p) {
       __syncthreads();
       load_tile<T, kGated, kZ>(zs, u, pre, t0 - P * kBlock, p.L);
       load_tile<T, kGated, kZ>(ws, dout, post, t0, p.L);
+      if constexpr (kDoc) doc_find<P, kTile + P * kBlock>(p, b, t0, *dt);
       __syncthreads();
+      bool dirty = false;
+      if constexpr (kDoc) {
+        dirty = dt->dirty;
+        if (dirty) doc_tables<P, kTile + P * kBlock>(p, b, t0, *dt);
+      }
       float acc[8][4];
       // element-wise epilogue over the tile's 16-byte vectors: f(t, 8 staged fp32 values)
       auto epilogue = [&](auto&& f) {
@@ -377,16 +572,38 @@ __global__ void __launch_bounds__(kThreads, 3) bwd(const Params p) {
         toeplitz_mma<T, P, false>(acc, zs, [&](int f, int r) { return frag_f[(f * 2 + r) * 32 + lane]; }, warp, lane);
         stage(sf, acc, unscale, warp, lane);
         __syncthreads();
+        if (dirty) {
+          fwd_dirty<T, P>(sf, zs, taps, *dt, unscale);
+          __syncthreads();
+        }
         epilogue([&](long long t, const float (&o)[8]) { scaled_store(dpost, dout, t, o); });
         __syncthreads();
       }
       toeplitz_mma<T, P, true>(acc, ws, [&](int f, int r) { return bt[f][r]; }, warp, lane);
       stage(sf, acc, unscale, warp, lane);
       __syncthreads();
+      if (dirty) {
+        du_dirty<T, P>(sf, ws, taps, *dt, unscale, Lk);
+        __syncthreads();
+      }
       epilogue([&](long long t, const float (&o)[8]) {     // du = round(pregate * dz), dpregate = round(u * dz)
         scaled_store(du, pre, t, o);
         if (kGated) scaled_store(dpre, u, t, o);
       });
+      if (dirty) {                                             // the cut outputs' dk pairs, in the free staging tile;
+        const int NL = Lk <= 8 ? 8 : Lk <= 16 ? 16 : Lk <= 32 ? 32 : Lk <= 64 ? 64 : 128;   // then their W entries
+        __syncthreads();                                       // leave the diagonal-sum GEMM
+        dk_pairs<T, P>(sf, ws, zs, *dt, t0, p.Ld, Lk, NL);
+        __syncthreads();
+        for (int i = threadIdx.x; i < kTile; i += kThreads)
+          if (dk_cut(*dt, i, i + P * kBlock, t0, p.Ld, Lk)) ws[(i >> 6) * kS + (i & 63)] = 0;
+        if (threadIdx.x < Lk) {
+          float sum = 0.f;
+          for (int c = 0; c < kThreads / NL; ++c) sum += sf[c * NL + threadIdx.x];
+          dkacc[threadIdx.x] += sum;
+        }
+        __syncthreads();
+      }
       // dk: C_r = W^T shift_r(Z); warp w owns C_r's rows j in [16 w, 16 w + 16), all 64 columns i
       const uint32_t wbase = smem_addr(ws), zbase = smem_addr(zs);
 #pragma unroll
@@ -436,6 +653,11 @@ __global__ void __launch_bounds__(kThreads, 3) bwd(const Params p) {
   }
 }
 
+template <class T, int P, bool kGated>
+__global__ void __launch_bounds__(kThreads, 3) bwd(const Params p) {
+  bwd_body<T, P, kGated, false>(p);
+}
+
 // dk[g, m] = sum of the group's slab partials: warp w sums partials q = w, w + 16, ... (q over member, channel of the
 // group, slab) in order, then the warps are summed in order.  One CTA per group.
 __global__ void __launch_bounds__(kReduceThreads) dk_reduce(const Params p) {
@@ -465,4 +687,20 @@ __global__ void __launch_bounds__(kReduceThreads) dk_reduce(const Params p) {
 }
 
 }  // namespace fir
+
+// The packed-document kernels (bffc_fir_fwd_varlen / bffc_fir_bwd_varlen): the plain ones plus the rule above; the
+// backward's dk partials go through fir::dk_reduce.
+namespace fir_docs {
+
+template <class T, int P, bool kGated>
+__global__ void __launch_bounds__(fir::kThreads, 4) fwd(const fir::Params p) {
+  fir::fwd_body<T, P, kGated, true>(p);
+}
+
+template <class T, int P, bool kGated>
+__global__ void __launch_bounds__(fir::kThreads, 3) bwd(const fir::Params p) {
+  fir::bwd_body<T, P, kGated, true>(p);
+}
+
+}  // namespace fir_docs
 }  // namespace bffc

@@ -151,6 +151,12 @@ SYMBOLS = {
     'bffc_fir_workspace_bytes': (_c.c_size_t, [_c.c_int, _c.c_int, _c.c_int64, _c.c_int]),
     'bffc_fir_bwd': (_c.c_int, [_c.c_void_p, _c.c_int64] * 4 + [_c.c_void_p] + [_c.c_int] * 4 + [_c.c_int64, _c.c_int]
                      + [_c.c_void_p, _c.c_int64] * 3 + [_c.c_void_p] * 2 + [_c.c_size_t, _c.c_void_p]),
+    'bffc_fir_fwd_varlen': (_c.c_int, [_c.c_void_p, _c.c_int64] * 3 + [_c.c_void_p] + [_c.c_int] * 4
+                            + [_c.c_int64, _c.c_int] + [_c.c_void_p, _c.c_int64, _c.c_void_p, _c.c_int, _c.c_int64,
+                                                        _c.c_void_p]),
+    'bffc_fir_bwd_varlen': (_c.c_int, [_c.c_void_p, _c.c_int64] * 4 + [_c.c_void_p] + [_c.c_int] * 4
+                            + [_c.c_int64, _c.c_int] + [_c.c_void_p, _c.c_int64] * 3 + [_c.c_void_p] * 2
+                            + [_c.c_size_t, _c.c_void_p, _c.c_int, _c.c_int64, _c.c_void_p]),
     'bffc_fir_decode_state_bytes': (_c.c_size_t, [_c.c_int] * 5),
     'bffc_fir_decode_row_len': (_c.c_int64, [_c.c_int] * 2),
     'bffc_fir_decode_step': (_c.c_int, [_c.c_void_p, _c.c_int64] * 3 + [_c.c_void_p] * 6 + [_c.c_int] * 4

@@ -10,6 +10,10 @@ L >= 1; channel slices of a projection are read in place (conv.batch_stride).  k
 dividing H and 1 <= Lk <= 128; channel h uses row h // (H // G) and dk is (G, Lk), summed over each group.  A ragged L
 is zero-padded to a multiple of 8, which does not change a causal result.
 
+docs=DocumentTable(...) keeps packed documents apart (bffc_fir_fwd_varlen / bffc_fir_bwd_varlen): each output sums the
+lags of its own document only, with the same rounded taps, and dk sums over every document.  Only the table's device
+offsets (cu_seqlens) are read, nothing on the host, so such a call can be captured in a CUDA graph.
+
 FirFilter(k) hands such a filter to the decoders (decode.py): LongConvDecoder(FirFilter(k), batch) and
 HyenaDecoder(short_filter, FirFilter(k), d_model, batch) decode fir_conv / fir_mixer with its rounded taps, in a state
 of the tail and the last Lk - 1 z values per (member, channel), whatever the context length.
@@ -77,21 +81,30 @@ def _view(t, Lp):
     return t, t.shape[1] * t.shape[2]
 
 
-def _fwd(u, k, pre, post):
+def _doc_args(docs, L):
+    """The trailing document arguments of bffc_fir_*_varlen: cu_seqlens, n_docs and the row length they count."""
+    return _ptr(docs.cu_seqlens), docs.n_docs, L
+
+
+def _fwd(u, k, pre, post, docs=None):
     B, H, L = u.shape
     Lp = (L + 7) // 8 * 8
     (uv, us), (pv, ps), (qv, qs) = _view(u, Lp), _view(pre, Lp), _view(post, Lp)
     k = k.contiguous()
     y = torch.empty((B, H, Lp), dtype=u.dtype, device=u.device)
+    args = (_ptr(uv), us, _ptr(pv), ps, _ptr(qv), qs, _ptr(k), k.shape[0], k.shape[1], B, H, Lp, _DT[u.dtype], _ptr(y),
+            H * Lp)
     with _on_device(u.device):
-        _lib.check(_lib.lib().bffc_fir_fwd(_ptr(uv), us, _ptr(pv), ps, _ptr(qv), qs, _ptr(k), k.shape[0], k.shape[1],
-                                           B, H, Lp, _DT[u.dtype], _ptr(y), H * Lp, _stream()))
+        if docs is None:
+            _lib.check(_lib.lib().bffc_fir_fwd(*args, _stream()))
+        else:
+            _lib.check(_lib.lib().bffc_fir_fwd_varlen(*args, *_doc_args(docs, L), _stream()))
     return y if Lp == L else y[..., :L].contiguous()
 
 
-def _bwd(dout, u, k, pre, post, out=None):
+def _bwd(dout, u, k, pre, post, out=None, docs=None):
     """(du, dk, dpre, dpost); out: (du, dpre, dpost) (B, H, L) views to write in place (rows contiguous, batch strides
-    qualifying, L a multiple of 8), else new tensors."""
+    qualifying, L a multiple of 8), else new tensors.  docs: a DocumentTable for (B, L)."""
     B, H, L = u.shape
     Lp = (L + 7) // 8 * 8
     gated = pre is not None
@@ -107,10 +120,13 @@ def _bwd(dout, u, k, pre, post, out=None):
     dk = torch.empty((G, Lk), dtype=torch.float32, device=u.device)
     l = _lib.lib()
     ws = torch.empty(l.bffc_fir_workspace_bytes(B, H, Lp, Lk), dtype=torch.uint8, device=u.device)
+    args = (_ptr(dv), ds, _ptr(uv), us, _ptr(pv), ps, _ptr(qv), qs, _ptr(k), G, Lk, B, H, Lp, _DT[u.dtype], _ptr(du),
+            dus, _ptr(dp), dps, _ptr(dq), dqs, _ptr(dk), _ptr(ws), ws.numel())
     with _on_device(u.device):
-        _lib.check(l.bffc_fir_bwd(_ptr(dv), ds, _ptr(uv), us, _ptr(pv), ps, _ptr(qv), qs, _ptr(k), G, Lk, B, H, Lp,
-                                  _DT[u.dtype], _ptr(du), dus, _ptr(dp), dps, _ptr(dq), dqs, _ptr(dk), _ptr(ws),
-                                  ws.numel(), _stream()))
+        if docs is None:
+            _lib.check(l.bffc_fir_bwd(*args, _stream()))
+        else:
+            _lib.check(l.bffc_fir_bwd_varlen(*args, *_doc_args(docs, L), _stream()))
     trim = (lambda t: t) if Lp == L else (lambda t: t[..., :L].contiguous())
     return trim(du), dk, (trim(dp) if gated else None), (trim(dq) if gated else None)
 
@@ -119,15 +135,16 @@ class FirConvFunc(torch.autograd.Function):
     """y = postgate * causal_conv(u * pregate, k) with k of at most 128 taps; gradients to u, k and the gates."""
 
     @staticmethod
-    def forward(ctx, u, k, pregate, postgate):
+    def forward(ctx, u, k, pregate, postgate, docs=None):
         ctx.save_for_backward(u, k, pregate, postgate)
-        return _fwd(u, k, pregate, postgate)
+        ctx.docs = docs
+        return _fwd(u, k, pregate, postgate, docs)
 
     @staticmethod
     def backward(ctx, dout):
         u, k, pre, post = ctx.saved_tensors
-        du, dk, dpre, dpost = _bwd(dout, u, k, pre, post)
-        return du, dk, dpre, dpost
+        du, dk, dpre, dpost = _bwd(dout, u, k, pre, post, docs=ctx.docs)
+        return du, dk, dpre, dpost, None
 
 
 class FirMixerFunc(torch.autograd.Function):
@@ -135,11 +152,11 @@ class FirMixerFunc(torch.autograd.Function):
     contiguous (B, 3D, L) gradient whose three slices the kernel writes directly."""
 
     @staticmethod
-    def forward(ctx, x1x2v, k, d_model):
+    def forward(ctx, x1x2v, k, d_model, docs=None):
         x1, x2, v = x1x2v.split(d_model, dim=1)
-        ctx.d_model = d_model
+        ctx.d_model, ctx.docs = d_model, docs
         ctx.save_for_backward(x1x2v, k)
-        return _fwd(v, k, x1, x2)
+        return _fwd(v, k, x1, x2, docs)
 
     @staticmethod
     def backward(ctx, dout):
@@ -151,8 +168,8 @@ class FirMixerFunc(torch.autograd.Function):
         dx1, dx2, dv = grad.split(D, dim=1)
         x1, x2, v = x1x2v.split(D, dim=1)
         # u = v, pregate = x1, postgate = x2: du -> [:, 2D:], dpregate -> [:, :D], dpostgate -> [:, D:2D]
-        _, dk, _, _ = _bwd(dout, v, k, x1, x2, out=(dv, dx1, dx2))
-        return (grad if Lp == L else grad[..., :L].contiguous()), dk, None
+        _, dk, _, _ = _bwd(dout, v, k, x1, x2, out=(dv, dx1, dx2), docs=ctx.docs)
+        return (grad if Lp == L else grad[..., :L].contiguous()), dk, None, None
 
 
 def fir_conv(u, k, pregate=None, postgate=None, docs=None):
@@ -160,20 +177,24 @@ def fir_conv(u, k, pregate=None, postgate=None, docs=None):
 
     u, pregate, postgate: (B, H, L) bf16 or fp16 CUDA tensors of one dtype, the gates both given or both None; channel
     slices of a projection are read in place.  k: fp32 (H, Lk) or (G, Lk) with G dividing H, 1 <= Lk <= 128.  Gradients
-    flow to u, k and the gates; dk has k's shape, summed over each group.  Packed documents are not supported: a
-    DocumentTable is refused."""
-    _docs.refuse(docs, 'fir_conv')
+    flow to u, k and the gates; dk has k's shape, summed over each group.  docs: a DocumentTable of (B, L) on u's device
+    keeps packed documents apart (each output sums the lags of its own document only); dk then sums over every
+    document."""
+    if docs is not None and isinstance(u, torch.Tensor) and u.dim() == 3:
+        _docs._check(docs, u)
     _check(u, k, (pregate, postgate), 'fir_conv')
-    return FirConvFunc.apply(u, k, pregate, postgate)
+    return FirConvFunc.apply(u, k, pregate, postgate, docs)
 
 
 def fir_mixer(x1x2v, k, d_model, docs=None):
     """y = x2 * causal_conv(x1 * v, k) with x1, x2, v = x1x2v.split(d_model, dim=1): hyena_mixer's gating for filters
     of 1 to 128 taps, on the (B, 3 d_model, L) projection in place.  k as for fir_conv.  The backward returns one
-    contiguous (B, 3 d_model, L) gradient, as hyena_mixer does."""
-    _docs.refuse(docs, 'fir_mixer')
+    contiguous (B, 3 d_model, L) gradient, as hyena_mixer does.  docs: as for fir_conv; Hyena-SE on packed rows is
+    fir_mixer(short_filter(x, table.cu_seqlens), k, d_model, docs=table)."""
     if not isinstance(x1x2v, torch.Tensor) or x1x2v.dim() != 3 or x1x2v.shape[1] != 3 * d_model:
         raise RuntimeError(f'fir_mixer: x1x2v must be (B, 3 * d_model = {3 * d_model}, L)')
     x1, x2, v = x1x2v.split(d_model, dim=1)
+    if docs is not None:
+        _docs._check(docs, v)
     _check(v, k, (x1, x2), 'fir_mixer')
-    return FirMixerFunc.apply(x1x2v, k, d_model)
+    return FirMixerFunc.apply(x1x2v, k, d_model, docs)

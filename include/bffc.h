@@ -754,6 +754,32 @@ int bffc_fir_bwd(const void* dout, int64_t dout_bstride, const void* u, int64_t 
                  size_t workspace_bytes, void* stream);
 
 /*
+ * Packed documents in the direct convolution (INTEGRATION.md §14.2): the arguments of bffc_fir_fwd / bffc_fir_bwd,
+ * then the documents as bffc_dwconv1d_*_varlen takes them: cu_seqlens (device int32, 4-byte aligned) holds n_docs + 1
+ * offsets into the flattened (B, L_docs) positions, non-decreasing from 0 to B * L_docs with every row start among
+ * them.  L_docs is the row length the offsets count, L - 8 < L_docs <= L (a caller that zero-pads a ragged row to L
+ * passes its own length); positions [L_docs, L) belong to no document, and their outputs are unspecified.  For a
+ * document [s, e) of row b and s <= t < e:
+ *   y[b, h, t] = postgate[b, h, t] * sum_{m <= min(Lk - 1, t - s)} k^[g, m] z[b, h, t - m]
+ * with the rounding points of the plain calls; du, dpregate, dpostgate are the gradients of that y and dk (G, Lk) the sum
+ * over every document.  Outputs whose blocks see no document boundary are the plain calls' bits; the others are summed
+ * on the CUDA cores over their own document only, so a NaN or inf in one document reaches no other one's outputs.  The
+ * backward uses bffc_fir_workspace_bytes of the shape; launches: 1 forward, 2 backward; dk is bit-reproducible.
+ * n_docs >= B and B * L_docs < 2^31 are checked with the other host arguments before the device is looked at; the
+ * contents of cu_seqlens are not (a malformed table may give wrong values, and every search stays inside it).
+ */
+int bffc_fir_fwd_varlen(const void* u, int64_t u_bstride, const void* pregate, int64_t pregate_bstride,
+                        const void* postgate, int64_t postgate_bstride, const float* k, int G, int Lk, int B, int H,
+                        int64_t L, int dtype, void* y, int64_t y_bstride, const int32_t* cu_seqlens, int n_docs,
+                        int64_t L_docs, void* stream);
+int bffc_fir_bwd_varlen(const void* dout, int64_t dout_bstride, const void* u, int64_t u_bstride, const void* pregate,
+                        int64_t pregate_bstride, const void* postgate, int64_t postgate_bstride, const float* k, int G,
+                        int Lk, int B, int H, int64_t L, int dtype, void* du, int64_t du_bstride, void* dpregate,
+                        int64_t dpregate_bstride, void* dpostgate, int64_t dpostgate_bstride, float* dk,
+                        void* workspace, size_t workspace_bytes, const int32_t* cu_seqlens, int n_docs,
+                        int64_t L_docs, void* stream);
+
+/*
  * Decoding with a short explicit filter of 1 to 128 taps (no plan; INTEGRATION.md §14.1): the operator bffc_fir_fwd
  * computes, y = round(s_postgate * 2^-s sum_{m < min(t + 1, Lk)} k^[g, m] z[t - m]) with fir_conv's rounded taps k^
  * (each group's row scaled by 2^s to max |k| in [1, 2) and rounded once to dtype) and z = round(s_u * s_pregate) of the
@@ -800,7 +826,7 @@ int bffc_fir_decode_finish(const void* ext_y, int dtype, int Lk, int64_t* pos, i
 /* Number of kernel launches the last bffc_fwd / bffc_bwd / bffc_fwd_host / filter-side transform /
  * bffc_dwconv1d_fwd (1) / bffc_dwconv1d_bwd (2) / bffc_conv_state_fill[_slots] (1) / bffc_conv_step[_slots] (2) /
  * bffc_conv_far_gather[_slots] (1) / bffc_conv_step_far[_slots] (2) / bffc_conv_extend_gather[_slots] (1) /
- * bffc_conv_extend_finish[_slots] (1) / bffc_docs_gather (1) / bffc_docs_scatter (1) / bffc_fir_fwd (1) / bffc_fir_bwd (2)
+ * bffc_conv_extend_finish[_slots] (1) / bffc_docs_gather (1) / bffc_docs_scatter (1) / bffc_fir_fwd[_varlen] (1) / bffc_fir_bwd[_varlen] (2)
  * / bffc_fir_decode_step (1) / bffc_fir_decode_gather (1) / bffc_fir_decode_finish (1) on this thread enqueued (bench.py).  A bffc_bwd* on a deterministic plan
  * counts the same launches as on a default plan, plus one slot sum per dk_f launch whose rows have S > 1 slabs. */
 int bffc_last_launch_count(void);
