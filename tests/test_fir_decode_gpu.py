@@ -3,9 +3,10 @@
 
 1. Per-element bound against fp64 of the rounded operator (fir_conv's taps k^, the decoder's s and z):
        |y - y64| <= ulp_dt(y64) + c * 2^-24 * |s_post| * sum_m |k^[m] z[t - m]|
-   for every output of a prefill, steps of T in {1, 5, 64} and an extend, at Lk in {1, 2, 7, 64, 65, 127, 128}, K in
-   {1, 3, 4}, bf16 and fp16, G in {H, H / 16, 1}, and (LongConvDecoder) every gate set.  The statistic
-   max (|y - y64| - ulp) / (2^-24 |s_post| sum|k^ z|) over all 193 cases (steps on the CUDA cores and prefills /
+   for every output of a prefill, steps of T in {1, 5, 64} and an extend, at Lk in {1, 2, 7, 9, 10, 33, 64, 65, 66, 100,
+   127, 128} (33 fills the step kernel's second group of lag slots m = lane + 32 i in part), K in {1, 3, 4}, bf16 and
+   fp16, G in {H, H / 16, 1}, and (LongConvDecoder) every gate set.  The model is tests/fir_model.py's.  The statistic
+   max (|y - y64| - ulp) / (2^-24 |s_post| sum|k^ z|) over all 312 cases (steps on the CUDA cores and prefills /
    extends on the tensor cores together) measured 0.48 on an H100 80GB HBM3 at 700 W (largest: LongConvDecoder,
    Lk = 127, postgate only, fp16); c = 1.5 is about 3x that.
 2. Bit identity: a fresh prefill's y is fir_mixer(short_filter(x)[..., :L], k, D) (fir_conv for LongConvDecoder) bit
@@ -23,11 +24,13 @@ import random
 import pytest
 import torch
 
+from fir_model import reference, rounded_taps, stat
+
 pytestmark = pytest.mark.gpu
 
 DEV = 'cuda'
 C_BOUND = 1.5
-LKS = [1, 2, 7, 64, 65, 127, 128]
+LKS = [1, 2, 7, 9, 10, 33, 64, 65, 66, 100, 127, 128]
 DTYPES = [torch.bfloat16, torch.float16]
 
 
@@ -50,40 +53,6 @@ def _short(ffc, D, K, g):
 
 def _filter(G, Lk, g):
     return (torch.randn(G, Lk, generator=g) / Lk ** 0.5).to(DEV).contiguous()
-
-
-def rounded_taps(k, dtype):
-    """fir_conv's k^ in fp64: each row scaled to max |k| in [1, 2), rounded once to dtype, unscaled"""
-    _, e = torch.frexp(k.abs().amax(1, keepdim=True))
-    e = e.clamp(-125, 127)
-    scaled = (k * torch.ldexp(torch.ones_like(k), 1 - e)).to(dtype)
-    return scaled.double() * torch.ldexp(torch.ones_like(k, dtype=torch.float64), (e - 1).double())
-
-
-def ulp(x, dtype):
-    mant, emin = (7, -126) if dtype == torch.bfloat16 else (10, -14)
-    e = torch.floor(torch.log2(x.abs().clamp_min(2.0 ** emin))).clamp_min(emin)
-    return 2.0 ** (e - mant)
-
-
-def reference(z, post, kh, H):
-    """(y64, |post| sum|k^ z|) of z (B, H, L) dtype, post (B, H, L) or None, k^ (G, Lk) fp64"""
-    kh = kh.repeat_interleave(H // kh.shape[0], 0)
-    zd, L = z.double(), z.shape[-1]
-    acc, mag = torch.zeros_like(zd), torch.zeros_like(zd)
-    for m in range(min(kh.shape[1], L)):
-        prod = kh[None, :, m, None] * zd[..., :L - m]
-        acc[..., m:] += prod
-        mag[..., m:] += prod.abs()
-    if post is not None:
-        acc, mag = acc * post.double(), mag * post.double().abs()
-    return acc, mag
-
-
-def stat(y, y64, mag, dtype):
-    """max over elements of (|y - y64| - ulp) / (2^-24 mag), 0 where the error is within one ulp"""
-    err = (y.double() - y64).abs() - ulp(y64, dtype)
-    return (err.clamp_min(0) / (mag * 2.0 ** -24).clamp_min(1e-300)).max().item()
 
 
 def hyena_z(sf, x, D):
